@@ -1,12 +1,12 @@
-"""bench.py -- images/s of the YOLOv5 hot path on B200 (BASELINE.json metric: images/sec @640 at 1/2/4/8 GPUs + NMS us/img +
+"""bench.py -- images/s of the YOLOv5 hot path on H100 (BASELINE.json metric: images/sec @640 at 1/2/4/8 GPUs + NMS us/img +
 conv tensor-pipe fraction).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload config3|yolov5s|...]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload config3|yolov5s|...] [--dump-outputs DIR]
 
 Default workload = BASELINE.json configs[2] ("config3", the configuration the >= 2x / >= 70 % targets are quoted on):
 yolov5l, 64 images of 640x640, bf16, forward + non_max_suppression through the public API of yolov5_b200.
   * N = 1: the whole batch of 64 on one GPU.  N > 1 (torchrun, one rank per GPU): the SAME 64 images sharded 64/N per GPU
-    ("scaling": "strong", as configs[2] states it: "bs=64 on 1/2/4/8 x B200 (data-parallel shard)"); the path shards over
+    ("scaling": "strong", as configs[2] states it: "bs=64 on 1/2/4/8 GPUs (data-parallel shard)"); the path shards over
     independent images, so there is NO data-path collective; value = 64 * steps / max-over-ranks time.  The sub-record
     `weak_scaling` runs 64 images PER GPU for N > 1.
   * value : inputs resident in HBM, CUDA-event timed, barrier + synchronize on both sides.
@@ -23,6 +23,12 @@ yolov5l, 64 images of 640x640, bf16, forward + non_max_suppression through the p
   * --impl reference : the reference's own CPU path.  The reference is pure Python and does not exist on the GPU box, so
     this is the oracle port (oracle/model_ref.py + oracle/nms_ref.py: the same torch-CPU fp32 expressions, pinned to the
     reference by tests/golden) on the host threads, on a bounded sample of the same workload.
+  * --dump-outputs DIR : after the timed steps of the main leg, rank 0 writes what the last timed step computed as
+    DIR/<name>.npy (float32 / float64).  Inference: the NMS detections (det_rows, det_index, det_count) and a fixed seeded sample
+    of the model output z (z_sample with its z_sample_rows).  Training: the loss items (loss_items: box, obj, cls) and a fixed
+    seeded sample of the updated parameters (param_sample with its param_sample_index into the concatenation of
+    model.parameters()).  Inputs and weights are seeded, so two builds run with the same arguments can be compared output for
+    output.  Not available with --impl reference (the CPU port is not the timed path).
 """
 from __future__ import annotations
 
@@ -64,7 +70,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    # data-sheet figures are not sustained rates: the "sustained" peak is left unknown instead of copied from the burst one
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=None, src="H100 SXM data sheet (not measured)")
 
 
 def synth_images_u8(bs, size, seed):
@@ -122,7 +129,7 @@ class StdoutGuard:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / power / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / power / throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -263,8 +270,36 @@ def timed(D: Dist, fn, steps, sampler=None):
 # ---------------------------------------------------------------------------------------------------------------------
 # inference leg
 # ---------------------------------------------------------------------------------------------------------------------
-def infer_leg(D: Dist, model_name, bs, size, dt, steps, warmup, extras=True, cpu_base=True, sustain_s=0.0, tag=""):
-    """forward + NMS on `bs` images per rank.  Returns the record dict on rank 0 (None elsewhere)."""
+def save_arrays(out_dir, arrays):
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), arr)
+
+
+def dump_outputs(out_dir, z, nms_out, sample_rows=1 << 16):
+    """Writes the last timed step's results: detections in full, z as a fixed seeded sample of (image, anchor) rows."""
+    rows, idx, cnt = nms_out
+    zf = z.reshape(-1, z.shape[-1])
+    n = min(sample_rows, zf.shape[0])
+    pick = np.sort(np.random.RandomState(0).choice(zf.shape[0], n, replace=False))
+    arrays = {"det_rows": rows.float().cpu().numpy(), "det_index": idx.cpu().numpy().astype(np.float64),
+              "det_count": cnt.cpu().numpy().astype(np.float64), "z_sample_rows": pick.astype(np.float64),
+              "z_sample": zf[torch.from_numpy(pick).to(zf.device)].float().cpu().numpy()}
+    save_arrays(out_dir, arrays)
+
+
+def dump_train_outputs(out_dir, items, model, sample=1 << 20):
+    """Writes the last timed training step's results: its loss items and a fixed seeded sample of the updated parameters."""
+    flat = torch.cat([q.detach().float().flatten() for q in model.parameters()])
+    n = min(sample, flat.numel())
+    pick = np.sort(np.random.RandomState(0).choice(flat.numel(), n, replace=False))
+    save_arrays(out_dir, {"loss_items": items.detach().float().cpu().numpy(), "param_sample_index": pick.astype(np.float64),
+                          "param_sample": flat[torch.from_numpy(pick).to(flat.device)].cpu().numpy()})
+
+
+def infer_leg(D: Dist, model_name, bs, size, dt, steps, warmup, extras=True, cpu_base=True, sustain_s=0.0, tag="", dump_dir=None):
+    """forward + NMS on `bs` images per rank.  Returns the record dict on rank 0 (None elsewhere).  `dump_dir`: rank 0 writes the
+    outputs of the last timed step there (see dump_outputs)."""
     from yolov5_b200 import _lib
     from yolov5_b200.cfg import model_cfg
     from yolov5_b200.models.yolo import DetectionModel, SegmentationModel
@@ -283,9 +318,13 @@ def infer_leg(D: Dist, model_name, bs, size, dt, steps, warmup, extras=True, cpu
     host_u8 = [torch.from_numpy(synth_images_u8(bs, size, 1000 + 10 * rank + i)).pin_memory() for i in range(n_rot)]
     dev_in = [(h.to(dev).to(TDT[dt]) / 255) for h in host_u8]
 
+    last = {}
+
     def step(i):
         z = model(dev_in[i % n_rot])[0]
-        return nms_device(z, **nms_kw)  # device-side result (rows, idx, count): no host sync inside `value`
+        last["z"] = z
+        last["nms"] = nms_device(z, **nms_kw)  # device-side result (rows, idx, count): no host sync inside `value`
+        return last["nms"]
 
     for i in range(warmup):
         out = step(i)
@@ -298,6 +337,8 @@ def infer_leg(D: Dist, model_name, bs, size, dt, steps, warmup, extras=True, cpu
     ms_total = timed(D, step, steps, sampler)
     clocks = sampler.stop() if sampler is not None else None
     eager_launches = _lib.launch_count() - l0
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, last["z"], last["nms"])
     prog = model._program(dev_in[0])
     graph_launches = len(prog.ops) * steps if prog.graph is not None else 0
     images, worst_ms = aggregate_throughput(bs * steps, ms_total, dev)
@@ -387,14 +428,15 @@ def infer_leg(D: Dist, model_name, bs, size, dt, steps, warmup, extras=True, cpu
         if os.path.exists(tp):
             traffic = json.load(open(tp)).get(model_name)
         hbm_bound = model_name in ("yolov5n", "yolov5s", "yolov5m")  # SURVEY.md section 8d: AI below machine balance
-        roof = {"kernel": "conv_gemm_kernel (tcgen05 implicit GEMM: every Conv / C3 / SPPF / Detect-head launch of one forward)",
+        roof = {"kernel": "conv_gemm_kernel (wgmma implicit GEMM: every Conv / C3 / SPPF / Detect-head launch of one forward)",
                 "bound": "hbm" if hbm_bound else "tensor",
-                "achieved": gbs if hbm_bound else tfs, "peak": pk["hbm"] if hbm_bound else pk["tf_sust"],
-                "unit": "GB/s" if hbm_bound else "TFLOP/s", "frac": (gbs / pk["hbm"]) if hbm_bound else (tfs / pk["tf_sust"]),
-                "traffic": traffic, "peak_source": pk["src"] + (" (sustained cuBLAS bf16: kernels timed inside a long step)" if not hbm_bound else " (copy)"),
+                "achieved": gbs if hbm_bound else tfs, "peak": pk["hbm"] if hbm_bound else (pk["tf_sust"] or pk["tf_burst"]),
+                "unit": "GB/s" if hbm_bound else "TFLOP/s", "frac": (gbs / pk["hbm"]) if hbm_bound else (tfs / (pk["tf_sust"] or pk["tf_burst"])),
+                "traffic": traffic, "peak_source": pk["src"] + ((" (sustained cuBLAS bf16: kernels timed inside a long step)" if pk["tf_sust"] else
+                                                                 " (dense bf16)") if not hbm_bound else (" (copy)" if pk["src"] == "measured" else " (HBM3)")),
                 "launches": n_conv, "avg_launch_us": 1e3 * conv_ms / max(n_conv, 1),
                 "algorithmic_bytes_per_launch": conv_bytes / max(n_conv, 1), "flops_per_launch": prog.flops / max(n_conv, 1),
-                "hbm_gbs": gbs, "tensor_tflops": tfs, "tensor_frac_of_sustained": tfs / pk["tf_sust"], "tensor_frac_of_burst": tfs / pk["tf_burst"],
+                "hbm_gbs": gbs, "tensor_tflops": tfs, "tensor_frac_of_sustained": tfs / pk["tf_sust"] if pk["tf_sust"] else None, "tensor_frac_of_burst": tfs / pk["tf_burst"],
                 "hbm_frac": gbs / pk["hbm"], "conv_ms_per_forward": conv_ms, "all_ops_ms_per_forward": all_ms}
 
         # ---------------- NMS us/img (second half of the metric) ----------------
@@ -496,7 +538,7 @@ def torch_cuda_reference(cfg, sd, dev_in, dt, steps, dev):
 # ---------------------------------------------------------------------------------------------------------------------
 # training leg (BASELINE configs[3])
 # ---------------------------------------------------------------------------------------------------------------------
-def train_leg(D: Dist, model_name, bs, size, dt, steps, warmup, extras=True):
+def train_leg(D: Dist, model_name, bs, size, dt, steps, warmup, extras=True, dump_dir=None):
     """images/s of one optimisation step through the public API: model.train() under autocast, ComputeLoss, GradScaler-scaled
     backward, fused un-scale + clip + SGD-Nesterov (3 groups) + zero_grad (+ ModelEMA on rank 0, as train.py:251 does); per-GPU
     batch fixed, gradients averaged over ranks for N > 1 by FusedSGD.data_parallel -- one NCCL all-reduce of the packed arena -- with the
@@ -557,9 +599,12 @@ def train_leg(D: Dist, model_name, bs, size, dt, steps, warmup, extras=True):
         step(dev_img[i % n_rot], dev_tgt[i % n_rot])
     sampler = ClockSampler(D.local) if rank == 0 else None
     l0 = _lib.launch_count()
-    ms = timed(D, lambda i: step(dev_img[i % n_rot], dev_tgt[i % n_rot]), steps, sampler)
+    last = {}
+    ms = timed(D, lambda i: last.__setitem__("items", step(dev_img[i % n_rot], dev_tgt[i % n_rot])), steps, sampler)
     clocks = sampler.stop() if sampler is not None else None
     launches = _lib.launch_count() - l0
+    if dump_dir and rank == 0:
+        dump_train_outputs(dump_dir, last["items"], model)
     images, worst_ms = aggregate_throughput(bs * steps, ms, dev)
     value = images / (worst_ms / 1e3)
 
@@ -743,6 +788,8 @@ def main():
     ap.add_argument("--batch", type=int, default=0, help="override the per-GPU batch")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-subrecords", action="store_true", help="main workload only (profiling runs)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step of the main inference leg as DIR/<name>.npy")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3)
     global _OUT
@@ -759,6 +806,8 @@ def main():
     if a.batch:
         bs = a.batch
     train = a.workload.endswith("-train")
+    if a.dump_outputs and a.impl == "reference":
+        raise SystemExit("bench.py: --dump-outputs writes what the timed GPU path computed; --impl reference has no such path")
     scaling = "strong" if rule == "total" and not a.batch else "weak"
     what = "training step" if train else "forward + NMS"
     cfg_desc = {"workload": f"{model_name} {what}, {bs * world} images of {size}x{size} per step ({bs}/GPU x {world}), {dt}"
@@ -789,11 +838,11 @@ def main():
     D.init()
     subs = not a.no_subrecords and a.workload == "config3"
     if train:
-        rec = train_leg(D, model_name, bs, size, dt, a.steps, a.warmup)
+        rec = train_leg(D, model_name, bs, size, dt, a.steps, a.warmup, dump_dir=a.dump_outputs)
         metric = "images/sec @640 (training step: forward + loss + backward + optimizer)"
     else:
         rec = infer_leg(D, model_name, bs, size, dt, a.steps, a.warmup, extras=True, cpu_base=not a.no_cpu_baseline,
-                        sustain_s=2.5 if subs else 0.0)
+                        sustain_s=2.5 if subs else 0.0, dump_dir=a.dump_outputs)
         metric = "images/sec @640 (forward + NMS)"
     sub = {}
     if subs:
@@ -821,7 +870,7 @@ def main():
                             + (", DDP gradient all-reduce" if D.world > 1 else ""))
             sub["train_ddp"] = rt
     if D.rank == 0:
-        cfg_desc.update({"model": model_name, "l2": "3 rotating input batches and GBs of activations streamed per step (>> 126 MB L2)",
+        cfg_desc.update({"model": model_name, "l2": "3 rotating input batches and GBs of activations streamed per step (>> 50 MB L2)",
                          "weights": "seeded synthetic (oracle.model_ref.synth_state_dict), head bias calibrated to ~2% anchors > 0.25"})
         cfg_desc.update(rec.pop("detail"))
         sustained = rec.pop("sustained", None)

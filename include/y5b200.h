@@ -1,4 +1,4 @@
-/* y5b200.h -- C ABI of liby5b200.so: the B200 (sm_100a) engine behind the YOLOv5 forward / NMS / loss hot path.
+/* y5b200.h -- C ABI of liby5b200.so: the H100 (sm_90a) engine behind the YOLOv5 forward / NMS / loss hot path.
  *
  * The reference (ultralytics/yolov5) is pure Python and has NO FFI / plugin interface for this path: the work
  * sits behind ordinary Python callables (SURVEY.md section 8b).  Each entry point below therefore names the
@@ -48,7 +48,7 @@ const char* y5_last_error(void);
 int64_t y5_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Fused Conv2d(bias=False) + folded BatchNorm + SiLU (+ residual add), implicit GEMM on tcgen05 tensor cores.
+ * Fused Conv2d(bias=False) + folded BatchNorm + SiLU (+ residual add), implicit GEMM on wgmma tensor cores.
  * Replaces: models/common.py:86-92 Conv.forward / forward_fuse (conv -> bn -> act), utils/torch_utils.py:224-254
  * (BN fold, done once by the caller when packing), models/common.py:181 Bottleneck's `x + ...` (residual),
  * and, through out pitch/offset, the torch.cat of models/common.py:246,340,453.
@@ -81,12 +81,12 @@ typedef struct y5_conv_desc {
     int64_t in_y_stride;  /* elements between rows   (0 = in_w * in_x_stride) */
     int64_t in_n_stride;  /* elements between images (0 = in_h * in_y_stride) */
     int32_t a_mode;       /* activation fetch: 0 auto, 1 force TMA-im2col, 2 force shifted-patch (stride-1 only) */
-    int32_t reserved;     /* flags.  bit 6 (64): the weights are constant -- not written by whatever precedes this launch in the
-                             stream -- so the kernel may fetch them before its programmatic-dependency wait (inference programs
-                             set it; a training forward that packs weights right before the conv must not).  Tuning / tests:
-                             bit 4 (16) row-strided stores instead of the TMA-store epilogue, bit 5 (32) one patch copy per
-                             horizontal tap instead of the wide patch; with a forced block_n >= 128 also bit 1 (2) = 256-row
-                             tiles, bit 2 (4) = CTA pairs, bits 8.. = cluster size (2|4) for weight-tile multicast */
+    int32_t reserved;     /* flags, 0 in normal use.  Tuning / tests: bit 3 (8) staged epilogue (each warpgroup's block goes
+                             through shared memory and leaves as 16-byte row segments), bit 4 (16) forces the default direct
+                             register stores; bit 7 (128) the wide patch fetch (one patch copy per channel chunk
+                             feeds every tap of a stride-1 k x k conv with 64-channel chunks), bit 5 (32) vetoes it; with a
+                             forced block_n also bit 1 (2) = 256-row tiles (block_n 128), bit 2 (4) = CTA pairs (2-CTA cluster),
+                             bits 8.. = cluster size (2|4): the CTAs of a cluster split every weight tile and TMA-multicast it */
 } y5_conv_desc;
 
 /* Tiling the library will use for a conv: block_k decides the weight packing (cin_pad = ceil(in_c/block_k)*block_k). */
@@ -221,7 +221,7 @@ int y5_loss_read_targets(const y5_loss_params* p, const void* workspace, int32_t
  *            column sums of y          -> y5_bn_stats
  *            z = act(bn(y))            -> y5_bn_act_fwd    (derives mean/invstd, updates running_mean / running_var)
  * Backward:  dy, dgamma, dbeta         -> y5_bn_act_bwd
- *            dW                        -> y5_conv_wgrad    (tcgen05, MN-major operands straight from NHWC)
+ *            dW                        -> y5_conv_wgrad    (wgmma, MN-major operands straight from NHWC)
  *            dx = conv(dy, W^T flipped)-> y5_conv_bn_silu_fwd again on transposed/flipped packed weights (stride-2
  *                                         layers first expand dy with y5_zero_stuff2x); `residual` = dx accumulates.
  * Detect.m[i] (models/yolo.py:97) has a bias and no BN: its bias gradient is y5_col_sum(dy).

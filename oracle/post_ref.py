@@ -6,7 +6,7 @@ rows are not built yet; this file and tests/golden/post.npz are the checker they
 
 Pinned: tests/golden/post.npz holds outputs of the real reference (tests/golden/make_golden.py post, through
 tests/golden/refshim.py); tests/test_oracle_golden.py checks this file against them.  `box_iou` / `clip_boxes` come from
-the absent `ultralytics` package in the reference: pinned only to the shim's restatement (see DESIGN.md section 4).
+the absent `ultralytics` package in the reference: pinned only to the shim's restatement.
 
 Reference lines restated (paths relative to /root/reference):
   utils/segment/general.py:10-22   crop_mask                      -> crop_mask

@@ -13,7 +13,7 @@ def pytest_configure(config):
 
     # the oracle's torch-CPU convs crawl when 128+ host threads fight over small layers (GPU box): cap the pool
     torch.set_num_threads(max(1, min(16, os.cpu_count() or 1)))
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -517,9 +517,29 @@ def gen_ckpt():
           f"{os.path.getsize(f'{HERE}/ref_tiny.pt') / 1e6:.2f} MB")
 
 
+def gen_signatures():
+    """The reference's call signatures of the drop-in surface listed in tests/test_compat_cpu.py (name, default repr, kind)."""
+    import importlib
+    import importlib.util
+    import inspect
+
+    spec = importlib.util.spec_from_file_location("test_compat_cpu", os.path.join(os.path.dirname(HERE), "test_compat_cpu.py"))
+    tmod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(tmod)
+    out = {}
+    for mod, qual in tmod.SURFACE:
+        obj = importlib.import_module(mod)
+        for part in qual.split("."):
+            obj = getattr(obj, part)
+        out[f"{mod}:{qual}"] = [(n, repr(p.default) if p.default is not inspect._empty else None, str(p.kind))
+                                for n, p in inspect.signature(obj).parameters.items()]
+    with open(f"{HERE}/ref_signatures.json", "w") as f:
+        json.dump(out, f, indent=1, sort_keys=True)
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["cfg", "model", "nms", "loss", "train", "post", "pre", "optim", "ckpt"]
+    which = sys.argv[1:] or ["cfg", "model", "nms", "loss", "train", "post", "pre", "optim", "ckpt", "signatures"]
     for w in which:
         {"cfg": gen_cfg, "model": gen_model, "nms": gen_nms, "loss": gen_loss, "train": gen_train, "post": gen_post, "pre": gen_pre,
-         "optim": gen_optim, "ckpt": gen_ckpt}[w]()
+         "optim": gen_optim, "ckpt": gen_ckpt, "signatures": gen_signatures}[w]()
     print("golden fixtures written to", HERE)

@@ -10,9 +10,12 @@ from yolov5_b200.engine import pack_weight
 
 
 def conv_case(dev, dtype, B, H, W, cin, cout, k, s, p, act=True, residual=False, in_extra=0, out_extra=0, seed=0, direct=False,
-              block_n=0, a_mode=0, mt2=False, cluster=1, cg2=False, direct_store=False, narrow_patch=False, wide_patch=False):
+              block_n=0, a_mode=0, mt2=False, cluster=1, cg2=False, direct_store=False, narrow_patch=False, wide_patch=False,
+              staged=False):
     """Runs y5_conv_bn_silu_fwd (or the direct cross-check kernel) on seeded data; returns (got NCHW fp32, oracle fp32).
-    `in_extra` / `out_extra` put the views inside wider buffers (channel offset 8, pitch + extra) to exercise slices."""
+    `in_extra` / `out_extra` put the views inside wider buffers (channel offset 8, pitch + extra) to exercise slices.
+    Stores: the library's default (direct from the registers) unless `staged` asks for the shared-memory staged epilogue;
+    `direct_store` forces the direct stores."""
     lib = _lib.lib()
     g = torch.Generator().manual_seed(seed)
     x = (torch.rand(B, cin, H, W, generator=g) * 2 - 1)
@@ -45,7 +48,7 @@ def conv_case(dev, dtype, B, H, W, cin, cout, k, s, p, act=True, residual=False,
     d.ksize, d.stride, d.pad = k, s, p
     d.act, d.dtype, d.block_k, d.block_n = int(act), _lib.dtype_code(dtype), bk.value, block_n
     d.a_mode = a_mode  # 0 auto, 1 TMA-im2col, 2 shifted patches
-    d.reserved = (2 if mt2 else 0) | (4 if cg2 else 0) | (16 if direct_store else 0) | (32 if narrow_patch else 0) | (128 if wide_patch else 0) | (cluster << 8 if cluster > 1 else 0)  # forced block_n >= 128: 256-row tiles / CTA pairs / multicast
+    d.reserved = (2 if mt2 else 0) | (4 if cg2 else 0) | (16 if direct_store else 0) | (8 if staged else 0) | (32 if narrow_patch else 0) | (128 if wide_patch else 0) | (cluster << 8 if cluster > 1 else 0)  # forced block_n: 256-row tiles / CTA pairs / multicast cluster
     fn = lib.y5_conv_direct_fwd if direct else lib.y5_conv_bn_silu_fwd
     _lib.check(fn(C.byref(d), C.c_void_p(_lib.stream_ptr(dev))), "conv")
     torch.cuda.synchronize()

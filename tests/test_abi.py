@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports every symbol include/y5b200.h declares
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports every symbol include/y5b200.h declares
 (no compute calls here -- there is no GPU in the build container)."""
 import ctypes
 import os
@@ -31,15 +31,15 @@ def test_library_exports_every_declared_symbol(built_lib):
     assert sorted(_lib.SIGNATURES) == _declared()  # the ctypes table mirrors the header one to one
 
 
-def test_library_is_sm100a_with_tcgen05_and_tma(built_lib):
+def test_library_is_sm90a_with_wgmma_and_tma(built_lib):
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "UTMALDG.4D.IM2COL"):  # tcgen05.mma, TMA, tcgen05.ld, im2col TMA
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA.64x", "UTMALDG", "UTMALDG.4D.IM2COL"):  # wgmma, TMA, im2col TMA
         assert mnemonic in sass, mnemonic
-    # the weight-gradient kernel is a tcgen05 kernel of its own (MN-major operands) with vector fp32 reductions
+    # the weight-gradient kernel is a wgmma kernel of its own (MN-major operands) with vector fp32 reductions
     wg = sass[sass.index("conv_wgrad_kernel"):]
     wg = wg[: wg.index("Function :", 10)] if "Function :" in wg[10:] else wg
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "REDG.E.ADD.F32x4"):
+    for mnemonic in ("HGMMA.64x64x16.F32", "UTMALDG", "REDG.E.ADD.F32x2"):
         assert mnemonic in wg, mnemonic
 
 

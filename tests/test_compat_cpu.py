@@ -11,7 +11,6 @@ import pytest
 import torch
 
 G = os.path.join(os.path.dirname(__file__), "golden")
-REF = "/root/reference"
 
 # (module under yolov5_b200 == module path in the reference, qualified name)
 SURFACE = [
@@ -38,32 +37,15 @@ def _resolve(mod, qual):
     return obj
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="the reference tree exists only in the build container")
 def test_signatures_match_the_reference():
     """Every reference parameter (name, position, default) is present in this package's callable; extra trailing keyword
-    parameters with defaults are allowed (e.g. non_max_suppression(..., return_indices=False))."""
+    parameters with defaults are allowed (e.g. non_max_suppression(..., return_indices=False)).  The reference's signatures
+    were recorded by running the reference itself (tests/golden/make_golden.py, ref_signatures.json)."""
     import importlib
-    import subprocess
 
-    # the reference must be imported in a clean interpreter: its top-level packages are called `models` / `utils` too
-    code = f"""
-import sys, json, inspect
-sys.path.insert(0, {os.path.join(os.path.dirname(__file__), 'golden')!r})
-import refshim; refshim.install()
-import importlib
-out = {{}}
-for mod, qual in {SURFACE!r}:
-    m = importlib.import_module(mod)
-    obj = m
-    for part in qual.split('.'):
-        obj = getattr(obj, part)
-    sig = inspect.signature(obj)
-    out[mod + ':' + qual] = [(n, repr(p.default) if p.default is not inspect._empty else None, str(p.kind)) for n, p in sig.parameters.items()]
-print(json.dumps(out))
-"""
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd="/tmp")
-    assert r.returncode == 0, r.stderr[-2000:]
-    ref = json.loads(r.stdout.strip().splitlines()[-1])
+    with open(os.path.join(G, "ref_signatures.json")) as f:
+        ref = json.load(f)
+    assert sorted(ref) == sorted(f"{mod}:{qual}" for mod, qual in SURFACE)
     bad = []
     for mod, qual in SURFACE:
         ours = inspect.signature(_resolve(importlib.import_module("yolov5_b200." + mod), qual))

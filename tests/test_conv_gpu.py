@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 implicit-GEMM conv (through the C ABI) against the fp32 oracle expression
+"""GPU: the wgmma implicit-GEMM conv (through the C ABI) against the fp32 oracle expression
 SiLU(conv2d(x, W') + b') [+ residual]  (reference models/common.py:86-92,181) on fp16/bf16-rounded operands.
 Tolerance: output is rounded once to fp16 (rel 2^-11) / bf16 (2^-8) after fp32 accumulation -> 2e-3 / 1.6e-2 of max|y|."""
 import pytest
@@ -30,16 +30,17 @@ CASES = [
 def test_conv_vs_oracle(cuda, dtype, case):
     got, ref, _ = conv_case(cuda, dtype, *case)
     assert rel_err(got, ref) < TOL[dtype], (case, rel_err(got, ref))
-    got, ref, _ = conv_case(cuda, dtype, *case, direct_store=True)
-    assert rel_err(got, ref) < TOL[dtype], (case, "direct stores", rel_err(got, ref))
+    got, ref, _ = conv_case(cuda, dtype, *case, staged=True)
+    assert rel_err(got, ref) < TOL[dtype], (case, "staged stores", rel_err(got, ref))
 
 
 @pytest.mark.parametrize("direct_store", [False, True])
 @pytest.mark.parametrize("case", [(2, 20, 20, 64, 64, 3, 1, 1), (2, 16, 16, 64, 128, 1, 1, 0), (5, 7, 9, 64, 40, 1, 1, 0), (3, 13, 27, 32, 72, 3, 1, 1)])
 def test_conv_residual_and_slices(cuda, case, direct_store):
-    """Both epilogue store paths (per-warp staging + cp.async.bulk.tensor store, and the direct row-strided stores) into a
+    """Both epilogue store paths (per-warpgroup staging + 16-byte row-segment stores, and the direct register stores) into a
     channel slice of a wider buffer: N tails inside a 32-channel chunk (40, 72 channels), partial spatial tiles, M tails."""
-    got, ref, untouched = conv_case(cuda, torch.float16, *case, residual=True, in_extra=24, out_extra=40, direct_store=direct_store)
+    got, ref, untouched = conv_case(cuda, torch.float16, *case, residual=True, in_extra=24, out_extra=40, direct_store=direct_store,
+                                    staged=not direct_store)
     assert rel_err(got, ref) < 2e-3
     assert untouched, "epilogue wrote outside its channel slice"
 
@@ -72,7 +73,7 @@ def test_conv_3x3_both_fetch_modes(cuda, case, a_mode):
 ])
 def test_conv_wide_patch(cuda, case, kw, dtype, narrow):
     """Stride-1 k x k convs with 64-channel chunks fetch ONE (16+k-1) x PW patch per chunk and read all k*k taps from it through
-    descriptor offsets + the swizzle base offset (`narrow=False`); the one-copy-per-horizontal-tap mode (`narrow=True`, reserved bit
+    descriptor offsets (`narrow=False`); the one-copy-per-horizontal-tap mode (`narrow=True`, reserved bit
     32) must give the same answer.  Residual + channel-slice views on both sides."""
     got, ref, untouched = conv_case(cuda, dtype, *case, a_mode=2, residual=True, in_extra=8, out_extra=24, narrow_patch=narrow, wide_patch=not narrow,
                                      **kw)
@@ -95,7 +96,8 @@ def test_conv_every_tile_width(cuda, bn):
 @pytest.mark.parametrize("case,a_mode", [((2, 20, 20, 64, 256, 3, 1, 1), 1), ((2, 20, 20, 64, 256, 3, 1, 1), 2),
                                          ((3, 16, 16, 128, 256, 1, 1, 0), 0), ((1, 40, 40, 128, 384, 3, 2, 1), 0)])
 def test_conv_256_row_tiles(cuda, bn, case, a_mode):
-    """MT = 2: two 128-row sub-tiles share every B tile (256x128 double-buffered, 256x256 single-buffered accumulators)."""
+    """MT = 2: two 128-row sub-tiles share every B tile (256x128 tiles; 256-wide weight tiles keep one sub-tile, 128 register columns
+    per thread being the limit)."""
     got, ref, _ = conv_case(cuda, torch.float16, *case, block_n=bn, mt2=True, a_mode=a_mode, residual=True)
     assert rel_err(got, ref) < 2e-3, (bn, case, a_mode, rel_err(got, ref))
 
@@ -105,7 +107,8 @@ def test_conv_256_row_tiles(cuda, bn, case, a_mode):
                                          ((3, 40, 40, 128, 384, 3, 2, 1), 0)])
 def test_conv_cluster_multicast(cuda, bn, mt2, case, a_mode):
     """2-CTA clusters: each CTA fetches half of every weight tile and TMA-multicasts it to its peer; odd super-tile
-    counts leave one CTA of the last cluster without work (it must still take part in the multicast protocol)."""
+    counts leave one CTA of the last cluster without work (it must still take part in the multicast protocol).  With block_n 256
+    the planner keeps one sub-tile (the accumulators of 256 x 256 do not fit the registers), so (256, True) repeats (256, False)."""
     got, ref, _ = conv_case(cuda, torch.float16, *case, block_n=bn, mt2=mt2, cluster=2, a_mode=a_mode, residual=True)
     assert rel_err(got, ref) < 2e-3, (bn, mt2, case, a_mode, rel_err(got, ref))
 
@@ -115,10 +118,11 @@ def test_conv_cluster_multicast(cuda, bn, mt2, case, a_mode):
 @pytest.mark.parametrize("case,a_mode", [((4, 40, 40, 64, 256, 3, 1, 1), 2), ((4, 40, 40, 64, 256, 3, 1, 1), 1), ((5, 24, 24, 128, 512, 1, 1, 0), 0),
                                          ((3, 40, 40, 128, 384, 3, 2, 1), 0), ((2, 80, 80, 128, 128, 3, 1, 1), 2), ((1, 20, 20, 512, 512, 3, 1, 1), 0)])
 def test_conv_cta_pairs(cuda, dtype, bn, mt2, case, a_mode):
-    """cta_group::2: the two CTAs of a cluster run ONE M = 256 MMA per k-step, each staging its own 128 activation rows and half
-    of the weight tile; full barriers in the leader collect both CTAs' TMA bytes, the follower's epilogue releases the leader's
-    accumulator barrier remotely.  Odd super-tile counts (the follower of the last pair has no rows), N tails (384 = 1.5 tiles of
-    256), every fetch mode, residual operand."""
+    """CTA pairs: the two CTAs of a cluster work on two M super-tiles of the same N tile, each fetching half of every weight tile
+    and multicasting it to both; a weight stage is refilled only after the consumers of both CTAs released it.  Odd super-tile
+    counts (the second CTA of the last pair has no rows), N tails (384 = 1.5 tiles of 256), every fetch mode, residual operand.
+    On Hopper this is the 2-CTA multicast cluster of test_conv_cluster_multicast, checked here in both dtypes and on two more
+    shapes; with block_n 256 the planner keeps one sub-tile, so the mt2=True cases of that width repeat mt2=False."""
     if case[4] % bn and bn == 256 and case[4] < 256:
         pytest.skip("N tile wider than the layer")
     got, ref, _ = conv_case(cuda, dtype, *case, block_n=bn, mt2=mt2, cg2=True, a_mode=a_mode, residual=True)
@@ -132,13 +136,13 @@ def test_conv_cta_pairs_many_tiles(cuda):
 
 
 def test_tensor_core_path_agrees_with_direct_kernel(cuda):
-    """Two independent device implementations of the same op (tcgen05 GEMM vs CUDA-core direct conv)."""
+    """Two independent device implementations of the same op (wgmma GEMM vs CUDA-core direct conv)."""
     a, ref, _ = conv_case(cuda, torch.float16, 2, 20, 20, 64, 64, 3, 1, 1, seed=5)
     b, _, _ = conv_case(cuda, torch.float16, 2, 20, 20, 64, 64, 3, 1, 1, seed=5, direct=True)
     assert rel_err(a, b) < 2e-3 and rel_err(b, ref) < 2e-3
 
 
 def test_large_m_many_tiles_per_cta(cuda):
-    """> 148 tiles so every persistent CTA loops, exercising barrier phase wrap-around."""
+    """More tiles than SMs so every persistent CTA loops, exercising barrier phase wrap-around."""
     got, ref, _ = conv_case(cuda, torch.float16, 8, 80, 80, 64, 64, 3, 1, 1)  # 400 M tiles
     assert rel_err(got, ref) < 2e-3

@@ -190,10 +190,9 @@ def _worker_graphed(rank, world, port, out_dir):
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
-@pytest.mark.skipif(not os.environ.get("Y5_TEST_GRAPH_DP"), reason="opt-in (Y5_TEST_GRAPH_DP=1): the first version of this test hung in "
-                    "destroy_process_group with the captured graph still alive, and the round's GPU budget ended before the fixed teardown "
-                    "could be re-run; the same path is exercised by `Y5_BENCH_GRAPH_DP=1 torchrun ... bench.py --gpus 2` "
-                    "(profiles/r02_bench_config3_n2.json, train_ddp.cuda_graph_step)")
+@pytest.mark.skipif(not os.environ.get("Y5_TEST_GRAPH_DP"), reason="opt-in (Y5_TEST_GRAPH_DP=1): an earlier version of this test hung in "
+                    "destroy_process_group with the captured graph still alive and the fixed teardown has not been run since; the same path "
+                    "is exercised by `Y5_BENCH_GRAPH_DP=1 torchrun ... bench.py --gpus 2` (train_ddp.cuda_graph_step)")
 def test_graphed_data_parallel_step_two_ranks(tmp_path):
     """GraphedTrainStep over FusedSGD.data_parallel: the captured step contains the all-reduce of the gradient arena; both ranks
     replay in lock-step and must end with identical parameters, equal (to the weight-gradient kernel's summation-order noise) to

@@ -1,4 +1,4 @@
-"""-m gpu parity tests of the training path: weight-gradient GEMM (MN-major tcgen05), BatchNorm/SiLU training kernels, the
+"""-m gpu parity tests of the training path: weight-gradient GEMM (MN-major wgmma), BatchNorm/SiLU training kernels, the
 Conv layer's forward/backward and a whole-model training step, against torch autograd on the same seeded data.
 
 Tolerances: activations and activation gradients are fp16/bf16 (rounding 2^-11 / 2^-8 relative per op); statistics and

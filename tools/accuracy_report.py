@@ -1,5 +1,5 @@
 """Prints max-abs error / max|oracle| of the engine and of torch's low-precision evaluation of the reference, per
-model output (z, raw levels, proto), on a B200.   python tools/accuracy_report.py"""
+model output (z, raw levels, proto), on an H100.   python tools/accuracy_report.py"""
 import os, sys
 
 import torch

@@ -1,7 +1,7 @@
 """Per-launch floor / per-tile slope of conv_gemm: times back-to-back launches of one plan inside a CUDA graph.
 
-usage: python tools/floor_probe.py            (on a B200)
-For each (N, K, ksize) the row count M is swept in whole waves of 148 x 128-row tiles; the intercept of time vs waves is
+usage: python tools/floor_probe.py            (on an H100)
+For each (N, K, ksize) the row count M is swept in whole waves of <SM count> x 128-row tiles; the intercept of time vs waves is
 the fixed cost of a launch, the slope the steady-state cost of one tile per CTA.
 """
 import ctypes as C
@@ -63,7 +63,7 @@ def main():
     for cout, cin, k in ((32, 32, 1), (64, 64, 1), (128, 128, 1), (256, 256, 1), (512, 512, 1), (128, 128, 3), (256, 256, 3), (64, 64, 3), (512, 1024, 1)):
         row = []
         for waves in (1, 2, 3, 4, 8, 16):
-            M = 128 * 148 * waves
+            M = 128 * torch.cuda.get_device_properties(0).multi_processor_count * waves
             plan, keep = plan_for(dev, dtype, M, cin, cout, k)
             row.append(time_plan(plan))
             _lib.lib().y5_conv_plan_destroy(plan)

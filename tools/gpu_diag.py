@@ -1,4 +1,4 @@
-"""First-contact diagnostics on a B200: each stage runs in its own subprocess (a trapped kernel kills only its stage)
+"""First-contact diagnostics on an H100: each stage runs in its own subprocess (a trapped kernel kills only its stage)
 and prints error summaries rather than asserting.   python tools/gpu_diag.py [stage ...]"""
 import os
 import subprocess

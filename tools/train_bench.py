@@ -1,4 +1,4 @@
-"""Training-step timing on a B200: engine (yolov5_b200 train path) vs torch autocast execution of the same model.
+"""Training-step timing on an H100: engine (yolov5_b200 train path) vs torch autocast execution of the same model.
 
     python tools/train_bench.py [--model yolov5s] [--batch 16] [--size 640] [--dtype fp16] [--steps 10]
 

@@ -1,4 +1,4 @@
-"""Per-shape timing of the training kernels (BN statistics / apply / backward, wgrad) on a B200, inside a CUDA graph of
+"""Per-shape timing of the training kernels (BN statistics / apply / backward, wgrad) on an H100, inside a CUDA graph of
 20 back-to-back launches.   python tools/train_kernel_probe.py [batch]"""
 import ctypes as C
 import os

@@ -1,4 +1,4 @@
-"""yolov5_b200 -- B200-native (sm_100a) engine for the YOLOv5 forward / NMS / loss hot path.
+"""yolov5_b200 -- H100-native (sm_90a) engine for the YOLOv5 forward / NMS / loss hot path.
 
 Public surface mirrors the reference's Python callables for that path:
     yolov5_b200.models.yolo.DetectionModel / SegmentationModel / Detect / Segment / parse_model

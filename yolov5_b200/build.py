@@ -1,10 +1,10 @@
-"""In-tree build of liby5b200.so (hand-written sm_100a kernels + C ABI) with nvcc.
+"""In-tree build of liby5b200.so (hand-written sm_90a kernels + C ABI) with nvcc.
 
     python -m yolov5_b200.build            # incremental
     python -m yolov5_b200.build --force
 
 The shared object is written next to this file (yolov5_b200/liby5b200.so) so it travels with the repo snapshot to
-the GPU box; nvcc cross-compiles for sm_100a without a GPU.
+the GPU machine; nvcc cross-compiles for sm_90a without a GPU.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "liby5b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 # file -> extra flags.  nms.cu / loss.cu hold bit-exact integer/index paths: no FMA contraction there.
 SOURCES = {

@@ -1,7 +1,6 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (tiled + im2col), tcgen05 (alloc / mma / commit / ld), fences.
-// Everything the kernels in this directory need from the Blackwell programming model lives here; there is no
-// dependency on CUTLASS/CuTe.  Descriptor bit layouts follow the PTX ISA "tcgen05 matrix / instruction descriptor"
-// tables (cross-checked against cute/arch/mma_sm100_desc.hpp shipped in this image).
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (tiled + im2col), wgmma descriptors / fences, register reallocation.
+// Everything the kernels in this directory need from the Hopper programming model lives here; there is no dependency
+// on CUTLASS/CuTe.  Descriptor bit layouts follow the PTX ISA "matrix descriptor" table of the wgmma section.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -68,16 +67,13 @@ __device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parit
         : "memory");
     return ok != 0;
 }
-// Bounded wait: a pipeline bug must surface as a trapped kernel (launch error), never as a hung GPU.
+// Bounded wait: a pipeline bug must surface as a trapped kernel (launch error), never as a hung GPU.  No printf here: a
+// function call inside a kernel that issues wgmma makes ptxas serialise every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     uint32_t spins = 0;
     while (!mbar_try_wait_hint(bar, parity, 20000u)) {       // <= 20 us asleep per probe
-        if (++spins > 200000u) {                             // ~4 s
-            printf("y5b200: mbarrier wait timed out (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x,
-                   smem_u32(bar), parity);
-            __trap();
-        }
+        if (++spins > 200000u) __trap();                     // ~4 s
     }
 }
 
@@ -110,6 +106,22 @@ __device__ __forceinline__ void tma_load_2d_mcast(const CUtensorMap* m, uint64_t
         "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
         : "memory");
 }
+// shared::cluster address of `p` (a shared-memory object of this CTA) as seen in CTA `rank` of the cluster (same offset)
+__device__ __forceinline__ uint32_t mapa_u32(const void* p, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
+    return r;
+}
+// arrive (count 1) on a barrier anywhere in the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_addr) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_addr) : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ uint32_t cluster_nctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
 // im2col mode over an NHWC tensor (dims C,W,H,N): {c,w,h,n} is the base pixel of the first filter window of the tile,
 // {off_w, off_h} the filter tap.  The unit walks `pixelsPerColumn` windows in (w,h,n) order, zero-filling padding.
 __device__ __forceinline__ void tma_load_im2col_4d(const CUtensorMap* m, uint64_t* bar, void* dst, int c, int w, int h,
@@ -119,43 +131,6 @@ __device__ __forceinline__ void tma_load_im2col_4d(const CUtensorMap* m, uint64_
         " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};" ::"r"(smem_u32(dst)),
         "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h)
         : "memory");
-}
-// ---- CTA-pair (cta_group::2) variants: the copy lands in THIS CTA's shared memory but signals the mbarrier at `bar_addr`, a
-// shared::cluster address that may belong to the pair's leader CTA (one barrier then collects the bytes of both CTAs' copies)
-__device__ __forceinline__ void tma_load_2d_cg2(const CUtensorMap* m, uint32_t bar_addr, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_cg2(const CUtensorMap* m, uint32_t bar_addr, void* dst, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
-            smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_im2col_4d_cg2(const CUtensorMap* m, uint32_t bar_addr, void* dst, int c, int w, int h, int n,
-                                                       uint16_t off_w, uint16_t off_h) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h)
-        : "memory");
-}
-// shared::cluster address of `p` (a shared-memory object of this CTA) as seen in CTA `rank` of the cluster (same offset)
-__device__ __forceinline__ uint32_t mapa_u32(const void* p, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
-    return r;
-}
-// arrive (count 1) on a barrier anywhere in the cluster.  Default semantics (.release.cta), as CUTLASS' ClusterBarrier::arrive
-// does for the accumulator-empty hand-shake of CTA pairs: the tcgen05.ld results were waited for and fenced
-// (tcgen05.fence::before_thread_sync) by the arriving warp; `.release.cluster` here made ptxas emit MEMBAR.ALL.GPU + ERRBAR per
-// tile and warp (8 % of the stall samples of a pair-mode layer under ncu).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_addr) : "memory");
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
@@ -174,168 +149,34 @@ __device__ __forceinline__ void tma_store_wait_read0() { asm volatile("cp.async.
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA) -- the instruction wrappers themselves are in wgmma.cuh
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp, ncols pow2 >= 32
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// K-major shared-memory operand descriptor.  Tile rows are `row_bytes` (32/64/128) wide with the matching TMA swizzle,
+// 8-row groups packed back to back (SBO = 8*row_bytes); LBO is unused for swizzled K-major layouts (encoded 1).
+// Stepping 16 elements along K is +32 bytes on the start address (+2 on the low word).
+__device__ __forceinline__ uint32_t gmma_desc_hi(uint32_t row_bytes) {
+    const uint32_t layout = row_bytes == 128 ? 1u : (row_bytes == 64 ? 2u : 3u);  // SW128 / SW64 / SW32
+    return (((8u * row_bytes) >> 4) & 0x3FFFu) | (layout << 30);
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// CTA-pair allocation: executed by the same warp index of BOTH CTAs of the pair; each CTA gets the same column range
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ uint32_t gmma_desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFFu) | (1u << 16); }
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t lo, uint32_t hi) { return (static_cast<uint64_t>(hi) << 32) | lo; }
 
-// K-major shared-memory operand descriptor.  Tile rows are `row_bytes` (32/64/128) wide, 8-row groups are packed
-// back to back (SBO = 8*row_bytes), swizzle span == row width; LBO is unused for swizzled K-major (encoded 1).
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t row_bytes) {
-    const uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);  // SW128 / SW64 / SW32
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-    d |= 1ull << 16;                                                  // leading byte offset (ignored)
-    d |= static_cast<uint64_t>(((8u * row_bytes) >> 4) & 0x3FFF) << 32;  // stride byte offset between 8-row groups
-    d |= 1ull << 46;                                                  // descriptor version (Blackwell)
-    d |= layout << 61;
-    return d;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers must not be touched by other instructions while a wgmma that uses them is in flight
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// kind::f16 instruction descriptor: D fp32, A/B fp16 or bf16, both K-major, M=128.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_f16(bool bf16, uint32_t n, uint32_t m = 128) {
-    uint32_t d = 0;
-    d |= 1u << 4;                   // D format: F32
-    d |= (bf16 ? 1u : 0u) << 7;     // A format
-    d |= (bf16 ? 1u : 0u) << 10;    // B format
-    d |= (n >> 3) << 17;            // N / 8
-    d |= (m >> 4) << 24;            // M / 16  (128 for one CTA, 256 for a CTA pair: 128 rows in each CTA's TMEM)
-    return d;
-}
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// Lean issue path for the MMA thread: the 64-bit operand descriptors are assembled from a precomputed high word
-// (SBO | version | swizzle mode) and a low word ((smem address >> 4) | LBO field), so stepping along K or to another
-// sub-tile is a single 32-bit add on the low word.
-__device__ __forceinline__ uint32_t umma_desc_hi(uint32_t row_bytes) {
-    const uint32_t layout = row_bytes == 128 ? 2u : (row_bytes == 64 ? 4u : 6u);
-    return (((8u * row_bytes) >> 4) & 0x3FFFu) | (1u << 14) | (layout << 29);
-}
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFFu) | (1u << 16); }
-__device__ __forceinline__ void umma_f16_ss_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc,
-                                                 uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %5, 0;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %3};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-        "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// CTA-pair MMA (issued by the leader CTA only): M = 256 = this CTA's 128 rows + the peer's, A read from both CTAs' shared memory
-// at the same offset, B = the two CTAs' N/2-row halves, D in both CTAs' TMEM at the same address
-__device__ __forceinline__ void umma_f16_ss_lohi_cg2(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc,
-                                                     uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %5, 0;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %3};\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(tmem_d),
-        "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// same with separate descriptor high words for A and B (A may carry a swizzle base offset / its own group stride)
-__device__ __forceinline__ void umma_f16_ss_lohi_ab(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                                    uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}" ::"r"(tmem_d),
-        "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accum)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_lohi_ab_cg2(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                                        uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n\t}" ::"r"(tmem_d),
-        "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// 64-bit descriptor forms (the compiler keeps lo/hi as a register pair: no per-instruction pair assembly)
-__device__ __forceinline__ void umma_f16_ss_desc(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_desc_cg2(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// pair commit: arrives on the barrier at this offset in every CTA of `mask` once the pair's MMAs issued so far have completed
-__device__ __forceinline__ void umma_commit_cg2(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-}
-// arrives (count 1) on `bar` once every tcgen05.mma issued so far by this thread has completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// same, arriving on the barrier at this offset in every CTA of `mask` (a smem stage filled by multicast is free only
-// when all CTAs of the cluster have consumed it)
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t cluster_nctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (base_lane + i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+// per-warpgroup register budget: the producer warpgroup gives registers back, the MMA / epilogue warpgroups take them
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // Programmatic dependent launch: `wait` blocks until the grid this one depends on has completed and its writes are
 // visible; `launch_dependents` lets the next grid in the stream start its prologue as soon as SMs free up.
@@ -351,9 +192,8 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
 // ---------------------------------------------------------------------------------------------------------------------
 #ifndef Y5_SILU_EXACT
 // x*sigmoid(x) = h + h*tanh(h), h = x/2: one MUFU op per element (tanh.approx, rel. error 2^-11) instead of two
-// (ex2 + rcp).  Measured on B200: model outputs' error against the fp32 oracle is unchanged to 3 digits in fp16 and
-// bf16 (tools/accuracy_report.py) -- the result is rounded to 11 / 8 significant bits right after -- and the forward
-// is 2-3 % faster.  -DY5_SILU_EXACT restores the ex2 + rcp form.
+// (ex2 + rcp); the result is rounded to 11 / 8 significant bits (fp16 / bf16) right after, so the approximation stays
+// below the output's own rounding.  -DY5_SILU_EXACT restores the ex2 + rcp form.
 __device__ __forceinline__ float silu_f(float x) {
     const float h = 0.5f * x;
     float t;

@@ -1,37 +1,38 @@
-// Implicit-GEMM convolution for sm_100a:  D[M = B*Ho*Wo, N = Cout] = im2col(X)[M, K = kh*kw*Cin] * W[N, K]^T
+// Implicit-GEMM convolution for sm_90a:  D[M = B*Ho*Wo, N = Cout] = im2col(X)[M, K = kh*kw*Cin] * W[N, K]^T
 //
 // Activation (A) fetch, three modes -- all by the TMA unit, all landing in 32/64/128-byte-swizzled K-major smem tiles
-// that tcgen05.mma reads through shared-memory descriptors:
+// that wgmma reads through shared-memory descriptors:
 //   LINEAR  1x1/s1 convs: 2-D tiles [128 pixels x BLOCK_K channels] of the [M, Cin] matrix.
 //   IM2COL  hardware im2col mode (cp.async.bulk.tensor.4d...im2col): a tile is 128 consecutive output pixels in
 //           (n,y,x) order whatever the row/image boundaries; padding zero-filled; stride via elementStrides.  One
 //           copy per filter tap: the input is re-read kh*kw times (from L2).  Used for stride-2 and small maps.
 //   PATCH   stride-1 convs: the tile is a th x tw block of output pixels (th*tw = 128) and, per channel chunk and
 //           horizontal tap s, ONE copy brings the (th+kh-1) x tw input patch; the kh vertical taps are the same smem
-//           patch read at row offsets r*tw (a plain descriptor offset, still 1024-B aligned because tw % 8 == 0).
-//           L2->smem traffic for A drops from kh*kw to kw*(th+kh-1)/th reads per input element.
+//           patch read at row offsets r*tw (a plain descriptor offset, still aligned to the 8-row swizzle pattern
+//           because tw % 8 == 0).  L2->smem traffic for A drops from kh*kw to kw*(th+kh-1)/th reads per input element.
 //   PATCH, wide (64-channel chunks = 128-byte rows, kw > 1): tile = 16 rows x 8 pixels, ONE copy per channel chunk brings the
 //           (16+kh-1) x PW patch (PW = 8*MT + 8 pixels: the MT sub-tiles sit side by side in it) and ALL kh*kw taps are read
-//           from it: tap (r, s) = descriptor start + (r*PW + s) rows, the 8 pixels of an output row are one 8-row swizzle
-//           group, consecutive output rows are PW*128 bytes apart (the descriptor's group stride).  The start is then s rows off the
-//           1024-byte swizzle pattern; the descriptor's base-offset field must stay 0 for that (measured on B200: the hardware
-//           swizzles on absolute shared-memory address bits, like the TMA write did; a non-zero base offset shifts the pattern twice).
-//           A traffic: (16+kh-1)*PW / (128*MT) reads per input element = 2.25 (MT 1) / 1.69 (MT 2) instead of 3.75.
+//           from it: tap (r, s) = descriptor start + (r*PW + s) rows, the 8 pixels of an output row are one 8-row swizzle group,
+//           consecutive output rows are PW*128 bytes apart (the descriptor's group stride).
 // Weights (B): 2-D TMA tiles of the packed [Cout][kh][kw][Cin_pad] matrix, one per (tap, channel chunk); A and B
-// have separate mbarrier rings because one A patch feeds kh B tiles.
-// MMA: one elected thread issues tcgen05.mma (M128 x BLOCK_N x K16, fp32 accumulate) into one of two TMEM
-// accumulators, so the epilogue of tile i overlaps the MMAs of tile i+1; tcgen05.commit releases smem stages and
-// publishes the accumulator.
-// Tiles: every tile owns 128 TMEM columns = MT sub-tiles of 128 rows x BLOCK_N (MT = 128/BLOCK_N for BLOCK_N < 128), so
-// narrow layers amortise the per-tile latencies like wide ones and one B tile feeds MT sub-tiles.
-// Epilogue (16 independent warps, no block barrier): warp = (TMEM lane quarter, slot); each drains its 32-column chunks
-// with tcgen05.ld -> + folded-BN bias (whole vector preloaded in smem) -> SiLU -> (+ residual, prefetched into
-// registers before the TMEM load) -> fp16/bf16 -> 64 contiguous bytes per row straight to the NHWC (slice) view, then
-// arrives on the accumulator's "empty" barrier and moves on to the next tile while its siblings may still be storing.
+// have separate mbarrier rings because one A patch feeds kh B tiles (PATCH mode: the kh tiles of a group may share one stage).
+// MMA + epilogue: two consumer warpgroups.  Warpgroup w owns rows [64w, 64w + 64) of every 128-row sub-tile and issues
+// wgmma m64 x BLOCK_N x k16 (fp32 accumulators in registers) for them; after the tile's last K block it applies the
+// folded-BN bias -> SiLU -> (+ residual) -> fp16/bf16 and stores straight from the registers to the NHWC (slice) view.
+// Epilogue stores: by default each thread stores its 4-byte pairs straight from the registers; on request each warpgroup stages
+// its packed 64 x BLOCK_N block in shared memory and writes whole 16-byte row segments instead.
+// Tiles: MT sub-tiles of 128 rows x BLOCK_N with MT * BLOCK_N <= 256 (128 accumulator registers per thread), so one weight
+// tile feeds MT sub-tiles and narrow layers do as much work per barrier round as wide ones.
+// Clusters (2 or 4 CTAs along M): the CTAs of a cluster work on different M super-tiles of the SAME N tile in lock-step, each
+// fetches 1/csize of every weight tile and TMA-multicasts it to all of them, so the L2 -> smem weight traffic per CTA drops by
+// the cluster size.  A weight stage is free again only when the consumers of every CTA of the cluster have released it.
 // Detect head (EPI=1): N tile == one anchor; raw logits and decoded predictions are staged in smem in the exact
 // global layout and copied out with 16-byte vectors.
-// Persistent grid (<= one CTA per SM), warp-specialised: warp 0 TMA producer, warp 1 MMA issuer + TMEM owner,
-// warps 2..17 epilogue.
+// Limits: a consumer waits for every K group's wgmma before releasing its stage, and both warpgroups run the epilogue of the
+// same tile, so the tensor cores idle during each epilogue; overlapping them (two accumulator sets or ping-pong warpgroups) is the
+// next step for this kernel.
+// Persistent grid (<= one CTA per SM), warp-specialised: warp 0 TMA producer (its warpgroup hands its registers to the
+// consumers through setmaxnreg), warpgroups 1 and 2 MMA + epilogue.
 //
 // Replaces reference models/common.py:86-92 (Conv), :181 (Bottleneck add), :246/:340/:453 (cat, via strided
 // output views) and models/yolo.py:95-113 (Detect level).
@@ -43,25 +44,18 @@
 #include "../../include/y5b200.h"
 #include "common.cuh"
 #include "host_util.h"
+#include "wgmma.cuh"
 
 namespace y5 {
 
 constexpr int kBlockM = 128;
-constexpr int kEpiWarps = 16;
-constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kThreads = 64 + kEpiThreads + 32;  // warp0 producer, warp1 mma, warps 2..17 epilogue, warp 18 second mma issuer (MT == 2)
-constexpr int kMma2Warp = 2 + kEpiWarps;         // (96 registers per thread either way: the allocation granule covers 640 threads)
+constexpr int kConsumers = 2;                          // MMA + epilogue warpgroups (64 rows of each sub-tile each)
+constexpr int kConsumerThreads = 128 * kConsumers;
+constexpr int kThreads = 128 + kConsumerThreads;       // warpgroup 0: TMA producer (warp 0 only)
 constexpr int kMaxStages = 8;
 constexpr int kHeadN = 128;                 // head GEMM: one anchor per 128-wide N tile (no <= 128)
 
 enum AMode { A_LINEAR = 0, A_IM2COL = 1, A_PATCH = 2 };
-
-// sub-tiles (128 rows each) per tile: every tile owns 128 TMEM columns (256 for BLOCK_N = 256), so the fixed per-tile
-// latencies (barrier round trips, TMEM load, first global access) are amortised over the same amount of output whatever
-// the channel count, and one B tile feeds MT sub-tiles.
-__host__ __device__ constexpr int mt_for(int block_n, int epi) { return (epi == 0 && block_n < 128) ? 128 / block_n : 1; }
-// For BLOCK_N >= 128 the host may also pick MT = 2 (tiles of 256 x 128 / 256 x 256): deep-K layers are bound by
-// L2->smem operand traffic, and a 256x256 tile needs half the bytes per flop of a 128x128 one.
 
 struct ConvParams {
     int M, N;                   // GEMM rows (B*Ho*Wo), output channels
@@ -73,17 +67,13 @@ struct ConvParams {
     int Ho, Wo, HoWo, stride, pad_h, pad_w;
     int tw, th, tiles_x, tiles_y;  // PATCH: spatial sub-tile th x tw (= 128 pixels), sub-tiles per image
     int b_grouped;              // PATCH: a weight stage holds all kh tiles of one (chunk, horizontal tap) group: one barrier round per group
-    uint32_t b_sub_bytes;       // bytes of one weight tile inside a (possibly grouped) stage
-    int cluster_n;              // thread-block cluster size of the launch (what %cluster_nctarank returns; read from here in the hot loops)
     int patch_pw;               // > 0: wide patch mode, patch row pitch in pixels (8*MT + 8); one A copy per channel chunk feeds kh*kw taps
+    int cluster_n;              // CTAs per cluster (1, 2, 4): weight tiles are split between them and multicast
+    uint32_t stg_bytes;         // EPI 0: shared-memory staging of the epilogue (0 = direct stores)
+    uint32_t b_sub_bytes;       // bytes of one weight tile inside a (possibly grouped) stage
     float rcp_per_img, rcp_tiles_x, rcp_HoWo, rcp_Wo;  // reciprocals for fdiv(): exact small-integer division in ~7 instructions
     int a_stages, b_stages;
-    int tma_store;              // epilogue: per-warp swizzled smem staging + cp.async.bulk.tensor store instead of row-strided STG
-    int c_bw, c_bh;             // PATCH + tma_store: store box = c_bw pixels x c_bh rows (c_bw * c_bh = 32)
-    int b_resident;             // weights of the (single) N tile stay in shared memory for the whole kernel: 1 = loaded with the first tile,
-                                // 2 = constant weights, fetched BEFORE the programmatic-dependency wait (overlaps the previous kernel's tail)
     uint32_t a_sub_bytes, a_stage_bytes, b_stage_bytes;
-    uint32_t idesc;
     int is_bf16, act;
     const float* bias;
     int bias_n;                 // floats preloaded into smem
@@ -101,11 +91,11 @@ struct ConvParams {
 };
 
 struct SmemLayout {
-    uint32_t off_a, off_b, off_out, off_bias, off_bars, off_tmem, total;
+    uint32_t off_a, off_b, off_out, off_bias, off_bars, total;
 };
 
 __host__ __device__ inline SmemLayout smem_layout(int epi, int no, int bias_n, int a_stages, int b_stages, uint32_t a_bytes,
-                                                   uint32_t b_bytes) {
+                                                   uint32_t b_bytes, uint32_t stg_bytes) {
     SmemLayout L;
     uint32_t o = 0;
     L.off_a = o;
@@ -115,14 +105,12 @@ __host__ __device__ inline SmemLayout smem_layout(int epi, int no, int bias_n, i
     o = (o + 1023) & ~1023u;
     L.off_out = o;
     if (epi == 1) o += 4 * ((kBlockM * no * 2 + 1023) & ~1023u);  // head: 2 sets x {raw, decoded} blocks [128][no], global layout
-    if (epi == 2) o += kEpiWarps * 2048;                           // EPI 0 with TMA store: one [32 rows][32 ch] staging tile per epilogue warp
+    else o += stg_bytes;                                            // EPI 0 staged stores: one [64 rows][BLOCK_N] block per consumer warpgroup
     L.off_bias = o;
     o += ((bias_n + 3) & ~3) * 4;
     o = (o + 7) & ~7u;
     L.off_bars = o;
-    o += (4 * kMaxStages + 4) * 8;
-    L.off_tmem = o;
-    o += 16;
+    o += 4 * kMaxStages * 8;
     L.total = o;
     return L;
 }
@@ -138,336 +126,17 @@ __device__ __forceinline__ int fdiv(int n, int d, float rd) {
     return q;
 }
 
-// Detect-head epilogue for one 32-column chunk of a row: logits -> raw + decoded (models/yolo.py:103-109), both written into the
-// shared-memory staging blocks that mirror the global [pixel][no] layout.  Values are packed in pairs and stored as 32-bit
-// words: a row starts on an odd 16-bit element when row*no is odd (no = 85), so the pairing shifts by one for those rows and
-// the two boundary elements go out as 16-bit stores (the neighbouring halves of those words belong to other threads).
-template <int C>
-__device__ __forceinline__ void head_chunk(const uint32_t (&v)[32], const float* __restrict__ bias, int no, int nc, float fgx, float fgy,
-                                           float det_stride, float aw, float ah, bool bf16, uint16_t* __restrict__ stage_raw,
-                                           uint16_t* __restrict__ stage_z, int row) {
-    // words wr[j] / wz[j] = elements (2j, 2j+1) of this chunk, converted two at a time (cvt.rn.f16x2 / bf16x2)
-    uint32_t wr[16], wz[16];
-    const float4* b4 = reinterpret_cast<const float4*>(bias + C * 32);  // 128-byte aligned: bias vector base and C*32 floats
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        const float4 bb = b4[q];
-        const float bv[4] = {bb.x, bb.y, bb.z, bb.w};
-        float x[4], d[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-            const int j = q * 4 + t;
-            const int o = C * 32 + j;
-            x[t] = __uint_as_float(v[j]) + bv[t];
-            d[t] = x[t];
-            if (o < 5 + nc) {
-                const float sg = sigmoid_f(x[t]);
-                if (C == 0 && j == 0) d[t] = (sg * 2.0f + fgx) * det_stride;
-                else if (C == 0 && j == 1) d[t] = (sg * 2.0f + fgy) * det_stride;
-                else if (C == 0 && j == 2) { const float u = sg * 2.0f; d[t] = u * u * aw; }
-                else if (C == 0 && j == 3) { const float u = sg * 2.0f; d[t] = u * u * ah; }
-                else d[t] = sg;
-            }
-        }
-        wr[2 * q] = pack2(x[0], x[1], bf16); wr[2 * q + 1] = pack2(x[2], x[3], bf16);
-        wz[2 * q] = pack2(d[0], d[1], bf16); wz[2 * q + 1] = pack2(d[2], d[3], bf16);
-    }
-    const int e0 = row * no + C * 32;     // first element of this thread's chunk inside the [128][no] block
-    const int n_here = min(32, no - C * 32);
-    uint16_t* pr = stage_raw + e0;
-    uint16_t* pz = stage_z + e0;
-    if (!(e0 & 1)) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            if (2 * j + 1 < n_here) {
-                *reinterpret_cast<uint32_t*>(pr + 2 * j) = wr[j];
-                *reinterpret_cast<uint32_t*>(pz + 2 * j) = wz[j];
-            } else if (2 * j < n_here) {
-                pr[2 * j] = static_cast<uint16_t>(wr[j]);
-                pz[2 * j] = static_cast<uint16_t>(wz[j]);
-            }
-        }
-    } else {  // odd start: element 0 alone, then words made of (2j+1, 2j+2) = funnel shift of two neighbouring pair-words
-        if (n_here > 0) { pr[0] = static_cast<uint16_t>(wr[0]); pz[0] = static_cast<uint16_t>(wz[0]); }
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            if (2 * j + 2 < n_here) {
-                *reinterpret_cast<uint32_t*>(pr + 2 * j + 1) = __funnelshift_r(wr[j], wr[j < 15 ? j + 1 : 15], 16);
-                *reinterpret_cast<uint32_t*>(pz + 2 * j + 1) = __funnelshift_r(wz[j], wz[j < 15 ? j + 1 : 15], 16);
-            } else if (2 * j + 1 < n_here) {
-                pr[2 * j + 1] = static_cast<uint16_t>(wr[j] >> 16);
-                pz[2 * j + 1] = static_cast<uint16_t>(wz[j] >> 16);
-            }
-        }
-    }
-}
-
-// The MMA-issuing warp's loop, specialised.  ncu (yolov5l, 64-channel 3x3 layer): this warp never waits on a barrier, it is busy
-// for the whole kernel executing ~120 SASS instructions per 8 MMAs at ~9 clocks each (uniform-datapath latencies, one warp), i.e.
-// ITS instruction count bounds every layer whose MMAs are short (N <= 128, or few K steps per barrier round).  Every run-time
-// mode test inside the loop costs a constant load + compare + branch per weight tile, so the common case -- 64-channel chunks
-// (4 K steps), streamed weights, no weight multicast, no wide patch -- gets its own straight-line loops here, chosen once per
-// kernel; the generic loop in the kernel body handles the rest.
-//   PATCH   : A groups of kh weight tiles (vertical taps read the same activation patch at row offsets)
-//   GROUPED : the kh tiles of a group share one weight stage (one barrier round and one commit per group)
-//   MI0, MI1: the sub-tiles [MI0, MI1) this warp issues for.  With MT == 2 two warps run this loop, one per sub-tile (independent
-//             accumulators, same operand stages): the MMA stream, the longest of the kernel for narrow tiles, is halved; every
-//             "empty" / "accumulator full" barrier then expects one commit from each of them.
-template <int BLOCK_N, int MT, int CG, bool PATCH, bool GROUPED, int MI0 = 0, int MI1 = MT>
-__device__ __forceinline__ void mma_issue_lean(const ConvParams& p, uint64_t* a_full, uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty,
-                                               uint64_t* tmem_full, uint64_t* tmem_empty, uint32_t tmem_base, uint32_t a_base, uint32_t b_base,
-                                               int tile0, int tile_step, int num_tiles) {
-    constexpr int kAccCols = MT * BLOCK_N;
-    constexpr int NACC = kAccCols <= 256 ? 2 : 1;
-    const uint32_t dhi = umma_desc_hi(128);
-    const uint32_t a_stage16 = p.a_stage_bytes >> 4, b_stage16 = p.b_stage_bytes >> 4, a_sub16 = p.a_sub_bytes >> 4, b_sub16 = p.b_sub_bytes >> 4;
-    const uint32_t a_shift16 = PATCH ? static_cast<uint32_t>(p.tw * 128) >> 4 : 0u;
-    const uint32_t idesc = p.idesc;
-    const int a_stages = p.a_stages, b_stages = p.b_stages;
-    const int grp = PATCH ? p.kh : 1;
-    const int num_groups = PATCH ? p.c_chunks * p.kw : p.kh * p.kw * p.c_chunks;
-    int as = 0, bs = 0, acc = 0;
-    uint32_t aph = 0, bph = 0, acc_phase = 0;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * kAccCols;
-        uint32_t accum = 0;
-        for (int g = 0; g < num_groups; ++g) {
-            mbar_wait(&a_full[as], aph);  // !PATCH: the stage's activation AND weight tiles (one barrier pair per stage, see producer_lean)
-            uint32_t a_lo = a_base + as * a_stage16;
-            const bool last_group = g == num_groups - 1;
-            if (!PATCH) {
-                tc_fence_after();
-                const uint32_t b_lo = b_base + as * b_stage16;
-                if (elect_one()) {
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-#pragma unroll
-                        for (int mi = MI0; mi < MI1; ++mi) {
-                            if (CG == 2) umma_f16_ss_lohi_cg2(d_tmem + mi * BLOCK_N, a_lo + mi * a_sub16 + 2 * k, b_lo + 2 * k, dhi, idesc, accum | k);
-                            else umma_f16_ss_lohi(d_tmem + mi * BLOCK_N, a_lo + mi * a_sub16 + 2 * k, b_lo + 2 * k, dhi, idesc, accum | k);
-                        }
-                    }
-                    if (CG == 2) {
-                        umma_commit_cg2(&a_empty[as], 3);
-                        if (last_group) umma_commit_cg2(&tmem_full[acc], 3);
-                    } else {
-                        umma_commit(&a_empty[as]);
-                        if (last_group) umma_commit(&tmem_full[acc]);
-                    }
-                }
-                __syncwarp();
-                accum = 1;
-            } else if (GROUPED) {  // the group's kh weight tiles arrived together: one wait, one elected region, one commit each
-                mbar_wait(&b_full[bs], bph);
-                tc_fence_after();
-                uint32_t b_lo = b_base + bs * b_stage16;
-                if (elect_one()) {
-                    for (int j = 0; j < grp; ++j) {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-#pragma unroll
-                            for (int mi = MI0; mi < MI1; ++mi) {
-                                if (CG == 2) umma_f16_ss_lohi_cg2(d_tmem + mi * BLOCK_N, a_lo + mi * a_sub16 + 2 * k, b_lo + 2 * k, dhi, idesc, accum | k);
-                                else umma_f16_ss_lohi(d_tmem + mi * BLOCK_N, a_lo + mi * a_sub16 + 2 * k, b_lo + 2 * k, dhi, idesc, accum | k);
-                            }
-                        }
-                        accum = 1;
-                        a_lo += a_shift16;
-                        b_lo += b_sub16;
-                    }
-                    if (CG == 2) {
-                        umma_commit_cg2(&b_empty[bs], 3);
-                        umma_commit_cg2(&a_empty[as], 3);
-                        if (last_group) umma_commit_cg2(&tmem_full[acc], 3);
-                    } else {
-                        umma_commit(&b_empty[bs]);
-                        umma_commit(&a_empty[as]);
-                        if (last_group) umma_commit(&tmem_full[acc]);
-                    }
-                }
-                __syncwarp();
-                accum = 1;
-                if (++bs == b_stages) { bs = 0; bph ^= 1; }
-            } else {
-                for (int j = 0; j < grp; ++j) {
-                    mbar_wait(&b_full[bs], bph);
-                    tc_fence_after();
-                    const uint32_t b_lo = b_base + bs * b_stage16;
-                    if (elect_one()) {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-#pragma unroll
-                            for (int mi = MI0; mi < MI1; ++mi) {
-                                if (CG == 2) umma_f16_ss_lohi_cg2(d_tmem + mi * BLOCK_N, a_lo + mi * a_sub16 + 2 * k, b_lo + 2 * k, dhi, idesc, accum | k);
-                                else umma_f16_ss_lohi(d_tmem + mi * BLOCK_N, a_lo + mi * a_sub16 + 2 * k, b_lo + 2 * k, dhi, idesc, accum | k);
-                            }
-                        }
-                        if (CG == 2) {
-                            umma_commit_cg2(&b_empty[bs], 3);
-                            if (j == grp - 1) umma_commit_cg2(&a_empty[as], 3);
-                            if (j == grp - 1 && last_group) umma_commit_cg2(&tmem_full[acc], 3);
-                        } else {
-                            umma_commit(&b_empty[bs]);
-                            if (j == grp - 1) umma_commit(&a_empty[as]);
-                            if (j == grp - 1 && last_group) umma_commit(&tmem_full[acc]);
-                        }
-                    }
-                    __syncwarp();
-                    accum = 1;
-                    if (++bs == b_stages) { bs = 0; bph ^= 1; }
-                    a_lo += a_shift16;
-                }
-            }
-            if (++as == a_stages) { as = 0; aph ^= 1; }
-        }
-        if (++acc == NACC) { acc = 0; acc_phase ^= 1; }
-    }
-}
-
-// The TMA-issuing warp's loop, specialised the same way (it is the other single-warp instruction stream of the kernel: for 1x1
-// and TMA-im2col layers, one activation + one weight copy per K block, it is the longer of the two).
-//   MODE != A_PATCH : activation and weight tile of a K block share ONE full / empty barrier pair (same ring index): half the
-//                     barrier round trips for this warp and for the MMA warp
-//   MODE == A_PATCH : per (chunk, horizontal tap) group one activation patch per sub-tile and kh weight tiles (GROUPED: in one stage)
-template <int BLOCK_N, int MT, int CG, int MODE, bool GROUPED>
-__device__ __forceinline__ void producer_lean(const CUtensorMap* tmA, const CUtensorMap* tmB, const ConvParams& p, uint8_t* sA, uint8_t* sB,
-                                              uint64_t* a_full, uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty, uint32_t crank, int tile0,
-                                              int tile_step, int num_tiles) {
-    const int csz = CG;  // lean mode: the cluster is exactly the CTA pair (or a single CTA)
-    const int nn = p.num_n_tiles;
-    const int step_q = tile_step / nn, step_r = tile_step - step_q * nn;
-    int tq = tile0 / nn, tr = tile0 - tq * nn;
-    const uint32_t a_stage_bytes = p.a_stage_bytes, b_stage_bytes = p.b_stage_bytes, a_sub_bytes = p.a_sub_bytes, b_sub_bytes = p.b_sub_bytes;
-    const int a_stages = p.a_stages, b_stages = p.b_stages;
-    const int c_chunks = p.c_chunks, kw = p.kw, kh = p.kh;
-    int as = 0, bs = 0;
-    uint32_t aph = 0, bph = 0;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        const int ms = tq * csz + static_cast<int>(crank);
-        const int n0 = tr * BLOCK_N + (CG == 2 ? static_cast<int>(crank) * (BLOCK_N / 2) : 0);  // pair mode: my half of the weight rows
-        tq += step_q;
-        tr += step_r;
-        if (tr >= nn) { tr -= nn; ++tq; }
-        int img[MT], y0[MT], x0[MT];
-#pragma unroll
-        for (int mi = 0; mi < MT; ++mi) {
-            const int mt = ms * MT + mi;
-            img[mi] = y0[mi] = x0[mi] = 0;
-            if (MODE == A_IM2COL) {
-                const int m0 = mt * kBlockM;
-                img[mi] = fdiv(m0, p.HoWo, p.rcp_HoWo);
-                const int rem = m0 - img[mi] * p.HoWo;
-                const int oy = fdiv(rem, p.Wo, p.rcp_Wo);
-                y0[mi] = oy * p.stride - p.pad_h;
-                x0[mi] = (rem - oy * p.Wo) * p.stride - p.pad_w;
-            } else if (MODE == A_PATCH) {
-                const int per_img = p.tiles_x * p.tiles_y;
-                img[mi] = fdiv(mt, per_img, p.rcp_per_img);
-                const int rem = mt - img[mi] * per_img;
-                const int ty = fdiv(rem, p.tiles_x, p.rcp_tiles_x);
-                y0[mi] = ty * p.th - p.pad_h;
-                x0[mi] = (rem - ty * p.tiles_x) * p.tw - p.pad_w;
-            }
-        }
-        if (MODE != A_PATCH) {
-            int r = 0, sx = 0, cc = 0;
-            const int num_kb = kh * kw * c_chunks;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait(&a_empty[as], aph ^ 1);
-                if (elect_one()) {
-                    if (CG == 1 || crank == 0) mbar_arrive_expect_tx(&a_full[as], CG * (a_stage_bytes + b_stage_bytes));
-                    const uint32_t bar = CG == 2 ? mapa_u32(&a_full[as], 0) : 0;
-#pragma unroll
-                    for (int mi = 0; mi < MT; ++mi) {
-                        uint8_t* a_dst = sA + as * a_stage_bytes + mi * a_sub_bytes;
-                        if (MODE == A_LINEAR) {
-                            if (CG == 2) tma_load_2d_cg2(tmA, bar, a_dst, cc * 64, (ms * MT + mi) * kBlockM);
-                            else tma_load_2d(tmA, &a_full[as], a_dst, cc * 64, (ms * MT + mi) * kBlockM);
-                        } else {
-                            if (CG == 2)
-                                tma_load_im2col_4d_cg2(tmA, bar, a_dst, cc * 64, x0[mi], y0[mi], img[mi], static_cast<uint16_t>(sx), static_cast<uint16_t>(r));
-                            else
-                                tma_load_im2col_4d(tmA, &a_full[as], a_dst, cc * 64, x0[mi], y0[mi], img[mi], static_cast<uint16_t>(sx), static_cast<uint16_t>(r));
-                        }
-                    }
-                    if (CG == 2) tma_load_2d_cg2(tmB, bar, sB + as * b_stage_bytes, kb * 64, n0);
-                    else tma_load_2d(tmB, &a_full[as], sB + as * b_stage_bytes, kb * 64, n0);
-                }
-                __syncwarp();
-                if (++as == a_stages) { as = 0; aph ^= 1; }
-                if (++cc == c_chunks) { cc = 0; if (++sx == kw) { sx = 0; ++r; } }
-            }
-        } else {
-            for (int cc = 0; cc < c_chunks; ++cc) {
-                for (int sx = 0; sx < kw; ++sx) {
-                    mbar_wait(&a_empty[as], aph ^ 1);
-                    if (GROUPED) mbar_wait(&b_empty[bs], bph ^ 1);
-                    if (elect_one()) {
-                        if (CG == 1 || crank == 0) mbar_arrive_expect_tx(&a_full[as], CG * a_stage_bytes);
-                        const uint32_t a_bar = CG == 2 ? mapa_u32(&a_full[as], 0) : 0;
-#pragma unroll
-                        for (int mi = 0; mi < MT; ++mi) {
-                            uint8_t* a_dst = sA + as * a_stage_bytes + mi * a_sub_bytes;
-                            if (CG == 2) tma_load_4d_cg2(tmA, a_bar, a_dst, cc * 64, x0[mi] + sx, y0[mi], img[mi]);
-                            else tma_load_4d(tmA, &a_full[as], a_dst, cc * 64, x0[mi] + sx, y0[mi], img[mi]);
-                        }
-                        if (GROUPED) {
-                            if (CG == 1 || crank == 0) mbar_arrive_expect_tx(&b_full[bs], CG * b_stage_bytes);
-                            const uint32_t b_bar = CG == 2 ? mapa_u32(&b_full[bs], 0) : 0;
-                            for (int j = 0; j < kh; ++j) {
-                                const int kb = (j * kw + sx) * c_chunks + cc;
-                                uint8_t* b_dst = sB + bs * b_stage_bytes + j * b_sub_bytes;
-                                if (CG == 2) tma_load_2d_cg2(tmB, b_bar, b_dst, kb * 64, n0);
-                                else tma_load_2d(tmB, &b_full[bs], b_dst, kb * 64, n0);
-                            }
-                        }
-                    }
-                    __syncwarp();
-                    if (++as == a_stages) { as = 0; aph ^= 1; }
-                    if (GROUPED) {
-                        if (++bs == b_stages) { bs = 0; bph ^= 1; }
-                    } else {
-                        for (int j = 0; j < kh; ++j) {
-                            const int kb = (j * kw + sx) * c_chunks + cc;
-                            mbar_wait(&b_empty[bs], bph ^ 1);
-                            if (elect_one()) {
-                                if (CG == 1 || crank == 0) mbar_arrive_expect_tx(&b_full[bs], CG * b_stage_bytes);
-                                if (CG == 2) tma_load_2d_cg2(tmB, mapa_u32(&b_full[bs], 0), sB + bs * b_stage_bytes, kb * 64, n0);
-                                else tma_load_2d(tmB, &b_full[bs], sB + bs * b_stage_bytes, kb * 64, n0);
-                            }
-                            __syncwarp();
-                            if (++bs == b_stages) { bs = 0; bph ^= 1; }
-                        }
-                    }
-                }
-            }
-        }
-    }
-}
-
-// CG = 2: CTA-pair mode (tcgen05 cta_group::2).  The two CTAs of a cluster work on two M super-tiles of the SAME N tile as ONE
-// M = 256 MMA: each CTA stages its own 128 activation rows and HALF of the weight tile (BLOCK_N / 2 rows), the leader's MMA
-// reads both CTAs' shared memory and writes 128 x BLOCK_N accumulators into each CTA's TMEM.  Weight traffic L2 -> smem per
-// CTA halves (it is the larger operand of the 3x3 layers), which is what bounds them with cta_group::1.  Barrier protocol:
-// "full" barriers live in the leader only and collect the transaction bytes of BOTH CTAs' TMA copies (cp.async.bulk.tensor
-// .cta_group::2 may signal the peer's barrier); "empty" / "accumulator full" arrive in both CTAs through the multicast form of
-// tcgen05.commit; the follower's epilogue warps arrive remotely on the leader's "accumulator empty" barrier.
-template <int BLOCK_N, int EPI, int MT, int CG = 1>
+// OPT: the instantiation that supports the optional modes (clusters, wide patch, staged stores); the default one compiles them out,
+// which keeps their run-time tests and live registers out of the hot loops (measured 8 % on yolov5l's conv stack).
+template <int BLOCK_N, int EPI, int MT, bool OPT>
 __global__ void __launch_bounds__(kThreads, 1)
-conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
-                 const ConvParams p) {
-    static_assert(CG == 1 || (EPI == 0 && BLOCK_N >= 64), "CTA pairs: plain epilogue, N tile >= 64");
-    constexpr int kAccCols = MT * BLOCK_N;          // TMEM columns per accumulator set (128, 256 or 512)
-    constexpr int NACC = kAccCols <= 256 ? 2 : 1;   // two sets when they fit: epilogue of tile i overlaps the MMAs of tile i+1
-    constexpr uint32_t kTmemCols = NACC * kAccCols < 32 ? 32 : NACC * kAccCols;
-    constexpr int kChunks = kAccCols / 32;          // 32-column epilogue work items per tile (4, 8 or 16)
-    constexpr int kChunksPerSub = BLOCK_N / 32;
+conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
+    static_assert(MT * BLOCK_N <= 256, "accumulators: at most 128 fp32 registers per consumer thread");
+    constexpr int kAcc = BLOCK_N / 2;  // accumulator registers per sub-tile and thread (64 x BLOCK_N over a warpgroup)
 
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const SmemLayout L = smem_layout(EPI == 1 ? 1 : (p.tma_store ? 2 : 0), p.no, p.bias_n, p.a_stages, p.b_stages, p.a_stage_bytes, p.b_stage_bytes);
+    const SmemLayout L = smem_layout(EPI, p.no, p.bias_n, p.a_stages, p.b_stages, p.a_stage_bytes, p.b_stage_bytes, p.stg_bytes);
     uint8_t* sA = smem + L.off_a;
     uint8_t* sB = smem + L.off_b;
     float* sBias = reinterpret_cast<float*>(smem + L.off_bias);
@@ -475,507 +144,347 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint64_t* a_empty = a_full + kMaxStages;
     uint64_t* b_full = a_empty + kMaxStages;
     uint64_t* b_empty = b_full + kMaxStages;
-    uint64_t* tmem_full = b_empty + kMaxStages;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + L.off_tmem);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    // Thread-block cluster (1 or 2+ CTAs along M): the CTAs of a cluster work on different M super-tiles of the SAME
-    // N tile in lock-step over K, each fetches 1/csize of every weight tile and TMA-multicasts it to all of them.
-    const uint32_t csize = cluster_nctarank();
-    const uint32_t crank = cluster_ctarank();
-    const uint16_t cmask = static_cast<uint16_t>((1u << csize) - 1u);
+    const int csize = OPT ? static_cast<int>(cluster_nctarank()) : 1;
+    const uint32_t crank = OPT ? cluster_ctarank() : 0u;
 
-    // MT == 2 on the specialised loops: two MMA-issuing warps, one per sub-tile (see mma_issue_lean)
-    const bool dual_mma = MT == 2 && p.block_k == 64 && !p.b_resident && p.patch_pw == 0 && p.cluster_n == CG;
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
-        if (EPI == 0 && p.tma_store) tma_prefetch_desc(&tmC);
         for (int s = 0; s < kMaxStages; ++s) {
             mbar_init(&a_full[s], 1);
-            mbar_init(&a_empty[s], dual_mma ? 2 : 1);
+            mbar_init(&a_empty[s], kConsumers);  // one arrival per consumer warpgroup
             mbar_init(&b_full[s], 1);
-            mbar_init(&b_empty[s], dual_mma ? 2 : (CG == 2 ? 1 : csize));  // multicast mode: released by the MMA thread of every CTA in the cluster
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&tmem_full[s], dual_mma ? 2 : 1);
-            mbar_init(&tmem_empty[s], CG * kEpiWarps);  // pair mode: the epilogue warps of both CTAs release the leader's barrier
+            mbar_init(&b_empty[s], kConsumers * csize);  // multicast stages: released by the consumers of every CTA of the cluster
         }
         fence_barrier_init();
     }
-    if (warp == 1) { if (CG == 2) tmem_alloc_cg2(tmem_ptr_smem, kTmemCols); else tmem_alloc(tmem_ptr_smem, kTmemCols); }
-    if (warp >= 2 && warp < kMma2Warp)  // whole folded-BN bias vector once: no per-tile global loads on the epilogue's critical path
-        for (int i = threadIdx.x - 64; i < p.bias_n; i += kEpiThreads) {
+    if (threadIdx.x >= 128)  // whole folded-BN bias vector once: no per-tile global loads in the epilogue
+        for (int i = threadIdx.x - 128; i < p.bias_n; i += kConsumerThreads) {
             // SiLU layers keep HALF the bias: the epilogue forms h = (acc + b) / 2 with one FMA and silu = h + h * tanh(h)
             const float b = i < p.N ? __ldg(p.bias + i) : 0.0f;
             sBias[i] = (EPI == 0 && p.act) ? 0.5f * b : b;
         }
-    tc_fence_before();
     __syncthreads();
-    if (csize > 1) cluster_sync_all();  // peers' barriers are initialised before anyone multicasts into them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    // PDL: everything above (barrier init, TMEM allocation, descriptor prefetch, bias preload of constant weights) may
-    // overlap the tail of the previous kernel in the stream; activations are only touched after this point.
-    if (warp == 0 && p.b_resident == 2) {  // the weights do not depend on the previous kernel: start fetching them now
-        const int num_kb = p.kh * p.kw * p.c_chunks;
-        if (elect_one()) {
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_arrive_expect_tx(&b_full[kb], p.b_stage_bytes);
-                tma_load_2d(&tmB, &b_full[kb], sB + kb * p.b_stage_bytes, kb * p.block_k, 0);
-            }
-        }
-        __syncwarp();
-    }
+    if (csize > 1) cluster_sync_all();  // peers' barriers are initialised before anyone multicasts into them or arrives on them
+    // PDL: everything above (barrier init, descriptor prefetch, bias preload) may overlap the tail of the previous kernel in
+    // the stream; activations are only touched after this point.
     griddep_wait();
     griddep_launch_dependents();
 
-    // tiles are (group of csize M super-tiles, N tile); this CTA takes super-tile group*csize + crank
-    const int num_tiles = ((p.num_m_super + static_cast<int>(csize) - 1) / static_cast<int>(csize)) * p.num_n_tiles;
-    const int tile0 = blockIdx.x / csize, tile_step = gridDim.x / csize;
-    // tile -> (M group tq, N tile tr) kept incrementally: one division per kernel instead of two per tile and role
+    // tile = (group of csize M super-tiles, N tile), N fastest: CTAs running at the same time share the activation rows through L2;
+    // this CTA takes super-tile group * csize + crank
     const int nn = p.num_n_tiles;
-    const int step_q = tile_step / nn, step_r = tile_step - step_q * nn;
-    const int tq0 = tile0 / nn, tr0 = tile0 - tq0 * nn;
-#define Y5_NEXT_TILE(tq, tr)            \
-    do {                                \
-        tq += step_q;                   \
-        tr += step_r;                   \
-        if (tr >= nn) { tr -= nn; ++tq; } \
-    } while (0)
+    const int num_tiles = ((p.num_m_super + csize - 1) / csize) * nn;
+    const int tile0 = blockIdx.x / csize, tile_step = gridDim.x / csize;
     const uint32_t row_bytes = p.block_k * 2;
     const bool patch = p.a_mode == A_PATCH;
     // K iteration: "A groups" each feeding `grp` consecutive B tiles.
     //   PATCH : groups = (chunk cc, horizontal tap s), members r = 0..kh-1   -> k-block (r*kw + s)*c_chunks + cc
     //   else  : groups = k-blocks in (r, s, cc) order, one member each
     //   PATCH wide: groups = channel chunks cc, members (r, s) in weight order   -> k-block (r*kw + s)*c_chunks + cc
-    const bool wide = p.patch_pw > 0;
+    const bool wide = OPT && p.patch_pw > 0;
     const int grp = wide ? p.kh * p.kw : (patch ? p.kh : 1);
     const int num_groups = wide ? p.c_chunks : (patch ? p.c_chunks * p.kw : p.kh * p.kw * p.c_chunks);
 
-    // the common case -- 64-channel chunks, streamed weights, no weight multicast, no wide patch -- runs specialised loops in both
-    // single-warp roles (see mma_issue_lean / producer_lean); everything else takes the generic loops below
-    const bool lean = p.block_k == 64 && !p.b_resident && !wide && p.cluster_n == CG;
-    if (warp == 0 && lean) {
-        if (p.a_mode == A_LINEAR)
-            producer_lean<BLOCK_N, MT, CG, A_LINEAR, false>(&tmA, &tmB, p, sA, sB, a_full, a_empty, b_full, b_empty, crank, tile0, tile_step, num_tiles);
-        else if (p.a_mode == A_IM2COL)
-            producer_lean<BLOCK_N, MT, CG, A_IM2COL, false>(&tmA, &tmB, p, sA, sB, a_full, a_empty, b_full, b_empty, crank, tile0, tile_step, num_tiles);
-        else if (p.b_grouped)
-            producer_lean<BLOCK_N, MT, CG, A_PATCH, true>(&tmA, &tmB, p, sA, sB, a_full, a_empty, b_full, b_empty, crank, tile0, tile_step, num_tiles);
-        else
-            producer_lean<BLOCK_N, MT, CG, A_PATCH, false>(&tmA, &tmB, p, sA, sB, a_full, a_empty, b_full, b_empty, crank, tile0, tile_step, num_tiles);
-    } else if (warp == 0) {
+    if (warp < 4) {
+        setmaxnreg_dec<56>();  // 56 / 224: no spills in any instantiation (40 / 232 spilled the producer's tile decode)
+    }
+    if (warp == 0) {
         // ===================================== TMA producer =====================================
-        {   // the whole warp runs the loop with warp-uniform state; one elected lane issues the copies (keeps the TMA
-            // operands in uniform registers: a divergent `lane == 0` region makes the compiler wrap every UTMALDG in a
-            // vote / elect / R2UR waterfall)
-            int as = 0, bs = 0;
-            uint32_t aph = 0, bph = 0;
-            int tq = tq0, tr = tr0;
-            for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-                const int ms = tq * csize + crank;
-                const int n0 = tr * BLOCK_N;
-                Y5_NEXT_TILE(tq, tr);
-                int img[MT], y0[MT], x0[MT];  // IM2COL: base pixel of the first window; PATCH: sub-tile origin
+        // the whole warp runs the loop with warp-uniform state; one elected lane issues the copies
+        int as = 0, bs = 0;
+        uint32_t aph = 0, bph = 0;
+        for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+            const int ms = (tile / nn) * csize + static_cast<int>(crank);
+            const int n0 = (tile - (tile / nn) * nn) * BLOCK_N;
+            int img[MT], y0[MT], x0[MT];  // IM2COL: base pixel of the first window; PATCH: sub-tile origin
 #pragma unroll
-                for (int mi = 0; mi < MT; ++mi) {
-                    const int mt = ms * MT + mi;
-                    img[mi] = y0[mi] = x0[mi] = 0;
-                    if (p.a_mode == A_IM2COL) {
-                        const int m0 = mt * kBlockM;
-                        img[mi] = fdiv(m0, p.HoWo, p.rcp_HoWo);
-                        const int rem = m0 - img[mi] * p.HoWo;
-                        const int oy = fdiv(rem, p.Wo, p.rcp_Wo);
-                        y0[mi] = oy * p.stride - p.pad_h;
-                        x0[mi] = (rem - oy * p.Wo) * p.stride - p.pad_w;
-                    } else if (patch) {
-                        const int per_img = p.tiles_x * p.tiles_y;
-                        img[mi] = fdiv(mt, per_img, p.rcp_per_img);
-                        const int rem = mt - img[mi] * per_img;
-                        const int ty = fdiv(rem, p.tiles_x, p.rcp_tiles_x);
-                        y0[mi] = ty * p.th - p.pad_h;
-                        x0[mi] = (rem - ty * p.tiles_x) * p.tw - p.pad_w;
+            for (int mi = 0; mi < MT; ++mi) {
+                const int mt = ms * MT + mi;
+                img[mi] = y0[mi] = x0[mi] = 0;
+                if (p.a_mode == A_IM2COL) {
+                    const int m0 = mt * kBlockM;
+                    img[mi] = fdiv(m0, p.HoWo, p.rcp_HoWo);
+                    const int rem = m0 - img[mi] * p.HoWo;
+                    const int oy = fdiv(rem, p.Wo, p.rcp_Wo);
+                    y0[mi] = oy * p.stride - p.pad_h;
+                    x0[mi] = (rem - oy * p.Wo) * p.stride - p.pad_w;
+                } else if (patch) {
+                    const int per_img = p.tiles_x * p.tiles_y;
+                    img[mi] = fdiv(mt, per_img, p.rcp_per_img);
+                    const int rem = mt - img[mi] * per_img;
+                    const int ty = fdiv(rem, p.tiles_x, p.rcp_tiles_x);
+                    y0[mi] = ty * p.th - p.pad_h;
+                    x0[mi] = (rem - ty * p.tiles_x) * p.tw - p.pad_w;
+                }
+            }
+            // one A group + its B tiles; PATCH walks (cc, s){r}, the other modes walk (r, s, cc)
+            auto issue_group = [&](int cc, int s, int r0) {
+                mbar_wait(&a_empty[as], aph ^ 1);
+                if (elect_one()) {
+                    mbar_arrive_expect_tx(&a_full[as], p.a_stage_bytes);
+#pragma unroll
+                    for (int mi = 0; mi < MT; ++mi) {
+                        uint8_t* a_dst = sA + as * p.a_stage_bytes + mi * p.a_sub_bytes;
+                        if (wide) {  // one patch for all sub-tiles and taps (sub-tile mi starts 8 pixels = 1024 bytes into it)
+                            if (mi == 0) tma_load_4d(&tmA, &a_full[as], a_dst, cc * p.block_k, x0[0], y0[0], img[0]);
+                        } else if (p.a_mode == A_LINEAR) tma_load_2d(&tmA, &a_full[as], a_dst, cc * p.block_k, (ms * MT + mi) * kBlockM);
+                        else if (p.a_mode == A_IM2COL)
+                            tma_load_im2col_4d(&tmA, &a_full[as], a_dst, cc * p.block_k, x0[mi], y0[mi], img[mi], static_cast<uint16_t>(s),
+                                               static_cast<uint16_t>(r0));
+                        else tma_load_4d(&tmA, &a_full[as], a_dst, cc * p.block_k, x0[mi] + s, y0[mi], img[mi]);
                     }
                 }
-                // one A group + its B tiles; PATCH walks (cc, s){r}, the other modes walk (r, s, cc)
-                auto issue_group = [&](int cc, int s, int r0) {
-                    mbar_wait(&a_empty[as], aph ^ 1);
+                __syncwarp();
+                if (++as == p.a_stages) { as = 0; aph ^= 1; }
+                for (int j = 0; j < grp; ++j) {
+                    const int r = patch ? j : r0;
+                    const int kb = wide ? j * p.c_chunks + cc : (r * p.kw + s) * p.c_chunks + cc;
+                    // grouped stages: the kh tiles of this group share one stage (one wait, one expect_tx covering all of them)
+                    const bool stage_first = !p.b_grouped || j == 0, stage_last = !p.b_grouped || j == grp - 1;
+                    if (stage_first) mbar_wait(&b_empty[bs], bph ^ 1);
                     if (elect_one()) {
-                        if (CG == 1 || crank == 0) mbar_arrive_expect_tx(&a_full[as], CG * p.a_stage_bytes);  // pair: both CTAs' bytes
-                        const uint32_t a_bar = CG == 2 ? mapa_u32(&a_full[as], 0) : 0;                      // the leader's barrier
-#pragma unroll
-                        for (int mi = 0; mi < MT; ++mi) {
-                            uint8_t* a_dst = sA + as * p.a_stage_bytes + mi * p.a_sub_bytes;
-                            if (wide) {  // one patch for all sub-tiles and taps (sub-tile mi starts 8 pixels = 1024 bytes into it)
-                                if (mi == 0) {
-                                    if (CG == 2) tma_load_4d_cg2(&tmA, a_bar, a_dst, cc * p.block_k, x0[0], y0[0], img[0]);
-                                    else tma_load_4d(&tmA, &a_full[as], a_dst, cc * p.block_k, x0[0], y0[0], img[0]);
-                                }
-                            } else if (CG == 2) {
-                                if (p.a_mode == A_LINEAR) tma_load_2d_cg2(&tmA, a_bar, a_dst, cc * p.block_k, (ms * MT + mi) * kBlockM);
-                                else if (p.a_mode == A_IM2COL)
-                                    tma_load_im2col_4d_cg2(&tmA, a_bar, a_dst, cc * p.block_k, x0[mi], y0[mi], img[mi],
-                                                           static_cast<uint16_t>(s), static_cast<uint16_t>(r0));
-                                else tma_load_4d_cg2(&tmA, a_bar, a_dst, cc * p.block_k, x0[mi] + s, y0[mi], img[mi]);
-                            } else if (p.a_mode == A_LINEAR) tma_load_2d(&tmA, &a_full[as], a_dst, cc * p.block_k, (ms * MT + mi) * kBlockM);
-                            else if (p.a_mode == A_IM2COL)
-                                tma_load_im2col_4d(&tmA, &a_full[as], a_dst, cc * p.block_k, x0[mi], y0[mi], img[mi],
-                                                   static_cast<uint16_t>(s), static_cast<uint16_t>(r0));
-                            else tma_load_4d(&tmA, &a_full[as], a_dst, cc * p.block_k, x0[mi] + s, y0[mi], img[mi]);
+                        if (stage_first) mbar_arrive_expect_tx(&b_full[bs], p.b_stage_bytes);
+                        uint8_t* b_dst = sB + bs * p.b_stage_bytes + (p.b_grouped ? j * p.b_sub_bytes : 0u);
+                        if (csize == 1) tma_load_2d(&tmB, &b_full[bs], b_dst, kb * p.block_k, n0);
+                        else {  // my slice of the rows, delivered to every CTA of the cluster
+                            const int slice_rows = BLOCK_N / csize;
+                            tma_load_2d_mcast(&tmB, &b_full[bs], b_dst + crank * slice_rows * row_bytes, kb * p.block_k,
+                                              n0 + static_cast<int>(crank) * slice_rows, static_cast<uint16_t>((1u << csize) - 1u));
                         }
                     }
                     __syncwarp();
-                    if (++as == p.a_stages) { as = 0; aph ^= 1; }
-                    for (int j = 0; j < grp; ++j) {
-                        const int r = patch ? j : r0;
-                        const int kb = wide ? j * p.c_chunks + cc : (r * p.kw + s) * p.c_chunks + cc;
-                        if (p.b_resident) {  // slot kb holds k-block kb for every tile of this CTA (single N tile)
-                            if (p.b_resident == 1 && tile == tile0 && elect_one()) {
-                                mbar_arrive_expect_tx(&b_full[kb], p.b_stage_bytes);
-                                tma_load_2d(&tmB, &b_full[kb], sB + kb * p.b_stage_bytes, kb * p.block_k, n0);
-                            }
-                            __syncwarp();
-                            continue;
-                        }
-                        // grouped stages: the kh tiles of this group share one stage (one wait, one expect_tx covering all of them)
-                        const bool stage_first = !p.b_grouped || j == 0, stage_last = !p.b_grouped || j == grp - 1;
-                        if (stage_first) mbar_wait(&b_empty[bs], bph ^ 1);
-                        if (elect_one()) {
-                            if (stage_first && (CG == 1 || crank == 0)) mbar_arrive_expect_tx(&b_full[bs], CG * p.b_stage_bytes);
-                            uint8_t* b_dst = sB + bs * p.b_stage_bytes + (p.b_grouped ? j * p.b_sub_bytes : 0u);
-                            if (CG == 2)  // my half of the weight tile's rows, into my own shared memory; bytes counted by the leader
-                                tma_load_2d_cg2(&tmB, mapa_u32(&b_full[bs], 0), b_dst, kb * p.block_k, n0 + static_cast<int>(crank) * (BLOCK_N / 2));
-                            else if (csize == 1) tma_load_2d(&tmB, &b_full[bs], b_dst, kb * p.block_k, n0);
-                            else {  // my slice of the rows, delivered to every CTA of the cluster
-                                const uint32_t slice_rows = BLOCK_N / csize;
-                                tma_load_2d_mcast(&tmB, &b_full[bs], b_dst + crank * slice_rows * row_bytes, kb * p.block_k, n0 + crank * slice_rows,
-                                                  cmask);
-                            }
-                        }
-                        __syncwarp();
-                        if (stage_last && ++bs == p.b_stages) { bs = 0; bph ^= 1; }
-                    }
-                };
-                if (wide) {
-                    for (int cc = 0; cc < p.c_chunks; ++cc) issue_group(cc, 0, 0);
-                } else if (patch) {
-                    for (int cc = 0; cc < p.c_chunks; ++cc)
-                        for (int s = 0; s < p.kw; ++s) issue_group(cc, s, 0);
-                } else {
-                    for (int r = 0; r < p.kh; ++r)
-                        for (int s = 0; s < p.kw; ++s)
-                            for (int cc = 0; cc < p.c_chunks; ++cc) issue_group(cc, s, r);
+                    if (stage_last && ++bs == p.b_stages) { bs = 0; bph ^= 1; }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================================== MMA issuer =====================================
-        if ((CG == 1 || crank == 0) && lean) {   // the common case: specialised straight-line loops (see mma_issue_lean)
-            const uint32_t a_base = umma_desc_lo(smem_u32(sA)), b_base = umma_desc_lo(smem_u32(sB));
-            constexpr int M1 = MT == 2 ? 1 : MT;  // MT == 2: this warp issues sub-tile 0, warp kMma2Warp sub-tile 1
-            if (!patch)
-                mma_issue_lean<BLOCK_N, MT, CG, false, false, 0, M1>(p, a_full, a_empty, b_full, b_empty, tmem_full, tmem_empty, tmem_base, a_base, b_base,
-                                                                     tile0, tile_step, num_tiles);
-            else if (p.b_grouped)
-                mma_issue_lean<BLOCK_N, MT, CG, true, true, 0, M1>(p, a_full, a_empty, b_full, b_empty, tmem_full, tmem_empty, tmem_base, a_base, b_base,
-                                                                   tile0, tile_step, num_tiles);
-            else
-                mma_issue_lean<BLOCK_N, MT, CG, true, false, 0, M1>(p, a_full, a_empty, b_full, b_empty, tmem_full, tmem_empty, tmem_base, a_base, b_base,
-                                                                    tile0, tile_step, num_tiles);
-        } else if (CG == 1 || crank == 0) {   // pair mode: the leader CTA issues for both.  whole warp, warp-uniform state; the elected lane issues tcgen05.mma / tcgen05.commit (see the producer's note)
-            int as = 0, bs = 0, acc = 0;
-            uint32_t aph = 0, bph = 0, acc_phase = 0;
-            const int k_steps = p.block_k / 16;
-            // descriptor halves: everything below is 32-bit adds on the low word (units of 16 bytes)
-            const uint32_t dhi = umma_desc_hi(row_bytes);
-            const uint32_t a_base = umma_desc_lo(smem_u32(sA)), b_base = umma_desc_lo(smem_u32(sB));
-            const uint32_t a_stage16 = p.a_stage_bytes >> 4, b_stage16 = p.b_stage_bytes >> 4, a_sub16 = p.a_sub_bytes >> 4;
-            const uint32_t b_sub16 = p.b_sub_bytes >> 4;
-            const uint32_t a_shift16 = patch ? (p.tw * row_bytes) >> 4 : 0;  // between vertical taps inside a patch
-            // wide patch: group stride = one patch row (PW pixels); the tap's horizontal offset s goes into the swizzle base offset
-            const uint32_t dhi_wide = (dhi & ~0x3FFFu) | (((static_cast<uint32_t>(p.patch_pw) * row_bytes) >> 4) & 0x3FFFu);
-            const uint32_t row16 = row_bytes >> 4;
-            const uint32_t idesc = p.idesc;
-            for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-                mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * kAccCols;
-                uint32_t accum = 0;
-                for (int g = 0; g < num_groups; ++g) {
-                    mbar_wait(&a_full[as], aph);
-                    uint32_t a_lo = a_base + as * a_stage16;
-                    const uint32_t a_stage_lo = a_lo;
-                    uint32_t a_hi = dhi;
-                    int tap_r = 0, tap_s = 0;
-                    for (int j = 0; j < grp; ++j) {
-                        if (wide) {
-                            a_lo = a_stage_lo + (tap_r * p.patch_pw + tap_s) * row16;
-                            a_hi = dhi_wide;  // base-offset field stays 0: the swizzle is a function of the absolute smem address (measured)
-                            if (++tap_s == p.kw) { tap_s = 0; ++tap_r; }
-                        }
-                        const bool stage_first = !p.b_grouped || j == 0, stage_last = !p.b_grouped || j == grp - 1;
-                        if (p.b_resident) {
-                            bs = g;  // non-patch: group index == k-block index
-                            if (tile == tile0) mbar_wait(&b_full[bs], 0);
-                        } else if (stage_first) {
-                            mbar_wait(&b_full[bs], bph);
-                        }
-                        tc_fence_after();
-                        const uint32_t b_lo = b_base + bs * b_stage16 + (p.b_grouped ? j * b_sub16 : 0u);
-                        if (elect_one()) {
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                if (k < k_steps) {
-#pragma unroll
-                                    for (int mi = 0; mi < MT; ++mi) {
-                                        if (CG == 2)
-                                            umma_f16_ss_lohi_ab_cg2(d_tmem + mi * BLOCK_N, a_lo + mi * a_sub16 + 2 * k, a_hi, b_lo + 2 * k, dhi, idesc,
-                                                                    (accum | k) != 0 ? 1u : 0u);
-                                        else
-                                            umma_f16_ss_lohi_ab(d_tmem + mi * BLOCK_N, a_lo + mi * a_sub16 + 2 * k, a_hi, b_lo + 2 * k, dhi, idesc,
-                                                                (accum | k) != 0 ? 1u : 0u);
-                                    }
-                                }
-                            }
-                            if (CG == 2) {  // every release / publication reaches both CTAs of the pair
-                                if (stage_last) umma_commit_cg2(&b_empty[bs], 3);
-                                if (j == grp - 1) umma_commit_cg2(&a_empty[as], 3);
-                                if (j == grp - 1 && g == num_groups - 1) umma_commit_cg2(&tmem_full[acc], 3);
-                            } else {
-                                if (p.b_resident || !stage_last) {}
-                                else if (p.cluster_n == 1) umma_commit(&b_empty[bs]);
-                                else umma_commit_mcast(&b_empty[bs], cmask);
-                                if (j == grp - 1) umma_commit(&a_empty[as]);
-                                if (j == grp - 1 && g == num_groups - 1) umma_commit(&tmem_full[acc]);
-                            }
-                        }
-                        __syncwarp();
-                        accum = 1;
-                        if (!p.b_resident && stage_last && ++bs == p.b_stages) { bs = 0; bph ^= 1; }
-                        a_lo += a_shift16;
-                    }
-                    if (++as == p.a_stages) { as = 0; aph ^= 1; }
-                }
-                if (++acc == NACC) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp == kMma2Warp) {
-        // ===================================== second MMA issuer (sub-tile 1 of MT == 2 tiles) =====================================
-        if (MT == 2 && dual_mma && (CG == 1 || crank == 0)) {
-            const uint32_t a_base = umma_desc_lo(smem_u32(sA)), b_base = umma_desc_lo(smem_u32(sB));
-            constexpr int M0 = MT == 2 ? 1 : 0;
-            if (!patch)
-                mma_issue_lean<BLOCK_N, MT, CG, false, false, M0, MT>(p, a_full, a_empty, b_full, b_empty, tmem_full, tmem_empty, tmem_base, a_base, b_base,
-                                                                      tile0, tile_step, num_tiles);
-            else if (p.b_grouped)
-                mma_issue_lean<BLOCK_N, MT, CG, true, true, M0, MT>(p, a_full, a_empty, b_full, b_empty, tmem_full, tmem_empty, tmem_base, a_base, b_base,
-                                                                    tile0, tile_step, num_tiles);
-            else
-                mma_issue_lean<BLOCK_N, MT, CG, true, false, M0, MT>(p, a_full, a_empty, b_full, b_empty, tmem_full, tmem_empty, tmem_base, a_base, b_base,
-                                                                     tile0, tile_step, num_tiles);
-        }
-    } else {
-        // ===================================== epilogue (warps 2..17) =====================================
-        // 16 independent warps: warp = (TMEM lane quarter, slot); slot s drains the 32-column chunks s, s+4, ...
-        // of every tile straight to global memory.  No block-level barrier: a warp that is done with tile i moves
-        // on to tile i+1 (other accumulator set) while its siblings may still be storing.
-        const int et = threadIdx.x - 64;          // 0..511
-        const int ew = warp - 2;                  // 0..15
-        const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-        const int slot = ew >> 2;                 // 0..3
-        const int row = quarter * 32 + lane;      // accumulator row (= TMEM lane) owned by this thread
-        const bool bf16 = p.is_bf16 != 0;
-        const int per_img = p.tiles_x * p.tiles_y;
-        const int tw_shift = patch ? __ffs(p.tw) - 1 : 0;
-        const int ry = row >> tw_shift, rx = row & ((1 << tw_shift) - 1);
-        int acc = 0, head_set = 0;
-        uint32_t acc_phase = 0;
-        int tq = tq0, tr = tr0;
-        const bool staged = EPI == 0 && p.tma_store != 0;
-        const bool any_res = p.res != nullptr;
-        uint8_t* stg = smem + L.off_out + ew * 2048;  // this warp's [32 rows][32 channels] tile, 64-byte rows, SWIZZLE_64B
-        const int pos0 = quarter * 32;                // first tile position of this warp (PATCH: th x tw block, row-major)
-        const int y_in = pos0 >> tw_shift, x_in = pos0 & ((1 << tw_shift) - 1);
-        for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-            const int ms = tq * csize + crank;
-            const int nt = tr;
-            const int n0 = nt * BLOCK_N;
-            Y5_NEXT_TILE(tq, tr);
-            const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * kAccCols;
-
-            if (EPI == 0) {
-                mbar_wait(&tmem_full[acc], acc_phase);
-                tc_fence_after();
-#pragma unroll 1
-                for (int c = slot; c < kChunks; c += 4) {
-                    const int mi = c / kChunksPerSub;             // sub-tile of this chunk
-                    const int col = (c - mi * kChunksPerSub) * 32;  // first column inside the N tile
-                    const int mt = ms * MT + mi;
-                    // warp-uniform decode of the sub-tile (PATCH: image + origin of the th x tw block)
-                    int img = 0, oy0 = 0, ox0 = 0;
-                    if (patch) {
-                        img = fdiv(mt, per_img, p.rcp_per_img);
-                        const int rem = mt - img * per_img;
-                        const int tyi = fdiv(rem, p.tiles_x, p.rcp_tiles_x);
-                        oy0 = tyi * p.th;
-                        ox0 = (rem - tyi * p.tiles_x) * p.tw;
-                    }
-                    // this thread's global output pixel: only the residual read and the direct-store path need it
-                    long long gpix = -1;
-                    if (any_res || !staged) {
-                        if (patch) {
-                            const int oy = oy0 + ry, ox = ox0 + rx;  // (ry, rx) is loop invariant because tw is a power of two
-                            if (mt < p.num_m_tiles && oy < p.Ho && ox < p.Wo) gpix = static_cast<long long>(img) * p.HoWo + oy * p.Wo + ox;
-                        } else {
-                            const long long m = static_cast<long long>(mt) * kBlockM + row;
-                            if (m < p.M) gpix = m;
-                        }
-                    }
-                    const bool live = gpix >= 0;
-                    // residual for this thread's 32 output channels: issued before the TMEM load so its latency overlaps
-                    uint4 rv[4];
-                    const bool has_res = any_res && live;
-                    if (has_res) {
-                        const uint8_t* rp = reinterpret_cast<const uint8_t*>(p.res) + (gpix * p.res_pitch + n0 + col) * 2;
-#pragma unroll
-                        for (int g = 0; g < 4; ++g)
-                            if (n0 + col + g * 8 < p.N) rv[g] = *reinterpret_cast<const uint4*>(rp + g * 16);
-                    }
-                    uint32_t v[32];
-                    tmem_ld_32x32(t_row + c * 32, v);
-                    if (staged) {  // the previous bulk store of this warp must have finished READING the staging tile
-                        if (lane == 0) tma_store_wait_read0();
-                        __syncwarp();
-                    }
-                    tmem_ld_wait();
-                    uint8_t* op = reinterpret_cast<uint8_t*>(p.out) + (gpix * p.out_pitch + n0 + col) * 2;
-                    const float4* b4 = reinterpret_cast<const float4*>(sBias + n0 + col);
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const float4 ba = b4[2 * g], bb = b4[2 * g + 1];
-                        const float bv[8] = {ba.x, ba.y, ba.z, ba.w, bb.x, bb.y, bb.z, bb.w};
-                        float f[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float a = __uint_as_float(v[g * 8 + j]);
-                            if (p.act) {  // bv holds bias / 2 (see the preload): 3 instructions per element
-                                const float h = fmaf(a, 0.5f, bv[j]);
-                                f[j] = silu_from_half(h);
-                            } else {
-                                f[j] = a + bv[j];
-                            }
-                        }
-                        if (has_res) {
-                            const uint32_t rr[4] = {rv[g].x, rv[g].y, rv[g].z, rv[g].w};
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const float2 t = unpack2(rr[j], bf16);
-                                f[2 * j] += t.x;
-                                f[2 * j + 1] += t.y;
-                            }
-                        }
-                        uint4 o;
-                        o.x = pack2(f[0], f[1], bf16);
-                        o.y = pack2(f[2], f[3], bf16);
-                        o.z = pack2(f[4], f[5], bf16);
-                        o.w = pack2(f[6], f[7], bf16);
-                        if (staged) *reinterpret_cast<uint4*>(stg + lane * 64 + ((g ^ ((lane >> 1) & 3)) << 4)) = o;
-                        else if (live && n0 + col + g * 8 < p.N) *reinterpret_cast<uint4*>(op + g * 16) = o;
-                    }
-                    if (staged) {
-                        // one bulk tensor store per (warp, chunk): the copy engine writes whole 64-byte row segments and clips
-                        // rows / pixels / channels beyond the tensor, so no per-thread masks are needed
-                        fence_proxy_async_smem();
-                        __syncwarp();
-                        if (lane == 0 && mt < p.num_m_tiles && n0 + col < p.N) {
-                            if (patch) tma_store_4d(&tmC, stg, n0 + col, ox0 + x_in, oy0 + y_in, img);
-                            else tma_store_2d(&tmC, stg, n0 + col, mt * kBlockM + pos0);
-                            tma_store_commit();
-                        }
-                    }
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {  // this warp is done with the accumulator set (pair mode: tell the leader, it issues the MMAs)
-                    if (CG == 2 && crank != 0) mbar_arrive_cluster(mapa_u32(&tmem_empty[acc], 0));
-                    else mbar_arrive(&tmem_empty[acc]);
-                }
+            };
+            if (wide) {
+                for (int cc = 0; cc < p.c_chunks; ++cc) issue_group(cc, 0, 0);
+            } else if (patch) {
+                for (int cc = 0; cc < p.c_chunks; ++cc)
+                    for (int s = 0; s < p.kw; ++s) issue_group(cc, s, 0);
             } else {
-                // ---- Detect head (models/yolo.py:95-113): N tile `nt` == anchor.  One TMEM pass produces the raw logits AND
-                // the decoded predictions into two smem blocks laid out exactly like their global destinations
-                // ([128 pixels][no] contiguous per anchor), one block barrier, then 16-byte vector copy-out.  Two staging
-                // sets alternate per tile, so the barrier of tile i+1 also fences the reuse of tile i-1's set.
-                const uint32_t blk = (kBlockM * p.no * 2 + 1023) & ~1023u;
-                const int set = head_set;
-                head_set ^= 1;
-                uint16_t* stage_raw = reinterpret_cast<uint16_t*>(smem + L.off_out + (2 * set) * blk);
-                uint16_t* stage_z = reinterpret_cast<uint16_t*>(smem + L.off_out + (2 * set + 1) * blk);
-                const int no = p.no;
-                const int a = nt;
-                const int m0 = ms * kBlockM;
+                for (int r = 0; r < p.kh; ++r)
+                    for (int s = 0; s < p.kw; ++s)
+                        for (int cc = 0; cc < p.c_chunks; ++cc) issue_group(cc, s, r);
+            }
+        }
+    } else if (warp >= 4) {
+    // ===================================== MMA + epilogue (warpgroups 1, 2) =====================================
+    setmaxnreg_inc<224>();
+    const int wg = (warp >> 2) - 1;                       // rows [64 wg, 64 wg + 64) of every sub-tile
+    const int ct = threadIdx.x - 128;                     // 0 .. kConsumerThreads-1
+    const int wrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's first accumulator row (the second is +8)
+    const int ccol = 2 * (lane & 3);                      // this thread's first column inside every 8-column group
+    const bool signal = (threadIdx.x & 127) == 0;         // the warpgroup's thread that releases smem stages
+    const bool bf16 = p.is_bf16 != 0;
+    const uint32_t dhi = gmma_desc_hi(row_bytes);
+    // wide patch: group stride = one patch row (PW pixels); warpgroup wg starts 8 output rows = 8 patch rows down
+    const uint32_t a_hi = wide ? (dhi & ~0x3FFFu) | (((static_cast<uint32_t>(p.patch_pw) * row_bytes) >> 4) & 0x3FFFu) : dhi;
+    const uint32_t a_base = gmma_desc_lo(smem_u32(sA) + (wide ? wg * 8 * p.patch_pw : wg * 64) * row_bytes), b_base = gmma_desc_lo(smem_u32(sB));
+    const uint32_t row16 = row_bytes >> 4;
+    const uint32_t a_stage16 = p.a_stage_bytes >> 4, b_stage16 = p.b_stage_bytes >> 4, a_sub16 = p.a_sub_bytes >> 4;
+    const uint32_t b_sub16 = p.b_sub_bytes >> 4;
+    const uint32_t a_shift16 = patch ? (p.tw * row_bytes) >> 4 : 0;  // between vertical taps inside a patch
+    const int k_steps = p.block_k / 16;
+    const int per_img = p.tiles_x * p.tiles_y;
+    const int tw_shift = patch ? __ffs(p.tw) - 1 : 0;
+    int as = 0, bs = 0, head_set = 0;
+    uint32_t aph = 0, bph = 0;
+    float acc[MT][kAcc];
+#pragma unroll
+    for (int mi = 0; mi < MT; ++mi)
+#pragma unroll
+        for (int i = 0; i < kAcc; ++i) acc[mi][i] = 0.0f;
+
+    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+        const int ms = (tile / nn) * csize + static_cast<int>(crank);
+        const int nt = tile - (tile / nn) * nn;
+        const int n0 = nt * BLOCK_N;
+        for (int g = 0; g < num_groups; ++g) {
+            mbar_wait(&a_full[as], aph);
+            const uint32_t a_stage_lo = a_base + as * a_stage16;
+            uint32_t a_lo = a_stage_lo;
+            for (int j = 0; j < grp; ++j) {
+                if (wide) {  // tap (r, s) of the shared patch
+                    const int tr = j / p.kw, ts = j - tr * p.kw;
+                    a_lo = a_stage_lo + (tr * p.patch_pw + ts) * row16;
+                }
+                const bool stage_first = !p.b_grouped || j == 0, stage_last = !p.b_grouped || j == grp - 1;
+                if (stage_first) mbar_wait(&b_full[bs], bph);
+                const uint32_t b_lo = b_base + bs * b_stage16 + (p.b_grouped ? j * b_sub16 : 0u);
+#pragma unroll
+                for (int mi = 0; mi < MT; ++mi) fence_regs(acc[mi]);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    if (k < k_steps) {
+                        const uint32_t scale_d = (g | j | k) != 0 ? 1u : 0u;  // the tile's first K step overwrites the accumulators
+#pragma unroll
+                        for (int mi = 0; mi < MT; ++mi) {
+                            const uint64_t da = gmma_desc(a_lo + mi * a_sub16 + 2 * k, a_hi), db = gmma_desc(b_lo + 2 * k, dhi);
+                            if (bf16) Wgmma<BLOCK_N>::template run<true, 0, 0>(acc[mi], da, db, scale_d);
+                            else Wgmma<BLOCK_N>::template run<false, 0, 0>(acc[mi], da, db, scale_d);
+                        }
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+#pragma unroll
+                for (int mi = 0; mi < MT; ++mi) fence_regs(acc[mi]);
+                if (stage_last) {
+                    if (signal) {
+                        if (csize == 1) mbar_arrive(&b_empty[bs]);
+                        else
+                            for (int r = 0; r < csize; ++r) mbar_arrive_cluster(mapa_u32(&b_empty[bs], static_cast<uint32_t>(r)));
+                    }
+                    if (++bs == p.b_stages) { bs = 0; bph ^= 1; }
+                }
+                a_lo += a_shift16;
+            }
+            if (signal) mbar_arrive(&a_empty[as]);
+            if (++as == p.a_stages) { as = 0; aph ^= 1; }
+        }
+
+        if (EPI == 0) {
+            const bool staged = OPT && p.stg_bytes != 0;
+            const uint32_t stg_pitch = BLOCK_N * 2 + 16;  // +16 bytes: the fragment's 8 rows x 4 column pairs hit 32 distinct banks
+            uint8_t* stg = smem + L.off_out + wg * 64 * stg_pitch;
+#pragma unroll
+            for (int mi = 0; mi < MT; ++mi) {
+                const int mt = ms * MT + mi;
+                int img = 0, oy0 = 0, ox0 = 0;
+                if (patch) {  // image + origin of the th x tw block
+                    img = fdiv(mt, per_img, p.rcp_per_img);
+                    const int rem = mt - img * per_img;
+                    const int tyi = fdiv(rem, p.tiles_x, p.rcp_tiles_x);
+                    oy0 = tyi * p.th;
+                    ox0 = (rem - tyi * p.tiles_x) * p.tw;
+                }
+                // global output pixel of tile row `row`, -1 outside the output
+                auto pixel_of = [&](int row) -> long long {
+                    if (patch) {
+                        const int oy = oy0 + (row >> tw_shift), ox = ox0 + (row & ((1 << tw_shift) - 1));
+                        return (mt < p.num_m_tiles && oy < p.Ho && ox < p.Wo) ? static_cast<long long>(img) * p.HoWo + oy * p.Wo + ox : -1;
+                    }
+                    const long long m = static_cast<long long>(mt) * kBlockM + row;
+                    return m < p.M ? m : -1;
+                };
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = wrow + 8 * h;
+                    const long long gpix = pixel_of(row);
+                    if (gpix < 0 && !staged) continue;
+                    uint16_t* op = reinterpret_cast<uint16_t*>(p.out) + gpix * p.out_pitch + n0 + ccol;
+                    const uint16_t* rp = (p.res && gpix >= 0) ? reinterpret_cast<const uint16_t*>(p.res) + gpix * p.res_pitch + n0 + ccol : nullptr;
+                    uint8_t* sp = stg + (row - wg * 64) * stg_pitch + ccol * 2;
+#pragma unroll
+                    for (int j = 0; j < BLOCK_N / 8; ++j) {
+                        if (n0 + 8 * j >= p.N) continue;  // N % 8 == 0: an 8-column group is all in or all out
+                        const float2 b = *reinterpret_cast<const float2*>(sBias + n0 + 8 * j + ccol);
+                        const float a0 = acc[mi][4 * j + 2 * h], a1 = acc[mi][4 * j + 2 * h + 1];
+                        float f0, f1;
+                        if (p.act) {  // b holds bias / 2 (see the preload)
+                            f0 = silu_from_half(fmaf(a0, 0.5f, b.x));
+                            f1 = silu_from_half(fmaf(a1, 0.5f, b.y));
+                        } else {
+                            f0 = a0 + b.x;
+                            f1 = a1 + b.y;
+                        }
+                        if (rp) {  // may alias the output: read here, written below (direct) or after the warpgroup barrier (staged)
+                            const float2 t = unpack2(*reinterpret_cast<const uint32_t*>(rp + 8 * j), bf16);
+                            f0 += t.x;
+                            f1 += t.y;
+                        }
+                        if (staged) *reinterpret_cast<uint32_t*>(sp + 16 * j) = pack2(f0, f1, bf16);
+                        else *reinterpret_cast<uint32_t*>(op + 8 * j) = pack2(f0, f1, bf16);
+                    }
+                }
+                if (staged) {  // the warpgroup's 64 rows leave as whole 16-byte row segments
+                    named_bar_sync(2 + wg, 128);
+                    constexpr int kSeg = BLOCK_N / 8;
+                    for (int i = threadIdx.x & 127; i < 64 * kSeg; i += 128) {
+                        const int lrow = i / kSeg, c = i - lrow * kSeg;
+                        const long long gpix = pixel_of(wg * 64 + lrow);
+                        if (gpix >= 0 && n0 + 8 * c < p.N)
+                            *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + gpix * p.out_pitch + n0 + 8 * c) =
+                                *reinterpret_cast<const uint4*>(stg + lrow * stg_pitch + c * 16);
+                    }
+                    named_bar_sync(2 + wg, 128);  // the staging block is rewritten by the next sub-tile / tile
+                }
+            }
+        } else {
+            // ---- Detect head (models/yolo.py:95-113): N tile `nt` == anchor.  The accumulators give the raw logits AND the
+            // decoded predictions, written into two smem blocks laid out exactly like their global destinations ([128 pixels][no]
+            // contiguous per anchor), one barrier of the consumer warpgroups, then 16-byte vector copy-out.  Two staging sets
+            // alternate per tile, so the barrier of tile i+1 also fences the reuse of tile i-1's set.
+            const uint32_t blk = (kBlockM * p.no * 2 + 1023) & ~1023u;
+            const int set = head_set;
+            head_set ^= 1;
+            uint16_t* stage_raw = reinterpret_cast<uint16_t*>(smem + L.off_out + (2 * set) * blk);
+            uint16_t* stage_z = reinterpret_cast<uint16_t*>(smem + L.off_out + (2 * set + 1) * blk);
+            const int no = p.no;
+            const int a = nt;
+            const float aw = p.anchor_wh[a * 2], ah = p.anchor_wh[a * 2 + 1];
+            const int m0 = ms * kBlockM;
+            const int rows_here = min(kBlockM, p.M - m0);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = wrow + 8 * h;
                 const int m = m0 + row;
                 int gx = 0, gy = 0;
                 if (m < p.M) { const int pix = m - fdiv(m, p.HoWo, p.rcp_HoWo) * p.HoWo; gy = fdiv(pix, p.nx, p.rcp_Wo); gx = pix - gy * p.nx; }
-                const int rows_here = min(kBlockM, p.M - m0);
-                const int b_lo = fdiv(m0, p.HoWo, p.rcp_HoWo), b_hi = fdiv(m0 + rows_here - 1, p.HoWo, p.rcp_HoWo);
-                mbar_wait(&tmem_full[acc], acc_phase);
-                tc_fence_after();
-                if (slot * 32 < no) {
-                    uint32_t v[32];
-                    tmem_ld_32x32(t_row + slot * 32, v);
-                    tmem_ld_wait();
-                    const float fgx = static_cast<float>(gx) - 0.5f, fgy = static_cast<float>(gy) - 0.5f;
-                    // column chunk as a compile-time constant: the xy / wh special cases exist only in chunk 0's code
-                    switch (slot) {
-                        case 0: head_chunk<0>(v, sBias + n0, no, p.nc, fgx, fgy, p.det_stride, p.anchor_wh[a * 2], p.anchor_wh[a * 2 + 1], bf16,
-                                              stage_raw, stage_z, row); break;
-                        case 1: head_chunk<1>(v, sBias + n0, no, p.nc, fgx, fgy, p.det_stride, 0.f, 0.f, bf16, stage_raw, stage_z, row); break;
-                        case 2: head_chunk<2>(v, sBias + n0, no, p.nc, fgx, fgy, p.det_stride, 0.f, 0.f, bf16, stage_raw, stage_z, row); break;
-                        default: head_chunk<3>(v, sBias + n0, no, p.nc, fgx, fgy, p.det_stride, 0.f, 0.f, bf16, stage_raw, stage_z, row); break;
-                    }
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-                named_bar_sync(1, kEpiThreads);
-                // copy out: for each image the tile touches, rows [r_lo, r_hi) are one contiguous global block per output
-                for (int b = b_lo; b <= b_hi; ++b) {
-                    const int r_lo = max(b * p.HoWo - m0, 0), r_hi = min((b + 1) * p.HoWo - m0, rows_here);
-                    const int pix_lo = m0 + r_lo - b * p.HoWo;
-                    const int n_el = (r_hi - r_lo) * no;
+                const float fgx = static_cast<float>(gx) - 0.5f, fgy = static_cast<float>(gy) - 0.5f;
 #pragma unroll
-                    for (int which = 0; which < 2; ++which) {
-                        const long long dst_el = which == 0
-                            ? ((static_cast<long long>(b) * p.na + a) * p.HoWo + pix_lo) * no
-                            : (static_cast<long long>(b) * p.z_rows + p.z_row0 + static_cast<long long>(a) * p.HoWo + pix_lo) * no;
-                        uint16_t* dst = reinterpret_cast<uint16_t*>(which == 0 ? p.raw : p.z) + dst_el;
-                        const uint16_t* src = (which == 0 ? stage_raw : stage_z) + r_lo * no;
-                        if ((((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src)) & 15) == 0) && (n_el & 7) == 0) {
-                            const uint4* s4 = reinterpret_cast<const uint4*>(src);
-                            uint4* d4 = reinterpret_cast<uint4*>(dst);
-                            for (int i = et; i < n_el / 8; i += kEpiThreads) d4[i] = s4[i];
-                        } else {
-                            for (int i = et; i < n_el; i += kEpiThreads) dst[i] = src[i];
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int o = 8 * j + ccol + e;
+                        if (o >= no) continue;
+                        const float x = acc[0][4 * j + 2 * h + e] + sBias[n0 + o];
+                        float d = x;
+                        if (o < 5 + p.nc) {
+                            const float sg = sigmoid_f(x);
+                            if (o == 0) d = (sg * 2.0f + fgx) * p.det_stride;
+                            else if (o == 1) d = (sg * 2.0f + fgy) * p.det_stride;
+                            else if (o == 2) { const float u = sg * 2.0f; d = u * u * aw; }
+                            else if (o == 3) { const float u = sg * 2.0f; d = u * u * ah; }
+                            else d = sg;
                         }
+                        stage_raw[row * no + o] = pack1(x, bf16);
+                        stage_z[row * no + o] = pack1(d, bf16);
                     }
                 }
             }
-            if (++acc == NACC) { acc = 0; acc_phase ^= 1; }
+            named_bar_sync(1, kConsumerThreads);
+            // copy out: for each image the tile touches, rows [r_lo, r_hi) are one contiguous global block per output
+            const int b_lo = fdiv(m0, p.HoWo, p.rcp_HoWo), b_hi = fdiv(m0 + rows_here - 1, p.HoWo, p.rcp_HoWo);
+            for (int b = b_lo; b <= b_hi; ++b) {
+                const int r_lo = max(b * p.HoWo - m0, 0), r_hi = min((b + 1) * p.HoWo - m0, rows_here);
+                const int pix_lo = m0 + r_lo - b * p.HoWo;
+                const int n_el = (r_hi - r_lo) * no;
+#pragma unroll
+                for (int which = 0; which < 2; ++which) {
+                    const long long dst_el = which == 0
+                        ? ((static_cast<long long>(b) * p.na + a) * p.HoWo + pix_lo) * no
+                        : (static_cast<long long>(b) * p.z_rows + p.z_row0 + static_cast<long long>(a) * p.HoWo + pix_lo) * no;
+                    uint16_t* dst = reinterpret_cast<uint16_t*>(which == 0 ? p.raw : p.z) + dst_el;
+                    const uint16_t* src = (which == 0 ? stage_raw : stage_z) + r_lo * no;
+                    if ((((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src)) & 15) == 0) && (n_el & 7) == 0) {
+                        const uint4* s4 = reinterpret_cast<const uint4*>(src);
+                        uint4* d4 = reinterpret_cast<uint4*>(dst);
+                        for (int i = ct; i < n_el / 8; i += kConsumerThreads) d4[i] = s4[i];
+                    } else {
+                        for (int i = ct; i < n_el; i += kConsumerThreads) dst[i] = src[i];
+                    }
+                }
+            }
         }
     }
-
-    if (EPI == 0 && p.tma_store && warp >= 2 && warp < kMma2Warp && lane == 0) tma_store_wait_all();  // bulk stores issued by this thread are complete
-    tc_fence_before();
-    __syncthreads();
-    if (csize > 1) cluster_sync_all();  // no CTA leaves while a peer may still arrive on its barriers
-    if (warp == 1) {
-        tc_fence_after();
-        if (CG == 2) tmem_dealloc_cg2(tmem_base, kTmemCols);
-        else tmem_dealloc(tmem_base, kTmemCols);
     }
+    if (csize > 1) cluster_sync_all();  // no CTA leaves while a peer may still multicast into it or arrive on its barriers
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1021,67 +530,42 @@ using namespace y5;
 namespace {
 
 int pick_block_k(int in_c) {
-    // 64-channel chunks (128-byte rows) run the specialised single-warp loops (mma_issue_lean / producer_lean); the generic loops
-    // that narrower chunks need cost more than the zero padding of K does (the copy engine zero-fills the channels beyond in_c,
-    // the packed weights carry zeros there).  Only very narrow inputs keep 16-/32-channel chunks.  Y5_BK_RULE=0: the round-1 rule
-    // (fewest padded K elements + a per-chunk cost).
-    // Measured: yolov5m forward 3.49 -> 3.19 ms (its 96-channel layers were on 32-channel chunks), training step 19.5 -> 18.3 ms;
-    // yolov5s forward 1.53 -> 1.46 ms with 64-channel chunks for its 32-channel layers too.
-    static const int rule = [] { const char* e = getenv("Y5_BK_RULE"); return e ? atoi(e) : 2; }();  // 0 round-1 cost rule, 1 = 64 above 32 channels, 2 (default) = 64 above 16
-    if (rule == 1) return in_c > 32 ? 64 : (in_c > 16 ? 32 : 16);
-    if (rule == 2) return in_c > 16 ? 64 : 16;
-    int best = 64;
-    long best_cost = -1;
-    for (int bk : {64, 32, 16}) {
-        const int chunks = (in_c + bk - 1) / bk;
-        const long cost = static_cast<long>(chunks) * (bk + 24);
-        if (best_cost < 0 || cost < best_cost) {
-            best_cost = cost;
-            best = bk;
-        }
+    // 64-channel chunks (128-byte rows, 4 K steps per barrier round) for everything wider than 16 channels: the zero padding of
+    // K (the copy engine zero-fills the channels beyond in_c, the packed weights carry zeros there) costs less than the extra
+    // barrier rounds of narrower chunks.  Only very narrow inputs (the 16-channel stem) keep 16-channel chunks.
+    return in_c > 16 ? 64 : 16;
+}
+
+// Tile shape (block_n, sub-tiles per tile), MT * block_n <= 256 (the accumulators live in the consumer warpgroups' registers).
+// Narrow layers fill the 256 columns with 128-row sub-tiles that share each weight tile (one barrier round feeds MT of them);
+// wider layers take 128 x 256 tiles when the layer has enough of them to keep every SM busy for two waves, else 128 x 128.
+void pick_tile(int out_c, int64_t m_tiles, int* block_n, int* mt) {
+    const int64_t sms = sm_count();
+    if (out_c <= 32) { *block_n = 32; *mt = 4; return; }
+    if (out_c <= 64) { *block_n = 64; *mt = 2; return; }
+    if (out_c <= 128) {
+        *block_n = 128;
+        *mt = ((m_tiles + 1) / 2) >= sms ? 2 : 1;  // 256 x 128 tiles only while they still make a full wave
+        return;
     }
-    return best;
+    const int64_t tiles256 = m_tiles * ((out_c + 255) / 256);
+    *block_n = (tiles256 >= 2 * sms && (out_c % 256 == 0 || out_c > 384)) ? 256 : 128;
+    *mt = 1;
 }
 
 int pick_block_n(int out_c, int64_t m_rows) {
-    if (out_c <= 32) return 32;
-    if (out_c <= 64) return 64;
-    if (out_c <= 128) return 128;
-    const int64_t m_tiles = (m_rows + kBlockM - 1) / kBlockM;
-    const int64_t tiles256 = m_tiles * ((out_c + 255) / 256);
-    if (tiles256 >= 2 * 148 && (out_c % 256 == 0 || out_c > 384)) return 256;
-    return 128;
+    int bn, mt;
+    pick_tile(out_c, m_rows > 0 ? (m_rows + kBlockM - 1) / kBlockM : 1, &bn, &mt);
+    return bn;
 }
 
-// Tile shape (block_n, sub-tiles per tile).  Rules measured on B200 (profiles/r01_tile_sweep.txt): narrow layers
-// always fill 128 TMEM columns (MT = 128 / block_n); for 128 output channels a 256x128 tile (one weight tile feeding two
-// sub-tiles) wins except for 1x1 convs; for >= 256 channels the double-buffered 128x256 tile wins for shifted-patch and
-// most 1x1 convs (its epilogue overlaps the next tile's MMAs), while TMA-im2col (stride-2) and very deep 1x1 convs are
-// faster with the single-buffered 256x256 tile (half the operand bytes per flop).
-void pick_tile(int out_c, int a_mode, int k_total, int64_t m_tiles, int* block_n, int* mt, int* cluster) {
-    *cluster = 1;
-    if (out_c <= 32) { *block_n = 32; *mt = 4; return; }
-    if (out_c <= 64) { *block_n = 64; *mt = 2; return; }
-    const int pad128 = (out_c + 127) / 128 * 128, pad256 = (out_c + 255) / 256 * 256;
-    if (out_c <= 128 || pad128 < pad256) {
-        *block_n = 128;
-        *mt = a_mode == A_LINEAR ? 1 : 2;
-        if (*mt == 2 && ((m_tiles + 1) / 2) * (pad128 / 128) < 120) *mt = 1;  // keep ~a wave of tiles on small maps
-        return;
-    }
-    *block_n = 256;
-    *mt = (a_mode == A_IM2COL || (a_mode == A_LINEAR && k_total >= 2048)) ? 2 : 1;
-    // small feature maps: big tiles would leave most of the 148 SMs without a tile -- shrink until ~one wave exists
-    auto tiles = [&](int bn, int m) { return ((m_tiles + m - 1) / m) * ((out_c + bn - 1) / bn); };
-    if (tiles(*block_n, *mt) < 120 && *mt == 2) *mt = 1;
-    // (going further down to 128-wide tiles was measured slower on yolov5s' 20x20 layers: 1.98 vs 1.83 ms per forward)
-}
-
-template <int BN, int EPI, int MT, int CG = 1>
-cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c, const ConvParams& p, int grid, int cluster, uint32_t smem, cudaStream_t st) {
-    const cudaError_t attr_err = ensure_dyn_smem(reinterpret_cast<const void*>(conv_gemm_kernel<BN, EPI, MT, CG>), 227 * 1024);
+template <int BN, int EPI, int MT, bool OPT>
+cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const ConvParams& p, int grid, int cluster, uint32_t smem,
+                        cudaStream_t st) {
+    const cudaError_t attr_err = ensure_dyn_smem(reinterpret_cast<const void*>(conv_gemm_kernel<BN, EPI, MT, OPT>), 227 * 1024);
     if (attr_err != cudaSuccess) return attr_err;
     count_launch();
+    if (cluster == 1) return launch_pdl(conv_gemm_kernel<BN, EPI, MT, OPT>, dim3(grid), dim3(kThreads), smem, st, a, b, p);
     static const bool pdl = [] { const char* e = getenv("Y5_PDL"); return !(e && e[0] == '0'); }();
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid);
@@ -1089,110 +573,77 @@ cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const CUtens
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (cluster > 1) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = cluster;
-        attr[na].val.clusterDim.y = 1;
-        attr[na].val.clusterDim.z = 1;
-        ++na;
-    }
-    if (pdl) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = cluster;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = na;
-    return cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, EPI, MT, CG>, a, b, c, p);
+    cfg.numAttrs = pdl ? 2 : 1;
+    return cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, EPI, MT, OPT>, a, b, p);
 }
 
 struct PlanCommon {
-    CUtensorMap tmA, tmB, tmC;
+    CUtensorMap tmA, tmB;
     ConvParams p;
     int block_n, epi, mt, grid, cluster;
-    int cg;  // 2 = CTA-pair MMA (cta_group::2): cluster == 2, each CTA stages half of every weight tile
-    int const_weights;  // desc.reserved bit 6: the weights are not written by the kernel that precedes this one in the stream
     uint32_t smem_bytes;
 };
 
 // stage counts from the shared-memory budget; fills p.a_stages/b_stages and pc.smem_bytes/grid.
 // Expects p.a_sub_bytes, p.b_stage_bytes, p.num_m_tiles set.
-int finish_plan(PlanCommon& pc, int block_n, int epi, int mt, int cluster = 1, int cg = 1) {
+int finish_plan(PlanCommon& pc, int block_n, int epi, int mt, int cluster = 1) {
     ConvParams& p = pc.p;
-    pc.cg = cg;
     p.cluster_n = cluster;
     p.a_stage_bytes = mt * p.a_sub_bytes;
     if (p.patch_pw > 0) p.a_stage_bytes = static_cast<uint32_t>(p.th + p.kh - 1) * p.patch_pw * p.block_k * 2;  // one shared patch per stage
     p.num_m_super = (p.num_m_tiles + mt - 1) / mt;
     p.num_n_tiles = epi == 1 ? p.na : (p.N + block_n - 1) / block_n;
     p.bias_n = p.num_n_tiles * block_n;
-    p.idesc = umma_idesc_f16(p.is_bf16 != 0, block_n, cg == 2 ? 256 : 128);
     const uint32_t budget = 225 * 1024 - 1024;
     const bool patch = p.a_mode == A_PATCH;
-    const int lay = epi == 1 ? 1 : (p.tma_store ? 2 : 0);  // shared-memory layout variant (see smem_layout)
-    const int num_kb = p.kh * p.kw * p.c_chunks;
     int a_st = 0, b_st = 0;
-    // tuning knobs (A/B runs): Y5_STAGE_CAP=1 restores the round-1 rule "no more stages than k-blocks + 1";
-    // Y5_B_RESIDENT=1 turns the resident-weights mode on (measured 5-15 % slower on the 1x1 layers of yolov5l: opt-in)
-    static const bool stage_cap = [] { const char* e = getenv("Y5_STAGE_CAP"); return e && e[0] == '1'; }();
-    // With constant weights (desc.reserved bit 6) the resident tile is fetched before the PDL dependency wait, i.e. during the
-    // previous kernel's tail, which removes the start-up serialisation that made mode 1 slower -- measured equal to streaming
-    // (profiles/r02_tile_store_sweep.md), so it stays opt-in: Y5_B_RESIDENT=1.
-    static const int resident_env = [] { const char* e = getenv("Y5_B_RESIDENT"); return e ? atoi(e) : 0; }();
-    const bool allow_resident = resident_env == 1;
-    p.b_resident = 0;
-    if (!patch && allow_resident && cluster == 1 && p.num_n_tiles == 1 && num_kb <= kMaxStages &&
-        static_cast<uint32_t>(num_kb) * p.b_stage_bytes <= 132u * 1024u) {
-        // one N tile: every tile of the CTA multiplies by the same weights -> keep all of its k-blocks in shared memory (loaded
-        // once) and give the rest of the budget to the activation ring.  Cuts the L2 -> smem traffic of small-K layers by the
-        // weight share (half of it for a 128x128x128 1x1 conv) and deepens the activation prefetch.
+    if (!patch) {
         for (int s = kMaxStages; s >= 2; --s)
-            if (smem_layout(lay, p.no, p.bias_n, s, num_kb, p.a_stage_bytes, p.b_stage_bytes).total <= budget) { a_st = s; break; }
-        if (a_st >= 2) { b_st = num_kb < 2 ? 2 : num_kb; p.b_resident = pc.const_weights ? 2 : 1; }
-    }
-    if (p.b_resident) {
-    } else if (!patch) {
-        for (int s = kMaxStages; s >= 2; --s)
-            if (smem_layout(lay, p.no, p.bias_n, s, s, p.a_stage_bytes, p.b_stage_bytes).total <= budget) { a_st = b_st = s; break; }
-        if (stage_cap && a_st > num_kb + 1) a_st = b_st = (num_kb + 1 < 2 ? 2 : num_kb + 1);
+            if (smem_layout(epi, p.no, p.bias_n, s, s, p.a_stage_bytes, p.b_stage_bytes, p.stg_bytes).total <= budget) { a_st = b_st = s; break; }
     } else {
         const int b_min = p.b_grouped ? 2 : 3, b_max = p.b_grouped ? 4 : kMaxStages;  // a grouped stage holds kh tiles
         for (int a = 3; a >= 2 && !a_st; --a)
             for (int b = b_max; b >= b_min; --b)
-                if (smem_layout(lay, p.no, p.bias_n, a, b, p.a_stage_bytes, p.b_stage_bytes).total <= budget) { a_st = a; b_st = b; break; }
+                if (smem_layout(epi, p.no, p.bias_n, a, b, p.a_stage_bytes, p.b_stage_bytes, p.stg_bytes).total <= budget) { a_st = a; b_st = b; break; }
     }
     if (a_st < 2 || b_st < 2) return set_error(Y5_E_UNSUPPORTED, "conv tile does not fit shared memory (block_n %d a %u b %u)", block_n,
                                                 p.a_stage_bytes, p.b_stage_bytes);
     p.a_stages = a_st;
     p.b_stages = b_st;
-    pc.smem_bytes = smem_layout(lay, p.no, p.bias_n, a_st, b_st, p.a_stage_bytes, p.b_stage_bytes).total + 1024;
+    pc.smem_bytes = smem_layout(epi, p.no, p.bias_n, a_st, b_st, p.a_stage_bytes, p.b_stage_bytes, p.stg_bytes).total + 1024;
     pc.block_n = block_n;
     pc.epi = epi;
     pc.mt = mt;
     pc.cluster = cluster;
     const long long tiles = static_cast<long long>((p.num_m_super + cluster - 1) / cluster) * p.num_n_tiles;  // per cluster
-    const int max_clusters = sm_count() / cluster;  // 1 CTA per SM (shared memory); pairs pack perfectly on 148 SMs
+    const int max_clusters = sm_count() / cluster;  // 1 CTA per SM (shared memory), persistent
     pc.grid = static_cast<int>(tiles < max_clusters ? tiles : max_clusters) * cluster;
     return 0;
 }
 
 int run_plan(const PlanCommon& pc, cudaStream_t st) {
     cudaError_t e = cudaErrorInvalidValue;
-    const int key = (pc.cg == 2 ? 100000 : 0) + pc.epi * 10000 + pc.block_n * 10 + pc.mt;
+    const bool opt = pc.cluster > 1 || pc.p.patch_pw > 0 || pc.p.stg_bytes > 0;
+    const int key = (opt ? 100000 : 0) + pc.epi * 10000 + pc.block_n * 10 + pc.mt;
     switch (key) {
-        case 100642: e = launch_conv<64, 0, 2, 2>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, 2, pc.smem_bytes, st); break;
-        case 101281: e = launch_conv<128, 0, 1, 2>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, 2, pc.smem_bytes, st); break;
-        case 101282: e = launch_conv<128, 0, 2, 2>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, 2, pc.smem_bytes, st); break;
-        case 102561: e = launch_conv<256, 0, 1, 2>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, 2, pc.smem_bytes, st); break;
-        case 102562: e = launch_conv<256, 0, 2, 2>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, 2, pc.smem_bytes, st); break;
-        case 324: e = launch_conv<32, 0, 4>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 642: e = launch_conv<64, 0, 2>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 1281: e = launch_conv<128, 0, 1>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 1282: e = launch_conv<128, 0, 2>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 2561: e = launch_conv<256, 0, 1>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 2562: e = launch_conv<256, 0, 2>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 11281: e = launch_conv<kHeadN, 1, 1>(pc.tmA, pc.tmB, pc.tmC, pc.p, pc.grid, 1, pc.smem_bytes, st); break;
+        case 324: e = launch_conv<32, 0, 4, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 642: e = launch_conv<64, 0, 2, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 1281: e = launch_conv<128, 0, 1, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 1282: e = launch_conv<128, 0, 2, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 2561: e = launch_conv<256, 0, 1, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 11281: e = launch_conv<kHeadN, 1, 1, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 100324: e = launch_conv<32, 0, 4, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 100642: e = launch_conv<64, 0, 2, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 101281: e = launch_conv<128, 0, 1, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 101282: e = launch_conv<128, 0, 2, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 102561: e = launch_conv<256, 0, 1, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
         default: return set_error(Y5_E_UNSUPPORTED, "conv: no kernel for block_n %d mt %d epi %d", pc.block_n, pc.mt, pc.epi);
     }
     if (e != cudaSuccess) return set_error(int(e), "conv_gemm launch failed: %s", cudaGetErrorString(e));
@@ -1282,85 +733,23 @@ extern "C" Y5_API int y5_conv_plan_create(const y5_conv_desc* d, y5_conv_plan** 
     else if (d->a_mode == 2 || (d->a_mode == 0 && d->stride == 1 && best_eff >= 0.75)) a_mode_sel = A_PATCH;
     else a_mode_sel = A_IM2COL;
 
-    int bn = d->block_n, mt_sel = 0, cl_sel = 1, cg_sel = 1;
+    int bn = d->block_n, mt_sel = 0, cl_sel = 1;
     {
         int bn_auto = 0;
-        pick_tile(d->out_c, a_mode_sel, g.kh * g.kw * d->in_c, (M64 + kBlockM - 1) / kBlockM, &bn_auto, &mt_sel, &cl_sel);
+        pick_tile(d->out_c, (M64 + kBlockM - 1) / kBlockM, &bn_auto, &mt_sel);
         if (!bn) bn = bn_auto;
-        else {  // forced block_n (tests / tuning): reserved bit 1 asks for MT = 2, bits 8.. give the cluster size
-            mt_sel = bn < 128 ? 128 / bn : ((d->reserved & 2) ? 2 : 1);
+        else {  // forced block_n (tests / tuning): narrow tiles fill 128 columns, reserved bit 1 asks for 256 x 128 tiles,
+                // bit 2 for CTA pairs (a 2-CTA cluster sharing every weight tile), bits 8.. for the cluster size (2 | 4)
+            mt_sel = bn < 128 ? 128 / bn : ((d->reserved & 2) && bn == 128 ? 2 : 1);
             cl_sel = (d->reserved >> 8) > 1 ? (d->reserved >> 8) : 1;
-            if ((d->reserved & 4) && bn >= 64) { cg_sel = 2; cl_sel = 2; }  // CTA-pair MMA (64-wide tiles: two sub-tiles per CTA)
-        }
-        if (const char* e = getenv("Y5_CLUSTER")) cl_sel = atoi(e) > 1 && bn >= 128 ? atoi(e) : 1;
-        if (const char* e = getenv("Y5_BIG_TILE")) {  // tuning: "<block_n>x<mt>" for layers with out_c >= 256, e.g. 256x1
-            int tb = 0, tm = 0;
-            if (!d->block_n && d->out_c >= 256 && sscanf(e, "%dx%d", &tb, &tm) == 2 && (tb == 128 || tb == 256) && (tm == 1 || tm == 2)) {
-                bn = tb;
-                mt_sel = tm;
-            }
-        }
-        if (const char* e = getenv("Y5_MID_TILE")) {  // same for 64 < out_c < 256: "128x1" | "128x2"
-            int tb = 0, tm = 0;
-            if (!d->block_n && d->out_c > 64 && d->out_c < 256 && sscanf(e, "%dx%d", &tb, &tm) == 2 && tb == 128 && (tm == 1 || tm == 2)) {
-                bn = tb;
-                mt_sel = tm;
-            }
-        }
-        if (cl_sel != 1 && cl_sel != 2 && cl_sel != 4) cl_sel = 1;
-        // CTA-pair (cta_group::2) selection.  Measured on B200 (yolov5l, 64 x 640 x 640 bf16, profiles/r02_tile_store_sweep.md): pairs
-        // win wherever the weight tile is the larger smem operand -- every 3x3 layer with >= 128 output channels (-10..-22 %) and
-        // 1x1 layers with K >= 512 and >= 256 output channels (-3..-8 %); shallow 1x1 layers are store / latency bound and lose
-        // (+20..+70 %), they keep cta_group::1.  Y5_CG2: 0 = never, 1 = every layer with >= 256 channels, 2 = 1 + 128-channel
-        // layers, unset / 3 = the measured rule.  A pair needs >= ~60 pair-tiles to fill the 74 SM pairs.
-        static const int cg2_mode = [] { const char* e = getenv("Y5_CG2"); return e ? atoi(e) : 3; }();
-        if (!d->block_n && cg2_mode > 0 && cg_sel == 1 && d->out_c % 128 == 0) {
-            const long long m_tiles = (M64 + kBlockM - 1) / kBlockM;
-            const bool linear = a_mode_sel == A_LINEAR;
-            const long long k_total = static_cast<long long>(g.kh) * g.kw * d->in_c;
-            bool want;
-            if (cg2_mode == 1) want = d->out_c >= 256;
-            else if (cg2_mode == 2) want = true;
-            else want = linear ? (k_total >= 512 && d->out_c >= 256) : true;
-            if (want && d->out_c >= 256) {
-                const int bn2 = d->out_c % 256 == 0 ? 256 : 128;
-                const long long pair_tiles = ((m_tiles + 1) / 2) * (d->out_c / bn2);
-                if (pair_tiles >= 60) { bn = bn2; mt_sel = 1; cg_sel = 2; cl_sel = 2; }
-                // 512 x 256 pair tiles (two sub-tiles per CTA, all 512 TMEM columns, single-buffered accumulators): half the weight
-                // bytes per flop again.  They paid (-6..-19 % on the stride-2 layers) while the generic single-warp loops bounded the
-                // kernel; with the specialised loops the double-buffered 256 x 256 tiles win everywhere (model.3 199 -> 160 us,
-                // model.5 179 -> 148 us): off by default.  Y5_CG2_MT2=2 restores the stride-2 rule, 1 = every non-1x1 layer.
-                static const int mt2_pairs = [] { const char* e = getenv("Y5_CG2_MT2"); return e ? atoi(e) : 0; }();
-                const long long tiles_mt2 = ((m_tiles + 3) / 4) * (d->out_c / 256);
-                if (mt2_pairs && cg_sel == 2 && bn == 256 && !linear &&
-                    (mt2_pairs == 1 ? tiles_mt2 >= 60 : (a_mode_sel == A_IM2COL && d->stride >= 2 && tiles_mt2 >= 150)))
-                    mt_sel = 2;
-            } else if (want && d->out_c == 128) {
-                const int mt2 = linear ? 1 : 2;
-                const long long pair_tiles = (m_tiles + 2 * mt2 - 1) / (2 * mt2);
-                if (pair_tiles >= 60) { bn = 128; mt_sel = mt2; cg_sel = 2; cl_sel = 2; }
-            }
-        }
-        // 64 output channels, k > 1: these layers are bound by the MMA ISSUE rate (one elected thread issues ~1 tcgen05.mma per
-        // ~130 clocks whatever its size; a 128x64x16 MMA is 32 clocks of tensor work) -> pairs double the work per issued
-        // instruction (256x64x16).  Y5_CG2_N64=0 disables.
-        static const bool cg2_n64 = [] { const char* e = getenv("Y5_CG2_N64"); return !(e && e[0] == '0'); }();
-        if (!d->block_n && cg2_mode > 0 && cg2_n64 && cg_sel == 1 && d->out_c == 64 && a_mode_sel != A_LINEAR) {
-            const long long m_tiles = (M64 + kBlockM - 1) / kBlockM;
-            if ((m_tiles + 3) / 4 >= 60) { bn = 64; mt_sel = 2; cg_sel = 2; cl_sel = 2; }
+            if (d->reserved & 4) cl_sel = 2;
+            if (cl_sel != 1 && cl_sel != 2 && cl_sel != 4) return set_error(Y5_E_INVALID, "conv: cluster size must be 1, 2 or 4");
         }
     }
-    // 256-wide tiles: the TMA-im2col path shares one barrier pair between the activation and the weight tile of a K block, the
-    // patch path keeps two rings; with the single-warp instruction streams as the bound that is worth more than the patch mode's
-    // smaller L2 traffic (measured: 99 -> 87 us on yolov5l's 256-channel 3x3 layers).  Narrower tiles keep the patch mode: their kh
-    // weight tiles travel in one grouped stage.  Y5_PATCH_256=1 restores the patch mode for them.
-    static const bool patch_256 = [] { const char* e = getenv("Y5_PATCH_256"); return e && e[0] == '1'; }();
-    if (a_mode_sel == A_PATCH && d->a_mode == 0 && bn == 256 && !patch_256) a_mode_sel = A_IM2COL;
     if (bn != 32 && bn != 64 && bn != 128 && bn != 256) return set_error(Y5_E_INVALID, "conv: block_n must be 32/64/128/256");
     auto* plan = new y5_conv_plan();
     PlanCommon& pc = plan->pc;
     std::memset(&pc.p, 0, sizeof(pc.p));
-    pc.const_weights = (d->reserved & 64) ? 1 : 0;
     ConvParams& p = pc.p;
     p.M = static_cast<int>(M64);
     p.N = d->out_c;
@@ -1380,7 +769,7 @@ extern "C" Y5_API int y5_conv_plan_create(const y5_conv_desc* d, y5_conv_plan** 
     p.block_k = bk;
     p.c_chunks = (d->in_c + bk - 1) / bk;
     const int row_bytes = bk * 2;
-    p.b_sub_bytes = bn / cg_sel * row_bytes;  // pair mode: each CTA stages half of the weight tile's rows
+    p.b_sub_bytes = bn * row_bytes;
     p.b_stage_bytes = p.b_sub_bytes;
     p.a_mode = a_mode_sel;
 
@@ -1402,14 +791,12 @@ extern "C" Y5_API int y5_conv_plan_create(const y5_conv_desc* d, y5_conv_plan** 
         p.tw = best_tw;
         p.th = 128 / best_tw;
         // wide patch mode (see the header): 128-byte rows, horizontal taps, and an 8-pixel-wide tiling that wastes no more than the
-        // chosen one; with MT = 2 the two sub-tiles must be neighbours in x (even number of 8-pixel tiles per row).
-        // Y5_PATCH_WIDE=1 / reserved bit 7 (128) enable it; reserved bit 5 (32) wins and disables it.
-        static const bool wide_env = [] { const char* e = getenv("Y5_PATCH_WIDE"); return e && e[0] == '1'; }();
-        const bool wide_ok = wide_env || (d->reserved & 128);  // measured 0..-9 % (slower) on yolov5l: opt-in (tests force it with bit 7)
+        // chosen one; with MT = 2 the two sub-tiles must be neighbours in x (even number of 8-pixel tiles per row).  Opt-in (reserved
+        // bit 7, 128); bit 5 (32) wins and keeps one patch copy per horizontal tap.
         {
             const int tx8 = (g.Wo + 7) / 8, ty16 = (g.Ho + 15) / 16;
             const double eff8 = (double)g.Wo * g.Ho / ((double)tx8 * 8 * ty16 * 16);
-            if (wide_ok && !(d->reserved & 32) && row_bytes == 128 && g.kw > 1 && g.kw <= 7 && (mt_sel == 1 || (mt_sel == 2 && tx8 % 2 == 0)) &&
+            if ((d->reserved & 128) && !(d->reserved & 32) && row_bytes == 128 && g.kw > 1 && (mt_sel == 1 || (mt_sel == 2 && tx8 % 2 == 0)) &&
                 eff8 >= best_eff - 1e-9) {
                 p.tw = 8;
                 p.th = 16;
@@ -1417,11 +804,8 @@ extern "C" Y5_API int y5_conv_plan_create(const y5_conv_desc* d, y5_conv_plan** 
             }
         }
         // grouped weight stages: the kh tiles of a (chunk, horizontal tap) group travel in ONE stage -- one full/empty barrier round
-        // and one commit per group instead of per tile.  The MMA-issuing warp is the bottleneck of the narrow layers (ncu: it never
-        // waits on a barrier, ~120 instructions per 8 MMAs at ~9 clocks each), so fewer round trips per MMA is what pays.
-        // Y5_B_GROUP: 0 off, 1 (default) tiles up to 128 channels wide, 2 every patch-mode layer.
-        static const int group_mode = [] { const char* e = getenv("Y5_B_GROUP"); return e ? atoi(e) : 1; }();
-        if (!p.patch_pw && g.kh > 1 && cl_sel == cg_sel && (group_mode == 2 || (group_mode == 1 && bn <= 128))) {
+        // per group instead of per tile; 256-wide weight tiles are too large to group kh of them.
+        if (!p.patch_pw && g.kh > 1 && bn <= 128) {
             p.b_grouped = 1;
             p.b_stage_bytes = g.kh * p.b_sub_bytes;
         }
@@ -1441,40 +825,18 @@ extern "C" Y5_API int y5_conv_plan_create(const y5_conv_desc* d, y5_conv_plan** 
     {
         cuuint64_t dims[2] = {ktot, (cuuint64_t)d->out_c};
         cuuint64_t str[1] = {ktot * 2};
-        cuuint32_t box[2] = {(cuuint32_t)bk, (cuuint32_t)(bn / cl_sel)};
+        cuuint32_t box[2] = {(cuuint32_t)bk, (cuuint32_t)(bn / cl_sel)};  // cluster: each CTA fetches its slice of the rows
         e = encode_tiled(&pc.tmB, d->dtype, d->weight, 2, dims, str, box, sw, "B");
     }
     if (e) { delete plan; return e; }
-    // epilogue store mode.  TMA store (per-warp staging + cp.async.bulk.tensor): a warp's 32 rows x 64 bytes leave as whole row
-    // segments instead of 4 x 32 row-strided 16-byte stores (128 L1 wavefronts per chunk), which is what bounds the memory-bound
-    // layers; costs 32 KB of the pipeline's shared memory.  Y5_TMA_STORE = 0 off, 1 on (default), reserved bit 4 (16) forces it off in tests.
-    static const int tma_store_mode = [] { const char* e = getenv("Y5_TMA_STORE"); return e ? atoi(e) : 1; }();
-    p.tma_store = (tma_store_mode != 0 && !(d->reserved & 16)) ? 1 : 0;
-    // single-CTA TMA-im2col layers with 256-wide tiles are stage-starved (256x256 tiles fill the shared memory): the 32 KB of
-    // staging cost them 5-25 %; Y5_TMA_STORE=2 forces the staged store everywhere
-    if (tma_store_mode == 1 && cg_sel == 1 && p.a_mode == A_IM2COL && bn == 256) p.tma_store = 0;
-    if (p.tma_store) {
-        int ce;
-        if (p.a_mode == A_PATCH) {
-            p.c_bw = p.tw < 32 ? p.tw : 32;
-            p.c_bh = 32 / p.c_bw;
-            cuuint64_t dims[4] = {(cuuint64_t)d->out_c, (cuuint64_t)g.Wo, (cuuint64_t)g.Ho, (cuuint64_t)d->batch};
-            cuuint64_t str[3] = {(cuuint64_t)d->out_pitch * 2, (cuuint64_t)g.Wo * d->out_pitch * 2, (cuuint64_t)g.Ho * g.Wo * d->out_pitch * 2};
-            cuuint32_t box[4] = {32, (cuuint32_t)p.c_bw, (cuuint32_t)p.c_bh, 1};
-            ce = encode_tiled(&pc.tmC, d->dtype, d->out, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B, "C patch");
-        } else {
-            cuuint64_t dims[2] = {(cuuint64_t)d->out_c, (cuuint64_t)p.M};
-            cuuint64_t str[1] = {(cuuint64_t)d->out_pitch * 2};
-            cuuint32_t box[2] = {32, 32};
-            ce = encode_tiled(&pc.tmC, d->dtype, d->out, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B, "C");
-        }
-        if (ce) p.tma_store = 0;  // a view the copy engine cannot describe: the direct-store epilogue handles everything
-    }
-    if (!p.tma_store) pc.tmC = pc.tmA;  // unused, but must be a valid descriptor for the launch
-    int e2 = finish_plan(pc, bn, 0, mt_sel, cl_sel, cg_sel);
-    if (e2 && p.tma_store) {  // no room for the staging tiles next to the pipeline stages: direct stores
-        p.tma_store = 0;
-        e2 = finish_plan(pc, bn, 0, mt_sel, cl_sel, cg_sel);
+    // epilogue stores: direct from the registers unless reserved bit 3 (8) asks for staged 16-byte row segments (bit 4, 16, forces
+    // direct).  Direct is the default: staging takes up to 66 KB (256-wide tiles) from the pipeline stages and has not been measured
+    // faster.  Staging falls back to direct when the blocks do not fit next to the pipeline stages.
+    p.stg_bytes = ((d->reserved & 8) && !(d->reserved & 16)) ? static_cast<uint32_t>(kConsumers * 64 * (bn * 2 + 16)) : 0u;
+    int e2 = finish_plan(pc, bn, 0, mt_sel, cl_sel);
+    if (e2 && p.stg_bytes) {
+        p.stg_bytes = 0;
+        e2 = finish_plan(pc, bn, 0, mt_sel, cl_sel);
     }
     if (e2) { delete plan; return e2; }
     *out = plan;
@@ -1563,7 +925,6 @@ extern "C" Y5_API int y5_detect_plan_create(const y5_detect_desc* d, y5_detect_p
     cuuint32_t bbox[2] = {(cuuint32_t)bk, (cuuint32_t)kHeadN};
     e = encode_tiled(&pc.tmB, d->dtype, d->weight, 2, bdims, bstr, bbox, sw, "head B");
     if (e) { delete plan; return e; }
-    pc.tmC = pc.tmA;  // the head stages its outputs itself
     if (int e2 = finish_plan(pc, kHeadN, 1, 1)) { delete plan; return e2; }
     *out = plan;
     return 0;

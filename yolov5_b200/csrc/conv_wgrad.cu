@@ -1,21 +1,21 @@
-// Weight gradient of a convolution for sm_100a:
+// Weight gradient of a convolution for sm_90a:
 //     dW[co][r][s][ci] = sum over output pixels m of  dY[m][co] * X[pixel(m) shifted by tap (r,s)][ci]
 // i.e. per filter tap a GEMM  dW_tap[Cout, Cin] = dY[M, Cout]^T * X_tap[M, Cin]  whose reduction dimension is the pixel
-// index -- the dimension that is OUTERMOST in the NHWC activations.  Both operands are therefore fed to tcgen05.mma as
-// MN-major shared-memory tiles: a TMA box of [64 pixels][64 channels] (128-byte rows, 128-byte swizzle) is exactly the
-// canonical MN-major SW128 layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units -- each pixel is one 128-byte line
-// of 64 channels, 8 pixels form a 1024-byte swizzle atom (SBO), further 64-channel blocks sit LBO bytes apart.  So
-// neither dY nor X is ever transposed in memory; the tensor core does it on the fly.
-//   A (dY)   : 1-2 boxes [P px][64 co] per stage -> UMMA M = 128 output channels (the upper box is not fetched when the
-//              layer has <= 64 of them left: its accumulator rows are never read)
-//   B (X_tap): n boxes [P px][64 ci] per stage per tap -> UMMA N = 64*n input channels (n <= 4); hardware im2col for
-//              k > 1 or strided convs (same tensor map type as the forward kernel), plain 2-D tiles for 1x1/s1
+// index -- the dimension that is OUTERMOST in the NHWC activations.  Both operands are therefore fed to wgmma as
+// MN-major shared-memory tiles (transpose flags set): a TMA box of [P pixels][64 channels] (128-byte rows, 128-byte
+// swizzle) is exactly the canonical MN-major SW128 layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units -- each pixel is
+// one 128-byte line of 64 channels, 8 pixels form a 1024-byte swizzle atom (SBO).  So neither dY nor X is ever transposed
+// in memory; the tensor core does it on the fly.
+//   A (dY)   : 1-2 boxes [P px][64 co] per stage -> 128 output channels per CTA, one 64-channel box per consumer warpgroup
+//              (the upper box is not fetched, and its warpgroup idles, when the layer has <= 64 of them left)
+//   B (X_tap): n boxes [P px][64 ci] per stage per tap (n <= 4); hardware im2col for k > 1 or strided convs (same tensor
+//              map type as the forward kernel), plain 2-D tiles for 1x1/s1
 // One CTA = one (co tile, tap group, ci tile, pixel range) work item.  A tap group is up to G filter taps whose
-// accumulators sit side by side in TMEM (G * 64n <= 512 columns): the dY tile of a pixel block is fetched once and
-// multiplied with the G shifted X tiles, which divides the dY traffic of 3x3 layers by G.  P (64/128/256 pixels per
-// pipeline stage) grows when channels are few so that a stage stays ~32-64 KB and the per-stage barrier / TMA issue
-// costs are amortised.  The [128 x 64n] fp32 tiles are added to the fp32 gradient with vector reductions
-// (red.global.add.v4.f32); the pixel range is split so the grid is about one CTA per SM (one wave).
+// accumulators sit side by side in registers (G * n <= 4 blocks of m64 x n64 = 128 fp32 registers per thread): the dY tile
+// of a pixel block is fetched once and multiplied with the G shifted X tiles, which divides the dY traffic of 3x3 layers
+// by G.  P (64/128/256 pixels per pipeline stage) grows when channels are few so that a stage stays ~32-56 KB and the
+// per-stage barrier / TMA issue costs are amortised.  The fp32 tiles are added to the fp32 gradient with vector
+// reductions (red.global.add.v2.f32); the pixel range is split so the grid is about one CTA per SM (one wave).
 // Summation order across pixel ranges is not fixed (fp32 atomics), like cuDNN's default wgrad.
 //
 // Gradient of reference models/common.py:86-88 (Conv.forward, the nn.Conv2d weight) / models/yolo.py:97 (Detect.m[i]).
@@ -26,11 +26,13 @@
 #include "../../include/y5b200.h"
 #include "common.cuh"
 #include "host_util.h"
+#include "wgmma.cuh"
 
 namespace y5 {
 
-constexpr int kWgThreads = 64 + 128;  // warp 0 TMA producer, warp 1 MMA issuer + TMEM owner, warps 2..5 epilogue
-constexpr int kWgCo = 128;            // output channels per tile (UMMA M)
+constexpr int kWgThreads = 128 + 256;  // warpgroup 0: TMA producer (warp 0), warpgroups 1-2: MMA + reductions, 64 co each
+constexpr int kWgCo = 128;            // output channels per tile
+constexpr int kWgSlots = 4;           // accumulator blocks (tap, 64-channel ci block) per thread: 4 x 32 fp32 registers
 constexpr int kWgStagesMax = 6;
 
 struct WgradParams {
@@ -44,9 +46,24 @@ struct WgradParams {
     int kblocks, splits, kb_per_split;
     int stages;
     uint32_t box_bytes, stage_bytes;
-    uint32_t idesc, tmem_cols;
+    int is_bf16;
     float* dw;
 };
+
+template <bool BF16>
+__device__ __forceinline__ void wgrad_mma(float (&acc)[kWgSlots][32], int nslots, int n_blocks, uint32_t a16, uint32_t b16, uint32_t box16,
+                                          uint32_t lbo, uint32_t dhi, int ksteps, uint32_t first) {
+#pragma unroll
+    for (int t = 0; t < kWgSlots; ++t) {
+        if (t < nslots) {
+            const int g = t / n_blocks, j = t - g * n_blocks;
+            const uint32_t bt16 = b16 + (g * n_blocks + j) * box16;
+            for (int k = 0; k < ksteps; ++k)  // 16 pixels = two 8-pixel swizzle atoms = +2048 bytes
+                Wgmma<64>::run<BF16, 1, 1>(acc[t], gmma_desc((a16 + k * 128) | lbo, dhi), gmma_desc((bt16 + k * 128) | lbo, dhi),
+                                           (first == 0 || k != 0) ? 1u : 0u);
+        }
+    }
+}
 
 __global__ void __launch_bounds__(kWgThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX, const WgradParams p) {
@@ -55,29 +72,9 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     uint8_t* ring = smem;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.stages * p.stage_bytes);
     uint64_t* empty = full + kWgStagesMax;
-    uint64_t* acc_full = empty + kWgStagesMax;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(acc_full + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmDy);
-        tma_prefetch_desc(&tmX);
-        for (int s = 0; s < kWgStagesMax; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
-        }
-        mbar_init(acc_full, 1);
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc(tmem_ptr_smem, p.tmem_cols);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    griddep_wait();  // PDL: barrier init / TMEM allocation above overlap the predecessor's tail
-    griddep_launch_dependents();
 
     // work item
     int t = blockIdx.x;
@@ -99,7 +96,22 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     // stage layout: [A box 0][A box 1][tap 0: n boxes][tap 1: n boxes]...
     const uint32_t tx_bytes = (a_boxes + ntaps * p.n_blocks) * p.box_bytes;
 
-    if (warp == 0) {
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmDy);
+        tma_prefetch_desc(&tmX);
+        for (int s = 0; s < kWgStagesMax; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], a_boxes);  // one arrival per working consumer warpgroup
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    griddep_wait();  // PDL: barrier init above overlaps the predecessor's tail
+    griddep_launch_dependents();
+
+    if (warp < 4) {
+        setmaxnreg_dec<40>();
+        if (warp != 0) return;
         // ===================================== TMA producer =====================================
         int st = 0;
         uint32_t ph = 0;
@@ -134,76 +146,66 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
             __syncwarp();
             if (++st == p.stages) { st = 0; ph ^= 1; }
         }
-    } else if (warp == 1) {
-        // ===================================== MMA issuer =====================================
-        int st = 0;
-        uint32_t ph = 0;
-        // MN-major SW128 descriptors: SBO = 1024 B between 8-pixel groups, LBO = one [P px][64 ch] box between
-        // 64-channel blocks; stepping 16 pixels along K = +2048 B on the start address
-        const uint32_t dhi = ((1024u >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);
-        const uint32_t lbo = ((p.box_bytes >> 4) & 0x3FFFu) << 16;
-        const uint32_t ring16 = (smem_u32(ring) >> 4) & 0x3FFFu;
-        const uint32_t box16 = p.box_bytes >> 4;
-        const int ksteps = p.pix / 16;
-        uint32_t accum = 0;
-        for (int i = 0; i < nkb; ++i) {
-            mbar_wait(&full[st], ph);
-            tc_fence_after();
-            const uint32_t a16 = ring16 + ((st * p.stage_bytes) >> 4);
-            if (elect_one()) {
-                for (int g = 0; g < ntaps; ++g) {
-                    const uint32_t b16 = a16 + (2 + g * p.n_blocks) * box16;
-                    const uint32_t d = tmem_base + g * bn;
-                    for (int k = 0; k < ksteps; ++k)
-                        umma_f16_ss_lohi(d, (a16 + k * 128) | lbo, (b16 + k * 128) | lbo, dhi, p.idesc, (accum | k) != 0 ? 1u : 0u);
-                }
-                umma_commit(&empty[st]);
-                if (i == nkb - 1) umma_commit(acc_full);
-            }
-            __syncwarp();
-            accum = 1;
-            if (++st == p.stages) { st = 0; ph ^= 1; }
-        }
-    } else if (nkb > 0) {
-        // ===================================== epilogue: TMEM -> fp32 reductions =====================================
-        const int q = warp & 3;  // TMEM lane quarter this warp may access
-        mbar_wait(acc_full, 0);
-        tc_fence_after();
-        const int co = co0 + q * 32 + lane;
-        const bool row_ok = co < p.Cout;
-        const bool vec_ok = (p.Cin & 3) == 0;
-        for (int g = 0; g < ntaps; ++g) {
-            float* row = p.dw + (static_cast<size_t>(row_ok ? co : 0) * p.taps + tap0 + g) * p.Cin;
-            for (int c = 0; c < p.n_blocks * 2; ++c) {
-                const int cbase = ci0 + c * 32;
-                if (cbase >= p.Cin) break;  // warp-uniform
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + g * bn + c * 32, v);
-                tmem_ld_wait();
-                if (row_ok) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int ci = cbase + 4 * j;
-                        if (vec_ok && ci + 3 < p.Cin) {
-                            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(row + ci), "f"(__uint_as_float(v[4 * j])),
-                                         "f"(__uint_as_float(v[4 * j + 1])), "f"(__uint_as_float(v[4 * j + 2])),
-                                         "f"(__uint_as_float(v[4 * j + 3]))
-                                         : "memory");
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 4; ++e)
-                                if (ci + e < p.Cin) atomicAdd(row + ci + e, __uint_as_float(v[4 * j + e]));
-                        }
-                    }
-                }
-            }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, p.tmem_cols);
+
+    // ===================================== MMA + fp32 reductions =====================================
+    setmaxnreg_inc<232>();
+    const int wg = (warp >> 2) - 1;  // output channels [co0 + 64 wg, co0 + 64 wg + 64): dY box wg
+    if (wg >= a_boxes || nkb <= 0) return;
+    // MN-major SW128 descriptors: SBO = 1024 B between 8-pixel groups, LBO = one [P px][64 ch] box between 64-channel blocks
+    const uint32_t dhi = ((1024u >> 4) & 0x3FFFu) | (1u << 30);
+    const uint32_t lbo = ((p.box_bytes >> 4) & 0x3FFFu) << 16;
+    const uint32_t ring16 = (smem_u32(ring) >> 4) & 0x3FFFu;
+    const uint32_t box16 = p.box_bytes >> 4;
+    const int ksteps = p.pix / 16;
+    const int nslots = ntaps * p.n_blocks;
+    const bool signal = (threadIdx.x & 127) == 0;
+    float acc[kWgSlots][32];
+#pragma unroll
+    for (int s = 0; s < kWgSlots; ++s)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[s][i] = 0.0f;
+    int st = 0;
+    uint32_t ph = 0;
+    for (int i = 0; i < nkb; ++i) {
+        mbar_wait(&full[st], ph);
+        const uint32_t a16 = ring16 + ((st * p.stage_bytes) >> 4);
+#pragma unroll
+        for (int s = 0; s < kWgSlots; ++s) fence_regs(acc[s]);
+        wgmma_fence();
+        if (p.is_bf16) wgrad_mma<true>(acc, nslots, p.n_blocks, a16 + wg * box16, a16 + 2 * box16, box16, lbo, dhi, ksteps, i == 0);
+        else wgrad_mma<false>(acc, nslots, p.n_blocks, a16 + wg * box16, a16 + 2 * box16, box16, lbo, dhi, ksteps, i == 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int s = 0; s < kWgSlots; ++s) fence_regs(acc[s]);
+        if (signal) mbar_arrive(&empty[st]);
+        if (++st == p.stages) { st = 0; ph ^= 1; }
+    }
+    // accumulator fragment: rows (co) 16*warp + lane/4 + 8h, columns (ci) 8q + 2*(lane%4) + e of each 64 x 64 block
+    const bool vec_ok = (p.Cin & 1) == 0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int co = co0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        if (co >= p.Cout) continue;
+#pragma unroll
+        for (int s = 0; s < kWgSlots; ++s) {
+            if (s >= nslots) continue;
+            const int g = s / p.n_blocks, j = s - g * p.n_blocks;
+            float* row = p.dw + (static_cast<size_t>(co) * p.taps + tap0 + g) * p.Cin;
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+                const int ci = ci0 + j * 64 + q * 8 + 2 * (lane & 3);
+                const float v0 = acc[s][4 * q + 2 * h], v1 = acc[s][4 * q + 2 * h + 1];
+                if (vec_ok && ci + 1 < p.Cin) {
+                    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(row + ci), "f"(v0), "f"(v1) : "memory");
+                } else {
+                    if (ci < p.Cin) atomicAdd(row + ci, v0);
+                    if (ci + 1 < p.Cin) atomicAdd(row + ci + 1, v1);
+                }
+            }
+        }
     }
 }
 
@@ -253,12 +255,11 @@ extern "C" Y5_API int y5_conv_wgrad(const y5_wgrad_desc* d, void* stream) {
     p.n_blocks = (blocks_total + p.ci_tiles - 1) / p.ci_tiles;
     const int co_tiles = (d->out_c + kWgCo - 1) / kWgCo;
     const int bn = p.n_blocks * 64;
-    // taps per CTA: accumulators of a group share TMEM (512 columns); a 256-wide tile keeps one tap (its stage is
-    // already 48 KB); groups are balanced (9 taps, limit 5 -> 5 + 4)
-    static const int g_cap = [] { const char* e = getenv("Y5_WG_GROUP_MAX"); return e && atoi(e) > 0 ? atoi(e) : 5; }();
-    static const unsigned stage_kb = [] { const char* e = getenv("Y5_WG_STAGE_KB"); return e && atoi(e) > 0 ? (unsigned)atoi(e) : 56u; }();
-    int gmax = bn >= 256 ? 1 : 512 / bn;
-    if (gmax > g_cap) gmax = g_cap;
+    // taps per CTA: the accumulators of a group share the consumer threads' registers (kWgSlots blocks of 64 ci); groups are
+    // balanced (9 taps, limit 4 -> 3 + 3 + 3)
+    const unsigned stage_kb = 56u;
+    int gmax = kWgSlots / p.n_blocks;
+    if (gmax < 1) gmax = 1;
     p.tap_groups = (p.taps + gmax - 1) / gmax;
     p.group = (p.taps + p.tap_groups - 1) / p.tap_groups;
     // pixels per stage: as many as keep a stage within ~56 KB (>= 3 stages in flight)
@@ -278,9 +279,7 @@ extern "C" Y5_API int y5_conv_wgrad(const y5_wgrad_desc* d, void* stream) {
     p.stages = static_cast<int>((200u * 1024u) / p.stage_bytes);
     if (p.stages > kWgStagesMax) p.stages = kWgStagesMax;
     if (p.stages < 2) return set_error(Y5_E_UNSUPPORTED, "wgrad: stage does not fit shared memory");
-    p.idesc = umma_idesc_f16(d->dtype == Y5_BF16, bn) | (1u << 15) | (1u << 16);  // A and B MN-major
-    const int cols = p.group * bn;
-    p.tmem_cols = cols <= 64 ? 64 : (cols <= 128 ? 128 : (cols <= 256 ? 256 : 512));
+    p.is_bf16 = d->dtype == Y5_BF16;
     p.dw = d->dweight;
 
     CUtensorMap tmDy, tmX;
@@ -310,7 +309,7 @@ extern "C" Y5_API int y5_conv_wgrad(const y5_wgrad_desc* d, void* stream) {
         cudaError_t me = cudaMemsetAsync(d->dweight, 0, dw_bytes, st);
         if (me != cudaSuccess) return set_error(int(me), "wgrad: memset failed: %s", cudaGetErrorString(me));
     }
-    const uint32_t smem = p.stages * p.stage_bytes + (2 * kWgStagesMax + 1) * 8 + 16 + 1024;
+    const uint32_t smem = p.stages * p.stage_bytes + 2 * kWgStagesMax * 8 + 1024;
     const cudaError_t attr_err = ensure_dyn_smem(reinterpret_cast<const void*>(conv_wgrad_kernel), 227 * 1024);
     if (attr_err != cudaSuccess) return set_error(int(attr_err), "wgrad: cudaFuncSetAttribute failed");
     const long long grid = items * p.splits;

@@ -29,7 +29,7 @@ int sm_count() {
     if (dev < 0 || dev >= 64) dev = 0;
     int n = per_dev[dev];
     if (n == 0) {
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         per_dev[dev] = n;
     }
     return n;

@@ -1,4 +1,4 @@
-// Batched non_max_suppression for sm_100a -- whole batch, no host synchronisation, bit-exact indices.
+// Batched non_max_suppression for sm_90a -- whole batch, no host synchronisation, bit-exact indices.
 // Replaces reference utils/general.py:658-767 (+ torchvision.ops.nms called at :750) and ultralytics box_iou.
 //
 // Pipeline (every kernel is launched unconditionally; per-image early exits happen on the device):
@@ -646,7 +646,7 @@ extern "C" Y5_API int y5_box_iou(const float* a, int32_t n, const float* b, int3
     const long long total = static_cast<long long>(n) * m;
     const int threads = 256;
     long long blocks = (total + threads - 1) / threads;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > sm_count() * 16) blocks = sm_count() * 16;
     box_iou_kernel<<<static_cast<int>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(a, n, b, m, eps, out);
     count_launch();
     cudaError_t e = cudaGetLastError();

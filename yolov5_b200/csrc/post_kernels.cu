@@ -416,7 +416,7 @@ extern "C" Y5_API int y5_process_mask(const void* protos, int32_t proto_dtype, i
                                                         mode == 1, low, 0);
         const long long total = static_cast<long long>(n) * in_h * in_w;
         const long long blocks = (total + 255) / 256;
-        mask_upsample_kernel<<<static_cast<unsigned>(blocks < 148LL * 32 ? blocks : 148LL * 32), 256, 0, st>>>(
+        mask_upsample_kernel<<<static_cast<unsigned>(blocks < sm_count() * 32LL ? blocks : sm_count() * 32LL), 256, 0, st>>>(
             low, n, mh, mw, wy, wx, wh, ww, in_h, in_w, mode == 2 ? boxes : nullptr, box_stride, out, out_dtype == Y5_U8);
         count_launch(2);
     }
@@ -429,7 +429,7 @@ extern "C" Y5_API int y5_crop_mask(const float* masks, const float* boxes, int32
     if (!masks || !boxes || !out || n < 0 || h <= 0 || w <= 0 || box_stride < 4) return set_error(Y5_E_INVALID, "crop_mask: bad argument");
     const long long total = static_cast<long long>(n) * h * w;
     const long long blocks = (total + 255) / 256;
-    crop_mask_kernel<<<static_cast<unsigned>(blocks < 148LL * 16 ? blocks : 148LL * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    crop_mask_kernel<<<static_cast<unsigned>(blocks < sm_count() * 16LL ? blocks : sm_count() * 16LL), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         masks, boxes, box_stride, n, h, w, out);
     count_launch();
     return last_status("crop_mask");
@@ -440,7 +440,7 @@ extern "C" Y5_API int y5_scale_boxes(float* boxes, int32_t row_stride, int64_t n
     if (n_rows == 0) return 0;
     if (!boxes || !meta || n_rows < 0 || row_stride < 4) return set_error(Y5_E_INVALID, "scale_boxes: bad argument");
     const long long blocks = (n_rows + 255) / 256;
-    scale_boxes_kernel<<<static_cast<unsigned>(blocks < 148 * 8 ? blocks : 148 * 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    scale_boxes_kernel<<<static_cast<unsigned>(blocks < sm_count() * 8 ? blocks : sm_count() * 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         boxes, row_stride, n_rows, img_index, rows_per_image, count, meta);
     count_launch();
     return last_status("scale_boxes");

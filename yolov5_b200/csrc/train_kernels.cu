@@ -732,7 +732,7 @@ extern "C" Y5_API int y5_zero_stuff2x(const void* x, int32_t x_pitch, void* y, i
     if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "zero_stuff2x: dtype must be fp16 or bf16");
     if (batch <= 0 || h <= 0 || w <= 0) return set_error(Y5_E_INVALID, "zero_stuff2x: bad shape");
     const long long total = static_cast<long long>(batch) * 4 * h * w * (c / 8);
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, 148LL * 16));
+    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 16LL));
     count_launch();
     launch_pdl(zero_stuff2x_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), static_cast<const uint4*>(x), x_pitch / 8, static_cast<uint4*>(y),
                                                                                y_pitch / 8, batch, h, w, c / 8);
@@ -748,7 +748,7 @@ extern "C" Y5_API int y5_weight_pack(const void* w, int32_t w_dtype, int32_t out
         return set_error(Y5_E_INVALID, "weight_pack: bad shape");
     const long long total = (fwd ? static_cast<long long>(out_c) * ksize * ksize * in_c_pad : 0) +
                             (dgrad ? static_cast<long long>(in_c) * ksize * ksize * out_c_pad : 0);
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, 148LL * 8));
+    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 8LL));
     count_launch();
     launch_pdl(weight_pack_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), w, w_dtype, out_c, in_c, ksize, static_cast<uint16_t*>(fwd), in_c_pad,
                                                                               static_cast<uint16_t*>(dgrad), out_c_pad, dtype == Y5_BF16);
@@ -779,7 +779,7 @@ extern "C" Y5_API int y5_fold_pack(const void* w, int32_t w_dtype, int32_t out_c
     if (out_c <= 0 || in_c <= 0 || kh <= 0 || kw <= 0 || in_c_pad < in_c || out_c_pad < out_c) return set_error(Y5_E_INVALID, "fold_pack: bad shape");
     if (gamma && (!beta || !mean || !var)) return set_error(Y5_E_INVALID, "fold_pack: BatchNorm needs gamma, beta, mean and var");
     const long long total = static_cast<long long>(out_c_pad) * kh * kw * in_c_pad;
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, 148LL * 8));
+    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 8LL));
     count_launch();
     fold_pack_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(w, w_dtype, out_c, in_c, kh, kw, conv_bias, gamma, beta, mean, var,
                                                                             bn_dtype, eps, static_cast<uint16_t*>(packed), in_c_pad, out_c_pad,
@@ -794,7 +794,7 @@ extern "C" Y5_API int y5_upsample2x_bwd(const void* dy, int32_t dy_pitch, void* 
     if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "upsample2x_bwd: dtype must be fp16 or bf16");
     if (batch <= 0 || h <= 0 || w <= 0) return set_error(Y5_E_INVALID, "upsample2x_bwd: bad shape");
     const long long total = static_cast<long long>(batch) * h * w * (c / 8);
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, 148LL * 16));
+    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 16LL));
     count_launch();
     launch_pdl(upsample2x_bwd_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), dy, dy_pitch, dx, dx_pitch, batch, h, w, c, dtype == Y5_BF16);
     return launch_status("upsample2x_bwd");
@@ -816,7 +816,7 @@ extern "C" Y5_API int y5_sppf_pool_bwd(const void* cat, int32_t cat_pitch, const
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long pixels = static_cast<long long>(batch) * h * w, total = pixels * c;
     const int bf = dtype == Y5_BF16;
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, 148LL * 16));
+    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 16LL));
     float* acc = static_cast<float*>(workspace);
     const uint16_t* cat16 = static_cast<const uint16_t*>(cat);
     const uint16_t* dcat16 = static_cast<const uint16_t*>(dcat);

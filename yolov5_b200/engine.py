@@ -8,7 +8,7 @@ What the reference does layer by layer through torch.nn (models/yolo.py:160-170 
   * C3's cv1 and cv2 (same input, models/common.py:246) run as ONE GEMM with stacked output channels that lands
     directly in the C3's concat buffer; each Bottleneck's residual add (models/common.py:181) is the epilogue of its
     3x3 conv, in place; SPPF's three pools are one kernel; Upsample writes into its Concat slice;
-  * Conv = conv + folded BN + SiLU in one tcgen05 implicit-GEMM kernel (weights are folded/packed once, here);
+  * Conv = conv + folded BN + SiLU in one wgmma implicit-GEMM kernel (weights are folded/packed once, here);
   * the Detect/Segment head levels run the GEMM with the decode epilogue and write fresh output tensors each call;
   * the whole fixed part is captured in a CUDA graph and replayed.
 
@@ -228,7 +228,6 @@ class Program:
         d.a_mode = int(os.environ.get("Y5_FORCE_A_MODE", "0"))
         if d.a_mode == 2 and s != 1:
             d.a_mode = 0
-        d.reserved = 64  # packed once at build time: constant weights, the kernel may fetch them before its dependency wait
         plan = C.c_void_p()
         _lib.check(self.lib.y5_conv_plan_create(C.byref(d), C.byref(plan)), f"conv_plan_create[{name}]")
         self._plans.append((self.lib.y5_conv_plan_destroy, plan))

@@ -164,7 +164,7 @@ class BaseModel(nn.Module):
     def _forward_once(self, x, profile=False, visualize=False):
         if not (isinstance(x, torch.Tensor) and x.is_cuda):
             raise RuntimeError("y5b200: the engine executes on CUDA tensors only (no CPU / PyTorch fallback); "
-                               "move the model and the input to a B200")
+                               "move the model and the input to an H100")
         if x.dim() != 4 or x.shape[1] != 3:
             raise ValueError(f"y5b200: expected a (B,3,H,W) image batch, got {tuple(x.shape)}")
         head = self.model[-1]

@@ -6,7 +6,7 @@ train.py:401-410 (autocast forward, scaled backward).
 
 What runs where
   * every convolution (forward, data gradient, weight gradient), BatchNorm batch statistics / normalise / backward and
-    SiLU forward / backward: liby5b200 kernels (tcgen05 implicit GEMMs + HBM-bound passes), wrapped in
+    SiLU forward / backward: liby5b200 kernels (wgmma implicit GEMMs + HBM-bound passes), wrapped in
     torch.autograd.Function so gradients land in the ordinary ``.grad`` of the nn.Parameters (DDP's bucketed NCCL
     all-reduce -- smart_DDP -- works unchanged);
   * the glue between convolutions is liby5b200 too: channel concat = strided slice copies whose backward is a set of
@@ -299,8 +299,7 @@ def conv_wgrad(x: torch.Tensor, dy: torch.Tensor, k: int, s: int, p: int) -> tor
 def stem_wide_enabled() -> bool:
     """Stem as a 3x1 conv over overlapping 48-channel "wide pixels" of the zero-padded space-to-depth image (the form the
     inference engine uses): 3 TMA rows per pixel instead of 9 for the forward and the weight gradient, which are bound by
-    the TMA row rate on this 16-channel input.  Measured on B200: 10.28 -> 9.79 ms per yolov5s step; on by default since round 2
-    (Y5_TRAIN_STEM_WIDE=0 restores the 3x3x16 form)."""
+    the TMA row rate on this 16-channel input.  On by default (Y5_TRAIN_STEM_WIDE=0 restores the 3x3x16 form)."""
     return os.environ.get("Y5_TRAIN_STEM_WIDE", "1") != "0"
 
 
