@@ -13,9 +13,10 @@
 // One CTA = one (co tile, tap group, ci tile, pixel range) work item.  A tap group is up to G filter taps whose
 // accumulators sit side by side in registers (G * n <= 4 blocks of m64 x n64 = 128 fp32 registers per thread): the dY tile
 // of a pixel block is fetched once and multiplied with the G shifted X tiles, which divides the dY traffic of 3x3 layers
-// by G.  P (64/128/256 pixels per pipeline stage) grows when channels are few so that a stage stays ~32-56 KB and the
-// per-stage barrier / TMA issue costs are amortised.  The fp32 tiles are added to the fp32 gradient with vector
-// reductions (red.global.add.v2.f32); the pixel range is split so the grid is about one CTA per SM (one wave).
+// by G.  P (pixels per pipeline stage) is 128 when a stage of 128-pixel boxes stays within 56 KB -- one dY box pair and one
+// X box, i.e. 1x1 filters with Cin <= 64 -- and 64 otherwise, which amortises the per-stage barrier / TMA issue costs.
+// The fp32 tiles are added to the fp32 gradient with vector reductions (red.global.add.v2.f32); the pixel range is split
+// so the grid is about one CTA per SM (one wave).
 // Summation order across pixel ranges is not fixed (fp32 atomics), like cuDNN's default wgrad.
 //
 // Gradient of reference models/common.py:86-88 (Conv.forward, the nn.Conv2d weight) / models/yolo.py:97 (Detect.m[i]).
@@ -42,7 +43,7 @@ struct WgradParams {
     int n_blocks;               // 64-channel blocks of Cin per tile
     int ci_tiles, taps;
     int group, tap_groups;      // taps per CTA, number of tap groups
-    int pix;                    // pixels (GEMM K) per pipeline stage: 64 | 128 | 256
+    int pix;                    // pixels (GEMM K) per pipeline stage: 64 | 128
     int kblocks, splits, kb_per_split;
     int stages;
     uint32_t box_bytes, stage_bytes;
@@ -262,11 +263,9 @@ extern "C" Y5_API int y5_conv_wgrad(const y5_wgrad_desc* d, void* stream) {
     if (gmax < 1) gmax = 1;
     p.tap_groups = (p.taps + gmax - 1) / gmax;
     p.group = (p.taps + p.tap_groups - 1) / p.tap_groups;
-    // pixels per stage: as many as keep a stage within ~56 KB (>= 3 stages in flight)
-    p.pix = 64;
-    for (int cand : {256, 128}) {
-        if (static_cast<uint32_t>(2 + p.group * p.n_blocks) * cand * 128u <= stage_kb * 1024u) { p.pix = cand; break; }
-    }
+    // pixels per stage: 128 if such a stage stays within ~56 KB (>= 3 stages in flight), else 64.  (A stage holds two dY boxes
+    // and at least one X box, so 256-pixel stages, 3 x 32 KB, never fit.)
+    p.pix = static_cast<uint32_t>(2 + p.group * p.n_blocks) * 128u * 128u <= stage_kb * 1024u ? 128 : 64;
     p.box_bytes = p.pix * 128u;
     p.kblocks = (p.M + p.pix - 1) / p.pix;
     const long long items = static_cast<long long>(co_tiles) * p.tap_groups * p.ci_tiles;
