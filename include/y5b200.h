@@ -215,6 +215,30 @@ int y5_loss_fwd_bwd_scaled(const y5_loss_params* p, const void* const* pl, const
 int y5_loss_read_targets(const y5_loss_params* p, const void* workspace, int32_t level, int64_t* idx5_host,
                          float* tbox_host, int32_t* count_host, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Segmentation ComputeLoss (utils/segment/loss.py:48-195): the detection terms above plus the cropped mask BCE.
+ *   p[l]       : (B, na, ny_l, nx_l, no) logits with no == 5 + nc + nm; p->batch <= 1024
+ *   proto      : (B, nm, mh, mw) of proto_dtype, element strides ps_* of a dense layout (NCHW or channels_last, no
+ *                gaps: grad_proto is written at the same offsets); nm <= 32
+ *   masks      : (n_masks, gt_h, gt_w) fp32 contiguous; overlap: n_masks == batch and pixel value v marks the image's
+ *                v-th target (1-based); otherwise n_masks >= nt and masks[t] is target row t's mask.  Sizes other than
+ *                (mh, mw) are read through nearest-neighbour downsampling (F.interpolate(mode="nearest"))
+ *   out_loss   : fp32[5] = [loss*bs, lbox, lseg, lobj, lcls]
+ *   grad[l]    : optional, as in y5_loss_fwd_bwd_scaled (mask-coefficient columns included)
+ *   grad_proto : optional, same dtype and strides as proto: d(out_loss[0] * upstream)/dproto, every element written
+ * Only pixels inside a match's crop are visited.  The loss and grad_proto are deterministic.  The workspace (256-byte
+ * aligned) is the detection loss's followed by the segmentation scratch; y5_loss_read_targets works on it too.
+ * ------------------------------------------------------------------------------------------------------------- */
+int64_t y5_seg_loss_workspace_bytes(const y5_loss_params* p);
+int y5_seg_loss_fwd_bwd_scaled(const y5_loss_params* p, const void* const* pl, const float* targets, const float* anchors,
+                               const void* proto, int32_t proto_dtype, int64_t ps_b, int64_t ps_k, int64_t ps_y, int64_t ps_x,
+                               int32_t nm, int32_t mh, int32_t mw, const float* masks, int32_t n_masks, int32_t gt_h,
+                               int32_t gt_w, int32_t overlap, float* out_loss, void* const* grad, void* grad_proto,
+                               const float* grad_scale_dev, void* workspace, int64_t workspace_bytes, void* stream);
+/* one level's tidx (int64) and xywhn (fp32 x4) of the last y5_seg_loss_fwd_bwd_scaled on this workspace (synchronises) */
+int y5_seg_loss_read_targets(const y5_loss_params* p, const void* workspace, int32_t level, int64_t* tidx_host,
+                             float* xywhn_host, int32_t* count_host, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Training-mode Conv = SiLU(BN(conv(x)))  (reference models/common.py:86-88; gradients of the same).
  * Forward:   y = conv(x, W)            -> y5_conv_bn_silu_fwd with act = Y5_ACT_NONE and a zero bias (same kernel)

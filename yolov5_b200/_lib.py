@@ -139,6 +139,10 @@ SIGNATURES = {
     "y5_loss_workspace_bytes": (_I64, [C.POINTER(LossParams)]),
     "y5_loss_fwd_bwd": (_I32, [C.POINTER(LossParams), C.POINTER(_P), _P, _P, _P, C.POINTER(_P), _P, _I64, _P]),
     "y5_loss_read_targets": (_I32, [C.POINTER(LossParams), _P, _I32, _P, _P, _P, _P]),
+    "y5_seg_loss_workspace_bytes": (_I64, [C.POINTER(LossParams)]),
+    "y5_seg_loss_fwd_bwd_scaled": (_I32, [C.POINTER(LossParams), C.POINTER(_P), _P, _P, _P, _I32, _I64, _I64, _I64, _I64, _I32, _I32, _I32,
+                                          _P, _I32, _I32, _I32, _I32, _P, C.POINTER(_P), _P, _P, _P, _I64, _P]),
+    "y5_seg_loss_read_targets": (_I32, [C.POINTER(LossParams), _P, _I32, _P, _P, _P, _P]),
     "y5_conv_wgrad": (_I32, [C.POINTER(WgradDesc), _P]),
     "y5_bn_workspace_bytes": (_I64, [_I32]),
     "y5_bn_stats": (_I32, [_P, _I32, _I64, _I32, _I32, _P, _P]),

@@ -27,6 +27,7 @@ ALIASES = {
     "utils.augmentations": "yolov5_b200.utils.augmentations",
     "utils.segment": "yolov5_b200.utils.segment",
     "utils.segment.general": "yolov5_b200.utils.segment.general",
+    "utils.segment.loss": "yolov5_b200.utils.segment.loss",
 }
 
 

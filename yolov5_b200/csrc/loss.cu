@@ -45,6 +45,7 @@ struct LossArgs {
     float* part_obj;                          // [nl][kPartials]
     float* part_cls;                          // [nl][kPartials]
     float* out_loss;
+    int* trow;                                // optional [nl][cap]: target row of each match (segmentation loss)
 };
 
 __device__ __forceinline__ float ldp(const void* base, long long i, int dtype) {
@@ -91,13 +92,13 @@ __global__ void loss_targets_kernel(LossArgs a) {
     for (int c0 = 0; c0 < total; c0 += blockDim.x) {
         const int c = c0 + threadIdx.x;
         bool ok = false;
-        int b = 0, cls = 0, an = 0, gi = 0, gj = 0;
+        int b = 0, cls = 0, an = 0, gi = 0, gj = 0, t = 0;
         float gx = 0, gy = 0, gw = 0, gh = 0;
         if (c < total) {
             const int k = c / (a.na * a.nt);
             const int rem = c - k * (a.na * a.nt);
             an = rem / a.nt;
-            const int t = rem - an * a.nt;
+            t = rem - an * a.nt;
             const float* tg = a.targets + static_cast<size_t>(t) * 6;
             // t = targets * gain  (gain = [1,1,nx,ny,nx,ny,1]); image / class columns are multiplied by 1.0
             gx = __fmul_rn(tg[2], fnx); gy = __fmul_rn(tg[3], fny);
@@ -136,6 +137,7 @@ __global__ void loss_targets_kernel(LossArgs a) {
             mi[0 * a.cap + pos] = b; mi[1 * a.cap + pos] = an; mi[2 * a.cap + pos] = gj; mi[3 * a.cap + pos] = gi;
             mi[4 * a.cap + pos] = cls;
             tb[pos] = make_float4(__fsub_rn(gx, static_cast<float>(gi)), __fsub_rn(gy, static_cast<float>(gj)), gw, gh);
+            if (a.trow) a.trow[static_cast<size_t>(l) * a.cap + pos] = t;
         }
         __syncthreads();
         if (threadIdx.x == 0) {
@@ -340,6 +342,328 @@ __global__ void loss_finalize_kernel(LossArgs a, int match_blocks, int dense_blo
     a.out_loss[3] = lcls;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Segmentation loss: the mask term of reference utils/segment/loss.py:88-99,116-120 on top of the launch set above.
+//
+//   7 seg_prep      one CTA: per-image target counts -> tidx (global row, or with `overlap` the position's value in the
+//                   concatenation [1..n_0, 1..n_1, ...]), xywhn = (t*nx)/nx; per (level, image) match counts and the
+//                   start of every image's match list
+//   8 seg_bucket    CTA per image: ordered compaction of that image's matches, level by level (stable)
+//   9 seg_match     CTA per match: crop bounds, BCE over the crop's pixels only, the mask-coefficient gradient
+//                   (fixed-order block reduction), added into grad[l] like the class gradients
+//  10 seg_proto     CTA per (image, 16x16 pixel tile): dproto = sum_j g_j(p) coef_j over the image's matches whose crop
+//                   meets the tile, recomputed in registers; every element written once (no atomics)
+//  11 seg_finalize  fixed-order reduction: per (level, image) mean, sum, gains -> out[5]
+// Pixels outside a crop contribute exactly zero, so the work is ~3*nm FMAs per pixel of crop summed over the matches.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kSegMaxNm = 32;
+constexpr int kSegMaxBatch = 1024;  // seg_prep keeps per-image counters in shared memory
+constexpr int kSegTile = 16;
+
+struct SegArgs {
+    int nl, B, na, no, nc, nm, mh, mw, gt_h, gt_w, overlap, nt, cap, dtype, pdtype;
+    int ny[kMaxLevels], nx[kMaxLevels];
+    const void* p[kMaxLevels];
+    void* grad[kMaxLevels];
+    const void* proto;
+    long long ps_b, ps_k, ps_y, ps_x;         // proto element strides (NCHW or channels_last)
+    void* grad_proto;                         // same dtype and strides as proto
+    const float* masks;                       // (n_masks, gt_h, gt_w)
+    const float* targets;
+    const float* grad_scale_dev;
+    float box_gain, grad_scale;
+    const int* count;                         // [nl]           detection workspace
+    const int* midx;                          // [nl][5][cap]   detection workspace
+    const int* trow;                          // [nl][cap]
+    int* tidx;                                // [nl][cap]
+    float4* xywhn;                            // [nl][cap]
+    int* nimg;                                // [nl][B]        matches of image b at level l
+    int* ioff;                                // [B+1]          start of image b's list
+    int* list;                                // [nl*cap]       l*cap + i, by image, then level, then match order
+    int4* crop;                               // [nl][cap]      x0, x1, y0, y1 (half-open, clipped to the map)
+    float* gs;                                // [nl][cap]      d(loss * upstream)/d logit = gs * (sigmoid - gt)
+    float* val;                               // [nl][cap]      crop BCE sum / (mh*mw) / area
+    const float* det_out;                     // [4]            detection items
+    float* out;                               // [5]
+};
+
+// gt of pixel (y, x) at proto resolution: F.interpolate(mode="nearest") folded into the read,
+// source index min(floor(dst * (in / out)), in - 1) in fp32
+__device__ __forceinline__ float seg_gt(const SegArgs& a, int b, int tidx, int y, int x) {
+    const float sy = __fdiv_rn(static_cast<float>(a.gt_h), static_cast<float>(a.mh));
+    const float sx = __fdiv_rn(static_cast<float>(a.gt_w), static_cast<float>(a.mw));
+    const int iy = min(static_cast<int>(floorf(__fmul_rn(static_cast<float>(y), sy))), a.gt_h - 1);
+    const int ix = min(static_cast<int>(floorf(__fmul_rn(static_cast<float>(x), sx))), a.gt_w - 1);
+    const int m = a.overlap ? b : tidx;
+    const float v = a.masks[(static_cast<long long>(m) * a.gt_h + iy) * a.gt_w + ix];
+    return a.overlap ? (v == static_cast<float>(tidx) ? 1.0f : 0.0f) : v;
+}
+
+__device__ __forceinline__ float seg_logit(const float* coef, const float* pr, int nm) {
+    float acc = 0.0f;
+#pragma unroll
+    for (int k = 0; k < kSegMaxNm; ++k)
+        if (k < nm) acc = __fmaf_rn(coef[k], pr[k], acc);
+    return acc;
+}
+
+__device__ __forceinline__ void seg_load_proto(const SegArgs& a, int b, int y, int x, float* pr) {
+    const long long base = b * a.ps_b + y * a.ps_y + x * a.ps_x;
+#pragma unroll
+    for (int k = 0; k < kSegMaxNm; ++k) pr[k] = k < a.nm ? ldp(a.proto, base + k * a.ps_k, a.pdtype) : 0.0f;
+}
+
+__global__ void seg_prep_kernel(SegArgs a) {
+    __shared__ int s_start[kSegMaxBatch + 1];
+    __shared__ int s_cnt[kMaxLevels * kSegMaxBatch];
+    for (int i = threadIdx.x; i <= a.B; i += blockDim.x) s_start[i] = 0;
+    for (int i = threadIdx.x; i < a.nl * a.B; i += blockDim.x) s_cnt[i] = 0;
+    __syncthreads();
+    // (targets[:, 0] == i).sum() per image (segment/loss.py:134)
+    for (int t = threadIdx.x; t < a.nt; t += blockDim.x) {
+        const float f = a.targets[static_cast<size_t>(t) * 6];
+        const int b = static_cast<int>(f);
+        if (f == static_cast<float>(b) && b >= 0 && b < a.B) atomicAdd(&s_start[b + 1], 1);
+    }
+    for (int l = 0; l < a.nl; ++l) {
+        const int n = a.count[l];
+        const int* mb = a.midx + static_cast<size_t>(l) * 5 * a.cap;
+        for (int i = threadIdx.x; i < n; i += blockDim.x) atomicAdd(&s_cnt[l * a.B + mb[i]], 1);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int off = 0;
+        for (int b = 0; b < a.B; ++b) {
+            s_start[b + 1] += s_start[b];
+            a.ioff[b] = off;
+            for (int l = 0; l < a.nl; ++l) off += s_cnt[l * a.B + b];
+        }
+        a.ioff[a.B] = off;
+    }
+    for (int i = threadIdx.x; i < a.nl * a.B; i += blockDim.x) a.nimg[i] = s_cnt[i];
+    __syncthreads();
+    for (int l = 0; l < a.nl; ++l) {
+        const int n = a.count[l];
+        const float fnx = static_cast<float>(a.nx[l]), fny = static_cast<float>(a.ny[l]);
+        for (int i = threadIdx.x; i < n; i += blockDim.x) {
+            const size_t q = static_cast<size_t>(l) * a.cap + i;
+            const int t = a.trow[q];
+            int v = t;
+            if (a.overlap) {  // value at position t of cat([arange(n_b) + 1 for b in range(B)]): the image is the POSITION's
+                int lo = 0, hi = a.B - 1;
+                while (lo < hi) {
+                    const int mid = (lo + hi + 1) >> 1;
+                    if (s_start[mid] <= t) lo = mid; else hi = mid - 1;
+                }
+                v = t - s_start[lo] + 1;
+            }
+            a.tidx[q] = v;
+            const float* tg = a.targets + static_cast<size_t>(t) * 6;
+            // xywhn = cat(gxy, gwh) / gain[2:6] with gxy, gwh = targets * gain: (t * nx) / nx, not always t in fp32
+            a.xywhn[q] = make_float4(__fdiv_rn(__fmul_rn(tg[2], fnx), fnx), __fdiv_rn(__fmul_rn(tg[3], fny), fny),
+                                     __fdiv_rn(__fmul_rn(tg[4], fnx), fnx), __fdiv_rn(__fmul_rn(tg[5], fny), fny));
+        }
+    }
+}
+
+__global__ void seg_bucket_kernel(SegArgs a) {
+    const int b = blockIdx.x;
+    __shared__ int warp_cnt[32];
+    __shared__ int base_s;
+    if (threadIdx.x == 0) base_s = a.ioff[b];
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    for (int l = 0; l < a.nl; ++l) {
+        const int n = a.count[l];
+        const int* mb = a.midx + static_cast<size_t>(l) * 5 * a.cap;
+        for (int c0 = 0; c0 < n; c0 += blockDim.x) {
+            const int i = c0 + threadIdx.x;
+            const bool ok = i < n && mb[i] == b;
+            const unsigned m = __ballot_sync(0xffffffffu, ok);
+            if (lane == 0) warp_cnt[warp] = __popc(m);
+            __syncthreads();
+            int before = base_s;
+            for (int w = 0; w < warp; ++w) before += warp_cnt[w];
+            if (ok) a.list[before + __popc(m & ((1u << lane) - 1u))] = l * a.cap + i;
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                int s = base_s;
+                for (int w = 0; w < nwarps; ++w) s += warp_cnt[w];
+                base_s = s;
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// fixed-order block sum of v[0..nv) (blockDim.x == 256): result valid in red_out[0..nv) after the call
+template <int NV>
+__device__ __forceinline__ void block_sum(float (&v)[NV], float (*red)[NV], float* red_out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < NV; ++k)
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < NV; ++k) red[warp][k] = v[k];
+    __syncthreads();
+    if (threadIdx.x < NV) {
+        float s = 0.0f;
+        for (int w = 0; w < (blockDim.x >> 5); ++w) s += red[w][threadIdx.x];
+        red_out[threadIdx.x] = s;
+    }
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(256) seg_match_kernel(SegArgs a) {
+    const int l = blockIdx.y;
+    const int n = a.count[l];
+    const int nx = a.nx[l], ny = a.ny[l];
+    const int* mi = a.midx + static_cast<size_t>(l) * 5 * a.cap;
+    const float up = a.grad_scale * (a.grad_scale_dev ? *a.grad_scale_dev : 1.0f);
+    const float hw = static_cast<float>(a.mh) * static_cast<float>(a.mw);
+    __shared__ float s_coef[kSegMaxNm];
+    __shared__ float red[8][kSegMaxNm + 1];
+    __shared__ float tot[kSegMaxNm + 1];
+    for (int i = blockIdx.x; i < n; i += gridDim.x) {
+        const size_t q = static_cast<size_t>(l) * a.cap + i;
+        const int b = mi[i], an = mi[a.cap + i], gj = mi[2 * a.cap + i], gi = mi[3 * a.cap + i];
+        const long long e = (((static_cast<long long>(b) * a.na + an) * ny + gj) * nx + gi) * a.no + 5 + a.nc;
+        if (threadIdx.x < a.nm) s_coef[threadIdx.x] = ldp(a.p[l], e + threadIdx.x, a.dtype);
+        const float4 xn = a.xywhn[q];
+        // mxyxy = xywh2xyxy(xywhn * [mw, mh, mw, mh]); crop_mask keeps r >= x1 & r < x2 -> columns [ceil(x1), ceil(x2))
+        const float bx = __fmul_rn(xn.x, static_cast<float>(a.mw)), by = __fmul_rn(xn.y, static_cast<float>(a.mh));
+        const float bw = __fdiv_rn(__fmul_rn(xn.z, static_cast<float>(a.mw)), 2.0f);
+        const float bh = __fdiv_rn(__fmul_rn(xn.w, static_cast<float>(a.mh)), 2.0f);
+        const int x0 = static_cast<int>(fminf(fmaxf(ceilf(__fsub_rn(bx, bw)), 0.0f), static_cast<float>(a.mw)));
+        const int x1 = static_cast<int>(fminf(fmaxf(ceilf(__fadd_rn(bx, bw)), 0.0f), static_cast<float>(a.mw)));
+        const int y0 = static_cast<int>(fminf(fmaxf(ceilf(__fsub_rn(by, bh)), 0.0f), static_cast<float>(a.mh)));
+        const int y1 = static_cast<int>(fminf(fmaxf(ceilf(__fadd_rn(by, bh)), 0.0f), static_cast<float>(a.mh)));
+        const float area = __fmul_rn(xn.z, xn.w);
+        const float nb = static_cast<float>(a.nimg[l * a.B + b]);
+        const float s = __fdiv_rn(__fdiv_rn(__fdiv_rn(__fmul_rn(up, a.box_gain), nb), hw), area);
+        const int tidx = a.tidx[q];
+        __syncthreads();
+        float coef[kSegMaxNm];
+#pragma unroll
+        for (int k = 0; k < kSegMaxNm; ++k) coef[k] = k < a.nm ? s_coef[k] : 0.0f;
+        float acc[kSegMaxNm + 1];
+#pragma unroll
+        for (int k = 0; k <= kSegMaxNm; ++k) acc[k] = 0.0f;
+        const int cw = max(x1 - x0, 0), ch = max(y1 - y0, 0);
+        const int npix = cw * ch;
+        for (int pix = threadIdx.x; pix < npix; pix += blockDim.x) {
+            const int y = y0 + pix / cw, x = x0 + pix % cw;
+            float pr[kSegMaxNm];
+            seg_load_proto(a, b, y, x, pr);
+            const float xl = seg_logit(coef, pr, a.nm);
+            const float gt = seg_gt(a, b, tidx, y, x);
+            acc[kSegMaxNm] += bce_logits(xl, gt, 1.0f);
+            const float g = __fmul_rn(__fsub_rn(sigmoid_f(xl), gt), s);
+#pragma unroll
+            for (int k = 0; k < kSegMaxNm; ++k) acc[k] = __fmaf_rn(g, pr[k], acc[k]);
+        }
+        block_sum<kSegMaxNm + 1>(acc, red, tot);
+        if (threadIdx.x < a.nm && a.grad[l]) atomic_add_elem(a.grad[l], e + threadIdx.x, tot[threadIdx.x], a.dtype);
+        if (threadIdx.x == 0) {
+            a.val[q] = __fdiv_rn(__fdiv_rn(tot[kSegMaxNm], hw), area);
+            a.crop[q] = make_int4(x0, x1, y0, y1);
+            a.gs[q] = s;
+        }
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(256) seg_proto_kernel(SegArgs a) {
+    constexpr int kBatch = 32;
+    const int b = blockIdx.y;
+    const int tiles_x = (a.mw + kSegTile - 1) / kSegTile;
+    const int tx0 = (blockIdx.x % tiles_x) * kSegTile, ty0 = (blockIdx.x / tiles_x) * kSegTile;
+    const int x = tx0 + (threadIdx.x % kSegTile), y = ty0 + (threadIdx.x / kSegTile);
+    const bool inside = x < a.mw && y < a.mh;
+    __shared__ float s_coef[kBatch][kSegMaxNm];
+    __shared__ int4 s_crop[kBatch];
+    __shared__ float s_gs[kBatch];
+    __shared__ int s_tidx[kBatch];
+    __shared__ int s_hit[kBatch];
+    float pr[kSegMaxNm], acc[kSegMaxNm];
+    seg_load_proto(a, b, inside ? y : 0, inside ? x : 0, pr);
+#pragma unroll
+    for (int k = 0; k < kSegMaxNm; ++k) acc[k] = 0.0f;
+    const int beg = a.ioff[b], end = a.ioff[b + 1];
+    for (int j0 = beg; j0 < end; j0 += kBatch) {
+        const int nb = min(kBatch, end - j0);
+        if (threadIdx.x < nb) {
+            const int q = a.list[j0 + threadIdx.x];
+            const int4 c = a.crop[q];
+            s_crop[threadIdx.x] = c;
+            s_gs[threadIdx.x] = a.gs[q];
+            s_tidx[threadIdx.x] = a.tidx[q];
+            s_hit[threadIdx.x] = max(c.x, tx0) < min(c.y, tx0 + kSegTile) && max(c.z, ty0) < min(c.w, ty0 + kSegTile);
+        }
+        __syncthreads();
+        for (int idx = threadIdx.x; idx < nb * kSegMaxNm; idx += blockDim.x) {
+            const int jj = idx / kSegMaxNm, k = idx % kSegMaxNm;
+            if (!s_hit[jj] || k >= a.nm) continue;
+            const int q = a.list[j0 + jj];
+            const int l = q / a.cap, i = q - l * a.cap;
+            const int* mi = a.midx + static_cast<size_t>(l) * 5 * a.cap;
+            const long long e = (((static_cast<long long>(mi[i]) * a.na + mi[a.cap + i]) * a.ny[l] + mi[2 * a.cap + i]) * a.nx[l] +
+                                 mi[3 * a.cap + i]) * a.no + 5 + a.nc;
+            s_coef[jj][k] = ldp(a.p[l], e + k, a.dtype);
+        }
+        __syncthreads();
+        for (int jj = 0; jj < nb; ++jj) {
+            if (!s_hit[jj]) continue;
+            const int4 c = s_crop[jj];
+            if (!inside || x < c.x || x >= c.y || y < c.z || y >= c.w) continue;
+            const float xl = seg_logit(s_coef[jj], pr, a.nm);
+            const float g = __fmul_rn(__fsub_rn(sigmoid_f(xl), seg_gt(a, b, s_tidx[jj], y, x)), s_gs[jj]);
+#pragma unroll
+            for (int k = 0; k < kSegMaxNm; ++k) acc[k] = __fmaf_rn(g, s_coef[jj][k < a.nm ? k : 0], acc[k]);
+        }
+        __syncthreads();
+    }
+    if (!inside) return;
+    const long long base = b * a.ps_b + y * a.ps_y + x * a.ps_x;
+#pragma unroll
+    for (int k = 0; k < kSegMaxNm; ++k)
+        if (k < a.nm) stg(a.grad_proto, base + k * a.ps_k, acc[k], a.pdtype);
+}
+
+__global__ void seg_finalize_kernel(SegArgs a) {
+    __shared__ float red[256];
+    float local = 0.0f;
+    for (int b = threadIdx.x; b < a.B; b += blockDim.x) {
+        // the image's list is level-ordered: mean per (level, image), as the reference's `for bi in b.unique()`
+        float cur = 0.0f;
+        int cur_l = -1;
+        for (int j = a.ioff[b]; j < a.ioff[b + 1]; ++j) {
+            const int q = a.list[j];
+            const int l = q / a.cap;
+            if (l != cur_l) {
+                if (cur_l >= 0) local += cur / static_cast<float>(a.nimg[cur_l * a.B + b]);
+                cur = 0.0f;
+                cur_l = l;
+            }
+            cur += a.val[q];
+        }
+        if (cur_l >= 0) local += cur / static_cast<float>(a.nimg[cur_l * a.B + b]);
+    }
+    red[threadIdx.x] = local;
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    float lseg = 0.0f;
+    for (int w = 0; w < blockDim.x; ++w) lseg += red[w];
+    lseg *= a.box_gain / static_cast<float>(a.B);
+    const float lbox = a.det_out[1], lobj = a.det_out[2], lcls = a.det_out[3];
+    a.out[0] = (lbox + lobj + lcls + lseg) * static_cast<float>(a.B);
+    a.out[1] = lbox;
+    a.out[2] = lseg;
+    a.out[3] = lobj;
+    a.out[4] = lcls;
+}
+
 }  // namespace y5
 
 using namespace y5;
@@ -405,9 +729,10 @@ extern "C" Y5_API int y5_loss_fwd_bwd(const y5_loss_params* p, const void* const
     return y5_loss_fwd_bwd_scaled(p, pl, targets, anchors, out_loss, grad, nullptr, workspace, workspace_bytes, stream);
 }
 
-extern "C" Y5_API int y5_loss_fwd_bwd_scaled(const y5_loss_params* p, const void* const* pl, const float* targets, const float* anchors,
-                                             float* out_loss, void* const* grad, const float* grad_scale_dev, void* workspace,
-                                             int64_t workspace_bytes, void* stream) {
+namespace {
+// the detection launch set; `trow` (segmentation loss only) receives each match's target row
+int loss_launch(const y5_loss_params* p, const void* const* pl, const float* targets, const float* anchors, float* out_loss,
+                void* const* grad, const float* grad_scale_dev, void* workspace, int64_t workspace_bytes, void* stream, int* trow) {
     if (int e = validate_loss(p)) return e;
     if (!pl || !anchors || !out_loss || !workspace || (p->nt > 0 && !targets)) return set_error(Y5_E_INVALID, "loss: null pointer");
     const LossWs L = loss_ws(p);
@@ -422,6 +747,7 @@ extern "C" Y5_API int y5_loss_fwd_bwd_scaled(const y5_loss_params* p, const void
     }
     a.targets = targets; a.anchors = anchors; a.out_loss = out_loss;
     a.grad_scale_dev = grad_scale_dev;
+    a.trow = trow;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int sms = sm_count();
     loss_zero_kernel<<<sms * 4, 256, 0, st>>>(a);
@@ -437,6 +763,13 @@ extern "C" Y5_API int y5_loss_fwd_bwd_scaled(const y5_loss_params* p, const void
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(int(e), "loss launch failed: %s", cudaGetErrorString(e));
     return 0;
+}
+}  // namespace
+
+extern "C" Y5_API int y5_loss_fwd_bwd_scaled(const y5_loss_params* p, const void* const* pl, const float* targets, const float* anchors,
+                                             float* out_loss, void* const* grad, const float* grad_scale_dev, void* workspace,
+                                             int64_t workspace_bytes, void* stream) {
+    return loss_launch(p, pl, targets, anchors, out_loss, grad, grad_scale_dev, workspace, workspace_bytes, stream, nullptr);
 }
 
 // Copies one level's build_targets result to host memory (synchronises the stream: test / debugging helper).
@@ -468,6 +801,144 @@ extern "C" Y5_API int y5_loss_read_targets(const y5_loss_params* p, const void* 
         e = cudaMemcpyAsync(tbox_host, ws + L.tbox + sizeof(float4) * level * cap, sizeof(float4) * n, cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) return set_error(int(e), "loss_read_targets: %s", cudaGetErrorString(e));
+    }
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// segmentation loss: detection workspace layout unchanged, the seg scratch follows it
+// ---------------------------------------------------------------------------------------------------------------------
+namespace {
+struct SegWs {
+    size_t trow, tidx, xywhn, nimg, ioff, list, crop, gs, val, det_out, total;
+};
+SegWs seg_ws(const y5_loss_params* p) {
+    SegWs S;
+    size_t o = loss_ws(p).total;
+    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~size_t(255); return r; };
+    const size_t m = static_cast<size_t>(p->nl) * 5 * p->na * (p->nt > 0 ? p->nt : 1);
+    S.trow = take(sizeof(int) * m);
+    S.tidx = take(sizeof(int) * m);
+    S.xywhn = take(sizeof(float4) * m);
+    S.nimg = take(sizeof(int) * kMaxLevels * p->batch);
+    S.ioff = take(sizeof(int) * (p->batch + 1));
+    S.list = take(sizeof(int) * m);
+    S.crop = take(sizeof(int4) * m);
+    S.gs = take(sizeof(float) * m);
+    S.val = take(sizeof(float) * m);
+    S.det_out = take(sizeof(float) * 4);
+    S.total = o;
+    return S;
+}
+int validate_seg(const y5_loss_params* p) {
+    if (int e = validate_loss(p)) return e;
+    if (p->batch > kSegMaxBatch) return set_error(Y5_E_INVALID, "seg_loss: batch %d > %d", p->batch, kSegMaxBatch);
+    if (static_cast<long long>(p->nl) * 5 * p->na * (p->nt > 0 ? p->nt : 1) > 0x3fffffff)
+        return set_error(Y5_E_UNSUPPORTED, "seg_loss: too many targets");
+    return 0;
+}
+}  // namespace
+
+extern "C" Y5_API int64_t y5_seg_loss_workspace_bytes(const y5_loss_params* p) {
+    if (validate_seg(p)) return -1;
+    return static_cast<int64_t>(seg_ws(p).total);
+}
+
+extern "C" Y5_API int y5_seg_loss_fwd_bwd_scaled(const y5_loss_params* p, const void* const* pl, const float* targets,
+                                                 const float* anchors, const void* proto, int32_t proto_dtype, int64_t ps_b,
+                                                 int64_t ps_k, int64_t ps_y, int64_t ps_x, int32_t nm, int32_t mh, int32_t mw,
+                                                 const float* masks, int32_t n_masks, int32_t gt_h, int32_t gt_w, int32_t overlap,
+                                                 float* out_loss, void* const* grad, void* grad_proto, const float* grad_scale_dev,
+                                                 void* workspace, int64_t workspace_bytes, void* stream) {
+    if (int e = validate_seg(p)) return e;
+    if (nm < 1 || nm > kSegMaxNm) return set_error(Y5_E_INVALID, "seg_loss: nm %d outside [1, %d]", nm, kSegMaxNm);
+    if (p->no != 5 + p->nc + nm) return set_error(Y5_E_INVALID, "seg_loss: no %d != 5 + nc %d + nm %d", p->no, p->nc, nm);
+    if (mh < 1 || mw < 1 || gt_h < 1 || gt_w < 1)
+        return set_error(Y5_E_INVALID, "seg_loss: bad mask sizes (proto %dx%d, masks %dx%d)", mh, mw, gt_h, gt_w);
+    if (overlap != 0 && overlap != 1) return set_error(Y5_E_INVALID, "seg_loss: overlap must be 0 or 1");
+    if (overlap ? n_masks != p->batch : n_masks < p->nt)
+        return set_error(Y5_E_INVALID, "seg_loss: %d masks for batch %d / %d targets (overlap %d)", n_masks, p->batch, p->nt, overlap);
+    if (proto_dtype != Y5_F16 && proto_dtype != Y5_BF16 && proto_dtype != Y5_F32) return set_error(Y5_E_UNSUPPORTED, "seg_loss: proto dtype");
+    if (ps_b < 0 || ps_k < 0 || ps_y < 0 || ps_x < 0) return set_error(Y5_E_INVALID, "seg_loss: negative proto stride");
+    if (!proto || !out_loss || !workspace || (p->nt > 0 && !masks)) return set_error(Y5_E_INVALID, "seg_loss: null pointer");
+    const SegWs S = seg_ws(p);
+    if (workspace_bytes < static_cast<int64_t>(S.total)) return set_error(Y5_E_INVALID, "seg_loss: workspace too small");
+    unsigned char* ws = static_cast<unsigned char*>(workspace);
+    if (int e = loss_launch(p, pl, targets, anchors, reinterpret_cast<float*>(ws + S.det_out), grad, grad_scale_dev, workspace,
+                            workspace_bytes, stream, reinterpret_cast<int*>(ws + S.trow)))
+        return e;
+    const LossWs L = loss_ws(p);
+    SegArgs a{};
+    a.nl = p->nl; a.B = p->batch; a.na = p->na; a.no = p->no; a.nc = p->nc; a.nm = nm; a.mh = mh; a.mw = mw;
+    a.gt_h = gt_h; a.gt_w = gt_w; a.overlap = overlap; a.nt = p->nt; a.cap = 5 * p->na * (p->nt > 0 ? p->nt : 1);
+    a.dtype = p->dtype; a.pdtype = proto_dtype;
+    for (int l = 0; l < p->nl; ++l) {
+        a.ny[l] = p->ny[l]; a.nx[l] = p->nx[l];
+        a.p[l] = pl[l];
+        a.grad[l] = grad ? grad[l] : nullptr;
+    }
+    a.proto = proto; a.ps_b = ps_b; a.ps_k = ps_k; a.ps_y = ps_y; a.ps_x = ps_x;
+    a.grad_proto = grad_proto; a.masks = masks; a.targets = targets; a.grad_scale_dev = grad_scale_dev;
+    a.box_gain = p->box_gain; a.grad_scale = p->grad_scale;
+    a.count = reinterpret_cast<const int*>(ws + L.count);
+    a.midx = reinterpret_cast<const int*>(ws + L.midx);
+    a.trow = reinterpret_cast<const int*>(ws + S.trow);
+    a.tidx = reinterpret_cast<int*>(ws + S.tidx);
+    a.xywhn = reinterpret_cast<float4*>(ws + S.xywhn);
+    a.nimg = reinterpret_cast<int*>(ws + S.nimg);
+    a.ioff = reinterpret_cast<int*>(ws + S.ioff);
+    a.list = reinterpret_cast<int*>(ws + S.list);
+    a.crop = reinterpret_cast<int4*>(ws + S.crop);
+    a.gs = reinterpret_cast<float*>(ws + S.gs);
+    a.val = reinterpret_cast<float*>(ws + S.val);
+    a.det_out = reinterpret_cast<const float*>(ws + S.det_out);
+    a.out = out_loss;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    seg_prep_kernel<<<1, 1024, 0, st>>>(a);
+    seg_bucket_kernel<<<p->batch, 256, 0, st>>>(a);
+    seg_match_kernel<<<dim3(min(a.cap, 4 * sm_count()), p->nl), 256, 0, st>>>(a);
+    int n = 4;
+    if (grad_proto) {
+        const int tiles = ((mw + kSegTile - 1) / kSegTile) * ((mh + kSegTile - 1) / kSegTile);
+        seg_proto_kernel<<<dim3(tiles, p->batch), kSegTile * kSegTile, 0, st>>>(a);
+        ++n;
+    }
+    seg_finalize_kernel<<<1, 256, 0, st>>>(a);
+    count_launch(n);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(int(e), "seg_loss launch failed: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+// Copies one level's tidx (int64) and xywhn (fp32 x4) to host memory (synchronises the stream: test / debugging helper).
+extern "C" Y5_API int y5_seg_loss_read_targets(const y5_loss_params* p, const void* workspace, int32_t level, int64_t* tidx_host,
+                                               float* xywhn_host, int32_t* count_host, void* stream) {
+    if (int e = validate_seg(p)) return e;
+    if (!workspace || level < 0 || level >= p->nl || !count_host) return set_error(Y5_E_INVALID, "seg_loss_read_targets: bad arguments");
+    const LossWs L = loss_ws(p);
+    const SegWs S = seg_ws(p);
+    const unsigned char* ws = static_cast<const unsigned char*>(workspace);
+    const size_t cap = static_cast<size_t>(5) * p->na * (p->nt > 0 ? p->nt : 1);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int counts[kMaxLevels];
+    cudaError_t e = cudaMemcpyAsync(counts, ws + L.count, sizeof(int) * kMaxLevels, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return set_error(int(e), "seg_loss_read_targets: %s", cudaGetErrorString(e));
+    const int n = counts[level];
+    *count_host = n;
+    if (n > 0 && tidx_host) {
+        int* tmp = new int[n];
+        e = cudaMemcpyAsync(tmp, ws + S.tidx + sizeof(int) * level * cap, sizeof(int) * n, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e == cudaSuccess)
+            for (int i = 0; i < n; ++i) tidx_host[i] = tmp[i];
+        delete[] tmp;
+        if (e != cudaSuccess) return set_error(int(e), "seg_loss_read_targets: %s", cudaGetErrorString(e));
+    }
+    if (n > 0 && xywhn_host) {
+        e = cudaMemcpyAsync(xywhn_host, ws + S.xywhn + sizeof(float4) * level * cap, sizeof(float4) * n, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return set_error(int(e), "seg_loss_read_targets: %s", cudaGetErrorString(e));
     }
     return 0;
 }
