@@ -388,6 +388,41 @@ int y5_match_batch(const float* det, int64_t img_stride, int32_t row_stride, con
                    int32_t max_det, const float* labels, int32_t nt, const float* iouv, int32_t niou, float eps,
                    uint8_t* correct, void* stream);
 
+/* Mask IoU of segment/val.py (utils/metrics.py:239-265 process_batch(masks=True); ultralytics' mask_iou) as a 1-bit GEMM.
+ * Bit rows: an (h, w) mask is y5_mask_row_words(h, w) uint32 words, pixel p = y*w + x at bit p%32 of word p/32, zero bits
+ * up to a multiple of 256 pixels.  y5_mask_row_words returns Y5_E_UNSUPPORTED when h*w > 2^23 (beyond that the reference's
+ * fp32 pixel sums stop being exact).
+ * label_index (device, batch + 1 + 2*nt int32, written by y5_mask_pack whenever it is given, nt = 0 included): [0..batch] the first row
+ * of each image's labels (image b owns rows [li[b], li[b+1]) in target order), then for every row its target index, then
+ * its image (-1: the target's image column is not an integer in [0, batch); such rows follow li[batch]). */
+int32_t y5_mask_row_words(int32_t h, int32_t w);
+/* Masks -> bit rows (out_h, out_w) + popcount (n_rows int32), reading `src` (contiguous planes of src_h*src_w, Y5_U8 (also
+ * bool) | Y5_F32 | Y5_F16 | Y5_BF16).  One block per row; an overlap index plane is read once per label of its image.
+ *   overlap == 0, label_index NULL : row r = plane r (direct 0/1 masks)
+ *   overlap == 0, label_index set  : rows of the nt = n_rows targets grouped by image: row = plane row_target (segment/val.py
+ *                                    `masks[targets[:, 0] == si]`, so src holds nt planes)
+ *   overlap != 0, label_index NULL : row k = (plane 0 == k + 1), k < n_rows (one image's index mask, `gt == arange(nl) + 1`)
+ *   overlap != 0, label_index set  : row of label k of image b = (plane b == k + 1) (src holds batch planes)
+ * With label_index, `batch` images and target_img (device: the image column of the (nt, target_stride) fp32 targets, may be
+ * NULL when nt == 0) lay out the label rows first.  When (src_h, src_w) != (out_h, out_w) each
+ * row's values (the 0/1 indicators in overlap mode) are resized as F.interpolate(bilinear, align_corners=False) and kept
+ * where > 0.5.  Direct values that are not 0 or 1 and enter unresized are added to *nonbinary (device int32). */
+int y5_mask_pack(const void* src, int32_t src_dtype, int32_t src_h, int32_t src_w, int32_t overlap, const float* target_img,
+                 int32_t target_stride, int32_t batch, int32_t n_rows, int32_t out_h, int32_t out_w, int32_t* label_index,
+                 uint32_t* bits, int32_t* popcount, int32_t* nonbinary, void* stream);
+/* iou[(l) * rows_per_image + d] = inter / (|gt_l| + |pred_d| - inter + eps) for images img0..img0+n_img-1: labels l of image b
+ * from label_index, predictions d < count[b] (NULL: all) at pred rows (b - img0) * rows_per_image + d.  label_index NULL: one
+ * image, labels 0..n_gt-1 (the single-pair mask_iou(gt, pred) -> (n_gt, rows_per_image)).  `words` = y5_mask_row_words. */
+int y5_mask_iou(const uint32_t* gt_bits, const int32_t* gt_pop, const int32_t* label_index, int32_t n_gt, const uint32_t* pred_bits,
+                const int32_t* pred_pop, const int32_t* count, int32_t img0, int32_t n_img, int32_t rows_per_image, int32_t words,
+                float eps, float* iou, void* stream);
+/* process_batch(masks=True)'s matching (utils/metrics.py:255-264) for every image of a batch, reading the IoU matrix of
+ * y5_mask_iou (rows_per_image = max_det): det / count / correct as y5_match_batch; label l's class at
+ * label_cls[target(l) * cls_stride] (target(l) from label_index, or l when label_index is NULL and batch == 1). */
+int y5_mask_match_batch(const float* det, int64_t img_stride, int32_t row_stride, const int32_t* count, int32_t batch, int32_t max_det,
+                        const float* label_cls, int32_t cls_stride, const int32_t* label_index, int32_t nt, const float* iou,
+                        const float* iouv, int32_t niou, uint8_t* correct, void* stream);
+
 /* Fused optimizer step (train.py:413-421): un-scale + clip_grad_norm_ + SGD(momentum, nesterov) over parameter groups
  * (utils/torch_utils.py:256-289) + optimizer.zero_grad + ModelEMA.update (utils/torch_utils.py:359-368) in two
  * multi-tensor launches.  All tensors fp32.  `table`, `chunk_*`, `hyper`, `partial` are DEVICE arrays owned by the caller:

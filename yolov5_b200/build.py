@@ -30,6 +30,7 @@ SOURCES = {
     "nms.cu": ["-fmad=false"],
     "loss.cu": ["-fmad=false"],
     "post_kernels.cu": ["-fmad=false"],
+    "mask_metrics.cu": ["-fmad=false"],
     "optim_kernels.cu": [],
 }
 

@@ -13,6 +13,7 @@
 #include "../../include/y5b200.h"
 #include "common.cuh"
 #include "host_util.h"
+#include "match_rule.cuh"
 
 namespace y5 {
 
@@ -281,11 +282,8 @@ __device__ __forceinline__ float iou_label_det(const float* l, const float* d, f
     return __fdiv_rn(inter, __fadd_rn(__fsub_rn(__fadd_rn(a1, a2), inter), eps));
 }
 
-constexpr int kMatchMaxDet = 4096;
-
 // One block per image.  Detection d's best label = the same-class label with the highest IoU (first label on ties: the
-// reference's stable descending sort keeps (label, detection) scan order); d is a true positive at threshold t when that IoU
-// >= iouv[t] and no lower-index detection claims the same label at t (np.unique keeps the first detection per label).
+// reference's stable descending sort keeps (label, detection) scan order); then match_assign (match_rule.cuh).
 __global__ void match_kernel(const float* __restrict__ det, long long img_stride, int row_stride, const int32_t* __restrict__ count,
                              int max_det, const float* __restrict__ labels, int nt, const float* __restrict__ iouv, int niou, float eps,
                              uint8_t* __restrict__ correct) {
@@ -310,16 +308,7 @@ __global__ void match_kernel(const float* __restrict__ det, long long img_stride
         s_iou[d] = best_iou;
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < n * niou; i += blockDim.x) {
-        const int d = i / niou, t = i - d * niou;
-        const float thr = iouv[t];
-        const int bl = s_best[d];
-        bool ok = bl >= 0 && s_iou[d] >= thr;
-        for (int e = 0; ok && e < d; ++e)
-            if (s_best[e] == bl && s_iou[e] >= thr) ok = false;
-        correct[(static_cast<long long>(b) * max_det + d) * niou + t] = ok ? 1 : 0;
-    }
-    for (int i = n * niou + threadIdx.x; i < max_det * niou; i += blockDim.x) correct[static_cast<long long>(b) * max_det * niou + i] = 0;
+    match_assign(s_best, s_iou, n, max_det, iouv, niou, correct + static_cast<long long>(b) * max_det * niou);
 }
 
 static int last_status(const char* what) {

@@ -1,6 +1,8 @@
 """Metric matching of the validation loop on the device (reference utils/metrics.py:224-265 process_batch, box_iou as used
-at :158,:252, and the per-image loop of val.py:282-318): IoU, class test and the detection<->label matching rule for the
-WHOLE batch in one launch, with no `.cpu()` round trip per image."""
+at :158,:252, and the per-image loops of val.py:282-318 and segment/val.py:263-298): box IoU or mask IoU, class test and the
+detection<->label matching rule for the WHOLE batch, with no `.cpu()` round trip per image.  Mask IoU (ultralytics'
+mask_iou, imported by the reference into utils.metrics) is a 1-bit GEMM on the tensor cores: every quantity before the one
+fp32 division is an integer pixel count, so it is bit-exact."""
 from __future__ import annotations
 
 import ctypes as C
@@ -48,10 +50,12 @@ def match_batch(det_rows: torch.Tensor, count, labels6: torch.Tensor, iouv: torc
 
 def process_batch(detections, labels, iouv, pred_masks=None, gt_masks=None, overlap=False, masks=False):
     """Reference signature (utils/metrics.py:224): detections (N,6) [x1,y1,x2,y2,conf,cls], labels (M,5) [cls,x1,y1,x2,y2],
-    iouv thresholds -> correct (N, len(iouv)) bool on iouv.device.  Box matching only (masks=True is the mask-IoU branch of
-    segment/val.py, outside this path)."""
+    iouv thresholds -> correct (N, len(iouv)) bool on iouv.device.  masks=True matches by mask IoU (segment/val.py:295):
+    pred_masks (N, h, w) 0/1; gt_masks (M, H, W) 0/1, or with `overlap` (1, H, W) holding label k as the value k + 1; gt masks
+    of another size are resized as the reference does (bilinear, then > 0.5).  Raises ValueError on 0/1 masks holding other
+    values (that one check reads the device, as the reference's own `.cpu()` does)."""
     if masks:
-        raise NotImplementedError("y5b200: mask-IoU matching (segment/val.py) is outside the engine's hot path")
+        return _process_batch_masks(detections, labels, iouv, pred_masks, gt_masks, overlap)
     n = detections.shape[0]
     dev = detections.device
     lab6 = torch.cat((torch.zeros(labels.shape[0], 1, device=labels.device, dtype=labels.dtype), labels), 1)
@@ -80,11 +84,161 @@ def val_batch_metrics(rows: torch.Tensor, count: torch.Tensor, targets: torch.Te
     """The metric part of val.py:282-318 for a whole batch, on the device: rows/count from nms_device (rows (B,max_det,6+nm)
     in network-input pixels), targets (nt,6) [img, cls, cx, cy, w, h] already in network-input pixels (val.py:274),
     im_shape = (height, width) of the network input, shapes[i] = ((h0, w0), ((ratio_h, ratio_w), (pad_w, pad_h))) as the
-    reference dataloader yields.  Returns (predn rows in native space, correct (B,max_det,niou) bool); nothing is synced."""
-    from .general import scale_meta, scale_boxes_batch
+    reference dataloader yields, or the (B,5) tensor scale_meta makes of them (already on the device, the loop can then be
+    captured in a CUDA graph).  Returns (predn rows in native space, correct (B,max_det,niou) bool); nothing is synced."""
+    from .general import scale_boxes_batch
 
-    meta = scale_meta(im_shape, [s[0] for s in shapes], [s[1] if len(s) > 1 else None for s in shapes]).to(rows.device)
+    meta = _meta(im_shape, shapes, rows.device)
     predn = rows.clone()
     scale_boxes_batch(predn, count, meta)
     labelsn = labels_to_native(targets, meta)
     return predn, match_batch(predn, count, labelsn, iouv)
+
+
+_STAGE_BYTES = 256 << 20  # seg_val_batch_metrics stages the uint8 prediction masks of at most this many bytes at a time
+
+
+def _meta(im_shape, shapes, device):
+    if isinstance(shapes, torch.Tensor):
+        return shapes.to(device, torch.float32)
+    from .general import scale_meta
+
+    return scale_meta(im_shape, [s[0] for s in shapes], [s[1] if len(s) > 1 else None for s in shapes]).to(device)
+
+
+def _row_words(h: int, w: int) -> int:
+    words = int(_lib.lib().y5_mask_row_words(int(h), int(w)))
+    if words < 0:
+        _lib.check(words, "mask_row_words")
+    return words
+
+
+def _pack(src, src_hw, out_hw, n_rows, nonbinary, overlap=False, targets=None, batch=1, label_index=None):
+    """y5_mask_pack: (bits (n_rows, words) int32, popcount (n_rows,) int32) of the masks in `src` (see include/y5b200.h)."""
+    if not src.is_cuda:
+        raise RuntimeError("y5b200: mask IoU runs on CUDA tensors only (no CPU / PyTorch fallback)")
+    m = src.contiguous()
+    if m.dtype == torch.bool:
+        m = m.view(torch.uint8)
+    dev = m.device
+    bits = torch.empty(n_rows, _row_words(*out_hw), dtype=torch.int32, device=dev)
+    pop = torch.empty(n_rows, dtype=torch.int32, device=dev)
+    timg, ts = (targets.data_ptr(), targets.stride(0)) if targets is not None else (None, 0)
+    _lib.check(_lib.lib().y5_mask_pack(m.data_ptr() if m.numel() else None, _lib.dtype_code(m.dtype), int(src_hw[0]), int(src_hw[1]),
+                                       int(bool(overlap)), timg, ts, batch, n_rows, int(out_hw[0]), int(out_hw[1]),
+                                       label_index.data_ptr() if label_index is not None else None, bits.data_ptr(), pop.data_ptr(),
+                                       nonbinary.data_ptr(), C.c_void_p(_lib.stream_ptr(dev))), "mask_pack")
+    return bits, pop
+
+
+def _raise_nonbinary(nonbinary: torch.Tensor) -> None:
+    bad = int(nonbinary.item())
+    if bad:
+        raise ValueError(f"y5b200: {bad} mask values are neither 0 nor 1 (mask IoU takes 0/1 masks)")
+
+
+def mask_iou(mask1, mask2, eps=1e-7):
+    """ultralytics.utils.metrics.mask_iou, which the reference imports into utils.metrics: mask1 (N, n), mask2 (M, n) flattened
+    0/1 masks -> (N, M) fp32 on the device, inter / (|mask1| + |mask2| - inter + eps).  The intersections are a 1-bit GEMM
+    (y5_mask_iou), bit-equal to the fp32 matmul expression.  Raises ValueError when a mask holds a value other than 0 or 1."""
+    if mask1.dim() != 2 or mask2.dim() != 2 or mask1.shape[1] != mask2.shape[1]:
+        raise ValueError(f"y5b200: mask_iou takes (N, n) and (M, n) masks, got {tuple(mask1.shape)} and {tuple(mask2.shape)}")
+    dev = mask1.device
+    n, m, px = mask1.shape[0], mask2.shape[0], mask1.shape[1]
+    out = torch.zeros(n, m, dtype=torch.float32, device=dev)
+    if n == 0 or m == 0 or px == 0:
+        return out
+    nonbinary = torch.zeros(1, dtype=torch.int32, device=dev)
+    with _lib.on(dev):
+        g, gp = _pack(mask1, (1, px), (1, px), n, nonbinary)
+        p, pp = _pack(mask2, (1, px), (1, px), m, nonbinary)
+        _lib.check(_lib.lib().y5_mask_iou(g.data_ptr(), gp.data_ptr(), None, n, p.data_ptr(), pp.data_ptr(), None, 0, 1, m, g.shape[1],
+                                          float(eps), out.data_ptr(), C.c_void_p(_lib.stream_ptr(dev))), "mask_iou")
+    _raise_nonbinary(nonbinary)
+    return out
+
+
+def _process_batch_masks(detections, labels, iouv, pred_masks, gt_masks, overlap):
+    """process_batch(masks=True) (utils/metrics.py:239-252): pack, bit-GEMM IoU and matching for one image."""
+    n, nl = detections.shape[0], labels.shape[0]
+    if n == 0 or nl == 0:
+        return torch.zeros(n, iouv.numel(), dtype=torch.bool, device=iouv.device)
+    if not detections.is_cuda:
+        raise RuntimeError("y5b200: process_batch runs on CUDA tensors only (no CPU / PyTorch fallback)")
+    if pred_masks.dim() != 3 or gt_masks.dim() != 3 or pred_masks.shape[0] != n or (not overlap and gt_masks.shape[0] != nl):
+        raise ValueError(f"y5b200: process_batch(masks=True): pred_masks {tuple(pred_masks.shape)}, gt_masks {tuple(gt_masks.shape)} "
+                         f"for {n} detections and {nl} labels (overlap={overlap})")
+    dev = detections.device
+    out_hw = tuple(pred_masks.shape[1:])
+    nonbinary = torch.zeros(1, dtype=torch.int32, device=dev)
+    iou = torch.empty(nl, n, dtype=torch.float32, device=dev)
+    det = detections.float().contiguous()[None]
+    lab = labels.to(dev, torch.float32).contiguous()
+    iv = iouv.to(dev, torch.float32).contiguous()
+    correct = torch.empty(1, n, iv.numel(), dtype=torch.uint8, device=dev)
+    lib = _lib.lib()
+    with _lib.on(dev):
+        g, gp = _pack(gt_masks, gt_masks.shape[1:], out_hw, nl, nonbinary, overlap=overlap)
+        p, pp = _pack(pred_masks, out_hw, out_hw, n, nonbinary)
+        st = C.c_void_p(_lib.stream_ptr(dev))
+        _lib.check(lib.y5_mask_iou(g.data_ptr(), gp.data_ptr(), None, nl, p.data_ptr(), pp.data_ptr(), None, 0, 1, n, g.shape[1], 1e-7,
+                                   iou.data_ptr(), st), "mask_iou")
+        _lib.check(lib.y5_mask_match_batch(det.data_ptr(), det.stride(0), det.stride(1), None, 1, n, lab.data_ptr(), lab.stride(0), None, nl,
+                                           iou.data_ptr(), iv.data_ptr(), iv.numel(), correct.data_ptr(), st), "mask_match_batch")
+    _raise_nonbinary(nonbinary)
+    return correct[0].view(torch.bool).to(iouv.device)
+
+
+def seg_val_batch_metrics(rows, count, protos, targets, masks, im_shape, shapes, iouv, overlap, native=False, check=False):
+    """The metric part of segment/val.py:263-298 for a whole batch, on the device.  rows/count from nms_device(nm=32) (rows
+    (B,max_det,38) in network-input pixels), protos (B,32,mh,mw), targets (nt,6) [img, cls, cx, cy, w, h] in network-input
+    pixels, masks as the reference dataloader yields them: (B,H,W) label indices with `overlap`, else (nt,H,W) 0/1 in
+    target order; im_shape / shapes as val_batch_metrics takes them.  Prediction masks are process_mask (native=True:
+    process_mask_native, --retina-masks) of the network-input boxes, staged as uint8 a chunk of images at a time; gt masks of
+    another size are resized as the reference does.  Returns (predn, correct_bboxes, correct_masks), both (B,max_det,niou)
+    bool, padding rows False.  Nothing is synced unless `check`, which reads the non-binary counter once and raises
+    ValueError when a 0/1 gt mask held another value."""
+    from .segment.general import process_mask_batch
+
+    b, max_det = rows.shape[:2]
+    nt = targets.numel() // 6
+    if protos.dim() != 4 or protos.shape[0] != b or rows.dim() != 3 or rows.shape[2] < 6 + protos.shape[1]:
+        raise ValueError(f"y5b200: seg_val_batch_metrics: rows {tuple(rows.shape)} need 6 + {protos.shape[1] if protos.dim() == 4 else '?'} "
+                         f"columns and protos {tuple(protos.shape)} one entry per image")
+    if masks.dim() != 3 or masks.shape[0] != (b if overlap else nt):
+        raise ValueError(f"y5b200: seg_val_batch_metrics: masks {tuple(masks.shape)} must be ({b if overlap else nt}, H, W) "
+                         f"({'one index image per image' if overlap else 'one mask per target'}, overlap={overlap})")
+    dev = rows.device
+    meta = _meta(im_shape, shapes, dev)
+    predn, correct_bboxes = val_batch_metrics(rows, count, targets, im_shape, meta, iouv)
+    ih, iw = int(im_shape[0]), int(im_shape[1])
+    out_hw = (ih, iw) if native else tuple(protos.shape[-2:])
+    t = targets.to(dev, torch.float32).contiguous().view(-1, 6)
+    iv = iouv.to(dev, torch.float32).contiguous()
+    cnt = count.to(dev, torch.int32).contiguous() if count is not None else None
+    nonbinary = torch.zeros(1, dtype=torch.int32, device=dev)
+    label_index = torch.empty(b + 1 + 2 * nt, dtype=torch.int32, device=dev)
+    iou = torch.empty(nt, max_det, dtype=torch.float32, device=dev)
+    correct = torch.empty(b, max_det, iv.numel(), dtype=torch.uint8, device=dev)
+    lib = _lib.lib()
+    with _lib.on(dev):
+        g, gp = _pack(masks, masks.shape[-2:], out_hw, nt, nonbinary, overlap=overlap, targets=t, batch=b, label_index=label_index)
+        if nt:
+            flat = rows.reshape(b * max_det, rows.shape[2])
+            chunk = max(1, min(b, _STAGE_BYTES // (max_det * out_hw[0] * out_hw[1])))
+            for b0 in range(0, b, chunk):
+                nb = min(chunk, b - b0)
+                r = flat[b0 * max_det:(b0 + nb) * max_det]
+                img = torch.div(torch.arange(nb * max_det, dtype=torch.int32, device=dev), max_det, rounding_mode="floor")
+                pm = process_mask_batch(protos[b0:b0 + nb], r[:, 6:], r[:, :4], img, (ih, iw), out_dtype=torch.uint8, native=native)
+                p, pp = _pack(pm, out_hw, out_hw, nb * max_det, nonbinary)
+                _lib.check(lib.y5_mask_iou(g.data_ptr(), gp.data_ptr(), label_index.data_ptr(), nt, p.data_ptr(), pp.data_ptr(),
+                                           cnt.data_ptr() if cnt is not None else None, b0, nb, max_det, g.shape[1], 1e-7, iou.data_ptr(),
+                                           C.c_void_p(_lib.stream_ptr(dev))), "mask_iou")
+        _lib.check(lib.y5_mask_match_batch(predn.data_ptr(), predn.stride(0), predn.stride(1), cnt.data_ptr() if cnt is not None else None, b,
+                                           max_det, t.data_ptr() + 4 if nt else None, 6, label_index.data_ptr(), nt,
+                                           iou.data_ptr() if nt else None, iv.data_ptr(), iv.numel(), correct.data_ptr(),
+                                           C.c_void_p(_lib.stream_ptr(dev))), "mask_match_batch")
+    if check:
+        _raise_nonbinary(nonbinary)
+    return predn, correct_bboxes, correct.view(torch.bool)
