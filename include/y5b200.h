@@ -454,6 +454,31 @@ int32_t y5_opt_chunk_elems(void);
 int y5_opt_step(const y5_opt_tensor* table, const int32_t* chunk_tensor, const int32_t* chunk_index, int32_t n_chunks,
                 float* hyper, float* partial, int32_t do_step, int32_t do_ema, int32_t zero_grad, void* stream);
 
+/* The same step with Adam / AdamW (utils/torch_utils.py:276-279: torch.optim.Adam(betas=(momentum, 0.999)) or
+ * AdamW(weight_decay=0) plus the two decay groups) in three launches: y5_opt_step's gradient-norm pass, the update, and a tail
+ * that advances the step counters and the EMA counter.  Per parameter with a gradient, after un-scaling and clipping:
+ *   Adam: g += wd*p   AdamW: p *= 1 - lr*wd;   m = lerp(m, g, 1 - b1);  v = v*b2 + (1 - b2)*g*g;  step += 1;
+ *   p += -(lr / (1 - b1^step)) * m / (sqrt(v) / sqrt(1 - b2^step) + eps)
+ * with torch.optim.Adam's order of operations; 1 - b1, 1 - b2, the powers and the two corrections are computed in double and
+ * rounded to fp32 where torch rounds its Python scalars.  A non-finite gradient skips the update (p, m, v and steps unchanged).
+ *   table, chunk_*, hyper, partial  as y5_opt_step (do_step is implied); the per-group block of `hyper` is unused.  table[t].mom
+ *                       points at tensor t's exp_avg, its exp_avg_sq is at exp_avg + sq_offset elements.
+ *   n_tensors           entries of `table`
+ *   group_hyper         DEVICE doubles (a separate argument, so 8-byte aligned by construction): per group g at
+ *                       Y5_ADAM_STRIDE * g: lr, beta1, beta2, eps, weight_decay, decoupled (!= 0: AdamW)
+ *   steps               DEVICE floats, steps[t] = step count of table entry t (torch's fp32 state["step"]); it advances
+ *                       only for entries with a gradient and mom on a step that was not skipped */
+#define Y5_ADAM_LR 0
+#define Y5_ADAM_BETA1 1
+#define Y5_ADAM_BETA2 2
+#define Y5_ADAM_EPS 3
+#define Y5_ADAM_WEIGHT_DECAY 4
+#define Y5_ADAM_DECOUPLED 5
+#define Y5_ADAM_STRIDE 8
+int y5_adam_step(const y5_opt_tensor* table, int32_t n_tensors, const int32_t* chunk_tensor, const int32_t* chunk_index, int32_t n_chunks,
+                 float* hyper, const double* group_hyper, int64_t sq_offset, float* steps, float* partial, int32_t do_ema,
+                 int32_t zero_grad, void* stream);
+
 /* Data-parallel gradient exchange, device half (utils/torch_utils.py:61-70 smart_DDP / train.py:404-414): copy every gradient
  * of `table` (entries with mom != NULL; a NULL grad contributes zeros) into ONE contiguous fp32 arena in a single launch, so the
  * all-reduce is one NCCL call over the arena and y5_opt_step reads the averaged gradients from it (a second table whose grad

@@ -110,6 +110,8 @@ class PackItem(C.Structure):
 
 # indices into the fused optimizer's `hyper` array (include/y5b200.h Y5_OPT_*)
 OPT_INV_SCALE, OPT_MAX_NORM, OPT_EMA_DECAY, OPT_EMA_TAU, OPT_EMA_UPDATES, OPT_OUT_NORM, OPT_OUT_SKIPPED, OPT_GROUPS = 0, 1, 2, 3, 4, 5, 6, 8
+# per-group block of y5_adam_step's fp64 `group_hyper` (include/y5b200.h Y5_ADAM_*)
+ADAM_LR, ADAM_BETA1, ADAM_BETA2, ADAM_EPS, ADAM_WEIGHT_DECAY, ADAM_DECOUPLED, ADAM_STRIDE = 0, 1, 2, 3, 4, 5, 8
 
 _P = C.c_void_p
 _I32, _I64, _F = C.c_int32, C.c_int64, C.c_float
@@ -172,6 +174,7 @@ SIGNATURES = {
     "y5_mask_match_batch": (_I32, [_P, _I64, _I32, _P, _I32, _I32, _P, _I32, _P, _I32, _P, _P, _I32, _P, _P]),
     "y5_opt_chunk_elems": (_I32, []),
     "y5_opt_step": (_I32, [_P, _P, _P, _I32, _P, _P, _I32, _I32, _I32, _P]),
+    "y5_adam_step": (_I32, [_P, _I32, _P, _P, _I32, _P, _P, _I64, _P, _P, _I32, _I32, _P]),
     "y5_grad_pack": (_I32, [_P, _P, _P, _I32, _P, _P, _P, _P]),
     "y5_grad_bind": (_I32, [_P, _I32, _P, _P, _P, _P]),
     "y5_fold_pack": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _I32, _F, _P, _I32, _I32, _P, _I32, _P]),

@@ -7,6 +7,8 @@
 //                  weights (and of the floating-point buffers), gradient zeroing -- one read of g, one read+write of
 //                  p / momentum / ema per element instead of ~10 passes of foreach kernels.  A non-finite gradient skips
 //                  the parameter update (what GradScaler.step does) but still advances the EMA, like the reference.
+// y5_adam_step is the same step with torch.optim.Adam / AdamW (utils/torch_utils.py:276-279) in place of SGD: the same norm
+// pass, one element pass over g / p / exp_avg / exp_avg_sq / ema, and a tail that advances the per-tensor step counters.
 // Hyper-parameters live in DEVICE memory (per-group lr / momentum / weight decay, loss-scale reciprocal, EMA decay
 // constants, update counter), so a captured CUDA graph sees schedule changes without re-capture and never syncs.
 #include <math.h>
@@ -65,12 +67,11 @@ __global__ void __launch_bounds__(kOptThreads) opt_grad_norm_kernel(const y5_opt
     }
 }
 
-__global__ void __launch_bounds__(kOptThreads) opt_step_kernel(const y5_opt_tensor* __restrict__ tab, const int32_t* __restrict__ chunk_tensor,
-                                                               const int32_t* __restrict__ chunk_index, int n_chunks, float* __restrict__ hyper,
-                                                               const float* __restrict__ partial, int do_step, int do_ema, int zero_grad) {
-    __shared__ float sh[kOptThreads / 32];
-    __shared__ float s_coef, s_skip, s_decay;
-    // every block re-reduces the per-chunk partials in the same fixed order: deterministic, no second launch, no atomics
+// The step's scalars, shared by the update kernels: clip coefficient, overflow skip flag and EMA decay.  Every block
+// re-reduces the per-chunk partials in the same fixed order: deterministic, no second launch, no atomics.  Block 0 publishes
+// the norm and the skip flag to `hyper`.  s_coef / s_skip / s_decay are __shared__ and valid after the call.
+__device__ __forceinline__ void opt_step_scalars(float* __restrict__ hyper, const float* __restrict__ partial, int n_chunks, int do_step,
+                                                 float* sh, float& s_coef, float& s_skip, float& s_decay) {
     float acc = 0.f, badf = 0.f;
     if (do_step)
         for (int i = threadIdx.x; i < n_chunks; i += kOptThreads) {
@@ -94,6 +95,14 @@ __global__ void __launch_bounds__(kOptThreads) opt_step_kernel(const y5_opt_tens
         }
     }
     __syncthreads();
+}
+
+__global__ void __launch_bounds__(kOptThreads) opt_step_kernel(const y5_opt_tensor* __restrict__ tab, const int32_t* __restrict__ chunk_tensor,
+                                                               const int32_t* __restrict__ chunk_index, int n_chunks, float* __restrict__ hyper,
+                                                               const float* __restrict__ partial, int do_step, int do_ema, int zero_grad) {
+    __shared__ float sh[kOptThreads / 32];
+    __shared__ float s_coef, s_skip, s_decay;
+    opt_step_scalars(hyper, partial, n_chunks, do_step, sh, s_coef, s_skip, s_decay);
     const y5_opt_tensor t = tab[chunk_tensor[blockIdx.x]];
     const long long e0 = static_cast<long long>(chunk_index[blockIdx.x]) * kOptChunk;
     const long long e1 = min(static_cast<long long>(t.numel), e0 + kOptChunk);
@@ -126,6 +135,77 @@ __global__ void __launch_bounds__(kOptThreads) opt_step_kernel(const y5_opt_tens
 // advances the EMA update counter once per step (separate 1-thread tail so every block of the step kernel reads the same value)
 __global__ void opt_tick_kernel(float* hyper, int do_ema) {
     if (do_ema) hyper[Y5_OPT_EMA_UPDATES] += 1.0f;
+}
+
+// Adam / AdamW (torch.optim.Adam's foreach CUDA path, amsgrad = maximize = False) with the same un-scale, clip, skip and EMA as
+// opt_step_kernel.  exp_avg is t.mom, exp_avg_sq sits `sq_offset` elements behind it; steps[t] is tensor t's step count BEFORE
+// this step (adam_tick_kernel advances it afterwards, so every block of a tensor sees the same count).
+__global__ void __launch_bounds__(kOptThreads) opt_adam_step_kernel(const y5_opt_tensor* __restrict__ tab, const int32_t* __restrict__ chunk_tensor,
+                                                                    const int32_t* __restrict__ chunk_index, int n_chunks, float* __restrict__ hyper,
+                                                                    const double* __restrict__ group_hyper, long long sq_offset,
+                                                                    const float* __restrict__ steps, const float* __restrict__ partial, int do_ema,
+                                                                    int zero_grad) {
+    __shared__ float sh[kOptThreads / 32];
+    __shared__ float s_coef, s_skip, s_decay;
+    __shared__ float s_step_size, s_bc2_sqrt, s_w1, s_beta2, s_w2, s_eps, s_wd_mul, s_wd_add;
+    const int ti = chunk_tensor[blockIdx.x];
+    const y5_opt_tensor t = tab[ti];
+    if (threadIdx.x == 0 && t.mom) {
+        // torch computes these in Python doubles and hands fp32 scalars to its kernels: same doubles, same rounding points
+        const double* h = group_hyper + Y5_ADAM_STRIDE * t.group;
+        const double lr = h[Y5_ADAM_LR], b1 = h[Y5_ADAM_BETA1], b2 = h[Y5_ADAM_BETA2], wd = h[Y5_ADAM_WEIGHT_DECAY];
+        const double step = static_cast<double>(steps[ti] + 1.0f);  // state["step"] += 1 (fp32), then step.item()
+        s_step_size = static_cast<float>(-(lr / (1.0 - pow(b1, step))));
+        s_bc2_sqrt = static_cast<float>(sqrt(1.0 - pow(b2, step)));
+        s_w1 = static_cast<float>(1.0 - b1);
+        s_beta2 = static_cast<float>(b2);
+        s_w2 = static_cast<float>(1.0 - b2);
+        s_eps = static_cast<float>(h[Y5_ADAM_EPS]);
+        const bool decoupled = h[Y5_ADAM_DECOUPLED] != 0.0;
+        s_wd_mul = decoupled ? static_cast<float>(1.0 - lr * wd) : 1.0f;  // AdamW: p.mul_(1 - lr * weight_decay)
+        s_wd_add = decoupled ? 0.0f : static_cast<float>(wd);              // Adam:  grad = grad.add(p, alpha=weight_decay)
+    }
+    opt_step_scalars(hyper, partial, n_chunks, 1, sh, s_coef, s_skip, s_decay);  // ends with __syncthreads
+    const long long e0 = static_cast<long long>(chunk_index[blockIdx.x]) * kOptChunk;
+    const long long e1 = min(static_cast<long long>(t.numel), e0 + kOptChunk);
+    const bool step = t.grad && t.mom && s_skip == 0.f;
+    const float gscale = hyper[Y5_OPT_INV_SCALE] * s_coef;
+    const float d = s_decay;
+    const float step_size = s_step_size, bc2_sqrt = s_bc2_sqrt, w1 = s_w1, beta2 = s_beta2, w2 = s_w2, eps = s_eps;
+    const float wd_mul = s_wd_mul, wd_add = s_wd_add;
+    float* p = static_cast<float*>(t.param);
+    float* g = static_cast<float*>(t.grad);
+    float* m = static_cast<float*>(t.mom);
+    float* v = m + sq_offset;
+    float* e = static_cast<float*>(t.ema);
+    for (long long i = e0 + threadIdx.x; i < e1; i += kOptThreads) {
+        float w = p[i];
+        if (step) {
+            float gi = g[i] * gscale;
+            w *= wd_mul;
+            if (wd_add != 0.f) gi = fmaf(wd_add, w, gi);
+            float mi = m[i];
+            const float dm = gi - mi;
+            mi = w1 < 0.5f ? fmaf(w1, dm, mi) : fmaf(-dm, 1.0f - w1, gi);  // torch's lerp(m, g, 1 - beta1)
+            const float vi = fmaf(w2, gi * gi, v[i] * beta2);              // v.mul_(beta2).addcmul_(g, g, value=1 - beta2)
+            const float den = sqrtf(vi) / bc2_sqrt + eps;                  // (v.sqrt() / sqrt(bc2)).add_(eps)
+            w = fmaf(step_size, mi / den, w);                              // p.addcdiv_(m, den, value=-lr / bc1)
+            m[i] = mi;
+            v[i] = vi;
+            p[i] = w;
+        }
+        if (g && zero_grad) g[i] = 0.f;
+        if (do_ema && e) e[i] = fmaf(d, e[i], (1.0f - d) * w);
+    }
+}
+
+// the Adam step's tail: tensor t's step count advances when it had a gradient and the step was not skipped; the EMA counter
+// advances like opt_tick_kernel's
+__global__ void adam_tick_kernel(const y5_opt_tensor* __restrict__ tab, int n_tensors, float* __restrict__ steps, float* __restrict__ hyper,
+                                 int do_ema) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n_tensors && tab[t].grad && tab[t].mom && hyper[Y5_OPT_OUT_SKIPPED] == 0.f) steps[t] += 1.0f;
+    if (t == 0 && do_ema) hyper[Y5_OPT_EMA_UPDATES] += 1.0f;
 }
 
 // Data-parallel gradient exchange, device side (reference utils/torch_utils.py:61-70 wraps the model in DistributedDataParallel;
@@ -180,6 +260,24 @@ extern "C" Y5_API int y5_opt_step(const y5_opt_tensor* table, const int32_t* chu
     count_launch(do_step ? 3 : 2);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(int(e), "opt_step launch failed: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+extern "C" Y5_API int y5_adam_step(const y5_opt_tensor* table, int32_t n_tensors, const int32_t* chunk_tensor, const int32_t* chunk_index,
+                                   int32_t n_chunks, float* hyper, const double* group_hyper, int64_t sq_offset, float* steps, float* partial,
+                                   int32_t do_ema, int32_t zero_grad, void* stream) {
+    if (n_chunks <= 0) return 0;
+    if (!table || !chunk_tensor || !chunk_index || !hyper || !group_hyper || !steps || !partial)
+        return set_error(Y5_E_INVALID, "adam_step: null pointer");
+    if (n_tensors <= 0 || sq_offset < 0) return set_error(Y5_E_INVALID, "adam_step: n_tensors %d, sq_offset %lld", n_tensors, (long long)sq_offset);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    opt_grad_norm_kernel<<<n_chunks, kOptThreads, 0, st>>>(table, chunk_tensor, chunk_index, hyper, partial);
+    opt_adam_step_kernel<<<n_chunks, kOptThreads, 0, st>>>(table, chunk_tensor, chunk_index, n_chunks, hyper, group_hyper, sq_offset, steps,
+                                                           partial, do_ema, zero_grad);
+    adam_tick_kernel<<<(n_tensors + 255) / 256, 256, 0, st>>>(table, n_tensors, steps, hyper, do_ema);
+    count_launch(3);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(int(e), "adam_step launch failed: %s", cudaGetErrorString(e));
     return 0;
 }
 

@@ -149,24 +149,14 @@ class ModelEMA:
         copy_attr(self.ema, model, include, exclude)
 
 
-class FusedSGD(torch.optim.Optimizer):
-    """SGD with momentum / Nesterov over parameter groups (what reference smart_optimizer builds, utils/torch_utils.py:256-289)
-    whose whole step -- GradScaler un-scale, clip_grad_norm_, weight decay, momentum, update, zero_grad and optionally
-    ModelEMA.update (reference train.py:413-421) -- is two multi-tensor launches of liby5b200 (y5_opt_step).
+class _FusedOptimizer(torch.optim.Optimizer):
+    """What FusedSGD and FusedAdam share: the device tables of every parameter (+ the EMA's tensors), the data-parallel
+    gradient arena, the device-side GradScaler handling, the per-step hyper-parameter upload and the step's device outputs.
+    A subclass owns its state buffers (`_bind_state`), its per-group hyper-parameters (`_fill_groups` / `_upload_groups`), the
+    update launch (`_launch`) and `zero_state`."""
 
-    `param_groups` carry lr / momentum / weight_decay / nesterov exactly like torch.optim.SGD, so LambdaLR schedulers and the
-    warm-up code that edits them (train.py:368-376) work unchanged; their values are uploaded each step (a captured CUDA graph
-    replays that upload, so schedules keep working under GraphedTrainStep).  Gradients are read where autograd left them
-    (`zero_grad(set_to_none=True)` semantics: no extra accumulate kernels); only their addresses are refreshed per step.
-
-        opt.fused_step(scaler=scaler, max_norm=10.0, ema=ema)     # == train.py:413-421
-        opt.step()                                                # plain optimizer.step() (no clipping / scaling / EMA)
-    """
-
-    def __init__(self, params, lr=1e-3, momentum=0.0, weight_decay=0.0, nesterov=False):
-        if nesterov and momentum <= 0:
-            raise ValueError("Nesterov momentum requires a momentum")
-        super().__init__(params, dict(lr=lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov))
+    def __init__(self, params, defaults):
+        super().__init__(params, defaults)
         self._tab = None
         self._tab_key = None
         self._dp = None  # (process group, world size) once data_parallel() was called
@@ -182,10 +172,11 @@ class FusedSGD(torch.optim.Optimizer):
         reference does not use SyncBatchNorm unless asked)."""
         import torch.distributed as dist
 
+        name = type(self).__name__
         if not (dist.is_available() and dist.is_initialized()):
-            raise RuntimeError("y5b200: FusedSGD.data_parallel needs an initialised torch.distributed process group")
+            raise RuntimeError(f"y5b200: {name}.data_parallel needs an initialised torch.distributed process group")
         if isinstance(model, (nn.parallel.DataParallel, nn.parallel.DistributedDataParallel)):
-            raise TypeError("y5b200: pass the plain module to FusedSGD.data_parallel (DistributedDataParallel would all-reduce a second time)")
+            raise TypeError(f"y5b200: pass the plain module to {name}.data_parallel (DistributedDataParallel would all-reduce a second time)")
         world = dist.get_world_size(process_group)
         with torch.no_grad():
             for t in list(model.parameters()) + list(model.buffers()):
@@ -205,25 +196,15 @@ class FusedSGD(torch.optim.Optimizer):
             return
         dev = ps[0][1].device
         if not ps[0][1].is_cuda:
-            raise RuntimeError("y5b200: FusedSGD runs on CUDA parameters only (no CPU / PyTorch fallback)")
-        total = sum(p.numel() for _, p in ps)
-        flat_m = torch.zeros(total, dtype=torch.float32, device=dev)  # momentum buffers: one allocation, fixed addresses
+            raise RuntimeError(f"y5b200: {type(self).__name__} runs on CUDA parameters only (no CPU / PyTorch fallback)")
         ema_pairs = ema.pairs(model) if ema is not None else []
         ema_of = {m_t.data_ptr(): e_t for m_t, e_t in ema_pairs}
-        off, entries = 0, []
-        for gi, p in ps:
-            n = p.numel()
-            st = self.state[p]
-            m = flat_m[off : off + n].view_as(p)
-            if st.get("momentum_buffer") is not None:
-                m.copy_(st["momentum_buffer"])
-            st["momentum_buffer"] = m
-            entries.append((p.detach(), m, ema_of.get(p.data_ptr()), gi))
-            off += n
         seen = {p.data_ptr() for _, p in ps}
-        for m_t, e_t in ema_pairs:  # floating-point buffers (BN running statistics) take part in the EMA only
-            if m_t.data_ptr() not in seen:
-                entries.append((m_t.detach(), None, e_t, 0))
+        buffers = [(m_t, e_t) for m_t, e_t in ema_pairs if m_t.data_ptr() not in seen]  # BN running statistics: EMA only
+        self._plist = [p for _, p in ps]
+        moms = self._bind_state(ps, len(ps) + len(buffers), dev)
+        entries = [(p.detach(), m, ema_of.get(p.data_ptr()), gi) for (gi, p), m in zip(ps, moms)]
+        entries += [(m_t.detach(), None, e_t, 0) for m_t, e_t in buffers]
         self._tab = _OptTable(entries, dev)
         self._tab_arena = None
         if self._dp is not None:
@@ -243,41 +224,36 @@ class FusedSGD(torch.optim.Optimizer):
             self._tab_arena.set_grads([self._arena.data_ptr() + 4 * off if e[1] is not None else 0 for e, off in zip(entries, offs)])
             self._tab_arena.upload()
         self._tab_key = key
-        self._plist = [p for _, p in ps]
-        self._flat_m = flat_m
-        n_groups = len(self.param_groups)
-        self._hyper = torch.zeros(_lib.OPT_GROUPS + 4 * n_groups, dtype=torch.float32, device=dev)
-        self._hyper_host = torch.zeros(_lib.OPT_GROUPS + 4 * n_groups, dtype=torch.float32).pin_memory()
+        n = _lib.OPT_GROUPS + self._GROUP_FLOATS * len(self.param_groups)
+        self._hyper = torch.zeros(n, dtype=torch.float32, device=dev)
+        self._hyper_host = torch.zeros(n, dtype=torch.float32).pin_memory()
         self._hyper[_lib.OPT_INV_SCALE] = 1.0
         if ema is not None:
             ema.hyper_init(self._hyper)
 
     def fill_hyper_host(self, max_norm):
-        """Write lr / momentum / weight decay / nesterov of every group and the clip norm into the pinned staging buffer."""
-        h = self._hyper_host
-        h[_lib.OPT_MAX_NORM] = float(max_norm) if max_norm else 0.0
-        for gi, g in enumerate(self.param_groups):
-            o = _lib.OPT_GROUPS + 4 * gi
-            h[o], h[o + 1], h[o + 2], h[o + 3] = g["lr"], g["momentum"], g["weight_decay"], 1.0 if g["nesterov"] else 0.0
+        """Write the clip norm and every group's hyper-parameters into the pinned staging buffers."""
+        self._hyper_host[_lib.OPT_MAX_NORM] = float(max_norm) if max_norm else 0.0
+        self._fill_groups()
 
     def _upload_hyper(self, max_norm):
         self.fill_hyper_host(max_norm)
         h = self._hyper_host
         self._hyper[_lib.OPT_MAX_NORM : _lib.OPT_MAX_NORM + 1].copy_(h[_lib.OPT_MAX_NORM : _lib.OPT_MAX_NORM + 1], non_blocking=True)
-        self._hyper[_lib.OPT_GROUPS :].copy_(h[_lib.OPT_GROUPS :], non_blocking=True)
+        self._upload_groups()
 
     # ------------------------------------------------------------------ steps
     @torch.no_grad()
     def fused_step(self, scaler=None, max_norm=10.0, ema=None, model=None):
-        """train.py:413-421 (minus zero_grad) in one call: un-scale by `scaler`'s current factor, clip to `max_norm`, SGD update
-        of every parameter that has a gradient, and -- with `ema` (+ the `model` it tracks) -- ModelEMA.update.  `scaler` is a
+        """train.py:413-421 (minus zero_grad) in one call: un-scale by `scaler`'s current factor, clip to `max_norm`, update
+        every parameter that has a gradient, and -- with `ema` (+ the `model` it tracks) -- ModelEMA.update.  `scaler` is a
         torch GradScaler: its scale is read, and its growth / back-off state advanced, on the device (what scaler.step +
         scaler.update do, without their host synchronisation); a non-finite gradient skips the update.  `last_grad_norm` /
         `last_step_skipped` read the device-side results (they synchronise)."""
         if ema is not None and model is None:
             model = getattr(self, "_ema_model", None)
             if model is None:
-                raise ValueError("FusedSGD.fused_step(ema=...) needs model= (the module the EMA tracks)")
+                raise ValueError(f"{type(self).__name__}.fused_step(ema=...) needs model= (the module the EMA tracks)")
         self._ema_model = model
         self._ensure(ema, model)
         dev = self._hyper.device
@@ -286,7 +262,7 @@ class FusedSGD(torch.optim.Optimizer):
         t.set_grads([p.grad.data_ptr() if p.grad is not None else 0 for p in self._plist])
         for p in self._plist:
             if p.grad is not None and (p.grad.dtype != torch.float32 or not p.grad.is_contiguous()):
-                raise TypeError("y5b200: FusedSGD needs contiguous fp32 gradients")
+                raise TypeError(f"y5b200: {type(self).__name__} needs contiguous fp32 gradients")
         t.upload()
         use_scaler = scaler is not None and scaler.is_enabled() and getattr(scaler, "_scale", None) is not None
         if use_scaler:
@@ -305,9 +281,7 @@ class FusedSGD(torch.optim.Optimizer):
                 _lib.check(_lib.lib().y5_grad_bind(t.table.data_ptr(), len(t.keep), self._arena_off.data_ptr(), self._arena.data_ptr(),
                                                    self._present.data_ptr(), C.c_void_p(_lib.stream_ptr(dev))), "grad_bind")
         with _lib.on(dev):
-            _lib.check(_lib.lib().y5_opt_step(t.table.data_ptr(), t.chunk_tensor.data_ptr(), t.chunk_index.data_ptr(), t.n_chunks,
-                                              self._hyper.data_ptr(), t.partial.data_ptr(), 1, 1 if ema is not None else 0, 0,
-                                              C.c_void_p(_lib.stream_ptr(dev))), "opt_step")
+            self._launch(t, 1 if ema is not None else 0, C.c_void_p(_lib.stream_ptr(dev)))
         if ema is not None:
             ema.updates += 1
         if use_scaler:  # what scaler.update() does after scaler.step(): back off on overflow, grow after growth_interval clean steps
@@ -316,7 +290,7 @@ class FusedSGD(torch.optim.Optimizer):
 
     @torch.no_grad()
     def step(self, closure=None):
-        """Plain optimizer.step(): SGD update only (no un-scaling, clipping or EMA), for code that drives those itself."""
+        """Plain optimizer.step(): the update only (no un-scaling, clipping or EMA), for code that drives those itself."""
         loss = None
         if closure is not None:
             with torch.enable_grad():
@@ -333,11 +307,171 @@ class FusedSGD(torch.optim.Optimizer):
         return bool(self._hyper[_lib.OPT_OUT_SKIPPED] != 0)
 
 
+class FusedSGD(_FusedOptimizer):
+    """SGD with momentum / Nesterov over parameter groups (what reference smart_optimizer builds, utils/torch_utils.py:256-289)
+    whose whole step -- GradScaler un-scale, clip_grad_norm_, weight decay, momentum, update, zero_grad and optionally
+    ModelEMA.update (reference train.py:413-421) -- is two multi-tensor launches of liby5b200 (y5_opt_step).
+
+    `param_groups` carry lr / momentum / weight_decay / nesterov exactly like torch.optim.SGD, so LambdaLR schedulers and the
+    warm-up code that edits them (train.py:368-376) work unchanged; their values are uploaded each step (a captured CUDA graph
+    replays that upload, so schedules keep working under GraphedTrainStep).  Gradients are read where autograd left them
+    (`zero_grad(set_to_none=True)` semantics: no extra accumulate kernels); only their addresses are refreshed per step.
+
+        opt.fused_step(scaler=scaler, max_norm=10.0, ema=ema)     # == train.py:413-421
+        opt.step()                                                # plain optimizer.step() (no clipping / scaling / EMA)
+    """
+
+    _GROUP_FLOATS = 4  # lr, momentum, weight_decay, nesterov at Y5_OPT_GROUPS + 4g of `hyper`
+
+    def __init__(self, params, lr=1e-3, momentum=0.0, weight_decay=0.0, nesterov=False):
+        if nesterov and momentum <= 0:
+            raise ValueError("Nesterov momentum requires a momentum")
+        super().__init__(params, dict(lr=lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov))
+
+    def _bind_state(self, ps, n_entries, dev):
+        total = sum(p.numel() for _, p in ps)
+        flat_m = torch.zeros(total, dtype=torch.float32, device=dev)  # momentum buffers: one allocation, fixed addresses
+        off, moms = 0, []
+        for _, p in ps:
+            n = p.numel()
+            st = self.state[p]
+            m = flat_m[off : off + n].view_as(p)
+            if st.get("momentum_buffer") is not None:
+                m.copy_(st["momentum_buffer"])
+            st["momentum_buffer"] = m
+            moms.append(m)
+            off += n
+        self._flat_m = flat_m
+        return moms
+
+    def _fill_groups(self):
+        h = self._hyper_host
+        for gi, g in enumerate(self.param_groups):
+            o = _lib.OPT_GROUPS + 4 * gi
+            h[o], h[o + 1], h[o + 2], h[o + 3] = g["lr"], g["momentum"], g["weight_decay"], 1.0 if g["nesterov"] else 0.0
+
+    def _upload_groups(self):
+        self._hyper[_lib.OPT_GROUPS :].copy_(self._hyper_host[_lib.OPT_GROUPS :], non_blocking=True)
+
+    def _launch(self, t, do_ema, stream):
+        _lib.check(_lib.lib().y5_opt_step(t.table.data_ptr(), t.chunk_tensor.data_ptr(), t.chunk_index.data_ptr(), t.n_chunks,
+                                          self._hyper.data_ptr(), t.partial.data_ptr(), 1, do_ema, 0, stream), "opt_step")
+
+    def zero_state(self):
+        """Zero the momentum buffers in place (their device addresses, which a captured graph holds, stay)."""
+        self._flat_m.zero_()
+
+
+class FusedAdam(_FusedOptimizer):
+    """torch.optim.Adam (decoupled_weight_decay=False) or AdamW (True) over parameter groups -- what reference smart_optimizer
+    builds for `--optimizer Adam | AdamW` (utils/torch_utils.py:276-279) -- with the same fused train.py:413-421 step as
+    FusedSGD: three multi-tensor launches of liby5b200 (y5_adam_step).  The arithmetic is torch's foreach CUDA path, with the
+    bias corrections computed in double like torch's Python scalars; amsgrad and maximize are not implemented.
+
+    `param_groups` carry torch.optim.Adam's keys and no `momentum` (train.py's warm-up leaves the betas alone, as it does for the
+    reference); lr / betas / eps / weight_decay are uploaded each step, also under GraphedTrainStep.  Each parameter's step
+    count is an fp32 counter on the device that advances when the parameter had a gradient and the step was not skipped; it is
+    never read back while training.  `state_dict()` / `load_state_dict()` use torch's Adam format (`step` a 0-d fp32 CPU
+    tensor, `exp_avg`, `exp_avg_sq`), so optimizer states move both ways between this class and torch.optim.Adam / AdamW."""
+
+    _GROUP_FLOATS = 0  # the per-group block is y5_adam_step's fp64 `group_hyper`
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *, maximize=False,
+                 decoupled_weight_decay=False):
+        if amsgrad:
+            raise NotImplementedError("y5b200: Adam(amsgrad=True) is outside the fused optimizer (reference smart_optimizer never sets it)")
+        if maximize:
+            raise NotImplementedError("y5b200: Adam(maximize=True) is outside the fused optimizer (reference smart_optimizer never sets it)")
+        if not 0.0 <= lr or not 0.0 <= eps or not 0.0 <= weight_decay or not all(0.0 <= b < 1.0 for b in betas):
+            raise ValueError(f"invalid Adam hyper-parameters lr={lr} betas={betas} eps={eps} weight_decay={weight_decay}")
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, amsgrad=False, maximize=False, foreach=None,
+                                      capturable=False, differentiable=False, fused=None, decoupled_weight_decay=decoupled_weight_decay))
+
+    def add_param_group(self, param_group):
+        for k in ("amsgrad", "maximize"):
+            if param_group.get(k):
+                raise NotImplementedError(f"y5b200: Adam({k}=True) is outside the fused optimizer")
+        super().add_param_group(param_group)
+
+    def _bind_state(self, ps, n_entries, dev):
+        self._total = sum(p.numel() for _, p in ps)
+        self._flat = torch.zeros(2 * self._total, dtype=torch.float32, device=dev)  # [exp_avg | exp_avg_sq]: fixed addresses
+        self._steps = torch.zeros(n_entries, dtype=torch.float32, device=dev)       # step count per table entry
+        n_groups = len(self.param_groups)
+        self._ghyper = torch.zeros(_lib.ADAM_STRIDE * n_groups, dtype=torch.float64, device=dev)
+        self._ghyper_host = torch.zeros(_lib.ADAM_STRIDE * n_groups, dtype=torch.float64).pin_memory()
+        self._adopt_state()
+        return [self.state[p]["exp_avg"] for p in self._plist]
+
+    def _adopt_state(self):
+        """Move every parameter's state (fresh, loaded from a state_dict, or already ours) into the flat device buffers and
+        point `state` at them: exp_avg / exp_avg_sq views and `step` a 0-d view of the device counter."""
+        steps, off = [], 0
+        for i, p in enumerate(self._plist):
+            n = p.numel()
+            st = self.state[p]
+            m = self._flat[off : off + n].view_as(p)
+            v = self._flat[self._total + off : self._total + off + n].view_as(p)
+            for key, buf in (("exp_avg", m), ("exp_avg_sq", v)):
+                if st.get(key) is not None:
+                    buf.copy_(st[key])
+                else:
+                    buf.zero_()
+            steps.append(float(st["step"]) if "step" in st else 0.0)
+            st["exp_avg"], st["exp_avg_sq"], st["step"] = m, v, self._steps[i]
+            off += n
+        self._steps[: len(steps)].copy_(torch.tensor(steps, dtype=torch.float32))
+
+    def load_state_dict(self, state_dict):
+        super().load_state_dict(state_dict)
+        if self._tab is not None:  # the tables hold the flat buffers' addresses: copy the loaded state into them
+            self._adopt_state()
+
+    def state_dict(self):
+        sd = super().state_dict()
+        if self._tab is not None:  # torch's format: `step` as a 0-d fp32 CPU tensor (one device-to-host copy for all)
+            host = self._steps.cpu()
+            row = {id(p): i for i, p in enumerate(self._plist)}
+            flat = [p for g in self.param_groups for p in g["params"]]
+            sd["state"] = {k: dict(st, step=host[row[id(flat[k])]].clone()) if id(flat[k]) in row else st for k, st in sd["state"].items()}
+        return sd
+
+    def _fill_groups(self):
+        h = self._ghyper_host
+        for gi, g in enumerate(self.param_groups):
+            o = _lib.ADAM_STRIDE * gi
+            h[o + _lib.ADAM_LR], h[o + _lib.ADAM_EPS], h[o + _lib.ADAM_WEIGHT_DECAY] = g["lr"], g["eps"], g["weight_decay"]
+            h[o + _lib.ADAM_BETA1], h[o + _lib.ADAM_BETA2] = g["betas"]
+            h[o + _lib.ADAM_DECOUPLED] = 1.0 if g["decoupled_weight_decay"] else 0.0
+
+    def _upload_groups(self):
+        self._ghyper.copy_(self._ghyper_host, non_blocking=True)
+
+    def _launch(self, t, do_ema, stream):
+        _lib.check(_lib.lib().y5_adam_step(t.table.data_ptr(), len(t.keep), t.chunk_tensor.data_ptr(), t.chunk_index.data_ptr(), t.n_chunks,
+                                           self._hyper.data_ptr(), self._ghyper.data_ptr(), self._total, self._steps.data_ptr(),
+                                           t.partial.data_ptr(), do_ema, 0, stream), "adam_step")
+
+    def zero_state(self):
+        """Zero both moments and the step counters in place (their device addresses, which a captured graph holds, stay): the
+        next step is step 1 with the full bias correction."""
+        self._flat.zero_()
+        self._steps.zero_()
+
+
+class FusedAdamW(FusedAdam):
+    """torch.optim.AdamW on the fused step: FusedAdam with decoupled weight decay and AdamW's default weight_decay=1e-2."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, amsgrad=False, *, maximize=False):
+        super().__init__(params, lr, betas, eps, weight_decay, amsgrad, maximize=maximize, decoupled_weight_decay=True)
+
+
 def smart_optimizer(model, name="Adam", lr=0.001, momentum=0.9, decay=1e-5):
     """Three parameter groups like reference utils/torch_utils.py:256-289 -- biases (no decay), BatchNorm weights (no decay),
-    other weights (decay) -- on the fused SGD-Nesterov step.  Only SGD is on this path (the reference's default optimizer)."""
-    if name != "SGD":
-        raise NotImplementedError(f"y5b200: optimizer {name} is outside the hot path (train.py defaults to SGD)")
+    other weights (decay) -- on the fused step: SGD-Nesterov, Adam(betas=(momentum, 0.999)) or AdamW(betas=(momentum, 0.999),
+    weight_decay=0 for the bias group).  RMSProp (not offered by train.py's --optimizer) is not implemented."""
+    if name not in ("SGD", "Adam", "AdamW"):
+        raise NotImplementedError(f"y5b200: optimizer {name} is outside the hot path (train.py offers SGD, Adam and AdamW)")
     g = [], [], []
     for v in model.modules():
         for p_name, p in v.named_parameters(recurse=False):
@@ -347,7 +481,12 @@ def smart_optimizer(model, name="Adam", lr=0.001, momentum=0.9, decay=1e-5):
                 g[1].append(p)
             else:
                 g[0].append(p)
-    opt = FusedSGD(g[2], lr=lr, momentum=momentum, nesterov=True)
+    if name == "Adam":
+        opt = FusedAdam(g[2], lr=lr, betas=(momentum, 0.999))
+    elif name == "AdamW":
+        opt = FusedAdamW(g[2], lr=lr, betas=(momentum, 0.999), weight_decay=0.0)
+    else:
+        opt = FusedSGD(g[2], lr=lr, momentum=momentum, nesterov=True)
     opt.add_param_group({"params": g[0], "weight_decay": decay})
     opt.add_param_group({"params": g[1], "weight_decay": 0.0})
     return opt
@@ -355,13 +494,13 @@ def smart_optimizer(model, name="Adam", lr=0.001, momentum=0.9, decay=1e-5):
 
 class GraphedTrainStep:
     """One optimisation step -- forward (batch-statistics BN), ComputeLoss, scaled backward, un-scale + gradient clipping +
-    SGD + zero_grad + EMA (reference train.py:401-421) -- captured once in a CUDA graph and replayed per batch.
+    SGD / Adam / AdamW + zero_grad + EMA (reference train.py:401-421) -- captured once in a CUDA graph and replayed per batch.
 
     The training path never synchronises with the host, so the whole step is capturable; replaying it removes the Python /
     launch-issue time that bounds the eager step.  Numerically it is the reference's AMP recipe: with fp16 autocast the loss
     is multiplied by a dynamic loss scale kept ON THE DEVICE (GradScaler semantics: init 65536, x0.5 on overflow with the step
     skipped, x2 after 2000 clean steps -- y5_opt_step reports overflow, torch._amp_update_scale_ advances the scale, both
-    inside the graph); bf16 autocast needs no scaling.  Learning rate / momentum / weight decay are re-read from
+    inside the graph); bf16 autocast needs no scaling.  The optimizer's group hyper-parameters (lr, momentum or betas, ...) are re-read from
     `optimizer.param_groups` at every call (uploaded through a pinned buffer the captured copy node reads at replay time), so
     warm-up and schedulers work.  Shapes are fixed at construction: `batch` uint8 images of `size` and up to `max_targets`
     label rows; shorter label tensors are padded with zero-size boxes, which build_targets can never match (the anchor ratio
@@ -378,8 +517,8 @@ class GraphedTrainStep:
 
     def __init__(self, model, compute_loss, optimizer, batch: int, size, max_targets: int | None = None, amp_dtype=torch.float16,
                  max_norm: float | None = 10.0, warmup_steps: int = 3, ema=None, init_scale: float = 65536.0):
-        if not isinstance(optimizer, FusedSGD):
-            raise TypeError("GraphedTrainStep needs the fused optimizer (yolov5_b200.utils.torch_utils.smart_optimizer / FusedSGD): its "
+        if not isinstance(optimizer, _FusedOptimizer):
+            raise TypeError("GraphedTrainStep needs a fused optimizer (yolov5_b200.utils.torch_utils.smart_optimizer / FusedSGD / FusedAdam): its "
                             "overflow-skipping step is what makes the loss-scaled update capturable")
         dev = next(model.parameters()).device
         h, w = (size, size) if isinstance(size, int) else size
@@ -440,9 +579,9 @@ class GraphedTrainStep:
         self._arena_buf = train_ops._arena.buf
         self._pack_plans = list(model.__dict__.get("_y5_pack_plans", {}).values())  # persistent packed-weight buffers + tables
         # undo what warm-up and capture touched: weights are unchanged (lr 0 / capture does not execute), BN running statistics
-        # and batch counters, momentum buffers, the EMA and its counter, the loss scale
+        # and batch counters, the optimizer state (momentum / moments and step counts), the EMA and its counter, the loss scale
         model.load_state_dict(state)
-        optimizer._flat_m.zero_()
+        optimizer.zero_state()
         if ema is not None:
             ema.ema.load_state_dict(ema_state)
             ema.updates = ema_updates
