@@ -500,6 +500,61 @@ int y5_fold_pack(const void* w, int32_t w_dtype, int32_t out_c, int32_t in_c, in
                  const void* gamma, const void* beta, const void* mean, const void* var, int32_t bn_dtype, float eps,
                  void* packed, int32_t in_c_pad, int32_t out_c_pad, float* bias_out, int32_t dtype, void* stream);
 
+/* Training augmentation (utils/dataloaders.py:696-855 __getitem__ / load_mosaic, utils/augmentations.py:69-82 augment_hsv,
+ * :118-197 random_perspective (affine), :225-233 mixup) for a batch, byte-exact with the reference's OpenCV arithmetic
+ * (oracle/aug_ref.py).  The host draws every random number; the device table below carries the result.
+ * A "mosaic" is a virtual canvas (canvas_w x canvas_h, 114 outside its tiles) made of up to 4 tiles: canvas pixel
+ * (x, y) inside tile t's rectangle [x1a, x2a) x [y1a, y2a) reads src + (y + dy) * row_bytes + (x + dx) * pixel_stride
+ * + channel * channel_stride (BGR channel order).  An output image is warp(mosaic 0), or with mixup
+ * trunc(warp(mosaic 0) * mix_r + warp(mosaic 1) * (1 - mix_r)), then the three HSV LUTs, then the flips.
+ * (Declared as struct + typedef; tests/test_augment_cpu.py checks their layout against the ctypes mirrors.) */
+struct y5_aug_tile {
+    const void* src;                /* uint8, device memory */
+    int32_t row_bytes, pixel_stride, channel_stride;
+    int32_t x1a, y1a, x2a, y2a;     /* rectangle on the canvas */
+    int32_t dx, dy;                 /* source pixel = canvas pixel + (dx, dy) */
+    int32_t reserved;
+};
+typedef struct y5_aug_tile y5_aug_tile;
+struct y5_aug_image {
+    double inv_m[2][6];     /* cv2.invertAffineTransform(M[:2]) per mosaic, row-major */
+    double m[2][6];         /* M[:2] per mosaic (labels) */
+    double mix_r;           /* mixup ratio r, used when n_mosaic == 2 */
+    float scale[2];         /* random_perspective's scale draw per mosaic (box_candidates) */
+    float clip_max;         /* load_mosaic's label clip bound 2*s (labels with Y5_AUG_CLIP) */
+    int32_t n_mosaic;       /* 1, or 2 with mixup */
+    int32_t n_tiles[2];     /* tiles [0, n_tiles[0]) belong to mosaic 0, [4, 4 + n_tiles[1]) to mosaic 1 */
+    int32_t canvas_w, canvas_h;
+    int32_t warp[2];        /* 0: M == I, the canvas is the image (random_perspective skips cv2.warpAffine) */
+    int32_t hsv, flipud, fliplr;
+    int32_t reserved;
+    y5_aug_tile tiles[8];
+    uint8_t lut[3][256];    /* hue, saturation, value LUTs (augment_hsv), used when hsv != 0 */
+};
+typedef struct y5_aug_image y5_aug_image;
+/* One input label row and its path to the output.  flags: Y5_AUG_CLIP clips the xyxy box to [0, clip_max] (load_mosaic);
+ * Y5_AUG_IN_XYXY: (x, y, w, h) already hold pixel x1, y1, x2, y2 (tile_w ... pad_h unused); Y5_AUG_OUT_XYXY: write the
+ * warped pixel xyxy box (random_perspective's return) instead of xyxy2xywhn(clip=True, eps=1e-3) + flips. */
+#define Y5_AUG_CLIP 1
+#define Y5_AUG_IN_XYXY 2
+#define Y5_AUG_OUT_XYXY 4
+struct y5_aug_label {
+    float cls, x, y, w, h;                  /* normalised xywh, float32 as the dataset stores it */
+    float tile_w, tile_h, pad_w, pad_h;     /* xywhn2xyxy's w, h, padw, padh, already rounded to float32 */
+    int32_t image, mosaic, flags;
+};
+typedef struct y5_aug_label y5_aug_label;
+/* out: (n, 3, out_h, out_w) Y5_U8 | Y5_F16 | Y5_BF16 | Y5_F32 (/255), RGB when swap_rb (BGR otherwise); s2d != 0
+ * (fp16/bf16, even sizes) writes the stem's space-to-depth cells instead (layout and out_row_px/out_x_off as in
+ * y5_stem_s2d).  hsv_simd_cols: columns [0, hsv_simd_cols) of a row truncate in HSV->BGR, the rest round (cv2's SIMD
+ * blocks and scalar tail: out_w - out_w % 32).  `table` is DEVICE memory. */
+int y5_aug_gather(const y5_aug_image* table, int32_t n_images, int32_t out_h, int32_t out_w, int32_t hsv_simd_cols, int32_t swap_rb,
+                  void* out, int32_t out_dtype, int32_t s2d, int32_t out_row_px, int32_t out_x_off, void* stream);
+/* Labels of a batch in input order -> the kept rows, compacted stably, as collate_fn's (nt, 6) float32 [image, cls, box]
+ * rows in `targets` (room for n_labels rows); *count (device int32) = nt.  `table` and `labels` are DEVICE memory. */
+int y5_aug_labels(const y5_aug_image* table, int32_t n_images, const y5_aug_label* labels, int32_t n_labels, int32_t out_h,
+                  int32_t out_w, float* targets, int32_t* count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -108,6 +108,33 @@ class PackItem(C.Structure):
     ]
 
 
+class AugTile(C.Structure):
+    _fields_ = [
+        ("src", C.c_void_p), ("row_bytes", C.c_int32), ("pixel_stride", C.c_int32), ("channel_stride", C.c_int32),
+        ("x1a", C.c_int32), ("y1a", C.c_int32), ("x2a", C.c_int32), ("y2a", C.c_int32), ("dx", C.c_int32), ("dy", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class AugImage(C.Structure):
+    _fields_ = [
+        ("inv_m", (C.c_double * 6) * 2), ("m", (C.c_double * 6) * 2), ("mix_r", C.c_double), ("scale", C.c_float * 2),
+        ("clip_max", C.c_float), ("n_mosaic", C.c_int32), ("n_tiles", C.c_int32 * 2), ("canvas_w", C.c_int32), ("canvas_h", C.c_int32),
+        ("warp", C.c_int32 * 2), ("hsv", C.c_int32), ("flipud", C.c_int32), ("fliplr", C.c_int32), ("reserved", C.c_int32),
+        ("tiles", AugTile * 8), ("lut", (C.c_uint8 * 256) * 3),
+    ]
+
+
+class AugLabel(C.Structure):
+    _fields_ = [
+        ("cls", C.c_float), ("x", C.c_float), ("y", C.c_float), ("w", C.c_float), ("h", C.c_float),
+        ("tile_w", C.c_float), ("tile_h", C.c_float), ("pad_w", C.c_float), ("pad_h", C.c_float),
+        ("image", C.c_int32), ("mosaic", C.c_int32), ("flags", C.c_int32),
+    ]
+
+
+AUG_CLIP, AUG_IN_XYXY, AUG_OUT_XYXY = 1, 2, 4  # y5_aug_label.flags (include/y5b200.h Y5_AUG_*)
+
 # indices into the fused optimizer's `hyper` array (include/y5b200.h Y5_OPT_*)
 OPT_INV_SCALE, OPT_MAX_NORM, OPT_EMA_DECAY, OPT_EMA_TAU, OPT_EMA_UPDATES, OPT_OUT_NORM, OPT_OUT_SKIPPED, OPT_GROUPS = 0, 1, 2, 3, 4, 5, 6, 8
 # per-group block of y5_adam_step's fp64 `group_hyper` (include/y5b200.h Y5_ADAM_*)
@@ -177,6 +204,8 @@ SIGNATURES = {
     "y5_adam_step": (_I32, [_P, _I32, _P, _P, _I32, _P, _P, _I64, _P, _P, _I32, _I32, _P]),
     "y5_grad_pack": (_I32, [_P, _P, _P, _I32, _P, _P, _P, _P]),
     "y5_grad_bind": (_I32, [_P, _I32, _P, _P, _P, _P]),
+    "y5_aug_gather": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _I32, _I32, _I32, _I32, _P]),
+    "y5_aug_labels": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _P, _P, _P]),
     "y5_fold_pack": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _I32, _F, _P, _I32, _I32, _P, _I32, _P]),
 }
 

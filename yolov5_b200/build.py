@@ -32,6 +32,7 @@ SOURCES = {
     "post_kernels.cu": ["-fmad=false"],
     "mask_metrics.cu": ["-fmad=false"],
     "optim_kernels.cu": [],
+    "aug_kernels.cu": ["-fmad=false"],
 }
 
 
