@@ -555,6 +555,28 @@ int y5_aug_gather(const y5_aug_image* table, int32_t n_images, int32_t out_h, in
 int y5_aug_labels(const y5_aug_image* table, int32_t n_images, const y5_aug_label* labels, int32_t n_labels, int32_t out_h,
                   int32_t out_w, float* targets, int32_t* count, void* stream);
 
+/* Classification head (models/common.py:1120-1140 Classify) and loss (utils/torch_utils.py:52-57 smartCrossEntropyLoss).
+ * Global average pool over an NHWC channel-slice view x (B, h, w, pitch x_pitch): y[b * y_pitch + c] = the h*w pixels of
+ * channel c summed in fp32 in pixel order, divided by h*w and rounded once to the dtype (Y5_F16 | Y5_BF16; c, pitches % 8).
+ * No atomics: the result repeats bit for bit. */
+int y5_global_avg_pool(const void* x, int32_t x_pitch, void* y, int32_t y_pitch, int32_t batch, int32_t h, int32_t w, int32_t c,
+                       int32_t dtype, void* stream);
+/* Its backward: dx (B, h, w, pitch dx_pitch) = dy[b * dy_pitch + c] / (h*w) at every pixel, computed in fp32, rounded once. */
+int y5_global_avg_pool_bwd(const void* dy, int32_t dy_pitch, void* dx, int32_t dx_pitch, int32_t batch, int32_t h, int32_t w, int32_t c,
+                           int32_t dtype, void* stream);
+/* nn.CrossEntropyLoss(label_smoothing=eps) with reduction 'mean' on logits (batch, nc) with row stride `row_stride` elements
+ * (Y5_F16 | Y5_BF16 | Y5_F32) and int64 labels (DEVICE):
+ *   row_loss[b] = (1 - eps) * (lse - x[y]) + (eps / nc) * sum_c (lse - x[c]),  lse = max + log(sum exp(x - max)), in fp32;
+ *   *loss       = sum_b row_loss[b] / batch, summed by one block in a fixed order (bitwise repeatable).
+ * dlogits != NULL also writes, in the logits dtype with row stride dlogits_stride,
+ *   dlogits[b][c] = g * (softmax[b][c] - q[b][c]) / batch,  q = (1 - eps) * onehot(y) + eps / nc,
+ * g = *grad_scale (DEVICE fp32, the upstream gradient, e.g. GradScaler's factor; NULL: 1) multiplied in fp32 before the one
+ * rounding.  A label outside [0, nc) gives a NaN row loss (so a NaN *loss) and NaN gradients for its row -- there is no device
+ * assert and no ignore_index.  row_loss: DEVICE scratch of `batch` floats.  No host synchronisation; nc >= 2, any size. */
+int y5_cross_entropy(const void* logits, int32_t dtype, int32_t batch, int32_t nc, int64_t row_stride, const int64_t* labels,
+                     float label_smoothing, const float* grad_scale, void* dlogits, int64_t dlogits_stride, float* row_loss, float* loss,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -207,6 +207,9 @@ SIGNATURES = {
     "y5_aug_gather": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _I32, _I32, _I32, _I32, _P]),
     "y5_aug_labels": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _P, _P, _P]),
     "y5_fold_pack": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _I32, _F, _P, _I32, _I32, _P, _I32, _P]),
+    "y5_global_avg_pool": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
+    "y5_global_avg_pool_bwd": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
+    "y5_cross_entropy": (_I32, [_P, _I32, _I32, _I32, _I64, _P, _F, _P, _P, _I64, _P, _P, _P]),
 }
 
 _lib = None

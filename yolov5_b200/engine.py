@@ -387,6 +387,28 @@ class Program:
             self.weight_bytes += 2 * na * no * v.c
             row0 += na * v.h * v.w
 
+    def lower_classify(self, m, x, name):
+        """Classify (models/common.py:1138-1140): conv + folded BN + SiLU, global average pool into a (B,1,1,1280) buffer, then
+        the Linear as a 1x1 conv with bias and no activation on that view (nc padded with zero rows to a multiple of 8).
+        Dropout is the identity in eval.  The logits stay in the (B,1,1,ncpad) buffer; run_classify exports them."""
+        if isinstance(x, list):
+            raise NotImplementedError("y5b200: Classify behind a Concat (list input) is outside the engine's hot path")
+        a = self.lower_conv(m.conv, x, None, f"{name}.conv")
+        pooled = self.new_view(1, 1, a.c)
+        self.ops.append(_Op(f"{name}.pool", self.lib.y5_global_avg_pool,
+                            (a.ptr, a.pitch, pooled.ptr, pooled.pitch, self.B, a.h, a.w, a.c, self.dt_code)))
+        lin = m.linear
+        nc, cin = lin.weight.shape
+        ncpad = _pad8(nc)
+        bk = self.block_k(cin, ncpad, self.B)
+        ipad = (cin + bk - 1) // bk * bk
+        wp = torch.empty(ncpad, 1, 1, ipad, dtype=self.dtype, device=self.device)
+        bias = torch.empty(ncpad, dtype=torch.float32, device=self.device)
+        self.fold_pack_into([(lin.weight.view(nc, cin, 1, 1), lin.bias, None)], wp, bias, 0, ipad, pad_rows_to=ncpad)
+        out = self.new_view(1, 1, ncpad)
+        self.conv(pooled, out, None, None, 1, 1, 0, False, None, f"{name}.linear", packed=(wp, bias, bk, cin))
+        self.cls_view = View(out.buf, 0, nc)
+
     # ------------------------------------------------------------------ builders
     def _build(self):
         from .models import common as mc
@@ -395,6 +417,7 @@ class Program:
         mod = self.module
         self.stem_in = None
         self.proto_view = None
+        self.cls_view = None
         self.single_out = None
         if isinstance(mod, my.BaseModel):
             self._build_model(mod)
@@ -471,6 +494,9 @@ class Program:
                     self.proto_view = self.lower_proto(m.proto, xs[0], f"{name}.proto")
                 self.lower_detect(m, xs, name)
                 continue
+            if isinstance(m, mc.Classify):
+                self.lower_classify(m, outs[i - 1] if f == -1 else (outs[f] if isinstance(f, int) else [outs[j] for j in f]), name)
+                continue
             if isinstance(m, mc.Concat):
                 cat = concat_buf[i]
                 off = 0
@@ -503,7 +529,7 @@ class Program:
             return (src[0], src[1] * 2, src[2] * 2)
         if isinstance(m, mc.Concat):
             return (sum(s[0] for s in src), src[0][1], src[0][2])
-        if isinstance(m, my.Detect):
+        if isinstance(m, (my.Detect, mc.Classify)):
             return None
         raise NotImplementedError(f"y5b200: module {type(m).__name__} is outside the engine's hot path")
 
@@ -525,8 +551,8 @@ class Program:
             self._run_fixed(torch.cuda.current_stream(self.device).cuda_stream)
         self.graph = g
 
-    def run_model(self, img: torch.Tensor, use_graph: bool = True):
-        """img: (B,3,H,W) NCHW uint8 (scaled by 1/255 on the fly) or fp16/bf16/fp32 in [0,1]."""
+    def _run_body(self, img: torch.Tensor, use_graph: bool) -> int:
+        """stem space-to-depth of `img`, then the fixed part (graph replay); returns the stream pointer."""
         assert img.is_cuda and img.shape == (self.B, 3, self.H, self.W), (img.shape, (self.B, 3, self.H, self.W))
         if not img.is_contiguous():
             img = img.contiguous()
@@ -539,6 +565,19 @@ class Program:
             self.graph.replay()
         else:
             self._run_fixed(st)
+        return st
+
+    def run_classify(self, img: torch.Tensor, use_graph: bool = True) -> torch.Tensor:
+        """ClassificationModel: img (B,3,H,W) as run_model takes it -> a fresh (B, nc) logits tensor every call."""
+        st = self._run_body(img, use_graph)
+        v = self.cls_view
+        y = torch.empty(self.B, v.c, dtype=self.dtype, device=self.device)
+        _lib.check(self.lib.y5_nhwc_to_nchw(v.ptr, v.pitch, y.data_ptr(), self.B, 1, 1, v.c, self.dt_code, C.c_void_p(st)), "nhwc_to_nchw")
+        return y
+
+    def run_model(self, img: torch.Tensor, use_graph: bool = True):
+        """img: (B,3,H,W) NCHW uint8 (scaled by 1/255 on the fly) or fp16/bf16/fp32 in [0,1]."""
+        st = self._run_body(img, use_graph)
         # head: fresh output tensors every call, like the reference
         no = self.det_shapes[0][-1]
         z = torch.empty(self.B, self.z_rows, no, dtype=self.dtype, device=self.device)
@@ -568,7 +607,7 @@ class Program:
 
     def launches_per_forward(self) -> int:
         n = len(self.ops) + len(self.head_ops) + (1 if self.stem_in is not None else 0) + (1 if self.proto_view is not None else 0)
-        return n
+        return n + (1 if self.cls_view is not None else 0)
 
     def __del__(self):
         try:

@@ -1,5 +1,5 @@
 """Layer zoo of the hot path with the reference's class names, constructor signatures, attribute names and
-state_dict keys (reference models/common.py:62-92,164-181,230-246,318-340,443-453,1104-1117), so checkpoints and
+state_dict keys (reference models/common.py:62-92,164-181,230-246,318-340,443-453,1104-1140), so checkpoints and
 state_dicts move between the two unchanged.  The modules only *hold* parameters: executing one (``forward``) lowers it
 to liby5b200 kernels through yolov5_b200.engine.Program (eval) or yolov5_b200.train_ops (training: batch-statistics
 BatchNorm, autograd) -- there is no torch.nn convolution behind them and CPU tensors are rejected.
@@ -169,3 +169,20 @@ class Proto(_EngineLayer):
         self.upsample = nn.Upsample(scale_factor=2, mode="nearest")
         self.cv2 = Conv(c_, c_, k=3)
         self.cv3 = Conv(c_, c2)
+
+
+class Classify(nn.Module):
+    """Classification head (reference models/common.py:1120-1140): Conv(c1, 1280) -> global average pool -> Dropout ->
+    Linear(1280, c2).  Inside ClassificationModel.forward it runs as conv_gemm + y5_global_avg_pool + conv_gemm (the Linear
+    as a 1x1 conv with bias); Dropout is the identity in eval, and p > 0 is refused in training."""
+
+    def __init__(self, c1, c2, k=1, s=1, p=None, g=1, dropout_p=0.0):
+        super().__init__()
+        c_ = 1280  # efficientnet_b0 size
+        self.conv = Conv(c1, c_, k, s, autopad(k, p), g)
+        self.pool = nn.AdaptiveAvgPool2d(1)
+        self.drop = nn.Dropout(p=dropout_p, inplace=True)
+        self.linear = nn.Linear(c_, c2)
+
+    def forward(self, x):
+        raise RuntimeError("y5b200: Classify runs inside ClassificationModel.forward (conv, pool and linear as liby5b200 kernels)")

@@ -1,6 +1,7 @@
-"""Model assembly with the reference's API surface (reference models/yolo.py:71-150,160-195,215-261,314-327,375-458):
+"""Model assembly with the reference's API surface (reference models/yolo.py:71-150,160-195,215-261,314-372,375-458):
 ``DetectionModel(cfg, ch, nc, anchors)``, ``.forward(x)``, ``.fuse()``, attributes ``yaml names stride model save nc
-inplace``, ``Detect`` / ``Segment`` with ``nc no nl na anchors m stride``, and identical ``state_dict`` keys.
+inplace``, ``Detect`` / ``Segment`` with ``nc no nl na anchors m stride``, ``ClassificationModel(cfg, model, nc, cutoff)``,
+and identical ``state_dict`` keys.
 
 Differences that follow from being an engine rather than a torch.nn graph:
   * strides are derived from the layer table instead of a 256x256 probe forward (models/yolo.py:250-256);
@@ -18,7 +19,8 @@ import torch
 from torch import nn
 
 from ..cfg import model_cfg
-from .common import C3, SPPF, Bottleneck, Concat, Conv, Proto, _cached_program, _drop_engine_cache, _lib_on, _param_version  # noqa: F401
+from .common import (C3, SPPF, Bottleneck, Classify, Concat, Conv, Proto, _cached_program, _drop_engine_cache, _lib_on,  # noqa: F401
+                     _param_version)
 
 
 def make_divisible(x, divisor):
@@ -177,7 +179,10 @@ class BaseModel(nn.Module):
             with _lib_on(x.device):
                 return forward_train(self, x)
         with _lib_on(x.device):
-            z, raws, proto = self._program(x).run_model(x)
+            prog = self._program(x)
+            if isinstance(head, Classify):  # (B, nc) logits, as models/yolo.py:160-170 returns for a ClassificationModel
+                return prog.run_classify(x)
+            z, raws, proto = prog.run_model(x)
         if isinstance(head, Segment):
             return (z, proto) if head.export else (z, proto, raws)
         return (z,) if head.export else (z, raws)
@@ -300,3 +305,41 @@ Model = DetectionModel
 class SegmentationModel(DetectionModel):
     def __init__(self, cfg="yolov5s-seg.yaml", ch=3, nc=None, anchors=None):
         super().__init__(cfg, ch, nc, anchors)
+
+
+class ClassificationModel(BaseModel):
+    """Reference models/yolo.py:343-372: a DetectionModel's backbone cut at `cutoff` with a Classify head in place of its last
+    layer.  ``forward(x)`` returns the (B, nc) logits -- in eval through a cached engine Program, in training mode through
+    yolov5_b200.train_ops (batch-statistics BN, autograd)."""
+
+    def __init__(self, cfg=None, model=None, nc=1000, cutoff=10):
+        super().__init__()
+        self._from_detection_model(model, nc, cutoff) if model is not None else self._from_yaml(cfg)
+
+    def _from_detection_model(self, model, nc=1000, cutoff=10):
+        model.model = model.model[:cutoff]  # backbone
+        m = model.model[-1]  # last layer
+        ch = m.conv.in_channels if hasattr(m, "conv") else m.cv1.conv.in_channels  # ch into module
+        c = Classify(ch, nc)
+        c.i, c.f, c.type = m.i, m.f, "models.common.Classify"
+        model.model[-1] = c
+        _drop_engine_cache(model)
+        self.model = model.model
+        self.stride = model.stride
+        self.save = []
+        self.nc = nc
+
+    def _from_yaml(self, cfg):
+        self.model = None  # the reference does not build classification models from a *.yaml either
+
+    def _program(self, x):
+        """As BaseModel._program, except that an fp32 model called under autocast computes in the autocast dtype:
+        classify/train.py validates its fp32 EMA model that way (classify/val.py:110)."""
+        from ..engine import Program
+
+        dt = x.dtype if x.dtype in (torch.float16, torch.bfloat16) else next(self.parameters()).dtype
+        if dt == torch.float32 and torch.is_autocast_enabled("cuda"):
+            dt = torch.get_autocast_dtype("cuda")
+        key = (tuple(x.shape), x.dtype, dt, x.device.index, _param_version(self))
+        b, _, h, w = x.shape
+        return _cached_program(self, key, lambda: Program(self, b, h, w, dt, x.device))

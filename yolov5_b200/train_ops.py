@@ -735,6 +735,44 @@ class _Concat(torch.autograd.Function):
         return tuple(outs)
 
 
+class _GlobalAvgPool(torch.autograd.Function):
+    """nn.AdaptiveAvgPool2d(1) of Classify (models/common.py:1140): (B,C,H,W) NHWC view -> (B,C,1,1) channels_last, summed in
+    fp32 and rounded once (y5_global_avg_pool); the backward spreads dy / (H*W) over every pixel (y5_global_avg_pool_bwd)."""
+
+    @staticmethod
+    def forward(ctx, x):
+        x, xp = _nhwc(x)
+        b, c, h, w = x.shape
+        y = _empty_cl(b, c, 1, 1, x.dtype, x.device)
+        _lib.check(_lib.lib().y5_global_avg_pool(x.data_ptr(), xp, y.data_ptr(), c, b, h, w, c, _lib.dtype_code(x.dtype), _st(x.device)),
+                   "global_avg_pool")
+        ctx.hw = (h, w)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        dy, dp = _nhwc(dy)
+        b, c = dy.shape[:2]
+        h, w = ctx.hw
+        dx = _empty_cl(b, c, h, w, dy.dtype, dy.device)
+        _lib.check(_lib.lib().y5_global_avg_pool_bwd(dy.data_ptr(), dp, dx.data_ptr(), c, b, h, w, c, _lib.dtype_code(dy.dtype), _st(dy.device)),
+                   "global_avg_pool_bwd")
+        return dx
+
+
+def _classify(m, x):
+    """Classify (models/common.py:1138-1140) in training: conv + batch-statistics BN + SiLU, pool, Linear as _ConvBias."""
+    if isinstance(x, list):
+        raise NotImplementedError("y5b200: Classify behind a Concat (list input) is outside the engine's hot path")
+    if m.drop.p > 0 and m.drop.training:
+        raise NotImplementedError("y5b200: Dropout(p > 0) in training is not implemented (its mask cannot follow torch's RNG); "
+                                  "train with the reference default dropout_p=0.0")
+    pooled = _GlobalAvgPool.apply(conv_module(m.conv, x))
+    nc, cin = m.linear.weight.shape
+    y = _ConvBias.apply(pooled, m.linear.weight.view(nc, cin, 1, 1), m.linear.bias)  # (B,1,1,ncpad) NHWC
+    return y.reshape(y.shape[0], -1)[:, :nc]
+
+
 def stem_input(img: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
     """(B,3,H,W) uint8 / float image -> (B,16,H/2,W/2) channels_last space-to-depth tensor (12 channels used)."""
     lib = _lib.lib()
@@ -783,6 +821,8 @@ def _run(m, x, dt):
         for sub in m:
             x = _run(sub, x, dt)
         return x
+    if isinstance(m, mc.Classify):
+        return _classify(m, x)
     if isinstance(m, my.Detect):
         outs = []
         for i, xi in enumerate(x):

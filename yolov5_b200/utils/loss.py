@@ -1,13 +1,15 @@
 """ComputeLoss with the reference's interface (reference utils/loss.py:101-247): ``ComputeLoss(model)(p, targets) ->
 (loss (1,), items (3,))`` and ``.build_targets(p, targets)``.  build_targets, the gather/CIoU/scatter and both BCE
 terms -- forward and backward -- run in liby5b200 (y5_loss_fwd_bwd); the returned loss carries a custom autograd
-node that hands the kernel-computed gradient of every prediction level back to PyTorch.
+node that hands the kernel-computed gradient of every prediction level back to PyTorch.  ``CrossEntropyLoss`` is the
+classification loss (nn.CrossEntropyLoss with label smoothing) on y5_cross_entropy.
 """
 from __future__ import annotations
 
 import ctypes as C
 
 import torch
+from torch import nn
 
 from .. import _lib
 from .._lib import LossParams
@@ -41,6 +43,72 @@ class _LossFn(torch.autograd.Function):
         scale = g_loss.detach().reshape(-1)[:1].to(p[0].device, torch.float32).contiguous()
         _, grads = ctx.crit._run(p, ctx.targets, want_grad=True, grad_scale=scale)
         return (None, None) + tuple(grads)
+
+
+class _CrossEntropyFn(torch.autograd.Function):
+    """loss = CrossEntropyLoss(label_smoothing)(logits, labels) on y5_cross_entropy.  As _LossFn: the forward launch computes the
+    loss only; the backward re-launches the kernel with the upstream gradient (a device scalar) multiplied in fp32 before the
+    gradient is rounded to the logits dtype -- where torch-autocast rounds it, since cross_entropy runs in fp32 under autocast."""
+
+    @staticmethod
+    def forward(ctx, eps, labels, logits):
+        ctx.eps = eps
+        ctx.save_for_backward(labels, logits)
+        return _cross_entropy(logits, labels, eps)[0]
+
+    @staticmethod
+    def backward(ctx, g_loss):
+        labels, logits = ctx.saved_tensors
+        if not ctx.needs_input_grad[2]:
+            return None, None, None
+        scale = g_loss.detach().reshape(-1)[:1].to(logits.device, torch.float32).contiguous()
+        return None, None, _cross_entropy(logits, labels, ctx.eps, grad_scale=scale)[1]
+
+
+def _cross_entropy(logits, labels, eps, grad_scale=None):
+    """(0-d fp32 loss, dlogits (B, nc) in the logits dtype or None) from one y5_cross_entropy call (no host synchronisation)."""
+    b, nc = logits.shape
+    if logits.stride(1) != 1:
+        logits = logits.contiguous()
+    dev = logits.device
+    row_loss = torch.empty(b, dtype=torch.float32, device=dev)
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    grad = torch.empty(b, nc, dtype=logits.dtype, device=dev) if grad_scale is not None else None
+    with _lib.on(dev):
+        _lib.check(_lib.lib().y5_cross_entropy(logits.data_ptr(), _lib.dtype_code(logits.dtype), b, nc, logits.stride(0), labels.data_ptr(),
+                                               float(eps), grad_scale.data_ptr() if grad_scale is not None else None,
+                                               grad.data_ptr() if grad is not None else None, nc, row_loss.data_ptr(), loss.data_ptr(),
+                                               C.c_void_p(_lib.stream_ptr(dev))), "cross_entropy")
+    return loss, grad
+
+
+class CrossEntropyLoss(nn.CrossEntropyLoss):
+    """nn.CrossEntropyLoss(label_smoothing=eps) with reduction='mean' on class-index targets -- what smartCrossEntropyLoss
+    returns to classify/train.py and classify/val.py -- computed forward and backward by y5_cross_entropy:
+    mean_i[(1 - eps) (-log p_{i,y_i}) + (eps / nc) sum_c (-log p_{i,c})] in fp32 with a max-subtracted log-sum-exp.
+    Logits (B, nc) in fp16 / bf16 / fp32; the loss is fp32, or the logits dtype outside autocast as torch returns it.
+    A label outside [0, nc) -- ignore_index's -100 included -- gives a NaN loss and NaN gradients for its row (the reference
+    stops at a device assert instead).  weight=, reduction != 'mean', a non-default ignore_index and probability targets are
+    not implemented; CPU tensors are refused (no PyTorch fallback)."""
+
+    def forward(self, input, target):
+        if self.weight is not None:
+            raise NotImplementedError("y5b200: CrossEntropyLoss(weight=...) is not implemented")
+        if self.reduction != "mean":
+            raise NotImplementedError(f"y5b200: CrossEntropyLoss(reduction='{self.reduction}') is not implemented (mean only)")
+        if self.ignore_index != -100:
+            raise NotImplementedError("y5b200: CrossEntropyLoss(ignore_index=...) is not implemented")
+        if target.is_floating_point():
+            raise NotImplementedError("y5b200: CrossEntropyLoss with class-probability targets is not implemented (class indices only)")
+        if not (input.is_cuda and target.is_cuda):
+            raise RuntimeError("y5b200: CrossEntropyLoss runs on CUDA tensors only (no CPU / PyTorch fallback)")
+        if input.dim() != 2 or target.shape != input.shape[:1]:
+            raise ValueError(f"y5b200: CrossEntropyLoss expects (B, nc) logits and (B,) labels, got {tuple(input.shape)} and {tuple(target.shape)}")
+        labels = target if target.dtype == torch.int64 and target.is_contiguous() else target.long().contiguous()
+        loss = _CrossEntropyFn.apply(float(self.label_smoothing), labels, input)
+        if input.dtype != torch.float32 and not torch.is_autocast_enabled("cuda"):
+            loss = loss.to(input.dtype)  # F.cross_entropy on fp16 / bf16 logits returns that dtype
+        return loss
 
 
 class ComputeLoss:

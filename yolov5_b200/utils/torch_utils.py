@@ -1,4 +1,5 @@
-"""Hot-path edges of the reference's utils/torch_utils.py: BatchNorm folding and the DDP wrapper."""
+"""Hot-path edges of the reference's utils/torch_utils.py: BatchNorm folding, the DDP wrapper, the fused optimizers and EMA,
+and the classification helpers (smartCrossEntropyLoss, reshape_classifier_output)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -22,6 +23,40 @@ def fuse_conv_and_bn(conv: nn.Conv2d, bn: nn.BatchNorm2d) -> nn.Conv2d:
     b0 = conv.bias if conv.bias is not None else torch.zeros_like(scale)
     fused.bias.copy_(bn.bias + (b0 - bn.running_mean) * scale)
     return fused
+
+
+def smartCrossEntropyLoss(label_smoothing=0.0):
+    """nn.CrossEntropyLoss(label_smoothing=...) as reference utils/torch_utils.py:52-57 returns it, on the engine's
+    y5_cross_entropy kernel (yolov5_b200.utils.loss.CrossEntropyLoss, an nn.CrossEntropyLoss subclass)."""
+    from .loss import CrossEntropyLoss
+
+    return CrossEntropyLoss(label_smoothing=label_smoothing)
+
+
+def reshape_classifier_output(model, n=1000):
+    """Give the last layer `n` outputs (reference utils/torch_utils.py:72-93) for a Classify head or a plain nn.Linear, and drop
+    the engine caches: the cached Programs and the parameter list behind _param_version still name the replaced Linear."""
+    from ..models.common import Classify, _drop_engine_cache
+
+    name, m = list((model.model if hasattr(model, "model") else model).named_children())[-1]
+    if isinstance(m, Classify):
+        if m.linear.out_features != n:
+            m.linear = nn.Linear(m.linear.in_features, n)
+    elif isinstance(m, nn.Linear):
+        if m.out_features != n:
+            setattr(model, name, nn.Linear(m.in_features, n))
+    elif isinstance(m, nn.Sequential):
+        types = [type(x) for x in m]
+        if nn.Linear in types:
+            i = len(types) - 1 - types[::-1].index(nn.Linear)
+            if m[i].out_features != n:
+                m[i] = nn.Linear(m[i].in_features, n)
+        elif nn.Conv2d in types:
+            i = len(types) - 1 - types[::-1].index(nn.Conv2d)
+            if m[i].out_channels != n:
+                m[i] = nn.Conv2d(m[i].in_channels, n, m[i].kernel_size, m[i].stride, bias=m[i].bias is not None)
+    for mod in model.modules():
+        _drop_engine_cache(mod)
 
 
 def smart_DDP(model):
