@@ -94,12 +94,13 @@ def compute_loss(p, targets, anchors, hyp, balance=(4.0, 1.0, 0.4)):
     anc = anchors.detach().cpu().numpy() if isinstance(anchors, torch.Tensor) else np.asarray(anchors)
     nc = p[0].shape[-1] - 5
     bt = build_targets(tg, anc, [tuple(pi.shape[2:4]) for pi in p], hyp["anchor_t"])
-    lcls = torch.zeros(1)
-    lbox = torch.zeros(1)
-    lobj = torch.zeros(1)
+    dt = p[0].dtype  # fp32 like the reference, or float64 for the tests' float64 cross-checks
+    lcls = torch.zeros(1, dtype=dt)
+    lbox = torch.zeros(1, dtype=dt)
+    lobj = torch.zeros(1, dtype=dt)
     cp, cn = 1.0 - 0.5 * hyp.get("label_smoothing", 0.0), 0.5 * hyp.get("label_smoothing", 0.0)
-    pw_cls = torch.tensor([hyp["cls_pw"]])
-    pw_obj = torch.tensor([hyp["obj_pw"]])
+    pw_cls = torch.tensor([hyp["cls_pw"]], dtype=dt)
+    pw_obj = torch.tensor([hyp["obj_pw"]], dtype=dt)
     for i, pi in enumerate(p):
         d = bt[i]
         b, a, gj, gi = (torch.from_numpy(d[k]) for k in ("b", "a", "gj", "gi"))
@@ -108,8 +109,8 @@ def compute_loss(p, targets, anchors, hyp, balance=(4.0, 1.0, 0.4)):
         if n:
             ps = pi[b, a, gj, gi]
             pxy = ps[:, 0:2].sigmoid() * 2 - 0.5
-            pwh = (ps[:, 2:4].sigmoid() * 2) ** 2 * torch.from_numpy(d["anch"])
-            iou = bbox_ciou(torch.cat((pxy, pwh), 1), torch.from_numpy(d["tbox"]))
+            pwh = (ps[:, 2:4].sigmoid() * 2) ** 2 * torch.from_numpy(d["anch"]).to(dt)
+            iou = bbox_ciou(torch.cat((pxy, pwh), 1), torch.from_numpy(d["tbox"]).to(dt))
             lbox = lbox + (1.0 - iou).mean()
             tobj[b, a, gj, gi] = iou.detach().clamp(0).type(tobj.dtype)  # duplicates: last writer wins
             if nc > 1:

@@ -163,9 +163,13 @@ __device__ __forceinline__ D4 operator-(const D4& a, const D4& b) { D4 r; r.v = 
 __device__ __forceinline__ D4 operator*(const D4& a, const D4& b) { D4 r; r.v = a.v * b.v; for (int i = 0; i < 4; ++i) r.d[i] = a.d[i] * b.v + a.v * b.d[i]; return r; }
 __device__ __forceinline__ D4 operator/(const D4& a, const D4& b) { D4 r; r.v = a.v / b.v; const float inv = 1.0f / b.v; for (int i = 0; i < 4; ++i) r.d[i] = (a.d[i] - r.v * b.d[i]) * inv; return r; }
 __device__ __forceinline__ D4 dscale(const D4& a, float s) { D4 r; r.v = a.v * s; for (int i = 0; i < 4; ++i) r.d[i] = a.d[i] * s; return r; }
-__device__ __forceinline__ D4 dmin(const D4& a, const D4& b) { return a.v <= b.v ? a : b; }  // torch min/max: grad to the selected operand
-__device__ __forceinline__ D4 dmax(const D4& a, const D4& b) { return a.v >= b.v ? a : b; }
-__device__ __forceinline__ D4 dclamp0(const D4& a) { return a.v > 0.f ? a : dconst(a.v < 0.f ? 0.f : a.v); }
+// torch.minimum / maximum backward: the gradient goes to the selected operand, and on a tie half to each
+// (a predicted box equal to its target, e.g. logits 0 on an anchor-sized target, ties every edge)
+__device__ __forceinline__ D4 dtie(const D4& a, const D4& b) { D4 r; r.v = a.v; for (int i = 0; i < 4; ++i) r.d[i] = 0.5f * (a.d[i] + b.d[i]); return r; }
+__device__ __forceinline__ D4 dmin(const D4& a, const D4& b) { return a.v < b.v ? a : b.v < a.v ? b : dtie(a, b); }
+__device__ __forceinline__ D4 dmax(const D4& a, const D4& b) { return a.v > b.v ? a : b.v > a.v ? b : dtie(a, b); }
+// clamp(min=0) backward passes the gradient where v >= 0 (touching boxes: intersection width exactly 0)
+__device__ __forceinline__ D4 dclamp0(const D4& a) { return a.v >= 0.f ? a : dconst(0.f); }
 __device__ __forceinline__ D4 datan(const D4& a) { D4 r; r.v = atanf(a.v); const float g = 1.0f / (1.0f + a.v * a.v); for (int i = 0; i < 4; ++i) r.d[i] = a.d[i] * g; return r; }
 
 // CIoU(pred xywh, target xywh), eps 1e-7  (ultralytics bbox_iou, SURVEY.md Appendix C); alpha is a constant (no_grad)

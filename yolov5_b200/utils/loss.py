@@ -145,7 +145,23 @@ class ComputeLoss:
         q.grad_scale = 1.0
         return q
 
+    def _check_shapes(self, p, targets, no):
+        """Shape checks before any launch: the kernels take batch, dtype and grid strides from these tensors, so a level
+        with another batch, anchor count, channel count or dtype would be read past its end."""
+        if len(p) != self.nl:
+            raise ValueError(f"y5b200: expected {self.nl} head maps, got {len(p)}")
+        bs, dt = p[0].shape[0] if p[0].dim() else -1, p[0].dtype
+        for t in p:
+            if t.dim() != 5 or t.shape[0] != bs or t.shape[1] != self.na or t.shape[4] != no:
+                raise ValueError(f"y5b200: head map {tuple(t.shape)} is not (B={bs}, na={self.na}, ny, nx, {no})")
+            if t.dtype != dt:
+                raise ValueError(f"y5b200: head maps must share one dtype, got {dt} and {t.dtype}")
+        if targets.dim() != 2 or targets.shape[1] != 6:
+            raise ValueError(f"y5b200: targets must be (n, 6) [image, class, x, y, w, h], got {tuple(targets.shape)}")
+        return bs
+
     def _run(self, p, targets, want_grad, grad_scale=None):
+        self._check_shapes(p, targets, 5 + self.nc)
         if not all(t.is_cuda for t in p):
             raise RuntimeError("y5b200: ComputeLoss runs on CUDA tensors only (no CPU / PyTorch fallback)")
         lib = _lib.lib()

@@ -49,12 +49,7 @@ class ComputeLoss(_DetComputeLoss):
 
     # -------------------------------------------------------------------------------------------------------------
     def _check(self, p, proto, targets, masks):
-        if len(p) != self.nl:
-            raise ValueError(f"y5b200: expected {self.nl} head maps, got {len(p)}")
-        bs, no = p[0].shape[0], 5 + self.nc + self.nm
-        for t in p:
-            if t.dim() != 5 or t.shape[0] != bs or t.shape[1] != self.na or t.shape[4] != no:
-                raise ValueError(f"y5b200: head map {tuple(t.shape)} is not (B={bs}, na={self.na}, ny, nx, {no})")
+        bs = self._check_shapes(p, targets, 5 + self.nc + self.nm)
         if proto.dim() != 4 or proto.shape[0] != bs or proto.shape[1] != self.nm:
             raise ValueError(f"y5b200: proto {tuple(proto.shape)} is not (B={bs}, nm={self.nm}, mh, mw)")
         if masks.dim() != 3:
