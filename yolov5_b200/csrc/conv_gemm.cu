@@ -28,9 +28,13 @@
 // the cluster size.  A weight stage is free again only when the consumers of every CTA of the cluster have released it.
 // Detect head (EPI=1): N tile == one anchor; raw logits and decoded predictions are staged in smem in the exact
 // global layout and copied out with 16-byte vectors.
-// Limits: a consumer waits for every K group's wgmma before releasing its stage, and both warpgroups run the epilogue of the
-// same tile, so the tensor cores idle during each epilogue; overlapping them (two accumulator sets or ping-pong warpgroups) is the
-// next step for this kernel.
+// Mainloop: one K block of a tile is one wgmma batch (block_k / 16 k16 steps x MT sub-tiles, issued back to back; the dtype is a
+// template parameter, the step count a per-block switch into unrolled batches).  One batch stays in flight: after issuing batch i a
+// consumer waits (wgmma.wait_group 1) only for batch i-1 and then releases the stages i-1 was the last reader of, so the tensor
+// pipe is not drained between K blocks.  At the end of a tile it drains (wait_group 0) and releases what is still pending before
+// the epilogue, so the producer fills the next tile's stages while the epilogue runs.
+// Limits: both warpgroups run the epilogue of the same tile, so the tensor cores idle during each epilogue; overlapping them (two
+// accumulator sets or ping-pong warpgroups) is the next step for this kernel.
 // Persistent grid (<= one CTA per SM), warp-specialised: warp 0 TMA producer (its warpgroup hands its registers to the
 // consumers through setmaxnreg), warpgroups 1 and 2 MMA + epilogue.
 //
@@ -126,9 +130,26 @@ __device__ __forceinline__ int fdiv(int n, int d, float rd) {
     return q;
 }
 
+// One K block (KS k16 steps) for all MT sub-tiles as one wgmma batch: fence, KS * MT back-to-back wgmmas, commit.  Nothing
+// between the wgmmas touches their registers, so ptxas issues them as one chain (only the last waits on the scoreboard).
+// scale_first == 0 overwrites the accumulators with the first k16 step (the tile's first K block).
+template <int BLOCK_N, int MT, int KS, bool BF16>
+__device__ __forceinline__ void mma_batch(float (&acc)[MT][BLOCK_N / 2], uint32_t a_lo, uint32_t a_sub16, uint32_t a_hi, uint32_t b_lo,
+                                          uint32_t b_hi, uint32_t scale_first) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KS; ++k)
+#pragma unroll
+        for (int mi = 0; mi < MT; ++mi)
+            Wgmma<BLOCK_N>::template run<BF16, 0, 0>(acc[mi], gmma_desc(a_lo + mi * a_sub16 + 2 * k, a_hi), gmma_desc(b_lo + 2 * k, b_hi),
+                                                     k == 0 ? scale_first : 1u);
+    wgmma_commit();
+}
+
 // OPT: the instantiation that supports the optional modes (clusters, wide patch, staged stores); the default one compiles them out,
 // which keeps their run-time tests and live registers out of the hot loops (measured 8 % on yolov5l's conv stack).
-template <int BLOCK_N, int EPI, int MT, bool OPT>
+// BF16: activation / weight dtype (bf16 or fp16), fixed per instantiation so the MMA batches and the epilogue carry no dtype branch.
+template <int BLOCK_N, int EPI, int MT, bool OPT, bool BF16>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
     static_assert(MT * BLOCK_N <= 256, "accumulators: at most 128 fp32 registers per consumer thread");
@@ -279,7 +300,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int wrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's first accumulator row (the second is +8)
     const int ccol = 2 * (lane & 3);                      // this thread's first column inside every 8-column group
     const bool signal = (threadIdx.x & 127) == 0;         // the warpgroup's thread that releases smem stages
-    const bool bf16 = p.is_bf16 != 0;
+    constexpr bool bf16 = BF16;
     const uint32_t dhi = gmma_desc_hi(row_bytes);
     // wide patch: group stride = one patch row (PW pixels); warpgroup wg starts 8 output rows = 8 patch rows down
     const uint32_t a_hi = wide ? (dhi & ~0x3FFFu) | (((static_cast<uint32_t>(p.patch_pw) * row_bytes) >> 4) & 0x3FFFu) : dhi;
@@ -299,6 +320,22 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
         for (int i = 0; i < kAcc; ++i) acc[mi][i] = 0.0f;
 
+    // Stage release, deferred by one batch: the stages a batch reads are handed back to the producer only once the NEXT batch has
+    // been issued and wgmma.wait_group 1 has confirmed this one complete, so the tensor pipe never drains between K blocks.  The
+    // record of the batch in flight: its A stage and whether it is that stage's last reader, its B stage and whether it is that
+    // stage's last reader (a grouped B stage feeds kh members, a wide-patch A stage kh*kw).
+    int pend_as = 0, pend_bs = 0;
+    bool pend_a_last = false, pend_b_last = false;
+    auto release_pending = [&]() {
+        if (!signal) return;
+        if (pend_b_last) {
+            if (csize == 1) mbar_arrive(&b_empty[pend_bs]);
+            else  // multicast stage: every CTA of the cluster waits for the consumers of all of them
+                for (int r = 0; r < csize; ++r) mbar_arrive_cluster(mapa_u32(&b_empty[pend_bs], static_cast<uint32_t>(r)));
+        }
+        if (pend_a_last) mbar_arrive(&a_empty[pend_as]);
+    };
+
     for (int tile = tile0; tile < num_tiles; tile += tile_step) {
         const int ms = (tile / nn) * csize + static_cast<int>(crank);
         const int nt = tile - (tile / nn) * nn;
@@ -315,38 +352,33 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 const bool stage_first = !p.b_grouped || j == 0, stage_last = !p.b_grouped || j == grp - 1;
                 if (stage_first) mbar_wait(&b_full[bs], bph);
                 const uint32_t b_lo = b_base + bs * b_stage16 + (p.b_grouped ? j * b_sub16 : 0u);
+                const uint32_t scale_first = (g | j) != 0 ? 1u : 0u;  // the tile's first K step overwrites the accumulators
 #pragma unroll
                 for (int mi = 0; mi < MT; ++mi) fence_regs(acc[mi]);
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    if (k < k_steps) {
-                        const uint32_t scale_d = (g | j | k) != 0 ? 1u : 0u;  // the tile's first K step overwrites the accumulators
-#pragma unroll
-                        for (int mi = 0; mi < MT; ++mi) {
-                            const uint64_t da = gmma_desc(a_lo + mi * a_sub16 + 2 * k, a_hi), db = gmma_desc(b_lo + 2 * k, dhi);
-                            if (bf16) Wgmma<BLOCK_N>::template run<true, 0, 0>(acc[mi], da, db, scale_d);
-                            else Wgmma<BLOCK_N>::template run<false, 0, 0>(acc[mi], da, db, scale_d);
-                        }
-                    }
+                switch (k_steps) {  // block_k 64 / 32 / 16
+                    case 4: mma_batch<BLOCK_N, MT, 4, BF16>(acc, a_lo, a_sub16, a_hi, b_lo, dhi, scale_first); break;
+                    case 2: mma_batch<BLOCK_N, MT, 2, BF16>(acc, a_lo, a_sub16, a_hi, b_lo, dhi, scale_first); break;
+                    default: mma_batch<BLOCK_N, MT, 1, BF16>(acc, a_lo, a_sub16, a_hi, b_lo, dhi, scale_first); break;
                 }
-                wgmma_commit();
-                wgmma_wait<0>();
+                wgmma_wait<1>();  // the previous batch (not this one) is complete: its stages can go back to the producer
 #pragma unroll
                 for (int mi = 0; mi < MT; ++mi) fence_regs(acc[mi]);
-                if (stage_last) {
-                    if (signal) {
-                        if (csize == 1) mbar_arrive(&b_empty[bs]);
-                        else
-                            for (int r = 0; r < csize; ++r) mbar_arrive_cluster(mapa_u32(&b_empty[bs], static_cast<uint32_t>(r)));
-                    }
-                    if (++bs == p.b_stages) { bs = 0; bph ^= 1; }
-                }
+                if (g | j) release_pending();  // the tile's first batch: everything before it was released at the previous tile's end
+                pend_as = as;
+                pend_a_last = j == grp - 1;
+                pend_bs = bs;
+                pend_b_last = stage_last;
+                if (stage_last && ++bs == p.b_stages) { bs = 0; bph ^= 1; }
                 a_lo += a_shift16;
             }
-            if (signal) mbar_arrive(&a_empty[as]);
             if (++as == p.a_stages) { as = 0; aph ^= 1; }
         }
+        // drain before the epilogue reads the accumulators; the last stages go back now, so the producer fills the next tile's
+        // stages while this tile's epilogue runs
+        wgmma_wait<0>();
+#pragma unroll
+        for (int mi = 0; mi < MT; ++mi) fence_regs(acc[mi]);
+        release_pending();
 
         if (EPI == 0) {
             const bool staged = OPT && p.stg_bytes != 0;
@@ -562,10 +594,11 @@ int pick_block_n(int out_c, int64_t m_rows) {
 template <int BN, int EPI, int MT, bool OPT>
 cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const ConvParams& p, int grid, int cluster, uint32_t smem,
                         cudaStream_t st) {
-    const cudaError_t attr_err = ensure_dyn_smem(reinterpret_cast<const void*>(conv_gemm_kernel<BN, EPI, MT, OPT>), 227 * 1024);
+    auto* kernel = p.is_bf16 ? conv_gemm_kernel<BN, EPI, MT, OPT, true> : conv_gemm_kernel<BN, EPI, MT, OPT, false>;
+    const cudaError_t attr_err = ensure_dyn_smem(reinterpret_cast<const void*>(kernel), 227 * 1024);
     if (attr_err != cudaSuccess) return attr_err;
     count_launch();
-    if (cluster == 1) return launch_pdl(conv_gemm_kernel<BN, EPI, MT, OPT>, dim3(grid), dim3(kThreads), smem, st, a, b, p);
+    if (cluster == 1) return launch_pdl(kernel, dim3(grid), dim3(kThreads), smem, st, a, b, p);
     static const bool pdl = [] { const char* e = getenv("Y5_PDL"); return !(e && e[0] == '0'); }();
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid);
@@ -581,7 +614,7 @@ cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const ConvPa
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 2 : 1;
-    return cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, EPI, MT, OPT>, a, b, p);
+    return cudaLaunchKernelEx(&cfg, kernel, a, b, p);
 }
 
 struct PlanCommon {
