@@ -555,6 +555,41 @@ int y5_aug_gather(const y5_aug_image* table, int32_t n_images, int32_t out_h, in
 int y5_aug_labels(const y5_aug_image* table, int32_t n_images, const y5_aug_label* labels, int32_t n_labels, int32_t out_h,
                   int32_t out_w, float* targets, int32_t* count, void* stream);
 
+/* Segmentation training augmentation (utils/segment/dataloaders.py:130-301, utils/segment/augmentations.py:26-91 and
+ * ultralytics' polygons2masks[_overlap]), exact with the reference's numpy / OpenCV arithmetic (oracle/seg_aug_ref.py).
+ * Images go through y5_aug_gather with the same table; each label row (y5_aug_label, with the xyn2xy parameters in
+ * tile_w .. pad_h) has one polygon: n_points normalised float32 (x, y) pairs starting at pair point_offset of `points`.
+ * All pointers are DEVICE memory.  Sizes: verts n_labels * Y5_SEG_POINTS * 2 int32, rows n_labels * 6, masks
+ * n_labels * (out_h / r) * (out_w / r) bytes. */
+#define Y5_SEG_POINTS 1000 /* resample_segments(n=1000) */
+#define Y5_SEG_I32 4       /* y5_seg_compose's int32 output (overlap masks of images with more than 255 labels) */
+struct y5_aug_segment {
+    int32_t point_offset, n_points;
+};
+typedef struct y5_aug_segment y5_aug_segment;
+/* Per label: the resampled, warped polygon as polygon2mask's int32 vertices (verts), keep = box_candidates(area_thr 0.01)
+ * of its segment2box box, and its collate_fn row [image, cls, xywhn] (flips applied) in rows.  max_points bounds n_points. */
+int y5_seg_warp(const y5_aug_image* table, int32_t n_images, const y5_aug_label* labels, const y5_aug_segment* segments,
+                const float* points, int32_t max_points, int32_t n_labels, int32_t out_h, int32_t out_w, int32_t* verts, float* rows,
+                int32_t* keep, void* stream);
+/* cv2.resize(cv2.fillPoly(zeros(out_h, out_w), [poly], 1), (out_w / r, out_h / r)) for every kept label, unflipped, and
+ * its area (sum of the mask).  Polygon i is verts[i * n_verts * 2 ...], n_verts int32 (x, y) vertices (y5_seg_warp's:
+ * Y5_SEG_POINTS).  ratio: 1 or 4 (Y5_E_UNSUPPORTED otherwise; out_h, out_w multiples of it). */
+int y5_seg_raster(const int32_t* verts, int32_t n_verts, const int32_t* keep, int32_t n_labels, int32_t out_h, int32_t out_w,
+                  int32_t ratio, uint8_t* masks, int32_t* areas, void* stream);
+/* Image b owns label rows [image_rows[b], image_rows[b + 1]).  Kept labels -> output positions: image order, and within an
+ * image label order, or with overlap the order of np.argsort(-areas) on uint64 (zero areas first, then larger areas
+ * first; equal areas in label order).  targets (room for n_labels rows) gets the rows in that order, plane[pos] the
+ * label row, counts (n_images + 1) = [total, kept per image]. */
+int y5_seg_order(const int32_t* image_rows, int32_t n_images, const int32_t* keep, const int32_t* areas, const float* rows,
+                 int32_t overlap, float* targets, int32_t* plane, int32_t* counts, void* stream);
+/* The batch's masks: overlap -> n_out = n_images planes, v = clip(v + m_i * (i + 1), 0, i + 1) over the image's labels in
+ * order, in uint8 (with its wrap-around) up to 255 labels, else int32; otherwise n_out = total planes, one per label.
+ * Flips from the table; out_dtype Y5_U8 | Y5_SEG_I32 | Y5_F32. */
+int y5_seg_compose(const y5_aug_image* table, const y5_aug_label* labels, const int32_t* counts, const int32_t* plane,
+                   const uint8_t* masks, int32_t n_out, int32_t mask_h, int32_t mask_w, int32_t overlap, void* out, int32_t out_dtype,
+                   void* stream);
+
 /* Classification head (models/common.py:1120-1140 Classify) and loss (utils/torch_utils.py:52-57 smartCrossEntropyLoss).
  * Global average pool over an NHWC channel-slice view x (B, h, w, pitch x_pitch): y[b * y_pitch + c] = the h*w pixels of
  * channel c summed in fp32 in pixel order, divided by h*w and rounded once to the dtype (Y5_F16 | Y5_BF16; c, pitches % 8).

@@ -135,6 +135,13 @@ class AugLabel(C.Structure):
 
 AUG_CLIP, AUG_IN_XYXY, AUG_OUT_XYXY = 1, 2, 4  # y5_aug_label.flags (include/y5b200.h Y5_AUG_*)
 
+
+class AugSegment(C.Structure):
+    _fields_ = [("point_offset", C.c_int32), ("n_points", C.c_int32)]
+
+
+SEG_POINTS, SEG_I32 = 1000, 4  # include/y5b200.h Y5_SEG_POINTS, Y5_SEG_I32
+
 # indices into the fused optimizer's `hyper` array (include/y5b200.h Y5_OPT_*)
 OPT_INV_SCALE, OPT_MAX_NORM, OPT_EMA_DECAY, OPT_EMA_TAU, OPT_EMA_UPDATES, OPT_OUT_NORM, OPT_OUT_SKIPPED, OPT_GROUPS = 0, 1, 2, 3, 4, 5, 6, 8
 # per-group block of y5_adam_step's fp64 `group_hyper` (include/y5b200.h Y5_ADAM_*)
@@ -206,6 +213,10 @@ SIGNATURES = {
     "y5_grad_bind": (_I32, [_P, _I32, _P, _P, _P, _P]),
     "y5_aug_gather": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _I32, _I32, _I32, _I32, _P]),
     "y5_aug_labels": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _P, _P, _P]),
+    "y5_seg_warp": (_I32, [_P, _I32, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P, _P]),
+    "y5_seg_raster": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _P, _P, _P]),
+    "y5_seg_order": (_I32, [_P, _I32, _P, _P, _P, _I32, _P, _P, _P, _P]),
+    "y5_seg_compose": (_I32, [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _I32, _P]),
     "y5_fold_pack": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _I32, _F, _P, _I32, _I32, _P, _I32, _P]),
     "y5_global_avg_pool": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "y5_global_avg_pool_bwd": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),

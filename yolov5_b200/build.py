@@ -33,6 +33,7 @@ SOURCES = {
     "mask_metrics.cu": ["-fmad=false"],
     "optim_kernels.cu": [],
     "aug_kernels.cu": ["-fmad=false"],
+    "seg_aug_kernels.cu": ["-fmad=false"],
     "cls_kernels.cu": [],
 }
 

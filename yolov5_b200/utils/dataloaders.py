@@ -45,25 +45,29 @@ def _check_dataset(ds):
         raise ValueError(f"y5b200: img_size {ds.img_size} outside (0, 16384]")
 
 
-def _mosaic_draws(ds, index):
+def _mosaic_draws(ds, index, shuffle_tiles=True):
     s = ds.img_size
     yc, xc = (int(random.uniform(-x, 2 * s + x)) for x in ds.mosaic_border)
     indices = [index, *random.choices(ds.indices, k=3)]
-    random.shuffle(indices)
+    if shuffle_tiles:
+        random.shuffle(indices)
     hyp = ds.hyp
     return dict(xc=xc, yc=yc, indices=[int(i) for i in indices],
                 persp=perspective_draws(hyp["degrees"], hyp["translate"], hyp["scale"], hyp["shear"], hyp["perspective"]))
 
 
-def draw_item(ds, i):
-    """Every random draw of __getitem__(i), in the reference's order (utils/dataloaders.py:696-756)."""
+def draw_item(ds, i, partner=None, shuffle_tiles=True):
+    """Every random draw of __getitem__(i), in the reference's order (utils/dataloaders.py:696-756).  The segmentation
+    loader (utils/segment/dataloaders.py:130-142, 235-243) differs in two draws: `partner()` draws the mixup partner's
+    index (random.randint(0, n - 1) instead of random.choice(ds.indices)) and its mosaics keep the tile order
+    (shuffle_tiles=False)."""
     hyp = ds.hyp
     p = dict(index=int(ds.indices[i]))
     p["mosaic"] = bool(ds.mosaic and random.random() < hyp["mosaic"])
     if p["mosaic"]:
-        p["m"] = [_mosaic_draws(ds, p["index"])]
+        p["m"] = [_mosaic_draws(ds, p["index"], shuffle_tiles)]
         if random.random() < hyp["mixup"]:  # drawn even when mixup == 0
-            p["m"].append(_mosaic_draws(ds, int(random.choice(ds.indices))))
+            p["m"].append(_mosaic_draws(ds, int(partner() if partner else random.choice(ds.indices)), shuffle_tiles))
             p["r"] = np.random.beta(32.0, 32.0)
     else:
         p["persp"] = perspective_draws(hyp["degrees"], hyp["translate"], hyp["scale"], hyp["shear"], hyp["perspective"])
