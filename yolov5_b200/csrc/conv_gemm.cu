@@ -20,7 +20,8 @@
 // wgmma m64 x BLOCK_N x k16 (fp32 accumulators in registers) for them; after the tile's last K block it applies the
 // folded-BN bias -> SiLU -> (+ residual) -> fp16/bf16 and stores straight from the registers to the NHWC (slice) view.
 // Epilogue stores: by default each thread stores its 4-byte pairs straight from the registers; on request each warpgroup stages
-// its packed 64 x BLOCK_N block in shared memory and writes whole 16-byte row segments instead.
+// its packed 64 x BLOCK_N block in shared memory and writes whole 16-byte row segments instead.  Residual words are loaded in
+// batches ahead of the stores (the residual may alias the output, so loads interleaved with stores would serialise).
 // Tiles: MT sub-tiles of 128 rows x BLOCK_N with MT * BLOCK_N <= 256 (128 accumulator registers per thread), so one weight
 // tile feeds MT sub-tiles and narrow layers do as much work per barrier round as wide ones.
 // Clusters (2 or 4 CTAs along M): the CTAs of a cluster work on different M super-tiles of the SAME N tile in lock-step, each
@@ -384,67 +385,85 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const bool staged = OPT && p.stg_bytes != 0;
             const uint32_t stg_pitch = BLOCK_N * 2 + 16;  // +16 bytes: the fragment's 8 rows x 4 column pairs hit 32 distinct banks
             uint8_t* stg = smem + L.off_out + wg * 64 * stg_pitch;
-#pragma unroll
-            for (int mi = 0; mi < MT; ++mi) {
-                const int mt = ms * MT + mi;
-                int img = 0, oy0 = 0, ox0 = 0;
+            // global output pixel of row `row` of sub-tile `mt`, -1 outside the output
+            auto pixel_of = [&](int mt, int row) -> long long {
                 if (patch) {  // image + origin of the th x tw block
-                    img = fdiv(mt, per_img, p.rcp_per_img);
+                    const int img = fdiv(mt, per_img, p.rcp_per_img);
                     const int rem = mt - img * per_img;
                     const int tyi = fdiv(rem, p.tiles_x, p.rcp_tiles_x);
-                    oy0 = tyi * p.th;
-                    ox0 = (rem - tyi * p.tiles_x) * p.tw;
+                    const int oy = tyi * p.th + (row >> tw_shift), ox = (rem - tyi * p.tiles_x) * p.tw + (row & ((1 << tw_shift) - 1));
+                    return (mt < p.num_m_tiles && oy < p.Ho && ox < p.Wo) ? static_cast<long long>(img) * p.HoWo + oy * p.Wo + ox : -1;
                 }
-                // global output pixel of tile row `row`, -1 outside the output
-                auto pixel_of = [&](int row) -> long long {
-                    if (patch) {
-                        const int oy = oy0 + (row >> tw_shift), ox = ox0 + (row & ((1 << tw_shift) - 1));
-                        return (mt < p.num_m_tiles && oy < p.Ho && ox < p.Wo) ? static_cast<long long>(img) * p.HoWo + oy * p.Wo + ox : -1;
-                    }
-                    const long long m = static_cast<long long>(mt) * kBlockM + row;
-                    return m < p.M ? m : -1;
-                };
+                const long long m = static_cast<long long>(mt) * kBlockM + row;
+                return m < p.M ? m : -1;
+            };
+            // The residual may alias the output (the in-place Bottleneck add), so a load placed after a store cannot be moved above
+            // it: read and written group by group, every 8-column group would cost one dependent global round trip.  Instead the
+            // thread's rows (MT sub-tiles x 2 row halves) go in batches of kBatch, and every residual word of a batch is loaded before
+            // its first store: one round trip per batch, and at most 2 per tile.  Legal in place because each thread reads only the
+            // elements it writes itself.  kBatch keeps the loaded words to 32 registers (64 spill next to 128 accumulators), 16 in
+            // the OPT instantiations, whose optional modes hold more live state.
+            constexpr int kRows = 2 * MT, kWords = (OPT ? 128 : 256) / BLOCK_N;
+            constexpr int kBatch = kWords < 1 ? 1 : (kWords < kRows ? kWords : kRows);
+            const bool has_res = p.res != nullptr;
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
+            for (int q0 = 0; q0 < kRows; q0 += kBatch) {
+                uint32_t rv[kBatch][BLOCK_N / 8];
+                long long gp[kBatch];  // output pixel of each row half of the batch, -1 outside the output
+#pragma unroll
+                for (int q = 0; q < kBatch; ++q) gp[q] = pixel_of(ms * MT + (q0 + q) / 2, wrow + 8 * ((q0 + q) & 1));
+                if (has_res) {
+#pragma unroll
+                    for (int q = 0; q < kBatch; ++q) {
+                        const uint16_t* rp = reinterpret_cast<const uint16_t*>(p.res) + (gp[q] < 0 ? 0 : gp[q] * p.res_pitch) + n0 + ccol;
+#pragma unroll
+                        for (int j = 0; j < BLOCK_N / 8; ++j)
+                            rv[q][j] = (gp[q] >= 0 && n0 + 8 * j < p.N) ? *reinterpret_cast<const uint32_t*>(rp + 8 * j) : 0u;
+                    }
+                }
+#pragma unroll
+                for (int q = 0; q < kBatch; ++q) {
+                    const int mi = (q0 + q) / 2, h = (q0 + q) & 1;  // sub-tile, row half
+                    const int mt = ms * MT + mi;
                     const int row = wrow + 8 * h;
-                    const long long gpix = pixel_of(row);
-                    if (gpix < 0 && !staged) continue;
-                    uint16_t* op = reinterpret_cast<uint16_t*>(p.out) + gpix * p.out_pitch + n0 + ccol;
-                    const uint16_t* rp = (p.res && gpix >= 0) ? reinterpret_cast<const uint16_t*>(p.res) + gpix * p.res_pitch + n0 + ccol : nullptr;
-                    uint8_t* sp = stg + (row - wg * 64) * stg_pitch + ccol * 2;
+                    const long long gpix = gp[q];
+                    if (gpix >= 0 || staged) {
+                        uint16_t* op = reinterpret_cast<uint16_t*>(p.out) + gpix * p.out_pitch + n0 + ccol;
+                        uint8_t* sp = stg + (row - wg * 64) * stg_pitch + ccol * 2;
 #pragma unroll
-                    for (int j = 0; j < BLOCK_N / 8; ++j) {
-                        if (n0 + 8 * j >= p.N) continue;  // N % 8 == 0: an 8-column group is all in or all out
-                        const float2 b = *reinterpret_cast<const float2*>(sBias + n0 + 8 * j + ccol);
-                        const float a0 = acc[mi][4 * j + 2 * h], a1 = acc[mi][4 * j + 2 * h + 1];
-                        float f0, f1;
-                        if (p.act) {  // b holds bias / 2 (see the preload)
-                            f0 = silu_from_half(fmaf(a0, 0.5f, b.x));
-                            f1 = silu_from_half(fmaf(a1, 0.5f, b.y));
-                        } else {
-                            f0 = a0 + b.x;
-                            f1 = a1 + b.y;
+                        for (int j = 0; j < BLOCK_N / 8; ++j) {
+                            if (n0 + 8 * j >= p.N) continue;  // N % 8 == 0: an 8-column group is all in or all out
+                            const float2 b = *reinterpret_cast<const float2*>(sBias + n0 + 8 * j + ccol);
+                            const float a0 = acc[mi][4 * j + 2 * h], a1 = acc[mi][4 * j + 2 * h + 1];
+                            float f0, f1;
+                            if (p.act) {  // b holds bias / 2 (see the preload)
+                                f0 = silu_from_half(fmaf(a0, 0.5f, b.x));
+                                f1 = silu_from_half(fmaf(a1, 0.5f, b.y));
+                            } else {
+                                f0 = a0 + b.x;
+                                f1 = a1 + b.y;
+                            }
+                            if (has_res && gpix >= 0) {
+                                const float2 t = unpack2(rv[q][j], bf16);
+                                f0 += t.x;
+                                f1 += t.y;
+                            }
+                            if (staged) *reinterpret_cast<uint32_t*>(sp + 16 * j) = pack2(f0, f1, bf16);
+                            else *reinterpret_cast<uint32_t*>(op + 8 * j) = pack2(f0, f1, bf16);
                         }
-                        if (rp) {  // may alias the output: read here, written below (direct) or after the warpgroup barrier (staged)
-                            const float2 t = unpack2(*reinterpret_cast<const uint32_t*>(rp + 8 * j), bf16);
-                            f0 += t.x;
-                            f1 += t.y;
+                    }
+                    if (staged && h == 1) {  // the sub-tile is complete: the warpgroup's 64 rows leave as whole 16-byte row segments
+                        named_bar_sync(2 + wg, 128);
+                        constexpr int kSeg = BLOCK_N / 8;
+                        for (int i = threadIdx.x & 127; i < 64 * kSeg; i += 128) {
+                            const int lrow = i / kSeg, c = i - lrow * kSeg;
+                            const long long gp = pixel_of(mt, wg * 64 + lrow);
+                            if (gp >= 0 && n0 + 8 * c < p.N)
+                                *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + gp * p.out_pitch + n0 + 8 * c) =
+                                    *reinterpret_cast<const uint4*>(stg + lrow * stg_pitch + c * 16);
                         }
-                        if (staged) *reinterpret_cast<uint32_t*>(sp + 16 * j) = pack2(f0, f1, bf16);
-                        else *reinterpret_cast<uint32_t*>(op + 8 * j) = pack2(f0, f1, bf16);
+                        named_bar_sync(2 + wg, 128);  // the staging block is rewritten by the next sub-tile / tile
                     }
-                }
-                if (staged) {  // the warpgroup's 64 rows leave as whole 16-byte row segments
-                    named_bar_sync(2 + wg, 128);
-                    constexpr int kSeg = BLOCK_N / 8;
-                    for (int i = threadIdx.x & 127; i < 64 * kSeg; i += 128) {
-                        const int lrow = i / kSeg, c = i - lrow * kSeg;
-                        const long long gpix = pixel_of(wg * 64 + lrow);
-                        if (gpix >= 0 && n0 + 8 * c < p.N)
-                            *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + gpix * p.out_pitch + n0 + 8 * c) =
-                                *reinterpret_cast<const uint4*>(stg + lrow * stg_pitch + c * 16);
-                    }
-                    named_bar_sync(2 + wg, 128);  // the staging block is rewritten by the next sub-tile / tile
                 }
             }
         } else {
