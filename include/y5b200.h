@@ -612,6 +612,27 @@ int y5_cross_entropy(const void* logits, int32_t dtype, int32_t batch, int32_t n
                      float label_smoothing, const float* grad_scale, void* dlogits, int64_t dlogits_stride, float* row_loss, float* loss,
                      void* stream);
 
+/* Validation AP (utils/metrics.py:25-126 ap_per_class, utils/segment/metrics.py:17-64 ap_per_class_box_and_mask) in float64.
+ * Rows: image b (0 <= b < n_img) holds rows r < count[b] (clamped to [0, rows_per_image]; count NULL: all), read in (image, row)
+ * order -- the flat form is n_img = 1, count NULL.  Row (b, r): conf / pred_cls at element b * img_stride + r * row_stride,
+ * its niou tp values (uint8, nonzero = true) at tp + b * tp_img_stride + r * tp_row_stride; tp2 (NULL or the same layout)
+ * is a second tp matrix evaluated on the same order (box and mask).  target_cls: nt labels.  Class values must be integers in
+ * [0, 4096); any other value sets a flag in meta[2] (1: a prediction, 2: a label) and its row counts as class 0.
+ * Order: np.argsort(-conf, kind="stable") (equal confidences keep row order, NaN last).  grid (DEVICE, 1101 float64):
+ * np.linspace(0, 1, 1000) then np.linspace(0, 1, 101).  nc_cap = min(nt, 4096).  Outputs (DEVICE):
+ *   out : per set s, at out + s * nc_cap * (5 + niou): tp, fp, p, r, f1 (nc_cap float64 each, at the max mean-F1 index),
+ *         then ap (nc_cap x niou); the first nc entries (rows) are valid
+ *   meta: Y5_AP_META + nc_cap int32 = [rows, nc, flags, max-F1 index of set 0, of set 1, unique classes ascending (nc)]
+ * Every output but the max-F1 index equals the reference's float64 bits at that index; the index comes from the smoothed
+ * mean-F1 curve, whose np.convolve summation order is not reproduced.  niou 1..32 (Y5_E_UNSUPPORTED above),
+ * n_img * rows_per_image < 2^31.  No allocation and no host synchronisation; workspace: y5_ap_workspace_bytes, sets = 1 or 2. */
+#define Y5_AP_META 5
+int64_t y5_ap_workspace_bytes(int32_t n_img, int32_t rows_per_image, int32_t niou, int32_t nt, int32_t sets);
+int y5_ap_per_class(const uint8_t* tp, const uint8_t* tp2, int64_t tp_img_stride, int32_t tp_row_stride, const float* conf,
+                    const float* pred_cls, int64_t img_stride, int32_t row_stride, const int32_t* count, int32_t n_img,
+                    int32_t rows_per_image, int32_t niou, const float* target_cls, int32_t nt, const double* grid, double eps,
+                    void* workspace, int64_t workspace_bytes, double* out, int32_t* meta, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -221,7 +221,11 @@ SIGNATURES = {
     "y5_global_avg_pool": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "y5_global_avg_pool_bwd": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "y5_cross_entropy": (_I32, [_P, _I32, _I32, _I32, _I64, _P, _F, _P, _P, _I64, _P, _P, _P]),
+    "y5_ap_workspace_bytes": (_I64, [_I32, _I32, _I32, _I32, _I32]),
+    "y5_ap_per_class": (_I32, [_P, _P, _I64, _I32, _P, _P, _I64, _I32, _P, _I32, _I32, _I32, _P, _I32, _P, C.c_double, _P, _I64, _P, _P, _P]),
 }
+
+AP_META = 5  # include/y5b200.h Y5_AP_META
 
 _lib = None
 

@@ -2,11 +2,16 @@
 at :158,:252, and the per-image loops of val.py:282-318 and segment/val.py:263-298): box IoU or mask IoU, class test and the
 detection<->label matching rule for the WHOLE batch, with no `.cpu()` round trip per image.  Mask IoU (ultralytics'
 mask_iou, imported by the reference into utils.metrics) is a 1-bit GEMM on the tensor cores: every quantity before the one
-fp32 division is an integer pixel count, so it is bit-exact."""
+fp32 division is an integer pixel count, so it is bit-exact.
+
+The last step of validation, ap_per_class (utils/metrics.py:25-126, val.py:328-330), runs on the device too (y5_ap_per_class):
+one sort of the predictions, then every class and IoU threshold in float64, equal to the reference's numpy arithmetic bit for
+bit under the stable confidence order (see DESIGN.md).  ap_per_class_batch reads the padded per-batch tensors directly."""
 from __future__ import annotations
 
 import ctypes as C
 
+import numpy as np
 import torch
 
 from .. import _lib
@@ -242,3 +247,132 @@ def seg_val_batch_metrics(rows, count, protos, targets, masks, im_shape, shapes,
     if check:
         _raise_nonbinary(nonbinary)
     return predn, correct_bboxes, correct.view(torch.bool)
+
+
+_AP_GRIDS = {}  # device -> np.linspace(0, 1, 1000) and np.linspace(0, 1, 101), the grids ap_per_class interpolates at
+_MAX_CLASSES = 4096
+
+
+def _ap_grid(dev):
+    g = _AP_GRIDS.get(dev)
+    if g is None:
+        g = _AP_GRIDS[dev] = torch.from_numpy(np.concatenate((np.linspace(0, 1, 1000), np.linspace(0, 1, 101)))).to(dev)
+    return g
+
+
+def _ap_device(*xs):
+    for x in xs:
+        if isinstance(x, torch.Tensor) and x.is_cuda:
+            return x.device
+    if not torch.cuda.is_available():
+        raise RuntimeError("y5b200: ap_per_class runs on CUDA only (no CPU / numpy fallback)")
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def _as_f32(x, dev, what):
+    """x as a contiguous float32 tensor on dev (numpy input uploaded once); ValueError when float32 cannot hold its values."""
+    t = torch.as_tensor(x)
+    if t.dtype != torch.float32:
+        f = t.to(torch.float32)
+        same = f.to(t.dtype) == t
+        if t.is_floating_point():
+            same |= torch.isnan(t)
+        if not bool(same.all()):
+            raise ValueError(f"y5b200: {what} ({t.dtype}) holds values float32 cannot represent")
+        t = f
+    return t.to(dev).contiguous().view(-1)
+
+
+def _as_tp(x, dev, what):
+    t = torch.as_tensor(x)
+    if t.dim() != 2:
+        raise ValueError(f"y5b200: {what} must be (n, niou), got {tuple(t.shape)}")
+    return t.to(dev).bool().contiguous().view(torch.uint8)
+
+
+def _ap_run(dev, tps, conf_ptr, cls_ptr, img_stride, row_stride, tp_img_stride, count, n_img, rows, niou, target_cls, eps):
+    """y5_ap_per_class over rows laid out as include/y5b200.h describes; one result tuple (tp, fp, p, r, f1, ap, classes) per
+    tp matrix in `tps`, as numpy arrays."""
+    lib = _lib.lib()
+    tcls = _as_f32(target_cls, dev, "target_cls")
+    nt = tcls.numel()
+    nc_cap = min(nt, _MAX_CLASSES)
+    sets = len(tps)
+    ws_bytes = int(lib.y5_ap_workspace_bytes(n_img, rows, niou, nt, sets))
+    if ws_bytes < 0:
+        _lib.check(ws_bytes, "ap_workspace_bytes")
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    out = torch.empty(max(sets * nc_cap * (5 + niou), 1), dtype=torch.float64, device=dev)
+    meta = torch.empty(_lib.AP_META + nc_cap, dtype=torch.int32, device=dev)
+    with _lib.on(dev):
+        _lib.check(lib.y5_ap_per_class(tps[0].data_ptr() or None, tps[1].data_ptr() or None if sets == 2 else None, tp_img_stride, niou,
+                                       conf_ptr or None, cls_ptr or None, img_stride, row_stride,
+                                       count.data_ptr() if count is not None else None, n_img, rows, niou,
+                                       tcls.data_ptr() if nt else None, nt, _ap_grid(dev).data_ptr(), float(eps), ws.data_ptr(), ws_bytes,
+                                       out.data_ptr(), meta.data_ptr(), C.c_void_p(_lib.stream_ptr(dev))), "ap_per_class")
+    meta_h = meta.cpu().numpy()
+    if meta_h[2]:
+        what = " and ".join(w for bit, w in ((1, "predicted classes"), (2, "target classes")) if meta_h[2] & bit)
+        raise ValueError(f"y5b200: ap_per_class takes integral class values in [0, {_MAX_CLASSES}); the {what} hold others")
+    nc = int(meta_h[1])
+    classes = meta_h[_lib.AP_META:_lib.AP_META + nc].astype(np.int64)
+    out_h = out.cpu().numpy()
+    results = []
+    for s in range(sets):
+        o = out_h[s * nc_cap * (5 + niou):(s + 1) * nc_cap * (5 + niou)]
+        tp, fp, p, r, f1 = (o[k * nc_cap:k * nc_cap + nc].copy() for k in range(5))
+        ap = o[5 * nc_cap:].reshape(nc_cap, niou)[:nc].copy()
+        results.append((tp, fp, p, r, f1, ap, classes.copy()))
+    return results
+
+
+def _ap_flat(tps, conf, pred_cls, target_cls, eps):
+    dev = _ap_device(*tps, conf, pred_cls, target_cls)
+    tps = [_as_tp(t, dev, "tp") for t in tps]
+    n, niou = tps[0].shape
+    cf, cl = _as_f32(conf, dev, "conf"), _as_f32(pred_cls, dev, "pred_cls")
+    if cf.numel() != n or cl.numel() != n or any(t.shape != tps[0].shape for t in tps):
+        raise ValueError(f"y5b200: ap_per_class: tp {[tuple(t.shape) for t in tps]}, conf ({cf.numel()},), pred_cls ({cl.numel()},) disagree")
+    return _ap_run(dev, tps, cf.data_ptr(), cl.data_ptr(), 0, 1, 0, None, 1, n, niou, target_cls, eps)
+
+
+def _box_and_mask(res_b, res_m):
+    return {k: {"p": r[2], "r": r[3], "ap": r[5], "f1": r[4], "ap_class": r[6]} for k, r in (("boxes", res_b), ("masks", res_m))}
+
+
+def ap_per_class(tp, conf, pred_cls, target_cls, plot=False, save_dir=".", names=(), eps=1e-16, prefix=""):
+    """Reference signature (utils/metrics.py:25): tp (n, niou) bool, conf (n,), pred_cls (n,), target_cls (m,) as numpy arrays
+    (uploaded once) or CUDA tensors -> numpy (tp, fp, p, r, f1, ap, unique_classes), float64 and int64, as the reference
+    returns them.  Rows are ordered by np.argsort(-conf, kind="stable"); class values must be integers in [0, 4096)
+    (ValueError otherwise).  Plots need matplotlib, which the engine does not depend on: plot=True raises."""
+    if plot:
+        raise NotImplementedError("y5b200: ap_per_class(plot=True): plotting is not ported (validation runs with plots=False)")
+    return _ap_flat([tp], conf, pred_cls, target_cls, eps)[0]
+
+
+def ap_per_class_batch(correct, rows, count, target_cls, eps=1e-16, correct_masks=None):
+    """ap_per_class over the padded tensors of a batched val loop, concatenated along dim 0 over batches: correct (I, max_det,
+    niou) bool (val_batch_metrics; correct_masks likewise from seg_val_batch_metrics), rows (I, max_det, >=6) float32 with conf
+    in column 4 and class in column 5, count (I,) valid rows per image, target_cls (m,) the labels' classes.  Reads rows
+    r < count[i] in (image, row) order, the order of val.py's per-image stats.append; padding rows are never read.  Returns
+    ap_per_class's tuple, or with correct_masks ap_per_class_box_and_mask's dict (one sort for both)."""
+    dev = _ap_device(correct, rows, count, target_cls)
+    if rows.dim() != 3 or rows.shape[2] < 6 or rows.dtype != torch.float32:
+        raise ValueError(f"y5b200: ap_per_class_batch: rows must be (I, max_det, >=6) float32, got {tuple(rows.shape)} {rows.dtype}")
+    n_img, max_det = rows.shape[:2]
+    tps = [correct] if correct_masks is None else [correct, correct_masks]
+    if any(t.dim() != 3 or tuple(t.shape[:2]) != (n_img, max_det) for t in tps):
+        raise ValueError(f"y5b200: ap_per_class_batch: correct {[tuple(t.shape) for t in tps]} must be ({n_img}, {max_det}, niou)")
+    if count.numel() != n_img:
+        raise ValueError(f"y5b200: ap_per_class_batch: count has {count.numel()} entries for {n_img} images")
+    niou = tps[0].shape[2]
+    if tps[-1].shape[2] != niou:
+        raise ValueError("y5b200: ap_per_class_batch: correct and correct_masks have different thresholds")
+    tps = [_as_tp(t.reshape(n_img * max_det, niou), dev, "correct") for t in tps]
+    r = rows.to(dev)
+    if r.stride(2) != 1:
+        r = r.contiguous()
+    cnt = count.to(dev, torch.int32).contiguous()
+    res = _ap_run(dev, tps, r.data_ptr() + 16, r.data_ptr() + 20, r.stride(0), r.stride(1), max_det * niou, cnt, n_img, max_det, niou,
+                  target_cls, eps)
+    return res[0] if correct_masks is None else _box_and_mask(*res)
