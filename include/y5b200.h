@@ -352,6 +352,32 @@ int y5_letterbox(const y5_letterbox_image* images, int32_t n_images, int32_t out
                  int32_t pad_value, void* out, int32_t out_dtype, int32_t s2d, int32_t out_row_px, int32_t out_x_off,
                  void* stream);
 
+/* Validation batch (utils/dataloaders.py:711-766, augment=False): load_image's resize of each ORIGINAL image to
+ * (res_h, res_w) = (ceil(h0 r), ceil(w0 r)) -- Y5_VAL_AREA (cv2 INTER_AREA, r < 1), Y5_VAL_LINEAR (cv2 INTER_LINEAR,
+ * r > 1) or Y5_VAL_COPY (r == 1) -- then letterbox(auto=False, scaleup=False) into the (out_h, out_w) canvas with
+ * border 114, CHW with RGB order.  Both resizes are OpenCV's arithmetic restated bit for bit (oracle/val_load_ref.py).
+ * When letterbox resizes again ((new_h, new_w) != (res_h, res_w)) the load_image result is written HWC BGR to the
+ * image's `scratch` (res_h * res_w * 3 bytes, DEVICE) and y5_letterbox takes it from there; otherwise scratch is unused
+ * and the image sits at (top, left) unchanged.  out: (n, 3, out_h, out_w) Y5_U8, or Y5_F16 | Y5_BF16 | Y5_F32 as
+ * float32(v) * float32(1 / 255) rounded once (what `im.half() / 255` computes on a CUDA tensor).  `images` is a HOST
+ * array; sources and out are DEVICE memory.  No allocation and no host synchronisation. */
+#define Y5_VAL_COPY 0
+#define Y5_VAL_LINEAR 1
+#define Y5_VAL_AREA 2
+struct y5_val_image {
+    const void* data;       /* the original image: uint8 HWC BGR, 3 channels */
+    void* scratch;          /* (res_h, res_w, 3) uint8 when new != res, else NULL */
+    int32_t src_h, src_w;
+    int32_t row_bytes;      /* bytes between source rows (>= 3 * src_w) */
+    int32_t res_h, res_w;   /* load_image's size */
+    int32_t interp;         /* Y5_VAL_* */
+    int32_t new_h, new_w;   /* letterbox's new_unpad */
+    int32_t top, left;      /* letterbox's border offsets inside the canvas */
+};
+typedef struct y5_val_image y5_val_image;
+int y5_val_letterbox(const y5_val_image* images, int32_t n_images, int32_t out_h, int32_t out_w, void* out, int32_t out_dtype,
+                     void* stream);
+
 /* process_mask (utils/segment/general.py:25-52, crop_mask :10-22): for detection i of image img_index[i] (NULL = image 0):
  * sigmoid(coef_i . protos[img]) at mask resolution, zeroed outside the box scaled by (mw/in_w, mh/in_h), optionally
  * bilinearly up-sampled (align_corners=False) to (in_h,in_w), thresholded at 0.5.

@@ -94,6 +94,17 @@ class LetterboxImage(C.Structure):
     ]
 
 
+class ValImage(C.Structure):
+    _fields_ = [
+        ("data", C.c_void_p), ("scratch", C.c_void_p), ("src_h", C.c_int32), ("src_w", C.c_int32), ("row_bytes", C.c_int32),
+        ("res_h", C.c_int32), ("res_w", C.c_int32), ("interp", C.c_int32), ("new_h", C.c_int32), ("new_w", C.c_int32),
+        ("top", C.c_int32), ("left", C.c_int32),
+    ]
+
+
+VAL_COPY, VAL_LINEAR, VAL_AREA = 0, 1, 2  # include/y5b200.h Y5_VAL_*
+
+
 class OptTensor(C.Structure):
     _fields_ = [
         ("param", C.c_void_p), ("grad", C.c_void_p), ("mom", C.c_void_p), ("ema", C.c_void_p),
@@ -195,6 +206,7 @@ SIGNATURES = {
     "y5_loss_fwd_bwd_scaled": (_I32, [C.POINTER(LossParams), C.POINTER(_P), _P, _P, _P, C.POINTER(_P), _P, _P, _I64, _P]),
     "y5_letterbox_max_images": (_I32, []),
     "y5_letterbox": (_I32, [C.POINTER(LetterboxImage), _I32, _I32, _I32, _I32, _I32, _P, _I32, _I32, _I32, _I32, _P]),
+    "y5_val_letterbox": (_I32, [C.POINTER(ValImage), _I32, _I32, _I32, _P, _I32, _P]),
     "y5_process_mask_workspace_bytes": (_I64, [_I32, _I32, _I32, _I32]),
     "y5_process_mask": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, C.POINTER(_I32), _P, _I32, _P, _I64,
                                 _P]),

@@ -43,6 +43,25 @@ __device__ __forceinline__ void lb_coeff(int d, double scale, int src, bool hori
     i1 = min(max(s + 1, 0), src - 1);
 }
 
+// cv2.resize INTER_LINEAR (uint8, 3 channels) of a src_h x src_w image to dst_h x dst_w, at destination pixel (rx, ry)
+__device__ __forceinline__ void linear_px(const uint8_t* src, int row_bytes, int src_h, int src_w, int dst_h, int dst_w, int rx, int ry,
+                                          int (&v)[3]) {
+    const double sx = 1.0 / (static_cast<double>(dst_w) / static_cast<double>(src_w));
+    const double sy = 1.0 / (static_cast<double>(dst_h) / static_cast<double>(src_h));
+    int x0, x1, a0, a1, y0, y1, b0, b1;
+    lb_coeff(rx, sx, src_w, true, x0, x1, a0, a1);
+    lb_coeff(ry, sy, src_h, false, y0, y1, b0, b1);
+    const uint8_t* r0 = src + static_cast<long long>(y0) * row_bytes;
+    const uint8_t* r1 = src + static_cast<long long>(y1) * row_bytes;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int s0 = r0[x0 * 3 + c] * a0 + r0[x1 * 3 + c] * a1;
+        const int s1 = r1[x0 * 3 + c] * a0 + r1[x1 * 3 + c] * a1;
+        const int o = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
+        v[c] = min(max(o, 0), 255);
+    }
+}
+
 // OUT: 0 = uint8 NCHW, 1 = fp16/bf16 NCHW (/255), 2 = fp32 NCHW (/255), 3 = stem space-to-depth cells (16 channels)
 template <int OUT>
 __global__ void letterbox_kernel(const LbBatch L, int n_img, int out_h, int out_w, int swap_rb, int pad_value, void* __restrict__ out,
@@ -51,8 +70,6 @@ __global__ void letterbox_kernel(const LbBatch L, int n_img, int out_h, int out_
     if (b >= n_img) return;
     const y5_letterbox_image im = L.im[b];
     const uint8_t* src = static_cast<const uint8_t*>(im.data);
-    const double sx = 1.0 / (static_cast<double>(im.new_w) / static_cast<double>(im.src_w));
-    const double sy = 1.0 / (static_cast<double>(im.new_h) / static_cast<double>(im.src_h));
     // OUT 3 handles a 2x2 block of output pixels per thread (one s2d cell); the others one pixel per thread
     const int step = OUT == 3 ? 2 : 1;
     const int cx = (blockIdx.x * blockDim.x + threadIdx.x) * step;
@@ -68,20 +85,7 @@ __global__ void letterbox_kernel(const LbBatch L, int n_img, int out_h, int out_
             const int ox = cx + dx, oy = cy + dy;
             int v[3] = {pad_value, pad_value, pad_value};
             const int rx = ox - im.left, ry = oy - im.top;
-            if (rx >= 0 && rx < im.new_w && ry >= 0 && ry < im.new_h) {
-                int x0, x1, a0, a1, y0, y1, b0, b1;
-                lb_coeff(rx, sx, im.src_w, true, x0, x1, a0, a1);
-                lb_coeff(ry, sy, im.src_h, false, y0, y1, b0, b1);
-                const uint8_t* r0 = src + static_cast<long long>(y0) * im.row_bytes;
-                const uint8_t* r1 = src + static_cast<long long>(y1) * im.row_bytes;
-#pragma unroll
-                for (int c = 0; c < 3; ++c) {
-                    const int s0 = r0[x0 * 3 + c] * a0 + r0[x1 * 3 + c] * a1;
-                    const int s1 = r1[x0 * 3 + c] * a0 + r1[x1 * 3 + c] * a1;
-                    int o = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
-                    v[c] = min(max(o, 0), 255);
-                }
-            }
+            if (rx >= 0 && rx < im.new_w && ry >= 0 && ry < im.new_h) linear_px(src, im.row_bytes, im.src_h, im.src_w, im.new_h, im.new_w, rx, ry, v);
             if (swap_rb) { const int t = v[0]; v[0] = v[2]; v[2] = t; }
             if (OUT == 3) {
 #pragma unroll
@@ -105,6 +109,132 @@ __global__ void letterbox_kernel(const LbBatch L, int n_img, int out_h, int out_
         const long long opx = (static_cast<long long>(b) * (out_h >> 1) + (cy >> 1)) * row_px + x_off + (cx >> 1);
         static_cast<uint4*>(out)[opx * 2] = lo;
         static_cast<uint4*>(out)[opx * 2 + 1] = hi;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// validation batch: load_image's resize + letterbox(scaleup=False)
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kValMaxImages = 64;  // descriptors travel by value in the kernel parameter block (64 x 56 bytes)
+
+// kVal*: to the canvas at (top, left), HWC BGR to `dst` (the scratch of a letterbox that resizes again), or not at all
+enum : int { kValCanvas = 0, kValScratch = 1, kValSkip = 2 };
+
+struct ValDesc {
+    const uint8_t* src;
+    uint8_t* dst;
+    int src_h, src_w, row_bytes, res_h, res_w, interp, top, left, mode, reserved;
+};
+
+struct ValBatch {
+    ValDesc im[kValMaxImages];
+};
+
+// OpenCV's computeResizeAreaTab for one destination index: the source cell [d s, d s + s) with s = 1 / (dst / src) as
+// taps s1 - first .. s2 - 1 + last; whole pixels weigh 1 / w, a partial first / last one its covered fraction / w
+struct AreaAxis {
+    int s1, n;
+    float w_first, w_mid, w_last;
+    bool first, last;
+};
+
+__device__ __forceinline__ AreaAxis area_axis(int d, double scale, int src) {
+    AreaAxis a;
+    const double f1 = __dmul_rn(static_cast<double>(d), scale);
+    const double f2 = __dadd_rn(f1, scale);
+    const double cw = fmin(scale, __dsub_rn(static_cast<double>(src), f1));
+    int s2 = min(static_cast<int>(floor(f2)), src - 1);
+    const int s1 = min(static_cast<int>(ceil(f1)), s2);
+    const double head = __dsub_rn(static_cast<double>(s1), f1), tail = __dsub_rn(f2, static_cast<double>(s2));
+    a.first = head > 1e-3;
+    a.last = tail > 1e-3;
+    a.w_first = static_cast<float>(__ddiv_rn(head, cw));
+    a.w_mid = static_cast<float>(__ddiv_rn(1.0, cw));
+    a.w_last = static_cast<float>(__ddiv_rn(fmin(fmin(tail, 1.0), cw), cw));
+    a.s1 = s1 - (a.first ? 1 : 0);
+    a.n = (s2 - s1) + (a.first ? 1 : 0) + (a.last ? 1 : 0);
+    return a;
+}
+
+__device__ __forceinline__ float area_weight(const AreaAxis& a, int t) {
+    return a.first && t == 0 ? a.w_first : (a.last && t == a.n - 1 ? a.w_last : a.w_mid);
+}
+
+__device__ __forceinline__ int round_u8(float f) { return min(max(__float2int_rn(f), 0), 255); }
+
+// cv2.resize INTER_AREA (uint8, 3 channels, shrinking in both axes) at destination pixel (rx, ry)
+__device__ void area_px(const uint8_t* src, int row_bytes, int src_h, int src_w, int dst_h, int dst_w, int rx, int ry, int (&v)[3]) {
+    const double sx = 1.0 / (static_cast<double>(dst_w) / static_cast<double>(src_w));
+    const double sy = 1.0 / (static_cast<double>(dst_h) / static_cast<double>(src_h));
+    const int kx = __double2int_rn(sx), ky = __double2int_rn(sy);
+    if (fabs(sx - kx) < 2.220446049250313e-16 && fabs(sy - ky) < 2.220446049250313e-16) {
+        // "area fast": integer cells summed exactly; 2 x 2 rounds as (sum + 2) >> 2, others as cvRound(sum * (1.f / area))
+        const uint8_t* p = src + static_cast<long long>(ry) * ky * row_bytes + rx * kx * 3;
+        int s[3] = {0, 0, 0};
+        for (int y = 0; y < ky; ++y)
+            for (int x = 0; x < kx; ++x)
+#pragma unroll
+                for (int c = 0; c < 3; ++c) s[c] += p[static_cast<long long>(y) * row_bytes + x * 3 + c];
+        const float inv = __fdiv_rn(1.0f, static_cast<float>(kx * ky));
+#pragma unroll
+        for (int c = 0; c < 3; ++c) v[c] = kx == 2 && ky == 2 ? (s[c] + 2) >> 2 : round_u8(__fmul_rn(static_cast<float>(s[c]), inv));
+        return;
+    }
+    // weighted cells: each source row summed across its x taps, then the rows across their y taps, in float32 in tap order
+    const AreaAxis ax = area_axis(rx, sx, src_w), ay = area_axis(ry, sy, src_h);
+    float sum[3] = {0.f, 0.f, 0.f};
+    for (int ty = 0; ty < ay.n; ++ty) {
+        const uint8_t* row = src + static_cast<long long>(ay.s1 + ty) * row_bytes;
+        const float beta = area_weight(ay, ty);
+        float buf[3] = {0.f, 0.f, 0.f};
+        for (int tx = 0; tx < ax.n; ++tx) {
+            const float alpha = area_weight(ax, tx);
+            const uint8_t* q = row + (ax.s1 + tx) * 3;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) buf[c] = __fadd_rn(buf[c], __fmul_rn(static_cast<float>(q[c]), alpha));
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) sum[c] = __fadd_rn(sum[c], __fmul_rn(beta, buf[c]));
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = round_u8(sum[c]);
+}
+
+// OUT: 0 = uint8, 1 = fp16/bf16, 2 = fp32 (float32(v) * float32(1/255), rounded once); CHW RGB
+template <int OUT>
+__global__ void val_letterbox_kernel(const ValBatch L, int out_h, int out_w, void* __restrict__ out, int bf16) {
+    const int b = blockIdx.z;
+    const ValDesc& im = L.im[b];
+    const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y * blockDim.y + threadIdx.y;
+    if (im.mode == kValSkip) return;
+    const bool to_scratch = im.mode == kValScratch;
+    const int rx = to_scratch ? ox : ox - im.left, ry = to_scratch ? oy : oy - im.top;
+    if (to_scratch ? (rx >= im.res_w || ry >= im.res_h) : (ox >= out_w || oy >= out_h)) return;
+    int v[3] = {114, 114, 114};
+    if (rx >= 0 && rx < im.res_w && ry >= 0 && ry < im.res_h) {
+        if (im.interp == Y5_VAL_AREA) {
+            area_px(im.src, im.row_bytes, im.src_h, im.src_w, im.res_h, im.res_w, rx, ry, v);
+        } else if (im.interp == Y5_VAL_LINEAR) {
+            linear_px(im.src, im.row_bytes, im.src_h, im.src_w, im.res_h, im.res_w, rx, ry, v);
+        } else {
+            const uint8_t* p = im.src + static_cast<long long>(ry) * im.row_bytes + rx * 3;
+            v[0] = p[0]; v[1] = p[1]; v[2] = p[2];
+        }
+    }
+    if (to_scratch) {
+        uint8_t* d = im.dst + (static_cast<long long>(ry) * im.res_w + rx) * 3;
+        d[0] = static_cast<uint8_t>(v[0]); d[1] = static_cast<uint8_t>(v[1]); d[2] = static_cast<uint8_t>(v[2]);
+        return;
+    }
+    const long long plane = static_cast<long long>(out_h) * out_w;
+    const long long o = static_cast<long long>(b) * 3 * plane + static_cast<long long>(oy) * out_w + ox;
+    const float inv255 = 1.0f / 255.0f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int x = v[2 - c];  // BGR -> RGB
+        if (OUT == 0) static_cast<uint8_t*>(out)[o + c * plane] = static_cast<uint8_t>(x);
+        else if (OUT == 1) static_cast<uint16_t*>(out)[o + c * plane] = pack1(__fmul_rn(static_cast<float>(x), inv255), bf16 != 0);
+        else static_cast<float*>(out)[o + c * plane] = __fmul_rn(static_cast<float>(x), inv255);
     }
 }
 
@@ -363,6 +493,68 @@ extern "C" Y5_API int y5_letterbox(const y5_letterbox_image* images, int32_t n_i
         count_launch();
     }
     return last_status("letterbox");
+}
+
+static void launch_val(const ValBatch& L, int nb, int grid_w, int grid_h, int out_h, int out_w, void* out, int out_dtype, cudaStream_t st) {
+    const dim3 block(32, 8);
+    const dim3 grid((grid_w + block.x - 1) / block.x, (grid_h + block.y - 1) / block.y, nb);
+    if (out_dtype == Y5_U8) val_letterbox_kernel<0><<<grid, block, 0, st>>>(L, out_h, out_w, out, 0);
+    else if (out_dtype == Y5_F32) val_letterbox_kernel<2><<<grid, block, 0, st>>>(L, out_h, out_w, out, 0);
+    else val_letterbox_kernel<1><<<grid, block, 0, st>>>(L, out_h, out_w, out, out_dtype == Y5_BF16);
+    count_launch();
+}
+
+extern "C" Y5_API int y5_val_letterbox(const y5_val_image* images, int32_t n_images, int32_t out_h, int32_t out_w, void* out, int32_t out_dtype,
+                                       void* stream) {
+    if (!images || !out || n_images <= 0 || out_h <= 0 || out_w <= 0) return set_error(Y5_E_INVALID, "val_letterbox: bad argument");
+    if (out_dtype != Y5_U8 && out_dtype != Y5_F16 && out_dtype != Y5_BF16 && out_dtype != Y5_F32)
+        return set_error(Y5_E_UNSUPPORTED, "val_letterbox: output dtype");
+    constexpr int kMaxSide = 1 << 15;
+    if (out_h > kMaxSide || out_w > kMaxSide) return set_error(Y5_E_UNSUPPORTED, "val_letterbox: canvas larger than %d", kMaxSide);
+    for (int i = 0; i < n_images; ++i) {
+        const y5_val_image& im = images[i];
+        const bool again = im.new_h != im.res_h || im.new_w != im.res_w;
+        if (!im.data || im.src_h <= 0 || im.src_w <= 0 || im.res_h <= 0 || im.res_w <= 0 || im.new_h <= 0 || im.new_w <= 0 ||
+            im.row_bytes < im.src_w * 3 || im.top < 0 || im.left < 0 || im.top + im.new_h > out_h || im.left + im.new_w > out_w ||
+            (again && !im.scratch))
+            return set_error(Y5_E_INVALID, "val_letterbox: image %d does not fit the %dx%d output (src %dx%d load %dx%d new %dx%d top %d left %d%s)", i,
+                             out_h, out_w, im.src_h, im.src_w, im.res_h, im.res_w, im.new_h, im.new_w, im.top, im.left,
+                             again && !im.scratch ? ", no scratch" : "");
+        if (im.src_h > kMaxSide || im.src_w > kMaxSide || im.res_h > kMaxSide || im.res_w > kMaxSide)
+            return set_error(Y5_E_UNSUPPORTED, "val_letterbox: image %d larger than %d", i, kMaxSide);
+        const bool ok = im.interp == Y5_VAL_COPY ? im.res_h == im.src_h && im.res_w == im.src_w
+                      : im.interp == Y5_VAL_AREA ? im.res_h <= im.src_h && im.res_w <= im.src_w
+                                                 : im.interp == Y5_VAL_LINEAR;
+        if (!ok) return set_error(Y5_E_UNSUPPORTED, "val_letterbox: image %d: interp %d from %dx%d to %dx%d", i, im.interp, im.src_h, im.src_w, im.res_h,
+                                  im.res_w);
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t elem = out_dtype == Y5_U8 ? 1 : (out_dtype == Y5_F32 ? 4 : 2);
+    const size_t img_bytes = static_cast<size_t>(3) * out_h * out_w * elem;
+    for (int i0 = 0; i0 < n_images; i0 += kValMaxImages) {
+        const int nb = n_images - i0 < kValMaxImages ? n_images - i0 : kValMaxImages;
+        ValBatch L, A;  // L: load_image (+ letterbox when it only pads); A: letterbox's own resize from the scratch
+        int gw = out_w, gh = out_h, again = 0;
+        for (int i = 0; i < nb; ++i) {
+            const y5_val_image& im = images[i0 + i];
+            ValDesc& d = L.im[i];
+            d = ValDesc{static_cast<const uint8_t*>(im.data), static_cast<uint8_t*>(im.scratch), im.src_h, im.src_w, im.row_bytes, im.res_h, im.res_w,
+                        im.interp, im.top, im.left, kValCanvas, 0};
+            A.im[i] = ValDesc{nullptr, nullptr, 0, 0, 0, 0, 0, 0, 0, 0, kValSkip, 0};
+            if (im.new_h != im.res_h || im.new_w != im.res_w) {
+                d.mode = kValScratch;
+                gw = gw > im.res_w ? gw : im.res_w;
+                gh = gh > im.res_h ? gh : im.res_h;
+                A.im[i] = ValDesc{static_cast<const uint8_t*>(im.scratch), nullptr, im.res_h, im.res_w, im.res_w * 3, im.new_h, im.new_w, Y5_VAL_LINEAR,
+                                  im.top, im.left, kValCanvas, 0};
+                again = 1;
+            }
+        }
+        void* o = static_cast<uint8_t*>(out) + static_cast<size_t>(i0) * img_bytes;
+        launch_val(L, nb, gw, gh, out_h, out_w, o, out_dtype, st);
+        if (again) launch_val(A, nb, out_w, out_h, out_h, out_w, o, out_dtype, st);
+    }
+    return last_status("val_letterbox");
 }
 
 extern "C" Y5_API int64_t y5_process_mask_workspace_bytes(int32_t n, int32_t mh, int32_t mw, int32_t mode) {

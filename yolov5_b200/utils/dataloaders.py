@@ -12,11 +12,17 @@ LoadImagesAndLabels.__getitem__ + collate_fn with augment=True, rect=False).
      letterboxed first (``y5_letterbox``) into a scratch canvas; ``y5_aug_labels`` transforms, filters and compacts the
      labels.  The one host synchronisation is the read of the label count that sizes ``targets``.
 With num_workers=0 and the same seeds the batches equal the reference's byte for byte (tests/test_augment_gpu.py).
+
+``DeviceValLoader`` is the validation loader (``create_dataloader(..., augment=False, rect=True, pad=0.5)``, reference
+utils/dataloaders.py:696-790): a pool of host threads decodes one batch ahead, and ``y5_val_letterbox`` does
+load_image's resize (cv2 INTER_AREA / INTER_LINEAR) and the letterbox in one launch; see its docstring.
 """
 from __future__ import annotations
 
 import ctypes
+import math
 import random
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -251,3 +257,262 @@ class DeviceAugmentLoader:
         nt = int(count.item())
         return imgs, padded[:nt], paths, tuple(shapes)
 
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# validation
+# ----------------------------------------------------------------------------------------------------------------------
+def load_val_image(ds, i):
+    """The validation loader's decode step for dataset image i -> (uint8 HWC BGR image, (h0, w0), cached).  cached: the
+    image is the RAM cache's ``ds.ims[i]``, already resized by load_image; otherwise it is the original image, from the
+    ``.npy`` disk cache or ``cv2.imread``.  Runs on the loader's worker threads (cv2 and np.load release the GIL)."""
+    ims = getattr(ds, "ims", None)
+    if ims is not None and ims[i] is not None:
+        return ims[i], tuple(int(v) for v in ds.im_hw0[i]), True
+    npy = getattr(ds, "npy_files", None)
+    if npy is not None and npy[i].exists():
+        im = np.load(npy[i])
+    else:
+        import cv2
+
+        im = cv2.imread(ds.im_files[i])
+        if im is None:
+            raise FileNotFoundError(f"Image Not Found {ds.im_files[i]}")
+    return im, tuple(int(v) for v in im.shape[:2]), False
+
+
+def check_val_dataset(ds, batch_size, name="DeviceValLoader"):
+    """Refuse what the validation path does not implement, before any work."""
+    if getattr(ds, "augment", False):
+        raise NotImplementedError(f"y5b200: {name} implements augment=False only (use the augment loaders for training batches)")
+    if getattr(ds, "image_weights", False):
+        raise NotImplementedError(f"y5b200: {name}: image_weights is not implemented")
+    s = int(ds.img_size)
+    if s <= 0 or s > 16384:
+        raise ValueError(f"y5b200: img_size {ds.img_size} outside (0, 16384]")
+    if getattr(ds, "rect", False):
+        n = len(ds.batch)
+        if not np.array_equal(np.asarray(ds.batch), np.arange(n) // int(batch_size)):
+            raise ValueError(f"y5b200: batch_size {batch_size} disagrees with the dataset's rect batches (built for another batch size)")
+
+
+def val_geometry(ds, k, hw0, cached, im_hw):
+    """(load_image size (h, w), interp, batch shape (H, W), letterbox geometry) of dataset image k."""
+    s = int(ds.img_size)
+    if cached:
+        (h, w), interp = im_hw, _lib.VAL_COPY
+    else:
+        h0, w0 = hw0
+        r = s / max(h0, w0)
+        if r == 1:
+            (h, w), interp = (h0, w0), _lib.VAL_COPY
+        else:
+            (h, w), interp = (math.ceil(h0 * r), math.ceil(w0 * r)), (_lib.VAL_LINEAR if r > 1 else _lib.VAL_AREA)
+    # the batch_shapes row as __getitem__ passes it: its numpy integers make letterbox's ratio and pads np.float64, which
+    # NumPy does not treat as weak scalars, so the label maths below round as the reference's do
+    shape = ds.batch_shapes[ds.batch[k]] if getattr(ds, "rect", False) else s
+    new_unpad, ratio, pad, (top, bottom, left, right) = letterbox_geometry((h, w), shape, auto=False, scaleup=False)
+    hw = (int(shape[0]), int(shape[1])) if getattr(ds, "rect", False) else (s, s)
+    return (h, w), interp, hw, ((int(new_unpad[0]), int(new_unpad[1])), ratio, pad, (int(top), int(bottom), int(left), int(right)))
+
+
+def val_label_rows(labels, ratio, w, h, pad, out_w, out_h):
+    """__getitem__'s label path (augment=False): xywhn2xyxy(ratio * w, ratio * h, pad) then xyxy2xywhn(clip=True,
+    eps=1e-3), in float32 as NumPy computes it from the float32 labels -> (n, 5) float32 [cls, xywhn]."""
+    lab = np.array(labels, dtype=np.float32, copy=True).reshape(-1, 5)
+    if not lab.size:
+        return lab
+    x = lab[:, 1:]
+    y = np.copy(x)
+    sw, sh = ratio[0] * w, ratio[1] * h
+    y[..., 0] = sw * (x[..., 0] - x[..., 2] / 2) + pad[0]
+    y[..., 1] = sh * (x[..., 1] - x[..., 3] / 2) + pad[1]
+    y[..., 2] = sw * (x[..., 0] + x[..., 2] / 2) + pad[0]
+    y[..., 3] = sh * (x[..., 1] + x[..., 3] / 2) + pad[1]
+    lab[:, 1:] = y
+    b = lab[:, 1:5]
+    b[..., [0, 2]] = b[..., [0, 2]].clip(0, out_w - 1e-3)
+    b[..., [1, 3]] = b[..., [1, 3]].clip(0, out_h - 1e-3)
+    y = np.copy(b)
+    y[..., 0] = ((b[..., 0] + b[..., 2]) / 2) / out_w
+    y[..., 1] = ((b[..., 1] + b[..., 3]) / 2) / out_h
+    y[..., 2] = (b[..., 2] - b[..., 0]) / out_w
+    y[..., 3] = (b[..., 3] - b[..., 1]) / out_h
+    lab[:, 1:5] = y
+    return lab
+
+
+class _Staging:
+    """Two pinned staging buffers used in turn; a buffer is reused once the copy that last read it has run."""
+
+    def __init__(self):
+        self.buf = [None, None]
+        self.done = [None, None]
+        self.turn = 0
+
+    def get(self, nbytes):
+        k = self.turn
+        self.turn ^= 1
+        if self.done[k] is not None:
+            self.done[k].synchronize()
+        if self.buf[k] is None or self.buf[k].numel() < nbytes:
+            self.buf[k] = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8).pin_memory()
+        return k, self.buf[k]
+
+    def mark(self, k, stream):
+        self.done[k] = torch.cuda.Event()
+        self.done[k].record(stream)
+
+
+class ValBatchLayout:
+    """Host side of one validation batch: decoded images, geometry, shapes and label rows, laid out in one staging
+    buffer as [sources | extra host blocks], plus the device scratch the letterboxes that resize again need."""
+
+    def __init__(self, ds, positions, loaded):
+        self.keys = [int(ds.indices[p]) for p in positions]
+        self.n = len(positions)
+        self.items, self.shapes, self.rows, self.offs = [], [], [], []
+        pos = scratch = 0
+        batch_shape = None
+        for b, (k, (im, hw0, cached)) in enumerate(zip(self.keys, loaded)):
+            if not isinstance(im, np.ndarray) or im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError(f"y5b200: image {k} must be a uint8 HWC BGR image with 3 channels")
+            if min(im.shape[:2]) < 1:
+                raise ValueError(f"y5b200: image {k} is empty")
+            im = np.ascontiguousarray(im)
+            (h, w), interp, shape, (new_unpad, ratio, pad, (top, _, left, _)) = val_geometry(ds, k, hw0, cached, im.shape[:2])
+            if batch_shape is None:
+                batch_shape = shape
+            elif shape != batch_shape:
+                raise ValueError(f"y5b200: image {k} has batch shape {shape}, the batch {batch_shape}")
+            again = tuple(new_unpad) != (w, h)
+            self.items.append(dict(im=im, res=(h, w), interp=interp, new=(new_unpad[1], new_unpad[0]), top=top, left=left,
+                                   scratch=scratch if again else None, ratio=ratio, pad=pad))
+            if again:
+                scratch += (h * w * 3 + _ALIGN - 1) // _ALIGN * _ALIGN
+            self.shapes.append(((int(hw0[0]), int(hw0[1])), ((h / hw0[0], w / hw0[1]), pad)))
+            self.offs.append(pos)
+            pos += (im.nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
+        self.out_hw = batch_shape
+        self.pos = pos
+        self.scratch_bytes = scratch
+        self.blocks = []
+
+    def label_rows(self, ds, b, out_w, out_h):
+        it = self.items[b]
+        return val_label_rows(ds.labels[self.keys[b]], it["ratio"], it["res"][1], it["res"][0], it["pad"], out_w, out_h)
+
+    def add_block(self, a):
+        """Append a host array to the staging layout -> its byte offset."""
+        a = np.ascontiguousarray(a)
+        off = self.pos
+        self.blocks.append((off, a))
+        self.pos += (a.nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
+        return off
+
+    def upload(self, staging, dev):
+        """One pinned host-to-device copy of the sources and blocks -> (device buffer, scratch base address)."""
+        total = self.pos
+        dev_buf = torch.empty(total + self.scratch_bytes, dtype=torch.uint8, device=dev)
+        k, pinned = staging.get(total)
+        host = pinned.numpy()
+        for off, it in zip(self.offs, self.items):
+            a = it["im"]
+            host[off: off + a.nbytes] = a.reshape(-1)
+        for off, a in self.blocks:
+            host[off: off + a.nbytes] = a.view(np.uint8).reshape(-1)
+        stream = torch.cuda.current_stream(dev)
+        dev_buf[:total].copy_(pinned[:total], non_blocking=True)
+        staging.mark(k, stream)
+        return dev_buf
+
+    def letterbox(self, dev_buf, dtype, dev):
+        """y5_val_letterbox over the uploaded sources -> (n, 3, H, W) `dtype`."""
+        H, W = self.out_hw
+        table = (_lib.ValImage * self.n)()
+        base = dev_buf.data_ptr()
+        for d, off, it in zip(table, self.offs, self.items):
+            im = it["im"]
+            d.data, d.src_h, d.src_w, d.row_bytes = base + off, im.shape[0], im.shape[1], im.shape[1] * 3
+            d.res_h, d.res_w = it["res"]
+            d.interp = it["interp"]
+            d.new_h, d.new_w = it["new"]
+            d.top, d.left = it["top"], it["left"]
+            d.scratch = base + self.pos + it["scratch"] if it["scratch"] is not None else None
+        imgs = torch.empty(self.n, 3, H, W, dtype=dtype, device=dev)
+        _lib.check(_lib.lib().y5_val_letterbox(table, self.n, H, W, imgs.data_ptr(), _lib.dtype_code(dtype),
+                                               ctypes.c_void_p(_lib.stream_ptr(dev))), "val_letterbox")
+        return imgs
+
+
+class DeviceValLoader:
+    """Drop-in for the validation ``create_dataloader(..., augment=False)`` loader over a ``LoadImagesAndLabels``-like
+    dataset (duck-typed on indices, labels, img_size, rect, batch, batch_shapes, im_files, ims, im_hw0, npy_files).
+    Yields collate_fn's ``(imgs, targets, paths, shapes)`` in dataset order with ``imgs`` and ``targets`` on ``device``;
+    ``dtype``: torch.uint8 (what collate_fn yields) or fp16/bf16/fp32 as ``imgs.to(dtype) / 255`` computes them.
+    Per batch:
+      1. ``workers`` host threads run ``decode`` (default ``load_val_image``: the RAM cache, the .npy cache or
+         cv2.imread) one batch ahead of the consumer;
+      2. the host works out load_image's size and interpolation, letterbox's geometry, ``shapes`` and the label rows
+         (float32, as the reference computes them), and makes one pinned host-to-device copy of the sources and rows;
+      3. ``y5_val_letterbox`` resizes (INTER_AREA when shrinking, INTER_LINEAR when enlarging) and letterboxes every
+         image in one launch.
+    Nothing waits for the device.  The batches equal the reference's byte for byte (tests/test_val_load_gpu.py)."""
+
+    def __init__(self, dataset, batch_size, device=None, dtype=torch.uint8, workers=8, decode=None):
+        check_val_dataset(dataset, batch_size)
+        if dtype not in (torch.uint8, torch.float16, torch.bfloat16, torch.float32):
+            raise ValueError(f"y5b200: unsupported output dtype {dtype}")
+        self.dataset = dataset
+        self.batch_size = int(batch_size)
+        self.dtype = dtype
+        self.workers = max(1, int(workers))
+        self.decode = decode or load_val_image
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self._staging = _Staging()
+
+    def __len__(self):
+        return (len(self.dataset.indices) + self.batch_size - 1) // self.batch_size
+
+    def _batches(self):
+        n = len(self.dataset.indices)
+        return [list(range(i, min(i + self.batch_size, n))) for i in range(0, n, self.batch_size)]
+
+    def __iter__(self):
+        ds = self.dataset
+        batches = self._batches()
+        if not batches:
+            return
+        with ThreadPoolExecutor(max_workers=self.workers) as pool:
+            def submit(b):
+                return [pool.submit(self.decode, ds, int(ds.indices[p])) for p in b]
+
+            ahead = submit(batches[0])
+            for j, b in enumerate(batches):
+                loaded = [f.result() for f in ahead]
+                if j + 1 < len(batches):
+                    ahead = submit(batches[j + 1])
+                yield self.collate(b, loaded)
+
+    def collate(self, positions, loaded=None):
+        """Batch of dataset positions (into dataset.indices) -> (imgs, targets, paths, shapes).  `loaded`: the decode
+        results, decoded here when None."""
+        ds, dev = self.dataset, self.device
+        if loaded is None:
+            loaded = [self.decode(ds, int(ds.indices[p])) for p in positions]
+        lay = ValBatchLayout(ds, positions, loaded)
+        H, W = lay.out_hw
+        rows = [lay.label_rows(ds, b, W, H) for b in range(lay.n)]
+        nt = sum(len(r) for r in rows)
+        tg = np.zeros((nt, 6), np.float32)
+        i = 0
+        for b, r in enumerate(rows):
+            tg[i: i + len(r), 0] = b
+            tg[i: i + len(r), 1:] = r
+            i += len(r)
+        t_off = lay.add_block(tg)
+        with _lib.on(dev):
+            dev_buf = lay.upload(self._staging, dev)
+            imgs = lay.letterbox(dev_buf, self.dtype, dev)
+        targets = dev_buf[t_off: t_off + tg.nbytes].view(torch.float32).view(nt, 6)
+        return imgs, targets, tuple(ds.im_files[k] for k in lay.keys), tuple(lay.shapes)

@@ -16,6 +16,9 @@ The one host synchronisation is the read of the kept-label counts, which size ``
 masks' dtype (torch.cat's promotion: uint8, int32 for an overlap image with more than 255 labels, float32 as soon as one
 image has no labels).  ``polygons2masks`` / ``polygons2masks_overlap`` expose the rasterizer with ultralytics'
 signatures.  With num_workers=0 and the same seeds the batches equal the reference's (tests/test_seg_augment_gpu.py).
+
+``DeviceSegValLoader`` is the segmentation validation loader (augment=False, rect batches): ``DeviceValLoader``'s
+images and label rows, plus the polygon masks through the same rasterizer, order and compose kernels.
 """
 from __future__ import annotations
 
@@ -27,7 +30,7 @@ import torch
 
 from ... import _lib
 from ..augmentations import affine_matrix, aug_gather, hsv_luts, invert_affine, letterbox_batch, letterbox_geometry, set_tile
-from ..dataloaders import _ALIGN, _label_rows, _placements, draw_item
+from ..dataloaders import _ALIGN, DeviceValLoader, ValBatchLayout, _label_rows, _placements, check_val_dataset, draw_item
 
 _RATIOS = (1, 4)  # r = 2 is cv2.resize's INTER_AREA special case, not implemented
 
@@ -326,3 +329,96 @@ def polygons2masks_overlap(imgsz, segments, downsample_ratio=1, device=None):
         _lib.check(lib.y5_seg_compose(table_dev.data_ptr(), None, counts.data_ptr(), plane.data_ptr(), masks.data_ptr(), 1, mh, mw, 1,
                                       out.data_ptr(), _MASK_CODE[mdtype], st), "seg_compose")
     return out[0], plane[:n].long()
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# validation
+# ----------------------------------------------------------------------------------------------------------------------
+def _check_val_segments(ds):
+    for k, (lab, segs) in enumerate(zip(ds.labels, ds.segments)):
+        if len(lab) and len(segs) != len(lab):
+            raise NotImplementedError(f"y5b200: image {k} has {len(lab)} labels and {len(segs)} segments (one segment per label is implemented)")
+        for seg in segs:
+            if not isinstance(seg, np.ndarray) or seg.dtype != np.float32 or seg.ndim != 2 or seg.shape[1] != 2 or len(seg) < 1:
+                raise ValueError(f"y5b200: image {k}: segments must be float32 (n >= 1, 2) arrays of normalised points")
+
+
+class DeviceSegValLoader(DeviceValLoader):
+    """``DeviceValLoader`` for a ``LoadImagesAndLabelsAndMasks``-like dataset (plus segments, overlap, downsample_ratio):
+    yields the segmentation collate_fn's ``(imgs, targets, paths, shapes, masks)`` with ``imgs``, ``targets`` and
+    ``masks`` on the device.  Each segment goes through xyn2xy with the letterbox's ratio and pad (float32 on the host)
+    and polygon2mask's int32 cast; ``y5_seg_raster`` rasterizes it at the batch shape (cv2.fillPoly + cv2.resize at
+    ``downsample_ratio`` 1 or 4), ``y5_seg_order`` orders an overlap image's labels by decreasing area (equal areas in
+    label order, as ``DeviceSegAugmentLoader`` does) and ``y5_seg_compose`` writes the masks.  Every label is kept, so
+    the counts and the masks' dtype (``_mask_dtype``: uint8, int32 past 255 labels in overlap mode, float32 once an
+    image has no labels) are known on the host: nothing waits for the device."""
+
+    def __init__(self, dataset, batch_size, device=None, dtype=torch.uint8, workers=8, decode=None, overlap=None, downsample_ratio=None):
+        self.overlap = bool(getattr(dataset, "overlap", False) if overlap is None else overlap)
+        self.downsample_ratio = int(getattr(dataset, "downsample_ratio", 1) if downsample_ratio is None else downsample_ratio)
+        if self.downsample_ratio not in _RATIOS:
+            raise NotImplementedError(f"y5b200: downsample_ratio {self.downsample_ratio} is not implemented (1 or 4)")
+        check_val_dataset(dataset, batch_size, "DeviceSegValLoader")
+        _check_val_segments(dataset)
+        super().__init__(dataset, batch_size, device=device, dtype=dtype, workers=workers, decode=decode)
+
+    def collate(self, positions, loaded=None):
+        """Batch of dataset positions -> (imgs, targets, paths, shapes, masks)."""
+        ds, dev, r = self.dataset, self.device, self.downsample_ratio
+        if loaded is None:
+            loaded = [self.decode(ds, int(ds.indices[p])) for p in positions]
+        lay = ValBatchLayout(ds, positions, loaded)
+        H, W = lay.out_hw
+        if H % r or W % r:
+            raise NotImplementedError(f"y5b200: batch shape {(H, W)} is not a multiple of downsample_ratio {r}")
+        if H > 4096 or W > 4096:
+            raise NotImplementedError(f"y5b200: batch shape {(H, W)}: masks are implemented up to 4096 x 4096")
+        rows, polys, image_rows = [], [], [0]
+        for b, k in enumerate(lay.keys):
+            lab = lay.label_rows(ds, b, W, H)
+            if len(lab):
+                it = lay.items[b]
+                (h, w), ratio, pad = it["res"], it["ratio"], it["pad"]
+                for seg in ds.segments[k]:
+                    xy = np.copy(seg)  # xyn2xy: float32, the python-float scales and pads are weak scalars
+                    xy[..., 0] = ratio[0] * w * seg[..., 0] + pad[0]
+                    xy[..., 1] = ratio[1] * h * seg[..., 1] + pad[1]
+                    polys.append(np.asarray(xy, dtype=np.int32).reshape(-1, 2))
+                r6 = np.zeros((len(lab), 6), np.float32)
+                r6[:, 0] = b
+                r6[:, 1:] = lab
+                rows.append(r6)
+            image_rows.append(image_rows[-1] + len(lab))
+        nl = image_rows[-1]
+        per_image = [image_rows[b + 1] - image_rows[b] for b in range(lay.n)]
+        nv = max([len(p) for p in polys], default=1)
+        verts = np.zeros((max(nl, 1), nv, 2), np.int32)
+        for i, p in enumerate(polys):  # shorter polygons repeat their last vertex (a zero-length edge draws nothing)
+            verts[i, :len(p)] = p
+            verts[i, len(p):] = p[-1]
+        lab6 = np.concatenate(rows, 0) if rows else np.zeros((1, 6), np.float32)
+        rec = np.zeros((max(nl, 1), 12), np.float32)  # y5_aug_label records: y5_seg_compose reads their image index
+        rec.view(np.int32)[:nl, 9] = lab6[:nl, 0].astype(np.int32)
+        table = np.zeros((lay.n, ctypes.sizeof(_lib.AugImage)), np.uint8)  # no flips
+        offs = [lay.add_block(a) for a in (verts, lab6, rec, table, np.asarray(image_rows, np.int32), np.ones(max(nl, 1), np.int32))]
+        mh, mw = H // r, W // r
+        mdtype = _mask_dtype(per_image, self.overlap)
+        n_out = lay.n if self.overlap else nl
+        lib = _lib.lib()
+        with _lib.on(dev):
+            st = ctypes.c_void_p(_lib.stream_ptr(dev))
+            dev_buf = lay.upload(self._staging, dev)
+            imgs = lay.letterbox(dev_buf, self.dtype, dev)
+            verts_p, rows_p, rec_p, table_p, image_rows_p, keep_p = (dev_buf.data_ptr() + o for o in offs)
+            raster = torch.empty(max(nl, 1), mh, mw, dtype=torch.uint8, device=dev)
+            areas = torch.empty(max(nl, 1), dtype=torch.int32, device=dev)
+            targets = torch.empty(max(nl, 1), 6, dtype=torch.float32, device=dev)
+            plane = torch.empty(max(nl, 1), dtype=torch.int32, device=dev)
+            counts = torch.empty(lay.n + 1, dtype=torch.int32, device=dev)
+            masks = torch.empty(n_out, mh, mw, dtype=mdtype, device=dev)
+            _lib.check(lib.y5_seg_raster(verts_p, nv, keep_p, nl, H, W, r, raster.data_ptr(), areas.data_ptr(), st), "seg_raster")
+            _lib.check(lib.y5_seg_order(image_rows_p, lay.n, keep_p, areas.data_ptr(), rows_p, int(self.overlap), targets.data_ptr(),
+                                        plane.data_ptr(), counts.data_ptr(), st), "seg_order")
+            _lib.check(lib.y5_seg_compose(table_p, rec_p, counts.data_ptr(), plane.data_ptr(), raster.data_ptr(), n_out, mh, mw,
+                                          int(self.overlap), masks.data_ptr(), _MASK_CODE[mdtype], st), "seg_compose")
+        return imgs, targets[:nl], tuple(ds.im_files[k] for k in lay.keys), tuple(lay.shapes), masks
