@@ -378,6 +378,22 @@ typedef struct y5_val_image y5_val_image;
 int y5_val_letterbox(const y5_val_image* images, int32_t n_images, int32_t out_h, int32_t out_w, void* out, int32_t out_dtype,
                      void* stream);
 
+/* Classification batch (utils/augmentations.py classify_transforms, utils/dataloaders.py:949-985 without Albumentations):
+ * CenterCrop's cv2.resize INTER_LINEAR of each image's center m x m square to (out_h, out_w), then ToTensor (BGR -> RGB,
+ * CHW, float32 v / 255 as a true division) and Normalize ((v - mean[c]) / std[c] in float32).  `data` holds only the
+ * square: m rows of `row_bytes` bytes, uint8 BGR.  out: (n, 3, out_h, out_w) Y5_F32, or Y5_F16 | Y5_BF16 as that float32
+ * value rounded once.  `images` is a DEVICE array of n descriptors (so one launch takes any batch size); the descriptors are
+ * the caller's to get right (an image with side <= 0 or row_bytes < 3 * side is skipped).  mean, std: 3 HOST float32 values
+ * each, in RGB order.  No allocation and no host synchronisation. */
+struct y5_cls_image {
+    const void* data;   /* the center square: uint8 HWC BGR, 3 channels, DEVICE */
+    int32_t side;       /* m = min(h, w) of the original image */
+    int32_t row_bytes;  /* bytes between rows (>= 3 * side) */
+};
+typedef struct y5_cls_image y5_cls_image;
+int y5_cls_batch(const y5_cls_image* images, int32_t n_images, int32_t out_h, int32_t out_w, const float* mean, const float* std, void* out,
+                 int32_t out_dtype, void* stream);
+
 /* process_mask (utils/segment/general.py:25-52, crop_mask :10-22): for detection i of image img_index[i] (NULL = image 0):
  * sigmoid(coef_i . protos[img]) at mask resolution, zeroed outside the box scaled by (mw/in_w, mh/in_h), optionally
  * bilinearly up-sampled (align_corners=False) to (in_h,in_w), thresholded at 0.5.

@@ -105,6 +105,10 @@ class ValImage(C.Structure):
 VAL_COPY, VAL_LINEAR, VAL_AREA = 0, 1, 2  # include/y5b200.h Y5_VAL_*
 
 
+class ClsImage(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("side", C.c_int32), ("row_bytes", C.c_int32)]
+
+
 class OptTensor(C.Structure):
     _fields_ = [
         ("param", C.c_void_p), ("grad", C.c_void_p), ("mom", C.c_void_p), ("ema", C.c_void_p),
@@ -207,6 +211,7 @@ SIGNATURES = {
     "y5_letterbox_max_images": (_I32, []),
     "y5_letterbox": (_I32, [C.POINTER(LetterboxImage), _I32, _I32, _I32, _I32, _I32, _P, _I32, _I32, _I32, _I32, _P]),
     "y5_val_letterbox": (_I32, [C.POINTER(ValImage), _I32, _I32, _I32, _P, _I32, _P]),
+    "y5_cls_batch": (_I32, [_P, _I32, _I32, _I32, C.POINTER(_F), C.POINTER(_F), _P, _I32, _P]),
     "y5_process_mask_workspace_bytes": (_I64, [_I32, _I32, _I32, _I32]),
     "y5_process_mask": (_I32, [_P, _I32, _I32, _I32, _I32, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, C.POINTER(_I32), _P, _I32, _P, _I64,
                                 _P]),

@@ -239,6 +239,36 @@ __global__ void val_letterbox_kernel(const ValBatch L, int out_h, int out_w, voi
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// classification batch: CenterCrop's resize + ToTensor + Normalize
+// ---------------------------------------------------------------------------------------------------------------------
+struct ClsNorm {
+    float mean[3], std[3];
+};
+
+// OUT: 1 = fp16/bf16, 2 = fp32; CHW RGB.  The descriptor table is in device memory: every thread of a block reads the
+// same 16 bytes, so the loads are broadcasts
+template <int OUT>
+__global__ void cls_batch_kernel(const y5_cls_image* __restrict__ images, int out_h, int out_w, const ClsNorm N, void* __restrict__ out, int bf16) {
+    const int b = blockIdx.z;
+    const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y * blockDim.y + threadIdx.y;
+    if (ox >= out_w || oy >= out_h) return;
+    const y5_cls_image im = images[b];
+    if (im.side <= 0 || im.row_bytes < 3 * im.side) return;
+    int v[3];
+    linear_px(static_cast<const uint8_t*>(im.data), im.row_bytes, im.side, im.side, out_h, out_w, ox, oy, v);
+    const long long plane = static_cast<long long>(out_h) * out_w;
+    const long long o = static_cast<long long>(b) * 3 * plane + static_cast<long long>(oy) * out_w + ox;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        // ToTensor's `/= 255` on a CPU float32 tensor is a true division (not a multiply by 1/255), then Normalize
+        const float x = __fdiv_rn(static_cast<float>(v[2 - c]), 255.0f);  // BGR -> RGB
+        const float y = __fdiv_rn(__fsub_rn(x, N.mean[c]), N.std[c]);
+        if (OUT == 1) static_cast<uint16_t*>(out)[o + c * plane] = pack1(y, bf16 != 0);
+        else static_cast<float*>(out)[o + c * plane] = y;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // process_mask
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int kMaskDets = 8;     // detections per thread pass (prototype vector stays in registers)
@@ -555,6 +585,28 @@ extern "C" Y5_API int y5_val_letterbox(const y5_val_image* images, int32_t n_ima
         if (again) launch_val(A, nb, out_w, out_h, out_h, out_w, o, out_dtype, st);
     }
     return last_status("val_letterbox");
+}
+
+extern "C" Y5_API int y5_cls_batch(const y5_cls_image* images, int32_t n_images, int32_t out_h, int32_t out_w, const float* mean, const float* std,
+                                   void* out, int32_t out_dtype, void* stream) {
+    if (!images || !out || !mean || !std || n_images <= 0 || out_h <= 0 || out_w <= 0) return set_error(Y5_E_INVALID, "cls_batch: bad argument");
+    if (out_dtype != Y5_F16 && out_dtype != Y5_BF16 && out_dtype != Y5_F32) return set_error(Y5_E_UNSUPPORTED, "cls_batch: output dtype");
+    constexpr int kMaxSide = 1 << 14, kMaxImages = 65535;  // grid.z carries the image
+    if (out_h > kMaxSide || out_w > kMaxSide) return set_error(Y5_E_UNSUPPORTED, "cls_batch: output larger than %d", kMaxSide);
+    if (n_images > kMaxImages) return set_error(Y5_E_UNSUPPORTED, "cls_batch: %d images (max %d per launch)", n_images, kMaxImages);
+    ClsNorm N;
+    for (int c = 0; c < 3; ++c) {
+        if (!(std[c] != 0.0f)) return set_error(Y5_E_INVALID, "cls_batch: std[%d] is zero", c);
+        N.mean[c] = mean[c];
+        N.std[c] = std[c];
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const dim3 block(32, 8);
+    const dim3 grid((out_w + block.x - 1) / block.x, (out_h + block.y - 1) / block.y, n_images);
+    if (out_dtype == Y5_F32) cls_batch_kernel<2><<<grid, block, 0, st>>>(images, out_h, out_w, N, out, 0);
+    else cls_batch_kernel<1><<<grid, block, 0, st>>>(images, out_h, out_w, N, out, out_dtype == Y5_BF16);
+    count_launch();
+    return last_status("cls_batch");
 }
 
 extern "C" Y5_API int64_t y5_process_mask_workspace_bytes(int32_t n, int32_t mh, int32_t mw, int32_t mode) {

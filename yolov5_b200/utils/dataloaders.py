@@ -16,12 +16,18 @@ With num_workers=0 and the same seeds the batches equal the reference's byte for
 ``DeviceValLoader`` is the validation loader (``create_dataloader(..., augment=False, rect=True, pad=0.5)``, reference
 utils/dataloaders.py:696-790): a pool of host threads decodes one batch ahead, and ``y5_val_letterbox`` does
 load_image's resize (cv2 INTER_AREA / INTER_LINEAR) and the letterbox in one launch; see its docstring.
+
+``DeviceClassifyLoader`` is ``create_classification_dataloader``'s loader (reference utils/dataloaders.py:949-1009,
+without Albumentations): host threads decode one batch ahead, and ``y5_cls_batch`` does classify_transforms' center
+crop, resize, ToTensor and Normalize in one launch; see its docstring.
 """
 from __future__ import annotations
 
 import ctypes
 import math
+import os
 import random
+import threading
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -364,6 +370,38 @@ class _Staging:
         self.done[k].record(stream)
 
 
+def stage_upload(staging, dev_buf, blocks, total):
+    """Write host arrays at byte offsets into a pinned `staging` buffer and copy its first `total` bytes to `dev_buf` on
+    the current stream.  blocks: (offset, array) pairs; an array may be a strided view (it is copied in place)."""
+    k, pinned = staging.get(total)
+    host = pinned.numpy()
+    for off, a in blocks:
+        np.copyto(host[off: off + a.nbytes].view(a.dtype).reshape(a.shape), a)
+    dev_buf[:total].copy_(pinned[:total], non_blocking=True)
+    staging.mark(k, torch.cuda.current_stream(dev_buf.device))
+
+
+def decode_ahead(ds, batches, decode, workers):
+    """(batch, decoded items) for each batch of the iterable `batches`, with `workers` threads running decode(ds, i) for
+    every i of the next batch while the caller works on the current one."""
+    it = iter(batches)
+    b = next(it, None)
+    if b is None:
+        return
+    with ThreadPoolExecutor(max_workers=workers) as pool:
+        def submit(b):
+            return [pool.submit(decode, ds, i) for i in b]
+
+        ahead = submit(b)
+        while b is not None:
+            loaded = [f.result() for f in ahead]
+            nxt = next(it, None)
+            if nxt is not None:
+                ahead = submit(nxt)
+            yield b, loaded
+            b = nxt
+
+
 class ValBatchLayout:
     """Host side of one validation batch: decoded images, geometry, shapes and label rows, laid out in one staging
     buffer as [sources | extra host blocks], plus the device scratch the letterboxes that resize again need."""
@@ -414,16 +452,7 @@ class ValBatchLayout:
         """One pinned host-to-device copy of the sources and blocks -> (device buffer, scratch base address)."""
         total = self.pos
         dev_buf = torch.empty(total + self.scratch_bytes, dtype=torch.uint8, device=dev)
-        k, pinned = staging.get(total)
-        host = pinned.numpy()
-        for off, it in zip(self.offs, self.items):
-            a = it["im"]
-            host[off: off + a.nbytes] = a.reshape(-1)
-        for off, a in self.blocks:
-            host[off: off + a.nbytes] = a.view(np.uint8).reshape(-1)
-        stream = torch.cuda.current_stream(dev)
-        dev_buf[:total].copy_(pinned[:total], non_blocking=True)
-        staging.mark(k, stream)
+        stage_upload(staging, dev_buf, [(off, it["im"]) for off, it in zip(self.offs, self.items)] + self.blocks, total)
         return dev_buf
 
     def letterbox(self, dev_buf, dtype, dev):
@@ -479,20 +508,8 @@ class DeviceValLoader:
         return [list(range(i, min(i + self.batch_size, n))) for i in range(0, n, self.batch_size)]
 
     def __iter__(self):
-        ds = self.dataset
-        batches = self._batches()
-        if not batches:
-            return
-        with ThreadPoolExecutor(max_workers=self.workers) as pool:
-            def submit(b):
-                return [pool.submit(self.decode, ds, int(ds.indices[p])) for p in b]
-
-            ahead = submit(batches[0])
-            for j, b in enumerate(batches):
-                loaded = [f.result() for f in ahead]
-                if j + 1 < len(batches):
-                    ahead = submit(batches[j + 1])
-                yield self.collate(b, loaded)
+        for b, loaded in decode_ahead(self.dataset, self._batches(), lambda ds, p: self.decode(ds, int(ds.indices[p])), self.workers):
+            yield self.collate(b, loaded)
 
     def collate(self, positions, loaded=None):
         """Batch of dataset positions (into dataset.indices) -> (imgs, targets, paths, shapes).  `loaded`: the decode
@@ -516,3 +533,176 @@ class DeviceValLoader:
             imgs = lay.letterbox(dev_buf, self.dtype, dev)
         targets = dev_buf[t_off: t_off + tg.nbytes].view(torch.float32).view(nt, 6)
         return imgs, targets, tuple(ds.im_files[k] for k in lay.keys), tuple(lay.shapes)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# classification
+# ----------------------------------------------------------------------------------------------------------------------
+IMAGENET_MEAN = 0.485, 0.456, 0.406  # RGB, as utils/augmentations.py defines them
+IMAGENET_STD = 0.229, 0.224, 0.225
+
+
+def load_cls_image(ds, i):
+    """The classification loader's decode step for dataset item i -> uint8 HWC BGR image, with
+    ClassificationDataset.__getitem__'s caches: the RAM cache keeps cv2.imread's result in ``samples[i][3]``, the disk
+    cache writes ``samples[i][2]`` (.npy) on first use and reads it with np.load.  A RAM-cached image is used as it is
+    (the reference's __getitem__ reads the file again once its cache is filled; the bytes are the same).  Runs on the
+    loader's worker threads."""
+    import cv2
+
+    f, _, fn, im = ds.samples[i]
+    if ds.cache_ram and im is not None:
+        return im
+    if ds.cache_disk and fn.exists():
+        return np.load(fn)
+    im = cv2.imread(str(f))
+    if im is None:
+        raise FileNotFoundError(f"Image Not Found {f}")
+    if ds.cache_ram:
+        ds.samples[i][3] = im
+    elif ds.cache_disk:  # written under a private name first: a padded DistributedSampler batch can hold an item twice
+        tmp = f"{fn.as_posix()}.{os.getpid()}.{threading.get_ident()}.npy"
+        np.save(tmp, im)
+        os.replace(tmp, fn)
+    return im
+
+
+# Where classify_transforms' CenterCrop and ToTensor may come from: the reference's utils/augmentations.py (also when it is
+# imported as part of a package, e.g. yolov5.utils.augmentations), or the call-compatible numpy stand-ins of the test oracle
+_CLS_TRANSFORM_MODULES = ("utils.augmentations", "oracle.cls_load_ref")
+
+
+def _from_module(t, modules):
+    m = type(t).__module__
+    return any(m == x or m.endswith("." + x) for x in modules)
+
+
+def check_cls_dataset(ds):
+    """Refuse what the classification path does not implement, before any work -> the output size (h, w).
+    torch_transforms must be classify_transforms' Compose([CenterCrop, ToTensor(half=False), Normalize(ImageNet)]): the
+    reference's CenterCrop and ToTensor classes (checked by class and module) and torchvision's Normalize."""
+    if getattr(ds, "album_transforms", None):  # __getitem__ takes this branch whenever the transform is truthy
+        raise NotImplementedError("y5b200: DeviceClassifyLoader: an active Albumentations transform is not implemented")
+    ts = list(getattr(getattr(ds, "torch_transforms", None), "transforms", None) or ())
+    names = [f"{type(t).__module__}.{type(t).__name__}" for t in ts]
+    if ([type(t).__name__ for t in ts] != ["CenterCrop", "ToTensor", "Normalize"] or not all(_from_module(t, _CLS_TRANSFORM_MODULES) for t in ts[:2])
+            or not _from_module(ts[2], ("torchvision.transforms.transforms",)) or not all(hasattr(ts[0], a) for a in ("h", "w"))):
+        raise NotImplementedError(f"y5b200: DeviceClassifyLoader implements classify_transforms (CenterCrop, ToTensor, Normalize) only, got {names}")
+    if getattr(ts[1], "half", None) is not False:
+        raise NotImplementedError("y5b200: DeviceClassifyLoader implements ToTensor(half=False) only")
+    mean, std = (tuple(float(v) for v in getattr(ts[2], a)) for a in ("mean", "std"))
+    if mean != IMAGENET_MEAN or std != IMAGENET_STD:
+        raise NotImplementedError(f"y5b200: DeviceClassifyLoader implements Normalize(IMAGENET_MEAN, IMAGENET_STD) only, got {mean}, {std}")
+    h, w = ts[0].h, ts[0].w
+    if not all(isinstance(v, (int, np.integer)) and 0 < v <= 16384 for v in (h, w)):
+        raise ValueError(f"y5b200: image size {(h, w)} outside (0, 16384]")
+    return int(h), int(w)
+
+
+class DeviceClassifyLoader:
+    """Drop-in for ``create_classification_dataloader``'s loader (reference utils/dataloaders.py:988-1009) over a
+    ``ClassificationDataset``-like dataset (duck-typed on samples, root, classes, torch_transforms, album_transforms,
+    cache_ram, cache_disk).  Yields ``(images (B, 3, h, w) dtype, labels (B,) int64)``, both on ``device``; ``dtype``
+    torch.float32 is what the reference yields, fp16 / bf16 that value rounded once (``images.half()``).
+
+    The batches are the reference's: the same ``min(batch_size, len(dataset))``, the same generator seed
+    (6148914691236517205 + RANK), shuffling or a ``DistributedSampler(dataset, shuffle=shuffle)`` when ``rank != -1``, and
+    one persistent index stream, as InfiniteDataLoader keeps it: each pass yields the next ``len(self)`` batches of
+    the stream, so ``next(iter(loader))`` advances it.  A pass draws its batches as it yields them (plus the one batch
+    being decoded ahead), so under DDP an epoch's DistributedSampler permutation is taken after classify/train.py's
+    ``set_epoch``.  The reference matches that with num_workers=0; with workers, its InfiniteDataLoader prefetches
+    ``prefetch_factor * num_workers`` batches and can take the next epoch's permutation before ``set_epoch`` runs, so its
+    later DDP epochs depend on its worker count.  Per batch:
+      1. ``workers`` host threads run ``decode`` (default ``load_cls_image``: the caches or cv2.imread) one batch ahead;
+      2. the host stages each image's center m x m square (m = min(h, w)), the y5_cls_image table and the labels in one
+         pinned buffer and makes one host-to-device copy;
+      3. ``y5_cls_batch`` resizes (cv2 INTER_LINEAR), converts and normalises the whole batch in one launch.
+    Nothing waits for the device.  The batches equal the reference's bit for bit (tests/test_cls_load_gpu.py)."""
+
+    def __init__(self, dataset, batch_size, rank=-1, shuffle=True, device=None, dtype=torch.float32, workers=8, decode=None):
+        self.size = check_cls_dataset(dataset)
+        if dtype not in (torch.float16, torch.bfloat16, torch.float32):
+            raise ValueError(f"y5b200: unsupported output dtype {dtype}")
+        self.dataset = dataset
+        n = len(dataset.samples)
+        self.batch_size = min(int(batch_size), n)
+        self.dtype = dtype
+        self.workers = max(1, int(workers))
+        self.decode = decode or load_cls_image
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.sampler = None if rank == -1 else torch.utils.data.DistributedSampler(dataset, shuffle=shuffle)
+        generator = torch.Generator()
+        generator.manual_seed(6148914691236517205 + int(os.getenv("RANK", "-1")))
+        index = torch.utils.data.DataLoader(range(n), batch_size=self.batch_size, shuffle=shuffle and self.sampler is None, sampler=self.sampler,
+                                            generator=generator, collate_fn=list)
+        self._batch_sampler = index.batch_sampler
+        object.__setattr__(index, "batch_sampler", _Repeat(index.batch_sampler))  # DataLoader refuses a plain assignment
+        self._stream = iter(index)  # created once: the iterator's base seed is drawn from the generator here, as the reference's is
+        self._carry = None  # a batch drawn from the stream but not yielded (a pass left early)
+        self._staging = _Staging()
+        self._mean = (ctypes.c_float * 3)(*IMAGENET_MEAN)
+        self._std = (ctypes.c_float * 3)(*IMAGENET_STD)
+
+    def __len__(self):
+        return len(self._batch_sampler)
+
+    def _draw(self):
+        for j in range(len(self)):
+            if j > 0 or self._carry is None:
+                self._carry = next(self._stream)
+            yield self._carry
+
+    def __iter__(self):
+        for b, loaded in decode_ahead(self.dataset, self._draw(), self.decode, self.workers):
+            if self._carry is b:  # nothing drawn ahead of this batch
+                self._carry = None
+            yield self.collate(b, loaded)
+
+    def collate(self, items, loaded=None):
+        """Dataset items -> (images, labels) on the device.  `loaded`: the decode results, decoded here when None."""
+        ds, dev = self.dataset, self.device
+        if loaded is None:
+            loaded = [self.decode(ds, i) for i in items]
+        n = len(items)
+        blocks, offs, sides, pos = [], [], [], 0
+        for i, im in zip(items, loaded):
+            if not isinstance(im, np.ndarray) or im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError(f"y5b200: image {i} must be a uint8 HWC BGR image with 3 channels")
+            h, w = im.shape[:2]
+            m = min(h, w)
+            if m < 1:
+                raise ValueError(f"y5b200: image {i} is empty")
+            top, left = (h - m) // 2, (w - m) // 2
+            blocks.append((pos, im[top: top + m, left: left + m]))
+            offs.append(pos)
+            sides.append(m)
+            pos += (m * m * 3 + _ALIGN - 1) // _ALIGN * _ALIGN
+        table = (_lib.ClsImage * n)()
+        table_off = pos
+        pos += (ctypes.sizeof(table) + _ALIGN - 1) // _ALIGN * _ALIGN
+        labels = np.array([ds.samples[i][1] for i in items], np.int64)
+        label_off = pos
+        pos += labels.nbytes
+        with _lib.on(dev):
+            dev_buf = torch.empty(pos, dtype=torch.uint8, device=dev)
+            base = dev_buf.data_ptr()
+            for d, off, m in zip(table, offs, sides):
+                d.data, d.side, d.row_bytes = base + off, m, 3 * m
+            blocks += [(table_off, np.frombuffer(table, np.uint8)), (label_off, labels)]
+            stage_upload(self._staging, dev_buf, blocks, pos)
+            h, w = self.size
+            images = torch.empty(n, 3, h, w, dtype=self.dtype, device=dev)
+            _lib.check(_lib.lib().y5_cls_batch(base + table_off, n, h, w, self._mean, self._std, images.data_ptr(), _lib.dtype_code(self.dtype),
+                                               ctypes.c_void_p(_lib.stream_ptr(dev))), "cls_batch")
+        return images, dev_buf[label_off: label_off + labels.nbytes].view(torch.int64)
+
+
+class _Repeat:
+    """A batch sampler that starts over whenever it runs out, so one DataLoader iterator is an endless stream."""
+
+    def __init__(self, batch_sampler):
+        self.sampler = batch_sampler
+
+    def __iter__(self):
+        while True:
+            yield from iter(self.sampler)
