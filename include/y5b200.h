@@ -96,6 +96,22 @@ typedef struct y5_conv_plan y5_conv_plan; /* opaque: encoded TMA descriptors + l
 int y5_conv_plan_create(const y5_conv_desc* desc, y5_conv_plan** plan);
 int y5_conv_plan_run(const y5_conv_plan* plan, void* stream);
 void y5_conv_plan_destroy(y5_conv_plan* plan);
+/* What a plan will run (read-only; tests assert the kernel path a case claims through it).  A plain struct tag, not a
+ * typedef: the query function has the same name. */
+struct y5_conv_plan_info {
+    int32_t a_mode;               /* activation fetch: 0 LINEAR (1x1/s1 GEMM), 1 TMA-im2col, 2 shifted patch */
+    int32_t tw, th;               /* patch: output pixels per tile row x rows (tw * th = 128); 0 in the other modes */
+    int32_t block_k, block_n, mt; /* K block, N tile, 128-row sub-tiles per tile */
+    int32_t cluster;              /* CTAs per cluster sharing (multicasting) every weight tile: 1, 2 or 4 */
+    int32_t patch_pw;             /* > 0: wide patch (one patch copy per channel chunk feeds every tap), its row pitch */
+    int32_t b_grouped;            /* patch: the kh weight tiles of a (chunk, horizontal tap) group share one stage */
+    int32_t staged;               /* epilogue stores go through shared memory (else straight from the registers) */
+    int32_t opt;                  /* runs the kernel instantiation with the optional modes compiled in */
+    int32_t epi;                  /* epilogue: 0 conv, 1 Detect head */
+    int32_t a_stages, b_stages;   /* shared-memory pipeline depth */
+    int32_t grid;                 /* CTAs launched (persistent, at most one per SM) */
+};
+int y5_conv_plan_info(const y5_conv_plan* plan, struct y5_conv_plan_info* info);
 /* one-shot convenience: create + run + destroy (tests) */
 int y5_conv_bn_silu_fwd(const y5_conv_desc* desc, void* stream);
 /* independent direct-convolution kernel (CUDA cores, fp32 accumulate) used by tests to cross-check the tensor-core
@@ -112,8 +128,8 @@ typedef struct y5_detect_desc {
     const void* in;
     int32_t in_pitch;
     int32_t batch, ny, nx, in_c;
-    const void* weight;   /* packed [na*no][cin_pad] */
-    const float* bias;    /* fp32 [na*no] */
+    const void* weight;   /* packed [na*128][cin_pad]: anchor a in rows [128a, 128a + no), the rest zero */
+    const float* bias;    /* fp32 [na*128], laid out like the weight rows */
     void* raw;
     void* z;
     int32_t z_rows, z_row0;

@@ -11,8 +11,9 @@ from yolov5_b200.engine import pack_weight
 
 def conv_case(dev, dtype, B, H, W, cin, cout, k, s, p, act=True, residual=False, in_extra=0, out_extra=0, seed=0, direct=False,
               block_n=0, a_mode=0, mt2=False, cluster=1, cg2=False, direct_store=False, narrow_patch=False, wide_patch=False,
-              staged=False):
+              staged=False, expect=None):
     """Runs y5_conv_bn_silu_fwd (or the direct cross-check kernel) on seeded data; returns (got NCHW fp32, oracle fp32).
+    `expect` ({y5_plan_info field: value}, "wide": bool for the wide patch) asserts the plan the case claims to run.
     `in_extra` / `out_extra` put the views inside wider buffers (channel offset 8, pitch + extra) to exercise slices.
     Stores: the library's default (direct from the registers) unless `staged` asks for the shared-memory staged epilogue;
     `direct_store` forces the direct stores."""
@@ -49,6 +50,8 @@ def conv_case(dev, dtype, B, H, W, cin, cout, k, s, p, act=True, residual=False,
     d.act, d.dtype, d.block_k, d.block_n = int(act), _lib.dtype_code(dtype), bk.value, block_n
     d.a_mode = a_mode  # 0 auto, 1 TMA-im2col, 2 shifted patches
     d.reserved = (2 if mt2 else 0) | (4 if cg2 else 0) | (16 if direct_store else 0) | (8 if staged else 0) | (32 if narrow_patch else 0) | (128 if wide_patch else 0) | (cluster << 8 if cluster > 1 else 0)  # forced block_n: 256-row tiles / CTA pairs / multicast cluster
+    if expect:
+        assert_plan(d, expect)
     fn = lib.y5_conv_direct_fwd if direct else lib.y5_conv_bn_silu_fwd
     _lib.check(fn(C.byref(d), C.c_void_p(_lib.stream_ptr(dev))), "conv")
     torch.cuda.synchronize()
@@ -57,6 +60,26 @@ def conv_case(dev, dtype, B, H, W, cin, cout, k, s, p, act=True, residual=False,
     if out_off:
         untouched = bool((obuf[..., :out_off] == -3.0).all() and (obuf[..., out_off + cout :] == -3.0).all())
     return got, y, untouched
+
+
+def plan_info(desc) -> dict:
+    """y5_conv_plan_info of the plan y5_conv_plan_create makes for `desc`, plus "wide" (the wide patch fetch)."""
+    lib = _lib.lib()
+    plan = C.c_void_p()
+    _lib.check(lib.y5_conv_plan_create(C.byref(desc), C.byref(plan)), "conv_plan_create")
+    try:
+        info = _lib.PlanInfo()
+        _lib.check(lib.y5_conv_plan_info(plan, C.byref(info)), "conv_plan_info")
+    finally:
+        lib.y5_conv_plan_destroy(plan)
+    out = info.as_dict()
+    out["wide"] = out["patch_pw"] > 0
+    return out
+
+
+def assert_plan(desc, expect: dict):
+    info = plan_info(desc)
+    assert {k: info[k] for k in expect} == expect, ("plan differs from the path the case names", info)
 
 
 def rel_err(got, ref):

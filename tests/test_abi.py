@@ -95,11 +95,18 @@ def test_argument_validation_without_gpu(built_lib):
     assert bk.value == 64 and bn.value in (128, 256)
 
 
+PLAIN_TAGS = ("y5_conv_plan_info",)
+
+
 def _header_structs():
-    """{struct name: [field names in declaration order]} parsed from include/y5b200.h"""
+    """{struct name: [field names in declaration order]} parsed from include/y5b200.h (typedefs and plain struct tags)"""
     src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
     out = {}
-    for body, name in re.findall(r"typedef struct \w+ \{(.*?)\}\s*(\w+);", src, flags=re.S):
+    found = re.findall(r"typedef struct \w+ \{(.*?)\}\s*(\w+);", src, flags=re.S)
+    # plain struct tags whose C type name is taken by a function of the same name
+    found += [(body, name) for name, body in re.findall(r"(?<!typedef )struct (\w+) \{(.*?)\};", src, flags=re.S)
+              if name in PLAIN_TAGS]
+    for body, name in found:
         fields = []
         for decl in body.split(";"):
             decl = decl.strip()
@@ -116,14 +123,16 @@ def test_ctypes_structs_match_the_c_layout(tmp_path):
     """sizeof / offsetof of every struct in the header (compiled by gcc) == the ctypes mirrors in yolov5_b200/_lib.py."""
     mirrors = {"y5_conv_desc": _lib.ConvDesc, "y5_detect_desc": _lib.DetectDesc, "y5_nms_params": _lib.NmsParams,
                "y5_loss_params": _lib.LossParams, "y5_wgrad_desc": _lib.WgradDesc, "y5_letterbox_image": _lib.LetterboxImage,
-               "y5_opt_tensor": _lib.OptTensor, "y5_pack_item": _lib.PackItem}
+               "y5_opt_tensor": _lib.OptTensor, "y5_pack_item": _lib.PackItem,
+               "y5_conv_plan_info": _lib.PlanInfo}
     structs = _header_structs()
     assert sorted(structs) == sorted(mirrors), (sorted(structs), sorted(mirrors))
     lines = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{HEADER}"', "int main(void) {"]
     for s, fields in structs.items():
-        lines.append(f'  printf("{s} %zu", sizeof({s}));')
+        t = f"struct {s}" if s in PLAIN_TAGS else s
+        lines.append(f'  printf("{s} %zu", sizeof({t}));')
         for f in fields:
-            lines.append(f'  printf(" %zu", offsetof({s}, {f}));')
+            lines.append(f'  printf(" %zu", offsetof({t}, {f}));')
         lines.append('  printf("\\n");')
     lines += ["  return 0;", "}"]
     src = tmp_path / "layout.c"

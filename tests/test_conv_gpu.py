@@ -30,7 +30,7 @@ CASES = [
 def test_conv_vs_oracle(cuda, dtype, case):
     got, ref, _ = conv_case(cuda, dtype, *case)
     assert rel_err(got, ref) < TOL[dtype], (case, rel_err(got, ref))
-    got, ref, _ = conv_case(cuda, dtype, *case, staged=True)
+    got, ref, _ = conv_case(cuda, dtype, *case, staged=True, expect=dict(staged=1))
     assert rel_err(got, ref) < TOL[dtype], (case, "staged stores", rel_err(got, ref))
 
 
@@ -40,7 +40,7 @@ def test_conv_residual_and_slices(cuda, case, direct_store):
     """Both epilogue store paths (per-warpgroup staging + 16-byte row-segment stores, and the direct register stores) into a
     channel slice of a wider buffer: N tails inside a 32-channel chunk (40, 72 channels), partial spatial tiles, M tails."""
     got, ref, untouched = conv_case(cuda, torch.float16, *case, residual=True, in_extra=24, out_extra=40, direct_store=direct_store,
-                                    staged=not direct_store)
+                                    staged=not direct_store, expect=dict(staged=int(not direct_store)))
     assert rel_err(got, ref) < 2e-3
     assert untouched, "epilogue wrote outside its channel slice"
 
@@ -54,6 +54,12 @@ def test_conv_3x3_both_fetch_modes(cuda, case, a_mode):
     got, ref, untouched = conv_case(cuda, torch.float16, *case, a_mode=a_mode, residual=True, in_extra=8, out_extra=24)
     assert rel_err(got, ref) < 2e-3, (case, a_mode, rel_err(got, ref))
     assert untouched
+
+
+# wide-patch requests the planner turns down: two sub-tiles need an even number of 8-pixel tiles per row, four sub-tiles (block_n
+# 32) never share a patch, and 9 x 130 tiles with fewer wasted pixels 32 wide than 8 wide
+WIDE_FALLS_BACK = {(2, 40, 40, 64, 64, 3, 1, 1), (2, 13, 27, 64, 32, 3, 1, 1), (1, 9, 130, 64, 96, 3, 1, 1), (2, 24, 24, 192, 64, 5, 1, 2),
+                   (3, 40, 40, 128, 64, 3, 1, 1)}
 
 
 @pytest.mark.parametrize("narrow", [False, True])
@@ -76,7 +82,7 @@ def test_conv_wide_patch(cuda, case, kw, dtype, narrow):
     descriptor offsets (`narrow=False`); the one-copy-per-horizontal-tap mode (`narrow=True`, reserved bit
     32) must give the same answer.  Residual + channel-slice views on both sides."""
     got, ref, untouched = conv_case(cuda, dtype, *case, a_mode=2, residual=True, in_extra=8, out_extra=24, narrow_patch=narrow, wide_patch=not narrow,
-                                     **kw)
+                                     expect=dict(wide=not narrow and case not in WIDE_FALLS_BACK), **kw)
     assert rel_err(got, ref) < TOL[dtype], (case, kw, narrow, rel_err(got, ref))
     assert untouched
 
@@ -109,7 +115,7 @@ def test_conv_cluster_multicast(cuda, bn, mt2, case, a_mode):
     """2-CTA clusters: each CTA fetches half of every weight tile and TMA-multicasts it to its peer; odd super-tile
     counts leave one CTA of the last cluster without work (it must still take part in the multicast protocol).  With block_n 256
     the planner keeps one sub-tile (the accumulators of 256 x 256 do not fit the registers), so (256, True) repeats (256, False)."""
-    got, ref, _ = conv_case(cuda, torch.float16, *case, block_n=bn, mt2=mt2, cluster=2, a_mode=a_mode, residual=True)
+    got, ref, _ = conv_case(cuda, torch.float16, *case, block_n=bn, mt2=mt2, cluster=2, a_mode=a_mode, residual=True, expect=dict(cluster=2))
     assert rel_err(got, ref) < 2e-3, (bn, mt2, case, a_mode, rel_err(got, ref))
 
 
@@ -125,13 +131,14 @@ def test_conv_cta_pairs(cuda, dtype, bn, mt2, case, a_mode):
     shapes; with block_n 256 the planner keeps one sub-tile, so the mt2=True cases of that width repeat mt2=False."""
     if case[4] % bn and bn == 256 and case[4] < 256:
         pytest.skip("N tile wider than the layer")
-    got, ref, _ = conv_case(cuda, dtype, *case, block_n=bn, mt2=mt2, cg2=True, a_mode=a_mode, residual=True)
+    got, ref, _ = conv_case(cuda, dtype, *case, block_n=bn, mt2=mt2, cg2=True, a_mode=a_mode, residual=True, expect=dict(cluster=2))
     assert rel_err(got, ref) < TOL[dtype], (bn, mt2, case, a_mode, rel_err(got, ref))
 
 
 def test_conv_cta_pairs_many_tiles(cuda):
     """Every pair loops over several tiles (barrier phase wrap-around across the pair protocol)."""
-    got, ref, _ = conv_case(cuda, torch.float16, 16, 80, 80, 64, 256, 3, 1, 1, block_n=256, cg2=True)  # 800 M tiles -> 400 pair tiles
+    got, ref, _ = conv_case(cuda, torch.float16, 16, 80, 80, 64, 256, 3, 1, 1, block_n=256, cg2=True,  # 800 M tiles -> 400 pair tiles
+                            expect=dict(cluster=2))
     assert rel_err(got, ref) < 2e-3
 
 

@@ -66,7 +66,7 @@ def test_grouped_weight_stages(cuda, dtype, bn, case):
     ((4, 32, 32, 64, 64, 3, 1, 1), dict(block_n=64, cg2=True)),     # wide patch inside a CTA pair
 ])
 def test_wide_patch(cuda, dtype, case, kw):
-    _check(cuda, dtype, case, a_mode=2, wide_patch=True, residual=True, in_extra=8, out_extra=24, **kw)
+    _check(cuda, dtype, case, a_mode=2, wide_patch=True, residual=True, in_extra=8, out_extra=24, expect=dict(wide=True), **kw)
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
@@ -79,7 +79,7 @@ def test_wide_patch(cuda, dtype, case, kw):
     ((16, 80, 80, 64, 256, 3, 1, 1), dict(block_n=256)),                      # many tiles per cluster: phases wrap
 ])
 def test_clusters(cuda, dtype, cluster, case, kw):
-    _check(cuda, dtype, case, cluster=cluster, residual=True, **kw)
+    _check(cuda, dtype, case, cluster=cluster, residual=True, expect=dict(cluster=cluster), **kw)
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

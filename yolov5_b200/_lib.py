@@ -54,6 +54,18 @@ class DetectDesc(C.Structure):
     ]
 
 
+class PlanInfo(C.Structure):
+    _fields_ = [
+        ("a_mode", C.c_int32), ("tw", C.c_int32), ("th", C.c_int32),
+        ("block_k", C.c_int32), ("block_n", C.c_int32), ("mt", C.c_int32), ("cluster", C.c_int32),
+        ("patch_pw", C.c_int32), ("b_grouped", C.c_int32), ("staged", C.c_int32), ("opt", C.c_int32), ("epi", C.c_int32),
+        ("a_stages", C.c_int32), ("b_stages", C.c_int32), ("grid", C.c_int32),
+    ]
+
+    def as_dict(self) -> dict:
+        return {f: getattr(self, f) for f, _ in self._fields_}
+
+
 class NmsParams(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("n_rows", C.c_int32), ("no", C.c_int32), ("nc", C.c_int32), ("nm", C.c_int32),
@@ -173,6 +185,7 @@ SIGNATURES = {
     "y5_conv_plan_create": (_I32, [C.POINTER(ConvDesc), C.POINTER(_P)]),
     "y5_conv_plan_run": (_I32, [_P, _P]),
     "y5_conv_plan_destroy": (None, [_P]),
+    "y5_conv_plan_info": (_I32, [_P, C.POINTER(PlanInfo)]),
     "y5_conv_bn_silu_fwd": (_I32, [C.POINTER(ConvDesc), _P]),
     "y5_conv_direct_fwd": (_I32, [C.POINTER(ConvDesc), _P]),
     "y5_detect_plan_create": (_I32, [C.POINTER(DetectDesc), C.POINTER(_P)]),

@@ -45,6 +45,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <type_traits>
 
 #include "../../include/y5b200.h"
 #include "common.cuh"
@@ -403,6 +404,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             // its first store: one round trip per batch, and at most 2 per tile.  Legal in place because each thread reads only the
             // elements it writes itself.  kBatch keeps the loaded words to 32 registers (64 spill next to 128 accumulators), 16 in
             // the OPT instantiations, whose optional modes hold more live state.
+            constexpr float kTail = BF16 ? 8.0f : 4.0f;  // silu_from_half is faithful down to -kTail (see common.cuh)
             constexpr int kRows = 2 * MT, kWords = (OPT ? 128 : 256) / BLOCK_N;
             constexpr int kBatch = kWords < 1 ? 1 : (kWords < kRows ? kWords : kRows);
             const bool has_res = p.res != nullptr;
@@ -430,27 +432,44 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     if (gpix >= 0 || staged) {
                         uint16_t* op = reinterpret_cast<uint16_t*>(p.out) + gpix * p.out_pitch + n0 + ccol;
                         uint8_t* sp = stg + (row - wg * 64) * stg_pitch + ccol * 2;
+                        float hmin = 0.0f;  // smallest SiLU input / 2 of the row half
+                        // the row half's 8-column groups: bias -> SiLU -> + residual -> pack -> store.  TAIL: the pass that recomputes
+                        // the SiLU inputs below -kTail with silu_tail (silu_from_half is not faithful there) and stores the row again
+                        auto row_half = [&](auto tail_pass) {
+                            constexpr bool TAIL = decltype(tail_pass)::value;
 #pragma unroll
-                        for (int j = 0; j < BLOCK_N / 8; ++j) {
-                            if (n0 + 8 * j >= p.N) continue;  // N % 8 == 0: an 8-column group is all in or all out
-                            const float2 b = *reinterpret_cast<const float2*>(sBias + n0 + 8 * j + ccol);
-                            const float a0 = acc[mi][4 * j + 2 * h], a1 = acc[mi][4 * j + 2 * h + 1];
-                            float f0, f1;
-                            if (p.act) {  // b holds bias / 2 (see the preload)
-                                f0 = silu_from_half(fmaf(a0, 0.5f, b.x));
-                                f1 = silu_from_half(fmaf(a1, 0.5f, b.y));
-                            } else {
-                                f0 = a0 + b.x;
-                                f1 = a1 + b.y;
+                            for (int j = 0; j < BLOCK_N / 8; ++j) {
+                                if (n0 + 8 * j >= p.N) continue;  // N % 8 == 0: an 8-column group is all in or all out
+                                const float2 b = *reinterpret_cast<const float2*>(sBias + n0 + 8 * j + ccol);
+                                const float a0 = acc[mi][4 * j + 2 * h], a1 = acc[mi][4 * j + 2 * h + 1];
+                                float f0, f1;
+                                if (p.act) {  // b holds bias / 2 (see the preload)
+                                    const float h0 = fmaf(a0, 0.5f, b.x), h1 = fmaf(a1, 0.5f, b.y);  // exactly fp32(acc + bias) / 2
+                                    f0 = silu_from_half(h0);
+                                    f1 = silu_from_half(h1);
+                                    if (TAIL) {
+                                        if (h0 < -0.5f * kTail) f0 = silu_tail(2.0f * h0);
+                                        if (h1 < -0.5f * kTail) f1 = silu_tail(2.0f * h1);
+                                    } else {
+                                        hmin = fminf(hmin, fminf(h0, h1));
+                                    }
+                                } else {
+                                    f0 = a0 + b.x;
+                                    f1 = a1 + b.y;
+                                }
+                                if (has_res && gpix >= 0) {
+                                    const float2 t = unpack2(rv[q][j], bf16);
+                                    f0 += t.x;
+                                    f1 += t.y;
+                                }
+                                if (staged) *reinterpret_cast<uint32_t*>(sp + 16 * j) = pack2(f0, f1, bf16);
+                                else *reinterpret_cast<uint32_t*>(op + 8 * j) = pack2(f0, f1, bf16);
                             }
-                            if (has_res && gpix >= 0) {
-                                const float2 t = unpack2(rv[q][j], bf16);
-                                f0 += t.x;
-                                f1 += t.y;
-                            }
-                            if (staged) *reinterpret_cast<uint32_t*>(sp + 16 * j) = pack2(f0, f1, bf16);
-                            else *reinterpret_cast<uint32_t*>(op + 8 * j) = pack2(f0, f1, bf16);
-                        }
+                        };
+                        row_half(std::false_type{});
+                        // inputs below -kTail are rare: one vote per row half, and only the warps holding some take the second pass
+                        // (the residual comes from the registers, so an in-place residual stays right)
+                        if (p.act && __any_sync(__activemask(), hmin < -0.5f * kTail)) row_half(std::true_type{});
                     }
                     if (staged && h == 1) {  // the sub-tile is complete: the warpgroup's 64 rows leave as whole 16-byte row segments
                         named_bar_sync(2 + wg, 128);
@@ -680,10 +699,12 @@ int finish_plan(PlanCommon& pc, int block_n, int epi, int mt, int cluster = 1) {
     return 0;
 }
 
+// the optional modes run in the OPT instantiation (see conv_gemm_kernel)
+bool plan_opt(const PlanCommon& pc) { return pc.cluster > 1 || pc.p.patch_pw > 0 || pc.p.stg_bytes > 0; }
+
 int run_plan(const PlanCommon& pc, cudaStream_t st) {
     cudaError_t e = cudaErrorInvalidValue;
-    const bool opt = pc.cluster > 1 || pc.p.patch_pw > 0 || pc.p.stg_bytes > 0;
-    const int key = (opt ? 100000 : 0) + pc.epi * 10000 + pc.block_n * 10 + pc.mt;
+    const int key = (plan_opt(pc) ? 100000 : 0) + pc.epi * 10000 + pc.block_n * 10 + pc.mt;
     switch (key) {
         case 324: e = launch_conv<32, 0, 4, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
         case 642: e = launch_conv<64, 0, 2, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
@@ -900,6 +921,28 @@ extern "C" Y5_API int y5_conv_plan_run(const y5_conv_plan* plan, void* stream) {
     return run_plan(plan->pc, static_cast<cudaStream_t>(stream));
 }
 extern "C" Y5_API void y5_conv_plan_destroy(y5_conv_plan* plan) { delete plan; }
+
+extern "C" Y5_API int y5_conv_plan_info(const y5_conv_plan* plan, struct y5_conv_plan_info* out) {
+    if (!plan || !out) return set_error(Y5_E_INVALID, "conv: null plan/info");
+    const PlanCommon& pc = plan->pc;
+    const ConvParams& p = pc.p;
+    out->a_mode = p.a_mode;
+    out->tw = p.tw;
+    out->th = p.th;
+    out->block_k = p.block_k;
+    out->block_n = pc.block_n;
+    out->mt = pc.mt;
+    out->cluster = pc.cluster;
+    out->patch_pw = p.patch_pw;
+    out->b_grouped = p.b_grouped;
+    out->staged = p.stg_bytes > 0;
+    out->opt = plan_opt(pc);
+    out->epi = pc.epi;
+    out->a_stages = p.a_stages;
+    out->b_stages = p.b_stages;
+    out->grid = pc.grid;
+    return 0;
+}
 
 extern "C" Y5_API int y5_conv_bn_silu_fwd(const y5_conv_desc* d, void* stream) {
     y5_conv_plan* plan = nullptr;
