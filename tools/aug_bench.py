@@ -13,6 +13,7 @@ LUT) single-threaded when cv2 is importable; without cv2 it reports that the com
 from __future__ import annotations
 
 import argparse
+import contextlib
 import json
 import os
 import random
@@ -26,6 +27,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from yolov5_b200.utils import dataloaders as D  # noqa: E402
 from yolov5_b200.utils.dataloaders import DeviceAugmentLoader  # noqa: E402
 
 S = 640
@@ -66,6 +68,24 @@ def gpu_info():
         return f"unknown ({e})"
 
 
+@contextlib.contextmanager
+def split_at_staging():
+    """Split host packing from the device work at the staging hand-off: while active, each stage_upload call first
+    synchronises the device and records the time in `.t` of the yielded wrapper."""
+    real = D.stage_upload
+
+    def staged(*a):
+        torch.cuda.synchronize()
+        staged.t = time.perf_counter()
+        return real(*a)
+
+    D.stage_upload = staged
+    try:
+        yield staged
+    finally:
+        D.stage_upload = real
+
+
 def time_engine(ds, batch, iters, dev):
     loader = DeviceAugmentLoader(ds, batch, device=dev)
     idx = list(range(batch))
@@ -73,22 +93,15 @@ def time_engine(ds, batch, iters, dev):
         loader.collate(idx)
     torch.cuda.synchronize()
     total, dev_part, host_part = [], [], []
-    orig = loader._staging
-
-    def staged(nbytes):  # split host packing from the device work at the staging hand-off
-        torch.cuda.synchronize()
-        staged.t = time.perf_counter()
-        return orig(nbytes)
-
-    loader._staging = staged
-    for _ in range(iters):
-        t0 = time.perf_counter()
-        imgs, targets, _, _ = loader.collate(idx)
-        torch.cuda.synchronize()
-        t1 = time.perf_counter()
-        total.append(t1 - t0)
-        host_part.append(staged.t - t0)
-        dev_part.append(t1 - staged.t)
+    with split_at_staging() as staged:
+        for _ in range(iters):
+            t0 = time.perf_counter()
+            imgs, targets, _, _ = loader.collate(idx)
+            torch.cuda.synchronize()
+            t1 = time.perf_counter()
+            total.append(t1 - t0)
+            host_part.append(staged.t - t0)
+            dev_part.append(t1 - staged.t)
     med = lambda v: float(np.median(v)) * 1e3  # noqa: E731
     return dict(batch_ms=med(total), host_draw_pack_ms=med(host_part), staging_h2d_kernels_count_ms=med(dev_part),
                 img_per_s=batch / (med(total) / 1e3), nt=int(targets.shape[0]))

@@ -26,7 +26,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from tools.aug_bench import HYP_LOW, SHAPES, gpu_info  # noqa: E402
+from tools.aug_bench import HYP_LOW, SHAPES, gpu_info, split_at_staging  # noqa: E402
 from yolov5_b200.utils.segment.dataloaders import DeviceSegAugmentLoader  # noqa: E402
 
 S = 640
@@ -71,22 +71,15 @@ def time_engine(ds, batch, iters, dev):
         loader.collate(idx)
     torch.cuda.synchronize()
     total, dev_part, host_part = [], [], []
-    orig = loader._staging
-
-    def staged(nbytes):  # split host packing from the device work at the staging hand-off
-        torch.cuda.synchronize()
-        staged.t = time.perf_counter()
-        return orig(nbytes)
-
-    loader._staging = staged
-    for _ in range(iters):
-        t0 = time.perf_counter()
-        imgs, targets, _, _, masks = loader.collate(idx)
-        torch.cuda.synchronize()
-        t1 = time.perf_counter()
-        total.append(t1 - t0)
-        host_part.append(staged.t - t0)
-        dev_part.append(t1 - staged.t)
+    with split_at_staging() as staged:
+        for _ in range(iters):
+            t0 = time.perf_counter()
+            imgs, targets, _, _, masks = loader.collate(idx)
+            torch.cuda.synchronize()
+            t1 = time.perf_counter()
+            total.append(t1 - t0)
+            host_part.append(staged.t - t0)
+            dev_part.append(t1 - staged.t)
     med = lambda v: float(np.median(v)) * 1e3  # noqa: E731
     return dict(batch_ms=med(total), host_draw_pack_ms=med(host_part), staging_h2d_kernels_masks_ms=med(dev_part),
                 img_per_s=batch / (med(total) / 1e3), nt=int(targets.shape[0]), masks=list(masks.shape), masks_dtype=str(masks.dtype))

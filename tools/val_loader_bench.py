@@ -134,7 +134,7 @@ def run_new(ds, batch, workers, dev):
 
     pos = list(range(min(batch, len(ds))))
     lay = ValBatchLayout(ds, pos, [load_val_image(ds, p) for p in pos])
-    staging = _Staging()
+    staging = _Staging(2)
     e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
     up, kern = [], []
     for _ in range(10):

@@ -20,6 +20,10 @@ load_image's resize (cv2 INTER_AREA / INTER_LINEAR) and the letterbox in one lau
 ``DeviceClassifyLoader`` is ``create_classification_dataloader``'s loader (reference utils/dataloaders.py:949-1009,
 without Albumentations): host threads decode one batch ahead, and ``y5_cls_batch`` does classify_transforms' center
 crop, resize, ToTensor and Normalize in one launch; see its docstring.
+
+Every loader lays out its host data with ``StagingLayout`` and uploads it with ``stage_upload``, one pinned
+host-to-device copy per batch.  The segmentation loaders (utils/segment/dataloaders.py) subclass ``DeviceAugmentLoader``
+and ``DeviceValLoader``.
 """
 from __future__ import annotations
 
@@ -40,21 +44,70 @@ from .augmentations import (affine_matrix, aug_gather, aug_labels, hsv_luts, inv
 _ALIGN = 16
 
 
-def _check_dataset(ds):
-    """Refuse what the device path does not implement, before any draw or launch."""
+def _aligned(nbytes):
+    return (nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
+
+
+class StagingLayout:
+    """Host arrays placed at _ALIGN-byte aligned offsets of one staging buffer: what one ``stage_upload`` copies."""
+
+    def __init__(self):
+        self.blocks = []  # (offset, array)
+        self.size = 0
+
+    def add(self, a):
+        """Place host array `a` after the blocks so far -> its byte offset.  `a` may be a strided view; it is read when
+        the layout is uploaded."""
+        off = self.size
+        self.blocks.append((off, a))
+        self.size += _aligned(a.nbytes)
+        return off
+
+
+class _Staging:
+    """`count` pinned staging buffers used in turn; a buffer is reused once the copy that last read it has run."""
+
+    def __init__(self, count):
+        self.buf = [None] * count
+        self.done = [None] * count
+        self.turn = 0
+
+    def get(self, nbytes):
+        k = self.turn
+        self.turn = (k + 1) % len(self.buf)
+        if self.done[k] is not None:
+            self.done[k].synchronize()
+        if self.buf[k] is None or self.buf[k].numel() < nbytes:
+            self.buf[k] = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8).pin_memory()
+        return k, self.buf[k]
+
+    def mark(self, k, stream):
+        self.done[k] = torch.cuda.Event()
+        self.done[k].record(stream)
+
+
+def stage_upload(staging, dev_buf, layout):
+    """Write the blocks of `layout` (a StagingLayout) into a pinned buffer of `staging` and copy its first `layout.size`
+    bytes to `dev_buf` on the current stream."""
+    total = layout.size
+    k, pinned = staging.get(total)
+    host = pinned.numpy()
+    for off, a in layout.blocks:
+        np.copyto(host[off: off + a.nbytes].view(a.dtype).reshape(a.shape), a)
+    dev_buf[:total].copy_(pinned[:total], non_blocking=True)
+    staging.mark(k, torch.cuda.current_stream(dev_buf.device))
+
+
+def _check_augment(ds, name):
+    """The refusals both training loaders share, before any draw or launch."""
     hyp = ds.hyp
     if getattr(ds, "rect", False) or not getattr(ds, "augment", True):
-        raise NotImplementedError("y5b200: DeviceAugmentLoader implements augment=True, rect=False only")
+        raise NotImplementedError(f"y5b200: {name} implements augment=True, rect=False only")
     if hyp.get("perspective", 0.0) > 0:
         raise NotImplementedError("y5b200: perspective > 0 (cv2.warpPerspective) is not implemented")
-    if any(len(s) for s in getattr(ds, "segments", ())):
-        # segments change random_perspective's box path and make copy_paste active: segmentation datasets
-        raise NotImplementedError("y5b200: datasets with segments (copy_paste, segment-derived boxes) are not implemented")
     alb = getattr(ds, "albumentations", None)
     if alb is not None and getattr(alb, "transform", None) is not None:
         raise NotImplementedError("y5b200: an active Albumentations transform is not implemented")
-    if int(ds.img_size) <= 0 or int(ds.img_size) > 16384:
-        raise ValueError(f"y5b200: img_size {ds.img_size} outside (0, 16384]")
 
 
 def _mosaic_draws(ds, index, shuffle_tiles=True):
@@ -127,7 +180,7 @@ class DeviceAugmentLoader:
     """
 
     def __init__(self, dataset, batch_size, sampler=None, shuffle=False, device=None, dtype=torch.uint8, generator=None, drop_last=False):
-        _check_dataset(dataset)
+        self._check_dataset(dataset)
         if dtype not in (torch.uint8, torch.float16, torch.bfloat16, torch.float32):
             raise ValueError(f"y5b200: unsupported output dtype {dtype}")
         self.dataset = dataset
@@ -137,8 +190,7 @@ class DeviceAugmentLoader:
         self.index_loader = torch.utils.data.DataLoader(range(len(dataset.indices)), batch_size=self.batch_size, shuffle=shuffle and sampler is None,
                                                         sampler=sampler, generator=generator, drop_last=drop_last, collate_fn=list)
         self.sampler = sampler
-        self._pinned = None
-        self._copied = None  # event: the last staging upload has been read
+        self._staging = _Staging(1)  # a batch's upload waits for the previous batch's copy
 
     def __len__(self):
         return len(self.index_loader)
@@ -147,18 +199,29 @@ class DeviceAugmentLoader:
         for batch in self.index_loader:
             yield self.collate(batch)
 
-    def _staging(self, nbytes):
-        if self._copied is not None:
-            self._copied.synchronize()  # the previous batch's copy still reads the pinned buffer
-        if self._pinned is None or self._pinned.numel() < nbytes:
-            self._pinned = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8).pin_memory()
-        return self._pinned
+    def _check_dataset(self, ds):
+        """Refuse what the device path does not implement, before any draw or launch."""
+        _check_augment(ds, "DeviceAugmentLoader")
+        if any(len(s) for s in getattr(ds, "segments", ())):
+            # segments change random_perspective's box path and make copy_paste active: segmentation datasets
+            raise NotImplementedError("y5b200: datasets with segments (copy_paste, segment-derived boxes) are not implemented")
+        if int(ds.img_size) <= 0 or int(ds.img_size) > 16384:
+            raise ValueError(f"y5b200: img_size {ds.img_size} outside (0, 16384]")
 
-    def collate(self, batch, sync=True):
-        """Augment dataset items `batch` (positions into dataset.indices) -> (imgs, targets, paths, shapes); with
-        sync=False targets is (padded (n, 6) rows, device int32 count) and nothing waits for the device."""
+    def _draw(self, i):
+        return draw_item(self.dataset, i)
+
+    def _stage_labels(self, lay, labelled, n):
+        """Add the batch's label data to the staging layout -> (offset of the y5_aug_label records, their count).
+        labelled: (image, dataset index, records) for each labelled tile, in table order; n: the batch size."""
+        rec = np.concatenate([r for _, _, r in labelled], 0) if labelled else np.zeros((0, 12), np.float32)
+        return lay.add(rec), len(rec)
+
+    def _augment(self, batch):
+        """Draw, load and stage dataset items `batch`, then letterbox the non-mosaic items and run y5_aug_gather ->
+        (imgs, device image table, device staging buffer, what _stage_labels returned, paths, shapes)."""
         ds, dev, s = self.dataset, self.device, int(self.dataset.img_size)
-        params = [draw_item(ds, i) for i in batch]
+        params = [self._draw(i) for i in batch]
         need = []
         for p in params:
             for k in ([i for m in p["m"] for i in m["indices"]] if p["mosaic"] else [p["index"]]):
@@ -172,16 +235,12 @@ class DeviceAugmentLoader:
             if max(im.shape[:2]) > 2 * s or min(im.shape[:2]) < 1:
                 raise ValueError(f"y5b200: load_image({k}) returned {im.shape[:2]}, outside [1, {2 * s}]")
             loaded[k] = (np.ascontiguousarray(im), hw0, hw)
-        # staging layout: sources | table | label rows
-        offs, pos = {}, 0
-        for k in need:
-            offs[k] = pos
-            pos += (loaded[k][0].nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
+        # staging layout: sources | table | label data
+        lay = StagingLayout()
+        offs = {k: lay.add(loaded[k][0]) for k in need}
         n = len(params)
         table = (_lib.AugImage * n)()
-        table_off = pos
-        pos += ctypes.sizeof(table)
-        rows, shapes, src_tiles = [], [], []
+        labelled, shapes, src_tiles = [], [], []
         lb_items = [b for b, p in enumerate(params) if not p["mosaic"]]
         canvas = torch.empty(len(lb_items), 3, s, s, dtype=torch.uint8, device=dev) if lb_items else None
         for b, p in enumerate(params):
@@ -206,7 +265,7 @@ class DeviceAugmentLoader:
                         tile.x1a, tile.y1a, tile.x2a, tile.y2a, tile.dx, tile.dy = x1a, y1a, x2a, y2a, x1b - x1a, y1b - y1a
                         lab = ds.labels[k]
                         if len(lab):
-                            rows.append(_label_rows(lab, b, m, w, h, x1a - x1b, y1a - y1b, _lib.AUG_CLIP))
+                            labelled.append((b, k, _label_rows(lab, b, m, w, h, x1a - x1b, y1a - y1b, _lib.AUG_CLIP)))
                 if len(p["m"]) == 2:
                     e.mix_r = p["r"]
                 shapes.append(None)
@@ -226,43 +285,38 @@ class DeviceAugmentLoader:
                 set_tile(e.tiles[0], canvas[lb_items.index(b)], 0, 0, s, s, 0, 0)
                 lab = ds.labels[k]
                 if len(lab):
-                    rows.append(_label_rows(lab, b, 0, ratio[0] * w, ratio[1] * h, pad[0], pad[1], 0))
+                    labelled.append((b, k, _label_rows(lab, b, 0, ratio[0] * w, ratio[1] * h, pad[0], pad[1], 0)))
             if p["hsv"] is not None:
                 e.hsv = 1
                 luts = hsv_luts(p["hsv"])
                 for c in range(3):
                     e.lut[c][:] = luts[c].tolist()
             e.flipud, e.fliplr = int(p["flipud"]), int(p["fliplr"])
-        rec = np.concatenate(rows, 0) if rows else np.zeros((0, 12), np.float32)
-        n_labels = len(rec)
-        total = pos + rec.nbytes
-        dev_buf = torch.empty(total, dtype=torch.uint8, device=dev)
+        table_off = lay.add(np.frombuffer(table, np.uint8))  # a view: the upload copies the table with the addresses below
+        labels = self._stage_labels(lay, labelled, n)
+        dev_buf = torch.empty(lay.size, dtype=torch.uint8, device=dev)
         for tile, off in src_tiles:
             tile.src = dev_buf.data_ptr() + off
-        pinned = self._staging(total)
-        host = pinned.numpy()
-        for k in need:
-            a = loaded[k][0]
-            host[offs[k]: offs[k] + a.nbytes] = a.reshape(-1)
-        host[table_off: table_off + ctypes.sizeof(table)] = np.frombuffer(bytes(table), np.uint8)
-        host[pos: total] = rec.view(np.uint8).reshape(-1)
         with _lib.on(dev):
-            stream = torch.cuda.current_stream(dev)
-            dev_buf[:total].copy_(pinned[:total], non_blocking=True)
-            self._copied = torch.cuda.Event()
-            self._copied.record(stream)
+            stage_upload(self._staging, dev_buf, lay)
             if lb_items:
                 views = [dev_buf[offs[k]: offs[k] + loaded[k][0].nbytes].view(loaded[k][0].shape) for k in (params[b]["index"] for b in lb_items)]
                 letterbox_batch(views, (s, s), auto=False, scaleup=True, swap_rb=False, device=dev, out=canvas)
             table_dev = dev_buf[table_off: table_off + ctypes.sizeof(table)]
             imgs = aug_gather(table_dev, n, s, s, swap_rb=True, dtype=self.dtype, device=dev)
-            padded, count = aug_labels(table_dev, n, dev_buf[pos: total], n_labels, s, s, device=dev)
-        paths = tuple(ds.im_files[p["index"]] for p in params)
-        if not sync:
-            return imgs, (padded, count), paths, tuple(shapes)
-        nt = int(count.item())
-        return imgs, padded[:nt], paths, tuple(shapes)
+        return imgs, table_dev, dev_buf, labels, tuple(ds.im_files[p["index"]] for p in params), tuple(shapes)
 
+    def collate(self, batch, sync=True):
+        """Augment dataset items `batch` (positions into dataset.indices) -> (imgs, targets, paths, shapes); with
+        sync=False targets is (padded (n, 6) rows, device int32 count) and nothing waits for the device."""
+        s = int(self.dataset.img_size)
+        imgs, table_dev, dev_buf, (off, n_labels), paths, shapes = self._augment(batch)
+        rec = dev_buf[off: off + n_labels * ctypes.sizeof(_lib.AugLabel)]
+        padded, count = aug_labels(table_dev, len(batch), rec, n_labels, s, s, device=self.device)
+        if not sync:
+            return imgs, (padded, count), paths, shapes
+        nt = int(count.item())
+        return imgs, padded[:nt], paths, shapes
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -348,39 +402,6 @@ def val_label_rows(labels, ratio, w, h, pad, out_w, out_h):
     return lab
 
 
-class _Staging:
-    """Two pinned staging buffers used in turn; a buffer is reused once the copy that last read it has run."""
-
-    def __init__(self):
-        self.buf = [None, None]
-        self.done = [None, None]
-        self.turn = 0
-
-    def get(self, nbytes):
-        k = self.turn
-        self.turn ^= 1
-        if self.done[k] is not None:
-            self.done[k].synchronize()
-        if self.buf[k] is None or self.buf[k].numel() < nbytes:
-            self.buf[k] = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8).pin_memory()
-        return k, self.buf[k]
-
-    def mark(self, k, stream):
-        self.done[k] = torch.cuda.Event()
-        self.done[k].record(stream)
-
-
-def stage_upload(staging, dev_buf, blocks, total):
-    """Write host arrays at byte offsets into a pinned `staging` buffer and copy its first `total` bytes to `dev_buf` on
-    the current stream.  blocks: (offset, array) pairs; an array may be a strided view (it is copied in place)."""
-    k, pinned = staging.get(total)
-    host = pinned.numpy()
-    for off, a in blocks:
-        np.copyto(host[off: off + a.nbytes].view(a.dtype).reshape(a.shape), a)
-    dev_buf[:total].copy_(pinned[:total], non_blocking=True)
-    staging.mark(k, torch.cuda.current_stream(dev_buf.device))
-
-
 def decode_ahead(ds, batches, decode, workers):
     """(batch, decoded items) for each batch of the iterable `batches`, with `workers` threads running decode(ds, i) for
     every i of the next batch while the caller works on the current one."""
@@ -402,15 +423,16 @@ def decode_ahead(ds, batches, decode, workers):
             b = nxt
 
 
-class ValBatchLayout:
+class ValBatchLayout(StagingLayout):
     """Host side of one validation batch: decoded images, geometry, shapes and label rows, laid out in one staging
-    buffer as [sources | extra host blocks], plus the device scratch the letterboxes that resize again need."""
+    buffer as [sources | blocks added later], plus the device scratch the letterboxes that resize again need."""
 
     def __init__(self, ds, positions, loaded):
+        super().__init__()
         self.keys = [int(ds.indices[p]) for p in positions]
         self.n = len(positions)
-        self.items, self.shapes, self.rows, self.offs = [], [], [], []
-        pos = scratch = 0
+        self.items, self.shapes, self.offs = [], [], []
+        scratch = 0
         batch_shape = None
         for b, (k, (im, hw0, cached)) in enumerate(zip(self.keys, loaded)):
             if not isinstance(im, np.ndarray) or im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
@@ -427,32 +449,20 @@ class ValBatchLayout:
             self.items.append(dict(im=im, res=(h, w), interp=interp, new=(new_unpad[1], new_unpad[0]), top=top, left=left,
                                    scratch=scratch if again else None, ratio=ratio, pad=pad))
             if again:
-                scratch += (h * w * 3 + _ALIGN - 1) // _ALIGN * _ALIGN
+                scratch += _aligned(h * w * 3)
             self.shapes.append(((int(hw0[0]), int(hw0[1])), ((h / hw0[0], w / hw0[1]), pad)))
-            self.offs.append(pos)
-            pos += (im.nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
+            self.offs.append(self.add(im))
         self.out_hw = batch_shape
-        self.pos = pos
         self.scratch_bytes = scratch
-        self.blocks = []
 
     def label_rows(self, ds, b, out_w, out_h):
         it = self.items[b]
         return val_label_rows(ds.labels[self.keys[b]], it["ratio"], it["res"][1], it["res"][0], it["pad"], out_w, out_h)
 
-    def add_block(self, a):
-        """Append a host array to the staging layout -> its byte offset."""
-        a = np.ascontiguousarray(a)
-        off = self.pos
-        self.blocks.append((off, a))
-        self.pos += (a.nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
-        return off
-
     def upload(self, staging, dev):
-        """One pinned host-to-device copy of the sources and blocks -> (device buffer, scratch base address)."""
-        total = self.pos
-        dev_buf = torch.empty(total + self.scratch_bytes, dtype=torch.uint8, device=dev)
-        stage_upload(staging, dev_buf, [(off, it["im"]) for off, it in zip(self.offs, self.items)] + self.blocks, total)
+        """One pinned host-to-device copy of the sources and blocks -> the device buffer, the scratch after them."""
+        dev_buf = torch.empty(self.size + self.scratch_bytes, dtype=torch.uint8, device=dev)
+        stage_upload(staging, dev_buf, self)
         return dev_buf
 
     def letterbox(self, dev_buf, dtype, dev):
@@ -467,7 +477,7 @@ class ValBatchLayout:
             d.interp = it["interp"]
             d.new_h, d.new_w = it["new"]
             d.top, d.left = it["top"], it["left"]
-            d.scratch = base + self.pos + it["scratch"] if it["scratch"] is not None else None
+            d.scratch = base + self.size + it["scratch"] if it["scratch"] is not None else None
         imgs = torch.empty(self.n, 3, H, W, dtype=dtype, device=dev)
         _lib.check(_lib.lib().y5_val_letterbox(table, self.n, H, W, imgs.data_ptr(), _lib.dtype_code(dtype),
                                                ctypes.c_void_p(_lib.stream_ptr(dev))), "val_letterbox")
@@ -498,7 +508,7 @@ class DeviceValLoader:
         self.workers = max(1, int(workers))
         self.decode = decode or load_val_image
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        self._staging = _Staging()
+        self._staging = _Staging(2)  # the next batch is staged while the previous copy may still run
 
     def __len__(self):
         return (len(self.dataset.indices) + self.batch_size - 1) // self.batch_size
@@ -527,7 +537,7 @@ class DeviceValLoader:
             tg[i: i + len(r), 0] = b
             tg[i: i + len(r), 1:] = r
             i += len(r)
-        t_off = lay.add_block(tg)
+        t_off = lay.add(tg)
         with _lib.on(dev):
             dev_buf = lay.upload(self._staging, dev)
             imgs = lay.letterbox(dev_buf, self.dtype, dev)
@@ -639,7 +649,7 @@ class DeviceClassifyLoader:
         object.__setattr__(index, "batch_sampler", _Repeat(index.batch_sampler))  # DataLoader refuses a plain assignment
         self._stream = iter(index)  # created once: the iterator's base seed is drawn from the generator here, as the reference's is
         self._carry = None  # a batch drawn from the stream but not yielded (a pass left early)
-        self._staging = _Staging()
+        self._staging = _Staging(2)  # the next batch is staged while the previous copy may still run
         self._mean = (ctypes.c_float * 3)(*IMAGENET_MEAN)
         self._std = (ctypes.c_float * 3)(*IMAGENET_STD)
 
@@ -664,7 +674,8 @@ class DeviceClassifyLoader:
         if loaded is None:
             loaded = [self.decode(ds, i) for i in items]
         n = len(items)
-        blocks, offs, sides, pos = [], [], [], 0
+        lay = StagingLayout()
+        offs, sides = [], []
         for i, im in zip(items, loaded):
             if not isinstance(im, np.ndarray) or im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
                 raise ValueError(f"y5b200: image {i} must be a uint8 HWC BGR image with 3 channels")
@@ -673,23 +684,18 @@ class DeviceClassifyLoader:
             if m < 1:
                 raise ValueError(f"y5b200: image {i} is empty")
             top, left = (h - m) // 2, (w - m) // 2
-            blocks.append((pos, im[top: top + m, left: left + m]))
-            offs.append(pos)
+            offs.append(lay.add(im[top: top + m, left: left + m]))
             sides.append(m)
-            pos += (m * m * 3 + _ALIGN - 1) // _ALIGN * _ALIGN
         table = (_lib.ClsImage * n)()
-        table_off = pos
-        pos += (ctypes.sizeof(table) + _ALIGN - 1) // _ALIGN * _ALIGN
+        table_off = lay.add(np.frombuffer(table, np.uint8))  # a view: the upload copies the table with the addresses below
         labels = np.array([ds.samples[i][1] for i in items], np.int64)
-        label_off = pos
-        pos += labels.nbytes
+        label_off = lay.add(labels)
         with _lib.on(dev):
-            dev_buf = torch.empty(pos, dtype=torch.uint8, device=dev)
+            dev_buf = torch.empty(lay.size, dtype=torch.uint8, device=dev)
             base = dev_buf.data_ptr()
             for d, off, m in zip(table, offs, sides):
                 d.data, d.side, d.row_bytes = base + off, m, 3 * m
-            blocks += [(table_off, np.frombuffer(table, np.uint8)), (label_off, labels)]
-            stage_upload(self._staging, dev_buf, blocks, pos)
+            stage_upload(self._staging, dev_buf, lay)
             h, w = self.size
             images = torch.empty(n, 3, h, w, dtype=self.dtype, device=dev)
             _lib.check(_lib.lib().y5_cls_batch(base + table_off, n, h, w, self._mean, self._std, images.data_ptr(), _lib.dtype_code(self.dtype),

@@ -1,13 +1,13 @@
 """The segmentation training dataloader's augmentation on the device (reference utils/segment/dataloaders.py:130-301,
 LoadImagesAndLabelsAndMasks.__getitem__ + collate_fn with augment=True, rect=False, copy_paste=0).
 
-``DeviceSegAugmentLoader`` yields ``(imgs, targets, paths, shapes, masks)`` as ``collate_fn`` builds them, with
-``imgs``, ``targets`` and ``masks`` on the device.  Per batch:
+``DeviceSegAugmentLoader`` is a ``DeviceAugmentLoader`` that yields ``(imgs, targets, paths, shapes, masks)`` as
+``collate_fn`` builds them, with ``imgs``, ``targets`` and ``masks`` on the device.  Per batch:
   1. host: every random draw in the reference's order (``draw_item``: the mixup partner is random.randint(0, n - 1)
      and the mosaic tiles keep their order),
      ``load_image``, and one pinned host-to-device copy of the sources, the image table, the label rows, the
      polygons' normalised points and the per-image label ranges;
-  2. device: ``y5_aug_gather`` writes the images exactly as the detection loader does (the segmentation loader's image
+  2. device: ``y5_aug_gather`` writes the images through the detection loader's code (the segmentation loader's image
      arithmetic is the same when copy_paste == 0); ``y5_seg_warp`` runs each label's segment through xyn2xy, the clip,
      resample_segments, the affine map, segment2box and box_candidates; ``y5_seg_raster`` rasterizes each kept polygon
      as cv2.fillPoly + cv2.resize do; ``y5_seg_order`` compacts the labels (in overlap mode in the order of
@@ -29,31 +29,13 @@ import numpy as np
 import torch
 
 from ... import _lib
-from ..augmentations import affine_matrix, aug_gather, hsv_luts, invert_affine, letterbox_batch, letterbox_geometry, set_tile
-from ..dataloaders import _ALIGN, DeviceValLoader, ValBatchLayout, _label_rows, _placements, check_val_dataset, draw_item
+from ..dataloaders import DeviceAugmentLoader, DeviceValLoader, ValBatchLayout, _check_augment, check_val_dataset, draw_item
 
 _RATIOS = (1, 4)  # r = 2 is cv2.resize's INTER_AREA special case, not implemented
 
 
-def _check_dataset(ds, overlap, downsample_ratio):
-    """Refuse what the device path does not implement, before any draw or launch."""
-    hyp = ds.hyp
-    if getattr(ds, "rect", False) or not getattr(ds, "augment", True):
-        raise NotImplementedError("y5b200: DeviceSegAugmentLoader implements augment=True, rect=False only")
-    if hyp.get("perspective", 0.0) > 0:
-        raise NotImplementedError("y5b200: perspective > 0 (cv2.warpPerspective) is not implemented")
-    if hyp.get("copy_paste", 0.0) > 0:
-        raise NotImplementedError("y5b200: copy_paste > 0 is not implemented")
-    alb = getattr(ds, "albumentations", None)
-    if alb is not None and getattr(alb, "transform", None) is not None:
-        raise NotImplementedError("y5b200: an active Albumentations transform is not implemented")
-    if downsample_ratio not in _RATIOS:
-        raise NotImplementedError(f"y5b200: downsample_ratio {downsample_ratio} is not implemented (1 or 4)")
-    s = int(ds.img_size)
-    if s <= 0 or s > 4096:
-        raise ValueError(f"y5b200: img_size {ds.img_size} outside (0, 4096]")
-    if s % downsample_ratio:
-        raise NotImplementedError(f"y5b200: img_size {s} is not a multiple of downsample_ratio {downsample_ratio}")
+def _check_segments(ds):
+    """One float32 (n >= 1, 2) segment of normalised points per label."""
     for k, (lab, segs) in enumerate(zip(ds.labels, ds.segments)):
         if len(lab) and len(segs) != len(lab):
             raise NotImplementedError(f"y5b200: image {k} has {len(lab)} labels and {len(segs)} segments (one segment per label is implemented)")
@@ -66,168 +48,62 @@ def _mixup_partner(ds):
     return lambda: random.randint(0, ds.n - 1)
 
 
-class DeviceSegAugmentLoader:
+class DeviceSegAugmentLoader(DeviceAugmentLoader):
     """Drop-in for utils/segment/dataloaders.py ``create_dataloader``'s loader over a ``LoadImagesAndLabelsAndMasks``-like
     dataset (duck-typed as ``DeviceAugmentLoader``'s, plus n, segments, overlap, downsample_ratio).  The index stream,
-    sampler / DDP behaviour and output ``dtype`` of the images are ``DeviceAugmentLoader``'s.  ``overlap`` and
+    sampler / DDP behaviour, the images and their output ``dtype`` are ``DeviceAugmentLoader``'s.  ``overlap`` and
     ``downsample_ratio`` default to the dataset's."""
 
     def __init__(self, dataset, batch_size, sampler=None, shuffle=False, device=None, dtype=torch.uint8, generator=None, drop_last=False,
                  overlap=None, downsample_ratio=None):
         self.overlap = bool(getattr(dataset, "overlap", False) if overlap is None else overlap)
         self.downsample_ratio = int(getattr(dataset, "downsample_ratio", 1) if downsample_ratio is None else downsample_ratio)
-        _check_dataset(dataset, self.overlap, self.downsample_ratio)
-        if dtype not in (torch.uint8, torch.float16, torch.bfloat16, torch.float32):
-            raise ValueError(f"y5b200: unsupported output dtype {dtype}")
-        self.dataset = dataset
-        self.batch_size = int(batch_size)
-        self.dtype = dtype
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        self.index_loader = torch.utils.data.DataLoader(range(len(dataset.indices)), batch_size=self.batch_size, shuffle=shuffle and sampler is None,
-                                                        sampler=sampler, generator=generator, drop_last=drop_last, collate_fn=list)
-        self.sampler = sampler
-        self._pinned = None
-        self._copied = None  # event: the last staging upload has been read
+        super().__init__(dataset, batch_size, sampler=sampler, shuffle=shuffle, device=device, dtype=dtype, generator=generator, drop_last=drop_last)
 
-    def __len__(self):
-        return len(self.index_loader)
+    def _check_dataset(self, ds):
+        """Refuse what the device path does not implement, before any draw or launch."""
+        _check_augment(ds, "DeviceSegAugmentLoader")
+        if ds.hyp.get("copy_paste", 0.0) > 0:
+            raise NotImplementedError("y5b200: copy_paste > 0 is not implemented")
+        r = self.downsample_ratio
+        if r not in _RATIOS:
+            raise NotImplementedError(f"y5b200: downsample_ratio {r} is not implemented (1 or 4)")
+        s = int(ds.img_size)
+        if s <= 0 or s > 4096:
+            raise ValueError(f"y5b200: img_size {ds.img_size} outside (0, 4096]")
+        if s % r:
+            raise NotImplementedError(f"y5b200: img_size {s} is not a multiple of downsample_ratio {r}")
+        _check_segments(ds)
 
-    def __iter__(self):
-        for batch in self.index_loader:
-            yield self.collate(batch)
+    def _draw(self, i):
+        return draw_item(self.dataset, i, _mixup_partner(self.dataset), shuffle_tiles=False)
 
-    def _staging(self, nbytes):
-        if self._copied is not None:
-            self._copied.synchronize()  # the previous batch's copy still reads the pinned buffer
-        if self._pinned is None or self._pinned.numel() < nbytes:
-            self._pinned = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8).pin_memory()
-        return self._pinned
-
-    def collate(self, batch):
-        """Augment dataset items `batch` (positions into dataset.indices) -> (imgs, targets, paths, shapes, masks)."""
-        ds, dev, s, r = self.dataset, self.device, int(self.dataset.img_size), self.downsample_ratio
-        partner = _mixup_partner(ds)
-        params = [draw_item(ds, i, partner, shuffle_tiles=False) for i in batch]
-        need = []
-        for p in params:
-            for k in ([i for m in p["m"] for i in m["indices"]] if p["mosaic"] else [p["index"]]):
-                if k not in need:
-                    need.append(k)
-        loaded = {}
-        for k in need:
-            im, hw0, hw = ds.load_image(k)
-            if not isinstance(im, np.ndarray) or im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
-                raise ValueError(f"y5b200: load_image({k}) must return a uint8 HWC BGR image with 3 channels")
-            if max(im.shape[:2]) > 2 * s or min(im.shape[:2]) < 1:
-                raise ValueError(f"y5b200: load_image({k}) returned {im.shape[:2]}, outside [1, {2 * s}]")
-            loaded[k] = (np.ascontiguousarray(im), hw0, hw)
-        offs, pos = {}, 0
-        for k in need:
-            offs[k] = pos
-            pos += (loaded[k][0].nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
-        n = len(params)
-        table = (_lib.AugImage * n)()
-        table_off = pos
-        pos += ctypes.sizeof(table)
-        rows, polys, image_rows, shapes, src_tiles = [], [], [0], [], []
-        n_rows = 0
-
-        def add_labels(k, b, m, tw, th, pw, ph, flags):
-            nonlocal n_rows
-            lab = ds.labels[k]
-            if len(lab):
-                rows.append(_label_rows(lab, b, m, tw, th, pw, ph, flags))
-                polys.extend(ds.segments[k])
-                n_rows += len(lab)
-
-        lb_items = [b for b, p in enumerate(params) if not p["mosaic"]]
-        canvas = torch.empty(len(lb_items), 3, s, s, dtype=torch.uint8, device=dev) if lb_items else None
-        for b, p in enumerate(params):
-            e = table[b]
-            if p["mosaic"]:
-                e.n_mosaic = len(p["m"])
-                e.canvas_w = e.canvas_h = 2 * s
-                e.clip_max = 2 * s
-                for m, md in enumerate(p["m"]):
-                    srcs = [loaded[k] for k in md["indices"]]
-                    M = affine_matrix(md["persp"], (2 * s, 2 * s), ds.mosaic_border)
-                    e.warp[m] = 1
-                    e.inv_m[m][:] = invert_affine(M)
-                    e.m[m][:] = [float(v) for v in M[:2].reshape(6)]
-                    e.scale[m] = md["persp"][3]
-                    e.n_tiles[m] = 4
-                    for t, ((x1a, y1a, x2a, y2a, x1b, y1b), k, (im, _, (h, w))) in enumerate(
-                            zip(_placements(md["xc"], md["yc"], s, [x[2] for x in srcs]), md["indices"], srcs)):
-                        tile = e.tiles[4 * m + t]
-                        src_tiles.append((tile, offs[k]))
-                        tile.row_bytes, tile.pixel_stride, tile.channel_stride = im.shape[1] * 3, 3, 1
-                        tile.x1a, tile.y1a, tile.x2a, tile.y2a, tile.dx, tile.dy = x1a, y1a, x2a, y2a, x1b - x1a, y1b - y1a
-                        add_labels(k, b, m, w, h, x1a - x1b, y1a - y1b, _lib.AUG_CLIP)
-                if len(p["m"]) == 2:
-                    e.mix_r = p["r"]
-                shapes.append(None)
-            else:
-                k = p["index"]
-                im, (h0, w0), (h, w) = loaded[k]
-                _, ratio, pad, _ = letterbox_geometry(im.shape[:2], s, auto=False, scaleup=True)
-                shapes.append(((h0, w0), ((h / h0, w / w0), pad)))
-                M = affine_matrix(p["persp"], (s, s), (0, 0))
-                e.n_mosaic = 1
-                e.canvas_w = e.canvas_h = s
-                e.warp[0] = int((M != np.eye(3)).any())
-                e.inv_m[0][:] = invert_affine(M)
-                e.m[0][:] = [float(v) for v in M[:2].reshape(6)]
-                e.scale[0] = p["persp"][3]
-                e.n_tiles[0] = 1
-                set_tile(e.tiles[0], canvas[lb_items.index(b)], 0, 0, s, s, 0, 0)
-                add_labels(k, b, 0, ratio[0] * w, ratio[1] * h, pad[0], pad[1], 0)
-            if p["hsv"] is not None:
-                e.hsv = 1
-                luts = hsv_luts(p["hsv"])
-                for c in range(3):
-                    e.lut[c][:] = luts[c].tolist()
-            e.flipud, e.fliplr = int(p["flipud"]), int(p["fliplr"])
-            image_rows.append(n_rows)
-        rec = np.concatenate(rows, 0) if rows else np.zeros((0, 12), np.float32)
+    def _stage_labels(self, lay, labelled, n):
+        """The label records, then each label's y5_aug_segment (point offset, point count), the segments' normalised points
+        and the per-image label ranges -> (their four offsets, label count, longest segment)."""
+        rec_off, n_rows = super()._stage_labels(lay, labelled, n)
+        polys = [seg for _, k, _ in labelled for seg in self.dataset.segments[k]]
         seg = np.zeros((max(n_rows, 1), 2), np.int32)
         lens = np.array([len(x) for x in polys], np.int64)
         seg[:n_rows, 0] = np.cumsum(lens) - lens
         seg[:n_rows, 1] = lens
         pts = np.concatenate(polys, 0) if polys else np.zeros((1, 2), np.float32)
-        max_points = int(lens.max()) if n_rows else 1
-        blocks = [rec.view(np.uint8).reshape(-1), seg.view(np.uint8).reshape(-1), pts.view(np.uint8).reshape(-1),
-                  np.asarray(image_rows, np.int32).view(np.uint8)]
-        block_off = []
-        for a in blocks:
-            block_off.append(pos)
-            pos += (a.nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
-        total = pos
-        dev_buf = torch.empty(total, dtype=torch.uint8, device=dev)
-        for tile, off in src_tiles:
-            tile.src = dev_buf.data_ptr() + off
-        pinned = self._staging(total)
-        host = pinned.numpy()
-        for k in need:
-            a = loaded[k][0]
-            host[offs[k]: offs[k] + a.nbytes] = a.reshape(-1)
-        host[table_off: table_off + ctypes.sizeof(table)] = np.frombuffer(bytes(table), np.uint8)
-        for off, a in zip(block_off, blocks):
-            host[off: off + a.nbytes] = a
-        lab_p, seg_p, pts_p, rows_p = (dev_buf.data_ptr() + off for off in block_off)
+        image_rows = np.zeros(n + 1, np.int32)
+        for b, _, rec in labelled:
+            image_rows[b + 1:] += len(rec)
+        offs = (rec_off, *(lay.add(a) for a in (seg, pts, image_rows)))
+        return offs, n_rows, int(lens.max()) if n_rows else 1
+
+    def collate(self, batch):
+        """Augment dataset items `batch` (positions into dataset.indices) -> (imgs, targets, paths, shapes, masks)."""
+        dev, s, r, n = self.device, int(self.dataset.img_size), self.downsample_ratio, len(batch)
+        imgs, table_dev, dev_buf, (offs, n_rows, max_points), paths, shapes = self._augment(batch)
+        lab_p, seg_p, pts_p, rows_p = (dev_buf.data_ptr() + off for off in offs)
         mh, mw = s // r, s // r
         nl = max(n_rows, 1)
         lib = _lib.lib()
         with _lib.on(dev):
-            stream = torch.cuda.current_stream(dev)
-            st = ctypes.c_void_p(stream.cuda_stream)
-            dev_buf[:total].copy_(pinned[:total], non_blocking=True)
-            self._copied = torch.cuda.Event()
-            self._copied.record(stream)
-            if lb_items:
-                views = [dev_buf[offs[k]: offs[k] + loaded[k][0].nbytes].view(loaded[k][0].shape) for k in (params[b]["index"] for b in lb_items)]
-                letterbox_batch(views, (s, s), auto=False, scaleup=True, swap_rb=False, device=dev, out=canvas)
-            table_dev = dev_buf[table_off: table_off + ctypes.sizeof(table)]
-            imgs = aug_gather(table_dev, n, s, s, swap_rb=True, dtype=self.dtype, device=dev)
+            st = ctypes.c_void_p(_lib.stream_ptr(dev))
             verts = torch.empty(nl, _lib.SEG_POINTS, 2, dtype=torch.int32, device=dev)
             label_rows = torch.empty(nl, 6, dtype=torch.float32, device=dev)
             keep = torch.empty(nl, dtype=torch.int32, device=dev)
@@ -249,8 +125,7 @@ class DeviceSegAugmentLoader:
             masks = torch.empty(n_out, mh, mw, dtype=mdtype, device=dev)
             _lib.check(lib.y5_seg_compose(table_dev.data_ptr(), lab_p, counts.data_ptr(), plane.data_ptr(), raster.data_ptr(), n_out, mh, mw,
                                           int(self.overlap), masks.data_ptr(), _MASK_CODE[mdtype], st), "seg_compose")
-        paths = tuple(ds.im_files[p["index"]] for p in params)
-        return imgs, targets[:nt], paths, tuple(shapes), masks
+        return imgs, targets[:nt], paths, shapes, masks
 
 
 _MASK_CODE = {torch.uint8: _lib.Y5_U8, torch.int32: _lib.SEG_I32, torch.float32: _lib.Y5_F32}
@@ -265,6 +140,16 @@ def _mask_dtype(kept_per_image, overlap):
     return dt
 
 
+def _pad_polygons(polys):
+    """Non-empty int32 (k, 2) polygons -> (max(n, 1), v, 2) int32 vertices for y5_seg_raster, v the longest polygon's
+    count: shorter polygons repeat their last vertex (a zero-length edge draws nothing new)."""
+    verts = np.zeros((max(len(polys), 1), max([len(p) for p in polys], default=1), 2), np.int32)
+    for i, p in enumerate(polys):
+        verts[i, :len(p)] = p
+        verts[i, len(p):] = p[-1]
+    return verts
+
+
 def _rasterize(imgsz, polygons, downsample_ratio, device):
     """Host polygons -> (uint8 (n, h / r, w / r) masks, int32 areas, device) through y5_seg_raster."""
     h, w = int(imgsz[0]), int(imgsz[1])
@@ -273,24 +158,18 @@ def _rasterize(imgsz, polygons, downsample_ratio, device):
         raise NotImplementedError(f"y5b200: downsample_ratio {r} is not implemented (1 or 4)")
     if h % r or w % r:
         raise NotImplementedError(f"y5b200: image size {(h, w)} is not a multiple of downsample_ratio {r}")
-    # np.asarray(polygons, dtype=np.int32) as polygon2mask does; shorter polygons are padded by repeating their last
-    # vertex (a zero-length edge draws nothing new), so all share one vertex count
-    polys = [np.asarray(p, dtype=np.int32).reshape(-1, 2) for p in polygons]
+    polys = [np.asarray(p, dtype=np.int32).reshape(-1, 2) for p in polygons]  # np.asarray(polygons, dtype=np.int32) as polygon2mask does
     if any(len(p) == 0 for p in polys):
         raise ValueError("y5b200: empty polygon")
     n = len(polys)
-    nv = max([len(p) for p in polys], default=1)
-    verts = np.zeros((max(n, 1), nv, 2), np.int32)
-    for i, p in enumerate(polys):
-        verts[i, :len(p)] = p
-        verts[i, len(p):] = p[-1]
+    verts = _pad_polygons(polys)
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     v = torch.from_numpy(verts).to(dev)
     keep = torch.ones(max(n, 1), dtype=torch.int32, device=dev)
     masks = torch.zeros(max(n, 1), h // r, w // r, dtype=torch.uint8, device=dev)
     areas = torch.zeros(max(n, 1), dtype=torch.int32, device=dev)
     with _lib.on(dev):
-        _lib.check(_lib.lib().y5_seg_raster(v.data_ptr(), nv, keep.data_ptr(), n, h, w, r, masks.data_ptr(), areas.data_ptr(),
+        _lib.check(_lib.lib().y5_seg_raster(v.data_ptr(), verts.shape[1], keep.data_ptr(), n, h, w, r, masks.data_ptr(), areas.data_ptr(),
                                             ctypes.c_void_p(_lib.stream_ptr(dev))), "seg_raster")
     return masks[:n], areas, dev
 
@@ -334,15 +213,6 @@ def polygons2masks_overlap(imgsz, segments, downsample_ratio=1, device=None):
 # ----------------------------------------------------------------------------------------------------------------------
 # validation
 # ----------------------------------------------------------------------------------------------------------------------
-def _check_val_segments(ds):
-    for k, (lab, segs) in enumerate(zip(ds.labels, ds.segments)):
-        if len(lab) and len(segs) != len(lab):
-            raise NotImplementedError(f"y5b200: image {k} has {len(lab)} labels and {len(segs)} segments (one segment per label is implemented)")
-        for seg in segs:
-            if not isinstance(seg, np.ndarray) or seg.dtype != np.float32 or seg.ndim != 2 or seg.shape[1] != 2 or len(seg) < 1:
-                raise ValueError(f"y5b200: image {k}: segments must be float32 (n >= 1, 2) arrays of normalised points")
-
-
 class DeviceSegValLoader(DeviceValLoader):
     """``DeviceValLoader`` for a ``LoadImagesAndLabelsAndMasks``-like dataset (plus segments, overlap, downsample_ratio):
     yields the segmentation collate_fn's ``(imgs, targets, paths, shapes, masks)`` with ``imgs``, ``targets`` and
@@ -359,7 +229,7 @@ class DeviceSegValLoader(DeviceValLoader):
         if self.downsample_ratio not in _RATIOS:
             raise NotImplementedError(f"y5b200: downsample_ratio {self.downsample_ratio} is not implemented (1 or 4)")
         check_val_dataset(dataset, batch_size, "DeviceSegValLoader")
-        _check_val_segments(dataset)
+        _check_segments(dataset)
         super().__init__(dataset, batch_size, device=device, dtype=dtype, workers=workers, decode=decode)
 
     def collate(self, positions, loaded=None):
@@ -391,16 +261,12 @@ class DeviceSegValLoader(DeviceValLoader):
             image_rows.append(image_rows[-1] + len(lab))
         nl = image_rows[-1]
         per_image = [image_rows[b + 1] - image_rows[b] for b in range(lay.n)]
-        nv = max([len(p) for p in polys], default=1)
-        verts = np.zeros((max(nl, 1), nv, 2), np.int32)
-        for i, p in enumerate(polys):  # shorter polygons repeat their last vertex (a zero-length edge draws nothing)
-            verts[i, :len(p)] = p
-            verts[i, len(p):] = p[-1]
+        verts = _pad_polygons(polys)
         lab6 = np.concatenate(rows, 0) if rows else np.zeros((1, 6), np.float32)
         rec = np.zeros((max(nl, 1), 12), np.float32)  # y5_aug_label records: y5_seg_compose reads their image index
         rec.view(np.int32)[:nl, 9] = lab6[:nl, 0].astype(np.int32)
         table = np.zeros((lay.n, ctypes.sizeof(_lib.AugImage)), np.uint8)  # no flips
-        offs = [lay.add_block(a) for a in (verts, lab6, rec, table, np.asarray(image_rows, np.int32), np.ones(max(nl, 1), np.int32))]
+        offs = [lay.add(a) for a in (verts, lab6, rec, table, np.asarray(image_rows, np.int32), np.ones(max(nl, 1), np.int32))]
         mh, mw = H // r, W // r
         mdtype = _mask_dtype(per_image, self.overlap)
         n_out = lay.n if self.overlap else nl
@@ -416,7 +282,7 @@ class DeviceSegValLoader(DeviceValLoader):
             plane = torch.empty(max(nl, 1), dtype=torch.int32, device=dev)
             counts = torch.empty(lay.n + 1, dtype=torch.int32, device=dev)
             masks = torch.empty(n_out, mh, mw, dtype=mdtype, device=dev)
-            _lib.check(lib.y5_seg_raster(verts_p, nv, keep_p, nl, H, W, r, raster.data_ptr(), areas.data_ptr(), st), "seg_raster")
+            _lib.check(lib.y5_seg_raster(verts_p, verts.shape[1], keep_p, nl, H, W, r, raster.data_ptr(), areas.data_ptr(), st), "seg_raster")
             _lib.check(lib.y5_seg_order(image_rows_p, lay.n, keep_p, areas.data_ptr(), rows_p, int(self.overlap), targets.data_ptr(),
                                         plane.data_ptr(), counts.data_ptr(), st), "seg_order")
             _lib.check(lib.y5_seg_compose(table_p, rec_p, counts.data_ptr(), plane.data_ptr(), raster.data_ptr(), n_out, mh, mw,
