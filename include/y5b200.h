@@ -445,6 +445,20 @@ int y5_labels_native(const float* targets, int32_t nt, const float* meta, float*
 int y5_match_batch(const float* det, int64_t img_stride, int32_t row_stride, const int32_t* count, int32_t batch,
                    int32_t max_det, const float* labels, int32_t nt, const float* iouv, int32_t niou, float eps,
                    uint8_t* correct, void* stream);
+/* ConfusionMatrix.process_batch (utils/metrics.py:139-183) for every image of a batch in one launch, added into `matrix`.
+ *   det / img_stride / row_stride / count as y5_match_batch (rows [x1,y1,x2,y2,conf,cls,...] in native pixels, row_stride >= 6);
+ *   labels (nt,6) [img, cls, x1,y1,x2,y2] in target order; matrix (nc+1, nc+1) int64, row = predicted class, column = true
+ *   class, index nc = background.  Per image: detections with conf > conf_thres (fp32 compare) are kept; a (label, kept
+ *   detection) pair is a candidate when box_iou > iou_thres; each detection keeps its best candidate label (first label on
+ *   equal IoU), then each label keeps, among the detections whose best it is, the one of highest IoU (first detection on
+ *   equal IoU).  A matched label adds 1 at [det class, label class], an unmatched one at [nc, label class]; when the image has
+ *   a match, every kept detection no label kept adds 1 at [det class, nc].  An image without rows counts its labels as
+ *   background, one without labels counts nothing (val.py's per-image branching gives these same counts).  Classes are
+ *   `.int()` of the value; one outside [0, nc) writes nothing and ORs 1 (a label's) or 2 (a detection's) into `*error`
+ *   (int32, device).  Integer atomics: repeatable bit for bit.  max_det <= 4096, nc <= 32768. */
+int y5_confusion_batch(const float* det, int64_t img_stride, int32_t row_stride, const int32_t* count, int32_t batch,
+                       int32_t max_det, const float* labels, int32_t nt, int32_t nc, float conf_thres, float iou_thres, float eps,
+                       int64_t* matrix, int32_t* error, void* stream);
 
 /* Mask IoU of segment/val.py (utils/metrics.py:239-265 process_batch(masks=True); ultralytics' mask_iou) as a 1-bit GEMM.
  * Bit rows: an (h, w) mask is y5_mask_row_words(h, w) uint32 words, pixel p = y*w + x at bit p%32 of word p/32, zero bits

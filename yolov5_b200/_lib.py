@@ -232,6 +232,7 @@ SIGNATURES = {
     "y5_scale_boxes": (_I32, [_P, _I32, _I64, _P, _I32, _P, _P, _P]),
     "y5_labels_native": (_I32, [_P, _I32, _P, _P, _P]),
     "y5_match_batch": (_I32, [_P, _I64, _I32, _P, _I32, _I32, _P, _I32, _P, _I32, _F, _P, _P]),
+    "y5_confusion_batch": (_I32, [_P, _I64, _I32, _P, _I32, _I32, _P, _I32, _I32, _F, _F, _F, _P, _P, _P]),
     "y5_mask_row_words": (_I32, [_I32, _I32]),
     "y5_mask_pack": (_I32, [_P, _I32, _I32, _I32, _I32, _P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P]),
     "y5_mask_iou": (_I32, [_P, _P, _P, _I32, _P, _P, _P, _I32, _I32, _I32, _I32, _F, _P, _P]),

@@ -1,7 +1,7 @@
 """Import-path compatibility with the reference: ``install()`` registers this package's modules under the names the
 reference's scripts and pickled checkpoints use (``models.common``, ``models.yolo``, ``models.experimental``,
 ``utils.general``, ``utils.loss``, ``utils.metrics``, ``utils.torch_utils``, ``utils.augmentations``,
-``utils.segment.general``), so
+``utils.segment.general``, ``utils.segment.loss``, ``utils.segment.metrics``), so
 
     from models.yolo import DetectionModel          # reference val.py:39 / train.py:49 style imports
     torch.load("reference_checkpoint.pt")           # pickles naming models.yolo.DetectionModel, models.common.Conv ...
@@ -28,6 +28,7 @@ ALIASES = {
     "utils.segment": "yolov5_b200.utils.segment",
     "utils.segment.general": "yolov5_b200.utils.segment.general",
     "utils.segment.loss": "yolov5_b200.utils.segment.loss",
+    "utils.segment.metrics": "yolov5_b200.utils.segment.metrics",
 }
 
 

@@ -4,7 +4,7 @@
 //         (reference utils/augmentations.py:85-115, utils/dataloaders.py:354-357, detect.py:205-208)
 //   post: process_mask / crop_mask (utils/segment/general.py:10-52), scale_boxes + clip_boxes (utils/general.py:613-626),
 //         xywh2xyxy + process_batch's detection<->label matching for a whole batch (utils/metrics.py:224-265,
-//         val.py:282-318)
+//         val.py:282-318), ConfusionMatrix.process_batch's counts for a whole batch (utils/metrics.py:139-183)
 // Integer / index results (letterboxed bytes, match matrices) are bit-exact w.r.t. oracle/pre_ref.py / oracle/post_ref.py;
 // this file is compiled with -fmad=false and uses explicit _rn intrinsics wherever a rounding point matters; fmaf() is
 // used only where the reference itself is a BLAS dot product (mask logits).
@@ -471,6 +471,78 @@ __global__ void match_kernel(const float* __restrict__ det, long long img_stride
     match_assign(s_best, s_iou, n, max_det, iouv, niou, correct + static_cast<long long>(b) * max_det * niou);
 }
 
+// ConfusionMatrix.process_batch (utils/metrics.py:139-183) for one image per block, counts added into `matrix` (nc+1)^2.
+// Kept detections: conf > conf_thres.  Candidates: iou > iou_thres, any classes.  Each kept detection keeps its best label
+// (highest IoU, first label on ties), then each label keeps, among the detections whose best it is, the one with the highest
+// IoU (first detection on ties).  A class is `.int()` of its value: values outside (-1, nc) set an error bit, never a write.
+constexpr int kConfusionLabelErr = 1, kConfusionDetErr = 2;  // bits of the error word
+constexpr int kNoLabel = -1, kDropped = -2;  // s_best of a kept detection without a candidate, of a detection at or below conf_thres
+
+__device__ __forceinline__ bool confusion_class(float c, int nc) { return c > -1.0f && c < static_cast<float>(nc); }  // .int() in [0, nc)
+
+__device__ __forceinline__ void confusion_add(unsigned long long* matrix, int nc, int row, int col) {
+    atomicAdd(matrix + static_cast<long long>(row) * (nc + 1) + col, 1ull);
+}
+
+__global__ void confusion_kernel(const float* __restrict__ det, long long img_stride, int row_stride, const int32_t* __restrict__ count,
+                                 int max_det, const float* __restrict__ labels, int nt, int nc, float conf_thres, float iou_thres, float eps,
+                                 unsigned long long* __restrict__ matrix, int* __restrict__ error) {
+    __shared__ int s_best[kMatchMaxDet];
+    __shared__ float s_iou[kMatchMaxDet];
+    __shared__ uint8_t s_won[kMatchMaxDet];
+    __shared__ int s_any;
+    const int b = blockIdx.x;
+    const int n = max(0, min(count ? count[b] : max_det, max_det));
+    const float* dbase = det + static_cast<long long>(b) * img_stride;
+    if (threadIdx.x == 0) s_any = 0;
+    for (int d = threadIdx.x; d < n; d += blockDim.x) {
+        const float* dp = dbase + static_cast<long long>(d) * row_stride;
+        s_won[d] = 0;
+        if (!(dp[4] > conf_thres)) {
+            s_best[d] = kDropped;
+            continue;
+        }
+        const float db[4] = {dp[0], dp[1], dp[2], dp[3]};
+        int best = kNoLabel;
+        float best_iou = 0.0f;
+        for (int l = 0; l < nt; ++l) {
+            const float* lp = labels + static_cast<long long>(l) * 6;
+            if (static_cast<int>(lp[0]) != b) continue;
+            const float v = iou_label_det(lp + 2, db, eps);
+            if (v > iou_thres && (best == kNoLabel || v > best_iou)) { best_iou = v; best = l; }
+        }
+        s_best[d] = best;
+        s_iou[d] = best_iou;
+    }
+    __syncthreads();
+    // one count per label of this image: at [class of its winning detection, class] or, without one, at [nc, class]
+    for (int l = threadIdx.x; l < nt; l += blockDim.x) {
+        const float* lp = labels + static_cast<long long>(l) * 6;
+        if (static_cast<int>(lp[0]) != b) continue;
+        int win = -1;
+        float win_iou = 0.0f;
+        for (int d = 0; d < n; ++d)
+            if (s_best[d] == l && (win < 0 || s_iou[d] > win_iou)) { win_iou = s_iou[d]; win = d; }
+        if (win >= 0) {
+            s_won[win] = 1;
+            s_any = 1;
+        }
+        const float gc = lp[1];
+        const float dc = win >= 0 ? dbase[static_cast<long long>(win) * row_stride + 5] : 0.0f;
+        if (!confusion_class(gc, nc)) atomicOr(error, kConfusionLabelErr);
+        else if (!confusion_class(dc, nc)) atomicOr(error, kConfusionDetErr);
+        else confusion_add(matrix, nc, win >= 0 ? static_cast<int>(dc) : nc, static_cast<int>(gc));
+    }
+    __syncthreads();
+    if (!s_any) return;  // the reference counts unmatched detections only in an image with at least one match
+    for (int d = threadIdx.x; d < n; d += blockDim.x) {
+        if (s_best[d] == kDropped || s_won[d]) continue;
+        const float dc = dbase[static_cast<long long>(d) * row_stride + 5];
+        if (confusion_class(dc, nc)) confusion_add(matrix, nc, static_cast<int>(dc), nc);
+        else atomicOr(error, kConfusionDetErr);
+    }
+}
+
 static int last_status(const char* what) {
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
@@ -698,4 +770,18 @@ extern "C" Y5_API int y5_match_batch(const float* det, int64_t img_stride, int32
                                                                         correct);
     count_launch();
     return last_status("match_batch");
+}
+
+extern "C" Y5_API int y5_confusion_batch(const float* det, int64_t img_stride, int32_t row_stride, const int32_t* count, int32_t batch,
+                                         int32_t max_det, const float* labels, int32_t nt, int32_t nc, float conf_thres, float iou_thres,
+                                         float eps, int64_t* matrix, int32_t* error, void* stream) {
+    if (batch == 0) return 0;
+    if (batch < 0 || max_det < 0 || nt < 0 || nc <= 0 || row_stride < 6 || !matrix || !error || (max_det > 0 && !det) || (nt > 0 && !labels))
+        return set_error(Y5_E_INVALID, "confusion_batch: bad argument");
+    if (max_det > kMatchMaxDet) return set_error(Y5_E_UNSUPPORTED, "confusion_batch: max_det %d > %d", max_det, kMatchMaxDet);
+    if (nc > (1 << 15)) return set_error(Y5_E_UNSUPPORTED, "confusion_batch: nc %d > %d", nc, 1 << 15);
+    confusion_kernel<<<batch, 256, 0, static_cast<cudaStream_t>(stream)>>>(det, img_stride, row_stride, count, max_det, labels, nt, nc, conf_thres,
+                                                                            iou_thres, eps, reinterpret_cast<unsigned long long*>(matrix), error);
+    count_launch();
+    return last_status("confusion_batch");
 }

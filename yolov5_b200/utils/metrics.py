@@ -6,10 +6,16 @@ fp32 division is an integer pixel count, so it is bit-exact.
 
 The last step of validation, ap_per_class (utils/metrics.py:25-126, val.py:328-330), runs on the device too (y5_ap_per_class):
 one sort of the predictions, then every class and IoU threshold in float64, equal to the reference's numpy arithmetic bit for
-bit under the stable confidence order (see DESIGN.md).  ap_per_class_batch reads the padded per-batch tensors directly."""
+bit under the stable confidence order (see DESIGN.md).  ap_per_class_batch reads the padded per-batch tensors directly.
+
+ConfusionMatrix (utils/metrics.py:129-221) counts on the device (y5_confusion_batch): its updates never wait for the device,
+and reading `matrix` syncs once.  `fitness` (utils/metrics.py:19-22) is the host weighting train.py applies to the results."""
 from __future__ import annotations
 
 import ctypes as C
+import logging
+import warnings
+from pathlib import Path
 
 import numpy as np
 import torch
@@ -85,18 +91,21 @@ def labels_to_native(targets: torch.Tensor, meta: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def val_batch_metrics(rows: torch.Tensor, count: torch.Tensor, targets: torch.Tensor, im_shape, shapes, iouv: torch.Tensor):
+def val_batch_metrics(rows: torch.Tensor, count: torch.Tensor, targets: torch.Tensor, im_shape, shapes, iouv: torch.Tensor, confusion=None):
     """The metric part of val.py:282-318 for a whole batch, on the device: rows/count from nms_device (rows (B,max_det,6+nm)
     in network-input pixels), targets (nt,6) [img, cls, cx, cy, w, h] already in network-input pixels (val.py:274),
     im_shape = (height, width) of the network input, shapes[i] = ((h0, w0), ((ratio_h, ratio_w), (pad_w, pad_h))) as the
     reference dataloader yields, or the (B,5) tensor scale_meta makes of them (already on the device, the loop can then be
-    captured in a CUDA graph).  Returns (predn rows in native space, correct (B,max_det,niou) bool); nothing is synced."""
+    captured in a CUDA graph).  Returns (predn rows in native space, correct (B,max_det,niou) bool); nothing is synced.
+    `confusion`, a ConfusionMatrix, is updated from the same native rows and labels as val.py's plots=True loop updates it."""
     from .general import scale_boxes_batch
 
     meta = _meta(im_shape, shapes, rows.device)
     predn = rows.clone()
     scale_boxes_batch(predn, count, meta)
     labelsn = labels_to_native(targets, meta)
+    if confusion is not None:
+        confusion.process_batch_padded(predn, count, labelsn)
     return predn, match_batch(predn, count, labelsn, iouv)
 
 
@@ -202,7 +211,8 @@ def seg_val_batch_metrics(rows, count, protos, targets, masks, im_shape, shapes,
     process_mask_native, --retina-masks) of the network-input boxes, staged as uint8 a chunk of images at a time; gt masks of
     another size are resized as the reference does.  Returns (predn, correct_bboxes, correct_masks), both (B,max_det,niou)
     bool, padding rows False.  Nothing is synced unless `check`, which reads the non-binary counter once and raises
-    ValueError when a 0/1 gt mask held another value."""
+    ValueError when a 0/1 gt mask held another value.  segment/val.py's confusion matrix (box IoU, segment/val.py:297) is
+    ConfusionMatrix.process_batch_padded(predn, count, labels_to_native(targets, meta)) on the returned predn."""
     from .segment.general import process_mask_batch
 
     b, max_det = rows.shape[:2]
@@ -376,3 +386,157 @@ def ap_per_class_batch(correct, rows, count, target_cls, eps=1e-16, correct_mask
     res = _ap_run(dev, tps, r.data_ptr() + 16, r.data_ptr() + 20, r.stride(0), r.stride(1), max_det * niou, cnt, n_img, max_det, niou,
                   target_cls, eps)
     return res[0] if correct_masks is None else _box_and_mask(*res)
+
+
+def fitness(x):
+    """Reference utils/metrics.py:19: per row of [P, R, mAP@0.5, mAP@0.5:0.95, ...] (numpy, on the host), the model's fitness
+    0.1 * mAP@0.5 + 0.9 * mAP@0.5:0.95, summed over the four weighted columns in column order."""
+    return np.sum(np.asarray(x)[:, :4] * np.array([0.0, 0.0, 0.1, 0.9]), axis=1)
+
+
+LOGGER = logging.getLogger("yolov5_b200")
+
+
+class ConfusionMatrix:
+    """Reference utils/metrics.py:129: the detection confusion matrix of val.py's plots, rows = predicted class, columns =
+    true class, index nc = background.  The counts accumulate on the device (y5_confusion_batch, one launch per update, no
+    host sync); `matrix` folds them into a host float64 array when read (see there).  Equal IoUs are resolved in (label,
+    detection) scan order (DESIGN.md, f11); the reference's own order among them depends on numpy's sort and the host."""
+
+    def __init__(self, nc, conf=0.25, iou_thres=0.45):
+        self.nc = nc
+        self.conf = conf
+        self.iou_thres = iou_thres
+        self._matrix = np.zeros((nc + 1, nc + 1))
+        self._acc = None  # device int64: (nc+1)^2 counts not yet read, then the error word (low 32 bits of the last entry)
+
+    @property
+    def matrix(self):
+        """The (nc+1, nc+1) float64 host array.  Reading it syncs once: the device counts since the last read are added into
+        it and the device accumulator is zeroed on the current stream; the same array is returned every time, so in-place
+        edits persist and later updates add on top.  Raises ValueError when an update met a class outside [0, nc) (the
+        reference would index out of range); the counts since the last read are dropped with the error."""
+        if self._acc is not None:
+            acc = self._acc.cpu().numpy()
+            self._acc.zero_()
+            k = (self.nc + 1) ** 2
+            if acc[k]:
+                what = " and ".join(w for bit, w in ((1, "a label"), (2, "a detection")) if acc[k] & bit)
+                raise ValueError(f"y5b200: ConfusionMatrix: {what} class is outside [0, {self.nc}) (nc={self.nc}); the counts since "
+                                 "the last read are dropped")
+            self._matrix += acc[:k].reshape(self.nc + 1, self.nc + 1)
+        return self._matrix
+
+    @matrix.setter
+    def matrix(self, value):
+        """Replace the host array; device counts not yet read are dropped, as the reference drops every earlier count."""
+        if self._acc is not None:
+            self._acc.zero_()
+        self._matrix = value
+
+    def _accumulator(self, dev):
+        if self._acc is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("y5b200: ConfusionMatrix allocates its device counts on the first update; make one update "
+                                   "(or read `matrix`) before capturing a CUDA graph")
+            self._acc = torch.zeros((self.nc + 1) ** 2 + 1, dtype=torch.int64, device=dev)
+        elif self._acc.device != dev:
+            raise ValueError(f"y5b200: ConfusionMatrix counts live on {self._acc.device}, got tensors on {dev}")
+        return self._acc
+
+    def _launch(self, det, img_stride, row_stride, count, batch, max_det, labels6):
+        dev = labels6.device if det is None else det.device
+        acc = self._accumulator(dev)
+        k = (self.nc + 1) ** 2
+        with _lib.on(dev):
+            _lib.check(_lib.lib().y5_confusion_batch(det.data_ptr() if det is not None and det.numel() else None, img_stride, row_stride,
+                                                     count.data_ptr() if count is not None else None, batch, max_det,
+                                                     labels6.data_ptr() if labels6.numel() else None, labels6.shape[0], self.nc,
+                                                     float(self.conf), float(self.iou_thres), 1e-7, acc.data_ptr(), acc.data_ptr() + 8 * k,
+                                                     C.c_void_p(_lib.stream_ptr(dev))), "confusion_batch")
+
+    def process_batch(self, detections, labels):
+        """Reference signature (utils/metrics.py:139): detections (N, >=6) float32 [x1,y1,x2,y2,conf,cls,...] and labels (M,5)
+        float32 [cls,x1,y1,x2,y2] in pixels, CUDA tensors; or detections=None and labels (M,) float32 classes, all counted as
+        background.  Launches one kernel; nothing is synced.  CPU tensors raise RuntimeError, other dtypes TypeError (the
+        reference computes the IoU in the input dtype)."""
+        if detections is None:
+            cls = _cuda_f32(labels, "labels", 1)
+            labels6 = torch.zeros(cls.shape[0], 6, dtype=torch.float32, device=cls.device)
+            labels6[:, 1] = cls
+            self._launch(None, 0, 6, None, 1, 0, labels6)
+            return
+        det = _cuda_f32(detections, "detections", 2)
+        lab = _cuda_f32(labels, "labels", 2)
+        if det.shape[1] < 6 or lab.shape[1] != 5 or det.device != lab.device:
+            raise ValueError(f"y5b200: ConfusionMatrix.process_batch takes detections (N, >=6) and labels (M, 5) on one device, got "
+                             f"{tuple(det.shape)} on {det.device} and {tuple(lab.shape)} on {lab.device}")
+        if det.stride(1) != 1:
+            det = det.contiguous()
+        labels6 = torch.cat((lab.new_zeros(lab.shape[0], 1), lab), 1)
+        self._launch(det, 0, det.stride(0), None, 1, det.shape[0], labels6)
+
+    def process_batch_padded(self, rows, count, labels6):
+        """The whole batch in one launch, as val.py's per-image loop with plots=True counts it: rows (B, max_det, >=6) float32
+        in native pixels (val_batch_metrics' predn, image b's valid rows r < count[b]; seg rows of 6 + nm columns work as
+        they are), count (B,) int32 or None (all rows valid), labels6 (nt, 6) [img, cls, x1,y1,x2,y2] in native pixels
+        (labels_to_native).  An image without rows counts its labels as background (val.py's detections=None call), one
+        without labels counts nothing.  No sync and no allocation once the first update has run: capturable in a CUDA graph."""
+        rows = _cuda_f32(rows, "rows", 3)
+        if rows.shape[2] < 6 or rows.stride(2) != 1:
+            raise ValueError(f"y5b200: process_batch_padded: rows must be (B, max_det, >=6) with unit column stride, got {tuple(rows.shape)}")
+        labels6 = _cuda_f32(labels6, "labels6", 2)
+        if labels6.shape[1] != 6:
+            raise ValueError(f"y5b200: process_batch_padded: labels6 must be (nt, 6), got {tuple(labels6.shape)}")
+        labels6 = labels6.contiguous()
+        b, max_det = rows.shape[:2]
+        cnt = None
+        if count is not None:
+            if count.numel() != b:
+                raise ValueError(f"y5b200: process_batch_padded: count has {count.numel()} entries for {b} images")
+            cnt = count.to(rows.device, torch.int32).contiguous()
+        self._launch(rows, rows.stride(0), rows.stride(1), cnt, b, max_det, labels6)
+
+    def plot(self, normalize=True, save_dir="", names=()):
+        """Reference utils/metrics.py:185 on the host from `matrix`: seaborn heatmap saved as save_dir/confusion_matrix.png.
+        As the reference's TryExcept does, a failure (seaborn or matplotlib missing included) is logged, not raised."""
+        try:
+            import matplotlib.pyplot as plt
+            import seaborn as sn
+
+            m = self.matrix
+            array = m / ((m.sum(0).reshape(1, -1) + 1e-9) if normalize else 1)  # each true class (column) sums to 1
+            array[array < 0.005] = np.nan  # left blank rather than annotated 0.00
+            fig, ax = plt.subplots(1, 1, figsize=(12, 9), tight_layout=True)
+            nc, nn = self.nc, len(names)
+            sn.set(font_scale=1.0 if nc < 50 else 0.8)
+            ticklabels = [*names, "background"] if 0 < nn < 99 and nn == nc else "auto"
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")  # an all-NaN column warns
+                sn.heatmap(array, ax=ax, annot=nc < 30, annot_kws={"size": 8}, cmap="Blues", fmt=".2f", square=True, vmin=0.0,
+                           xticklabels=ticklabels, yticklabels=ticklabels).set_facecolor((1, 1, 1))
+            ax.set_xlabel("True")
+            ax.set_ylabel("Predicted")
+            ax.set_title("Confusion Matrix")
+            fig.savefig(Path(save_dir) / "confusion_matrix.png", dpi=250)
+            plt.close(fig)
+        except Exception as e:
+            LOGGER.warning(f"ConfusionMatrix plot failure: {e}")
+
+    def print(self):
+        """Reference utils/metrics.py:218: log each of the nc + 1 rows of `matrix`, values separated by spaces."""
+        m = self.matrix
+        for i in range(self.nc + 1):
+            LOGGER.info(" ".join(map(str, m[i])))
+
+
+def _cuda_f32(x, what, dim):
+    if not isinstance(x, torch.Tensor):
+        raise TypeError(f"y5b200: ConfusionMatrix takes torch tensors, got {type(x).__name__} for {what}")
+    if not x.is_cuda:
+        raise RuntimeError("y5b200: ConfusionMatrix runs on CUDA tensors only (no CPU / PyTorch fallback)")
+    if x.dtype != torch.float32:
+        raise TypeError(f"y5b200: ConfusionMatrix takes float32 {what}, got {x.dtype}")
+    if x.dim() != dim:
+        raise ValueError(f"y5b200: ConfusionMatrix: {what} must have {dim} dimension(s), got {tuple(x.shape)}")
+    return x
