@@ -308,6 +308,29 @@ int y5_bn_act_bwd(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pit
                   int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
                   const float* gamma, const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace,
                   void* stream);
+/* SyncBatchNorm (torch.nn.SyncBatchNorm in training under torch.distributed): the same passes split where the column sums
+ * of every rank must be added, with the caller's SUM all-reduce in between.  The workspace is 2 * channels + 1 doubles,
+ * ZERO on entry; slot 2 * channels is the row count.
+ * Forward:  y5_bn_stats_sync (y5_bn_stats that also adds `rows` to ws[2C]) -> all-reduce ws[0 .. 2C] -> y5_bn_act_fwd_sync
+ *           (y5_bn_act_fwd in training mode, `sums` required, dividing by the global N = sums[2C] instead of `rows`;
+ *           running_var takes the unbiased factor N / (N - 1)).
+ * Backward: y5_bn_act_bwd_reduce (the reduce pass of y5_bn_act_bwd; writes THIS rank's dgamma / dbeta and, for
+ *           Y5_ACT_SILU, leaves du in dy) -> all-reduce ws[0 .. 2C) -> y5_bn_act_bwd_apply (the apply pass with the summed
+ *           `sums` and `count` -> the forward's N, one double; dgamma / dbeta untouched).
+ * Without the all-reduce, the pairs compute exactly what y5_bn_stats + y5_bn_act_fwd and y5_bn_act_bwd compute. */
+int y5_bn_stats_sync(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace,
+                     void* stream);
+int y5_bn_act_fwd_sync(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels,
+                       int32_t dtype, float* mean, float* invstd, const float* gamma, const float* beta, int32_t act,
+                       const void* sums, float eps, float momentum, float* running_mean, float* running_var,
+                       const void* residual, int32_t res_pitch, void* stream);
+int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                         int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
+                         const float* gamma, const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace,
+                         void* stream);
+int y5_bn_act_bwd_apply(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                        int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
+                        const float* gamma, int32_t act, const void* sums, const void* count, void* stream);
 /* out[c] = sum over rows of y[row][c] (fp32) */
 int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, float* out, void* workspace,
                void* stream);

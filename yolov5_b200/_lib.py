@@ -216,6 +216,10 @@ SIGNATURES = {
     "y5_sppf_pool_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P]),
     "y5_bn_act_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _P, _P, _P]),
     "y5_col_sum": (_I32, [_P, _I32, _I64, _I32, _I32, _P, _P, _P]),
+    "y5_bn_stats_sync": (_I32, [_P, _I32, _I64, _I32, _I32, _P, _P]),
+    "y5_bn_act_fwd_sync": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _F, _F, _P, _P, _P, _I32, _P]),
+    "y5_bn_act_bwd_reduce": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _P, _P, _P]),
+    "y5_bn_act_bwd_apply": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _I32, _P, _P, _P]),
     "y5_weight_pack": (_I32, [_P, _I32, _I32, _I32, _I32, _P, _I32, _P, _I32, _I32, _P]),
     "y5_weight_pack_chunk_elems": (_I32, []),
     "y5_weight_pack_multi": (_I32, [_P, _P, _P, _I32, _I32, _P]),

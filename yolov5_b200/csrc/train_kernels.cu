@@ -119,9 +119,10 @@ __device__ __forceinline__ void block_publish(float (&acc)[NV][8], int cgx, int 
 // mode 0: sum, sum of squares;  mode 1: sum only
 template <int MODE>
 __global__ void __launch_bounds__(kRedThreads) col_stats_kernel(const void* __restrict__ y, int pitch, long long rows, int channels, int bf16,
-                                                                int cgx, int rpb, double* __restrict__ ws) {
+                                                                int cgx, int rpb, double* __restrict__ ws, double* __restrict__ count) {
     griddep_wait();  // PDL: the predecessor kernel has completed and flushed beyond this point
     griddep_launch_dependents();
+    if (count && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *count += static_cast<double>(rows);  // SyncBN: this rank's rows
     const int nrows = kRedThreads / cgx;
     const int tx = threadIdx.x % cgx, ty = threadIdx.x / cgx;
     const int cg = blockIdx.x * cgx + tx;
@@ -158,6 +159,17 @@ __global__ void __launch_bounds__(kRedThreads) col_stats_kernel(const void* __re
     }
 }
 
+// dbeta / dgamma of the reduce pass alone (SyncBN): this rank's sums, rounded as the apply pass rounds them
+__global__ void bn_affine_grad_kernel(const double* __restrict__ ws, int channels, float* __restrict__ dgamma, float* __restrict__ dbeta) {
+    griddep_wait();  // PDL: the predecessor kernel has completed and flushed beyond this point
+    griddep_launch_dependents();
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c < channels) {
+        dbeta[c] = static_cast<float>(ws[c]);
+        dgamma[c] = static_cast<float>(ws[channels + c]);
+    }
+}
+
 __global__ void col_sum_finalize_kernel(const double* __restrict__ ws, int channels, float* __restrict__ out) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c < channels) out[c] = static_cast<float>(ws[c]);
@@ -190,11 +202,17 @@ __global__ void __launch_bounds__(kRedThreads, RES ? 3 : 4) bn_act_fwd_kernel(co
                                                                     long long rows, int channels, int bf16, int act, int cgx, int rpb,
                                                                     float* __restrict__ mean, float* __restrict__ invstd,
                                                                     const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                                    const double* __restrict__ sums, double inv_rows, double unbias, float eps,
+                                                                    const double* __restrict__ sums, const double* __restrict__ count,
+                                                                    double inv_rows, double unbias, float eps,
                                                                     float momentum, float* __restrict__ running_mean,
                                                                     float* __restrict__ running_var, const void* __restrict__ res, int res_pitch) {
     griddep_wait();  // PDL: the predecessor kernel has completed and flushed beyond this point
     griddep_launch_dependents();
+    if (count) {  // SyncBN: the row count N of all ranks, summed with the column sums; the same double arithmetic as the host's
+        const double n = *count;
+        inv_rows = 1.0 / n;
+        unbias = n > 1.0 ? n / (n - 1.0) : 1.0;
+    }
     __shared__ float2 tab[kRedThreads];
     const int nrows = kRedThreads / cgx;
     const int tx = threadIdx.x % cgx, ty = threadIdx.x / cgx;
@@ -357,8 +375,8 @@ __global__ void __launch_bounds__(kRedThreads, 4) bn_act_bwd_apply_kernel(const 
                                                                           void* dy, int dy_pitch, long long rows, int channels, int bf16,
                                                                           int cgx, int rpb, const float* __restrict__ mean,
                                                                           const float* __restrict__ invstd, const float* __restrict__ gamma,
-                                                                          const double* __restrict__ ws, float* __restrict__ dgamma,
-                                                                          float* __restrict__ dbeta) {
+                                                                          const double* __restrict__ ws, const double* __restrict__ count,
+                                                                          float* __restrict__ dgamma, float* __restrict__ dbeta) {
     // dy = du*a + y*c1 + c0 (see the table above).  du = dz * act'(t) comes from the reduce pass (stored in the dy buffer itself
     // for SiLU layers -- each thread reads its 16 bytes before it overwrites them -- or is dz for linear layers): no
     // transcendental work is left here, the pass is a pure 2-read 1-write stream.
@@ -369,14 +387,15 @@ __global__ void __launch_bounds__(kRedThreads, 4) bn_act_bwd_apply_kernel(const 
     const int nrows = kRedThreads / cgx;
     const int tx = threadIdx.x % cgx, ty = threadIdx.x / cgx;
     const int cg = blockIdx.x * cgx + tx;
-    const float inv_rows = 1.0f / static_cast<float>(rows);
+    // count != NULL (SyncBN): ws holds the sums of all ranks and *count their row count N
+    const float inv_rows = 1.0f / (count ? static_cast<float>(*count) : static_cast<float>(rows));
     for (int i = threadIdx.x; i < cgx * 8; i += kRedThreads) {
         const int c = blockIdx.x * cgx * 8 + i;
         float2 ac = make_float2(0.f, 0.f);
         float d = 0.f;
         if (c < channels) {
             const float db = static_cast<float>(ws[c]), dg = static_cast<float>(ws[channels + c]);
-            if (blockIdx.y == 0) {
+            if (blockIdx.y == 0 && dgamma) {
                 dbeta[c] = db;
                 dgamma[c] = dg;
             }
@@ -644,15 +663,96 @@ using namespace y5;
 
 extern "C" Y5_API int64_t y5_bn_workspace_bytes(int32_t channels) { return static_cast<int64_t>(channels) * 2 * sizeof(double); }
 
-extern "C" Y5_API int y5_bn_stats(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace, void* stream) {
-    if (int e = check_view(y, pitch, channels, "bn_stats")) return e;
-    if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "bn_stats: dtype must be fp16 or bf16");
-    if (!workspace || rows <= 0) return set_error(Y5_E_INVALID, "bn_stats: bad argument");
+// check_view with the operand named after the entry point ("bn_act_fwd y")
+static int check_operand(const char* what, const char* operand, const void* p, int pitch, int channels) {
+    char name[64];
+    snprintf(name, sizeof(name), "%s %s", what, operand);
+    return check_view(p, pitch, channels, name);
+}
+
+// The BatchNorm entry points and their SyncBatchNorm splits share these launches.  `count` (SyncBN) is the fp64 slot after
+// the 2*channels column sums: bn_stats adds this rank's rows to it, and after the caller's SUM all-reduce of the whole
+// workspace it holds N, which the forward and the apply pass divide by instead of the host's `rows`.
+static int bn_stats_launch(const char* what, const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace,
+                           bool sync, void* stream) {
+    if (int e = check_view(y, pitch, channels, what)) return e;
+    if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "%s: dtype must be fp16 or bf16", what);
+    if (!workspace || rows <= 0) return set_error(Y5_E_INVALID, "%s: bad argument", what);
+    double* ws = static_cast<double*>(workspace);
     const RowGeom g = row_geom(channels, rows, true);
     count_launch();
     launch_pdl(col_stats_kernel<0>, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream), 
-        y, pitch, rows, channels, dtype == Y5_BF16, g.cgx, g.rpb, static_cast<double*>(workspace));
-    return launch_status("bn_stats");
+        y, pitch, rows, channels, dtype == Y5_BF16, g.cgx, g.rpb, ws, sync ? ws + 2 * static_cast<int64_t>(channels) : static_cast<double*>(nullptr));
+    return launch_status(what);
+}
+
+static int bn_act_fwd_launch(const char* what, const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
+                             float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, const void* sums, bool sync,
+                             float eps, float momentum, float* running_mean, float* running_var, const void* residual, int32_t res_pitch,
+                             void* stream) {
+    if (int e = check_operand(what, "y", y, y_pitch, channels)) return e;
+    if (int e = check_operand(what, "z", z, z_pitch, channels)) return e;
+    if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "%s: dtype must be fp16 or bf16", what);
+    if (!mean || !invstd || !gamma || !beta || rows <= 0 || (sync && !sums)) return set_error(Y5_E_INVALID, "%s: bad argument", what);
+    if (residual)
+        if (int e = check_operand(what, "residual", residual, res_pitch, channels)) return e;
+    const RowGeom g = row_geom(channels, rows, false, residual ? 3 : 4);
+    const double inv_rows = 1.0 / static_cast<double>(rows);
+    const double unbias = rows > 1 ? static_cast<double>(rows) / static_cast<double>(rows - 1) : 1.0;
+    const double* s = static_cast<const double*>(sums);
+    count_launch();
+    launch_pdl(residual ? bn_act_fwd_kernel<true> : bn_act_fwd_kernel<false>, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream), 
+        y, y_pitch, z, z_pitch, rows, channels, dtype == Y5_BF16, act, g.cgx, g.rpb, mean, invstd, gamma, beta, s,
+        sync ? s + 2 * static_cast<int64_t>(channels) : static_cast<const double*>(nullptr), inv_rows, unbias, eps, momentum,
+        running_mean, running_var, residual, res_pitch);
+    return launch_status(what);
+}
+
+static int bn_bwd_check(const char* what, const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
+                        int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, const void* workspace) {
+    if (int e = check_operand(what, "y", y, y_pitch, channels)) return e;
+    if (int e = check_operand(what, "dz", dz, dz_pitch, channels)) return e;
+    if (int e = check_operand(what, "dy", dy, dy_pitch, channels)) return e;
+    if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "%s: dtype must be fp16 or bf16", what);
+    if (!mean || !invstd || !gamma || !workspace || rows <= 0) return set_error(Y5_E_INVALID, "%s: bad argument", what);
+    return 0;
+}
+
+// reduce pass: du = dz * act'(t) and its two column sums into the workspace.  SiLU layers: du is left in the dy buffer and the
+// apply pass finishes it in place; linear layers have du == dz
+static void bn_bwd_reduce_launch(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
+                                 int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                                 int32_t act, void* workspace, cudaStream_t st) {
+    static const int red_u = env_int("Y5_BN_RED_U", 4);
+    const RowGeom g = row_geom(channels, rows, true, red_u == 2 ? 3 : 2);
+    using RedFn = void (*)(const void*, int, const void*, int, long long, int, int, int, const float*, const float*, const float*, const float*,
+                           double*, void*, int);
+    static const RedFn table[2][2][2] = {
+        {{bn_act_bwd_reduce_kernel<4, false, false>, bn_act_bwd_reduce_kernel<4, false, true>},
+         {bn_act_bwd_reduce_kernel<4, true, false>, bn_act_bwd_reduce_kernel<4, true, true>}},
+        {{bn_act_bwd_reduce_kernel<2, false, false>, bn_act_bwd_reduce_kernel<2, false, true>},
+         {bn_act_bwd_reduce_kernel<2, true, false>, bn_act_bwd_reduce_kernel<2, true, true>}}};
+    launch_pdl(table[red_u == 2 ? 1 : 0][dtype == Y5_BF16 ? 1 : 0][act ? 1 : 0], row_grid(g, channels, rows), dim3(kRedThreads), 0, st, y, y_pitch, dz,
+               dz_pitch, rows, channels, g.cgx, g.rpb, mean, invstd, gamma, beta, static_cast<double*>(workspace),
+               act ? dy : static_cast<void*>(nullptr), dy_pitch);
+}
+
+// apply pass: dy from du and the column sums (count == NULL: divided by this call's rows); dgamma / dbeta written when non-NULL
+static void bn_bwd_apply_launch(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
+                                int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, int32_t act,
+                                const double* sums, const double* count, float* dgamma, float* dbeta, cudaStream_t st) {
+    const RowGeom ga = row_geom(channels, rows, false, 4);
+    launch_pdl(bn_act_bwd_apply_kernel, row_grid(ga, channels, rows), dim3(kRedThreads), 0, st, y, y_pitch, act ? static_cast<const void*>(dy) : dz,
+               act ? dy_pitch : dz_pitch, dy, dy_pitch, rows, channels, dtype == Y5_BF16, ga.cgx, ga.rpb, mean, invstd, gamma, sums, count, dgamma,
+               dbeta);
+}
+
+extern "C" Y5_API int y5_bn_stats(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace, void* stream) {
+    return bn_stats_launch("bn_stats", y, pitch, rows, channels, dtype, workspace, false, stream);
+}
+
+extern "C" Y5_API int y5_bn_stats_sync(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace, void* stream) {
+    return bn_stats_launch("bn_stats_sync", y, pitch, rows, channels, dtype, workspace, true, stream);
 }
 
 extern "C" Y5_API int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, float* out, void* workspace,
@@ -665,7 +765,7 @@ extern "C" Y5_API int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int
     const RowGeom g = row_geom(channels, rows, true);
     count_launch(2);
     launch_pdl(col_stats_kernel<1>, row_grid(g, channels, rows), dim3(kRedThreads), 0, st, y, pitch, rows, channels, dtype == Y5_BF16, g.cgx, g.rpb,
-                                                                              static_cast<double*>(workspace));
+                                                                              static_cast<double*>(workspace), static_cast<double*>(nullptr));
     col_sum_finalize_kernel<<<(channels + 127) / 128, 128, 0, st>>>(static_cast<const double*>(workspace), channels, out);
     return launch_status("col_sum");
 }
@@ -674,55 +774,55 @@ extern "C" Y5_API int y5_bn_act_fwd(const void* y, int32_t y_pitch, void* z, int
                                     float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, const void* sums,
                                     float eps, float momentum, float* running_mean, float* running_var, const void* residual,
                                     int32_t res_pitch, void* stream) {
-    if (int e = check_view(y, y_pitch, channels, "bn_act_fwd y")) return e;
-    if (int e = check_view(z, z_pitch, channels, "bn_act_fwd z")) return e;
-    if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "bn_act_fwd: dtype must be fp16 or bf16");
-    if (!mean || !invstd || !gamma || !beta || rows <= 0) return set_error(Y5_E_INVALID, "bn_act_fwd: bad argument");
-    if (residual)
-        if (int e = check_view(residual, res_pitch, channels, "bn_act_fwd residual")) return e;
-    const RowGeom g = row_geom(channels, rows, false, residual ? 3 : 4);
-    const double inv_rows = 1.0 / static_cast<double>(rows);
-    const double unbias = rows > 1 ? static_cast<double>(rows) / static_cast<double>(rows - 1) : 1.0;
-    count_launch();
-    launch_pdl(residual ? bn_act_fwd_kernel<true> : bn_act_fwd_kernel<false>, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream), 
-        y, y_pitch, z, z_pitch, rows, channels, dtype == Y5_BF16, act, g.cgx, g.rpb, mean, invstd, gamma, beta, static_cast<const double*>(sums), inv_rows, unbias, eps, momentum,
-        running_mean, running_var, residual, res_pitch);
-    return launch_status("bn_act_fwd");
+    return bn_act_fwd_launch("bn_act_fwd", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, sums, false, eps, momentum,
+                             running_mean, running_var, residual, res_pitch, stream);
+}
+
+extern "C" Y5_API int y5_bn_act_fwd_sync(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
+                                         float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, const void* sums,
+                                         float eps, float momentum, float* running_mean, float* running_var, const void* residual,
+                                         int32_t res_pitch, void* stream) {
+    return bn_act_fwd_launch("bn_act_fwd_sync", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, sums, true, eps,
+                             momentum, running_mean, running_var, residual, res_pitch, stream);
 }
 
 extern "C" Y5_API int y5_bn_act_bwd(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
                                     int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
                                     const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace, void* stream) {
-    if (int e = check_view(y, y_pitch, channels, "bn_act_bwd y")) return e;
-    if (int e = check_view(dz, dz_pitch, channels, "bn_act_bwd dz")) return e;
-    if (int e = check_view(dy, dy_pitch, channels, "bn_act_bwd dy")) return e;
-    if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "bn_act_bwd: dtype must be fp16 or bf16");
-    if (!mean || !invstd || !gamma || !beta || !dgamma || !dbeta || !workspace || rows <= 0)
-        return set_error(Y5_E_INVALID, "bn_act_bwd: bad argument");
+    if (int e = bn_bwd_check("bn_act_bwd", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace)) return e;
+    if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "bn_act_bwd: bad argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    static const int red_u = env_int("Y5_BN_RED_U", 4);
-    const RowGeom g = row_geom(channels, rows, true, red_u == 2 ? 3 : 2), ga = row_geom(channels, rows, false, 4);
-    const dim3 grid = row_grid(g, channels, rows);
     count_launch(2);
-    // SiLU layers: the reduce pass leaves du = dz * silu'(t) in the dy buffer and the apply pass finishes it in place; linear
-    // layers have du == dz
-    {
-        using RedFn = void (*)(const void*, int, const void*, int, long long, int, int, int, const float*, const float*, const float*, const float*,
-                               double*, void*, int);
-        static const RedFn table[2][2][2] = {
-            {{bn_act_bwd_reduce_kernel<4, false, false>, bn_act_bwd_reduce_kernel<4, false, true>},
-             {bn_act_bwd_reduce_kernel<4, true, false>, bn_act_bwd_reduce_kernel<4, true, true>}},
-            {{bn_act_bwd_reduce_kernel<2, false, false>, bn_act_bwd_reduce_kernel<2, false, true>},
-             {bn_act_bwd_reduce_kernel<2, true, false>, bn_act_bwd_reduce_kernel<2, true, true>}}};
-        // SiLU layers: the reduce pass leaves du = dz * silu'(t) in the dy buffer and the apply pass finishes it in place; linear
-        // layers have du == dz
-        launch_pdl(table[red_u == 2 ? 1 : 0][dtype == Y5_BF16 ? 1 : 0][act ? 1 : 0], grid, dim3(kRedThreads), 0, st, y, y_pitch, dz, dz_pitch, rows,
-                   channels, g.cgx, g.rpb, mean, invstd, gamma, beta, static_cast<double*>(workspace), act ? dy : static_cast<void*>(nullptr), dy_pitch);
-    }
-    launch_pdl(bn_act_bwd_apply_kernel, row_grid(ga, channels, rows), dim3(kRedThreads), 0, st, y, y_pitch, act ? static_cast<const void*>(dy) : dz,
-               act ? dy_pitch : dz_pitch, dy, dy_pitch, rows, channels, dtype == Y5_BF16, ga.cgx, ga.rpb, mean, invstd, gamma,
-               static_cast<const double*>(workspace), dgamma, dbeta);
+    bn_bwd_reduce_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, workspace, st);
+    bn_bwd_apply_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, act, static_cast<const double*>(workspace),
+                        nullptr, dgamma, dbeta, st);
     return launch_status("bn_act_bwd");
+}
+
+extern "C" Y5_API int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                                           int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
+                                           const float* gamma, const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace,
+                                           void* stream) {
+    if (int e = bn_bwd_check("bn_act_bwd_reduce", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace))
+        return e;
+    if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "bn_act_bwd_reduce: bad argument");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    count_launch(2);
+    bn_bwd_reduce_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, workspace, st);
+    launch_pdl(bn_affine_grad_kernel, dim3((channels + 127) / 128), dim3(128), 0, st, static_cast<const double*>(workspace), static_cast<int>(channels),
+               dgamma, dbeta);
+    return launch_status("bn_act_bwd_reduce");
+}
+
+extern "C" Y5_API int y5_bn_act_bwd_apply(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                                          int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
+                                          const float* gamma, int32_t act, const void* sums, const void* count, void* stream) {
+    if (int e = bn_bwd_check("bn_act_bwd_apply", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, sums)) return e;
+    if (!count) return set_error(Y5_E_INVALID, "bn_act_bwd_apply: bad argument");
+    count_launch();
+    bn_bwd_apply_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, act, static_cast<const double*>(sums),
+                        static_cast<const double*>(count), nullptr, nullptr, static_cast<cudaStream_t>(stream));
+    return launch_status("bn_act_bwd_apply");
 }
 
 extern "C" Y5_API int y5_zero_stuff2x(const void* x, int32_t x_pitch, void* y, int32_t y_pitch, int32_t batch, int32_t h, int32_t w, int32_t c,

@@ -8,7 +8,8 @@ What runs where
   * every convolution (forward, data gradient, weight gradient), BatchNorm batch statistics / normalise / backward and
     SiLU forward / backward: liby5b200 kernels (wgmma implicit GEMMs + HBM-bound passes), wrapped in
     torch.autograd.Function so gradients land in the ordinary ``.grad`` of the nn.Parameters (DDP's bucketed NCCL
-    all-reduce -- smart_DDP -- works unchanged);
+    all-reduce -- smart_DDP -- works unchanged); a torch.nn.SyncBatchNorm that syncs (bn_sync_group) all-reduces its column
+    sums between the split BN passes (train.py --sync-bn);
   * the glue between convolutions is liby5b200 too: channel concat = strided slice copies whose backward is a set of
     views, 2x nearest upsample and its 2x2-sum backward, SPPF's pooling chain and its arg-max backward, the Bottleneck
     shortcut as a residual operand of cv2's normalise+activate pass.  What is left to torch autograd is bookkeeping: the
@@ -473,7 +474,7 @@ class _ConvBnAct(torch.autograd.Function):
     """z = act(BN(conv(x, w)))  with batch statistics (training) or running statistics (eval inside a training graph)."""
 
     @staticmethod
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, residual, k, s, p, act, eps, momentum, training, stem):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, residual, k, s, p, act, eps, momentum, training, stem, pg=None):
         lib = _lib.lib()
         dev = x.device
         if stem:  # x is already the 16-channel space-to-depth image; weight is the (O,3,6,6) stem filter
@@ -509,14 +510,22 @@ class _ConvBnAct(torch.autograd.Function):
         b, c, ho, wo = y.shape
         rows = b * ho * wo
         code = _lib.dtype_code(y.dtype)
+        fwd_fn, n_rows = lib.y5_bn_act_fwd, None
         if training:
             mean = torch.empty(c, dtype=torch.float32, device=dev)
             invstd = torch.empty(c, dtype=torch.float32, device=dev)
-            ws = _bn_ws(c, dev)
             # the kernel updates fp32 running statistics in place; a model cast to fp16/bf16 goes through fp32 copies
             rm = running_mean if running_mean is None or running_mean.dtype == torch.float32 else running_mean.float()
             rv = running_var if running_var is None or running_var.dtype == torch.float32 else running_var.float()
-            _lib.check(lib.y5_bn_stats(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats")
+            if pg is None:
+                ws = _bn_ws(c, dev)
+                _lib.check(lib.y5_bn_stats(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats")
+            else:  # SyncBatchNorm: [column sums | row count] of every rank in one all-reduce, then the statistics of all rows
+                ws = _arena.take(2 * c + 1, dev)
+                _lib.check(lib.y5_bn_stats_sync(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats_sync")
+                _all_reduce(ws[: 2 * c + 1], pg)
+                n_rows = ws[2 * c : 2 * c + 1].clone()  # N for the backward: the arena is cleared by the next forward
+                fwd_fn = lib.y5_bn_act_fwd_sync
             sums = ws.data_ptr()
         else:
             mean = running_mean.float().contiguous()
@@ -525,10 +534,10 @@ class _ConvBnAct(torch.autograd.Function):
         g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
         z = torch.empty_like(y)
         res, resp = (None, 0) if residual is None else _nhwc(residual)
-        _lib.check(lib.y5_bn_act_fwd(y.data_ptr(), c, z.data_ptr(), c, rows, c, code, mean.data_ptr(), invstd.data_ptr(), g32.data_ptr(),
-                                     b32.data_ptr(), 1 if act else 0, sums, eps, momentum, rm.data_ptr() if rm is not None else None,
-                                     rv.data_ptr() if rv is not None else None, res.data_ptr() if res is not None else None, resp,
-                                     _st(dev)), "bn_act_fwd")
+        _lib.check(fwd_fn(y.data_ptr(), c, z.data_ptr(), c, rows, c, code, mean.data_ptr(), invstd.data_ptr(), g32.data_ptr(),
+                          b32.data_ptr(), 1 if act else 0, sums, eps, momentum, rm.data_ptr() if rm is not None else None,
+                          rv.data_ptr() if rv is not None else None, res.data_ptr() if res is not None else None, resp,
+                          _st(dev)), "bn_act_fwd")
         if training:
             if rm is not running_mean:
                 running_mean.copy_(rm)
@@ -539,6 +548,7 @@ class _ConvBnAct(torch.autograd.Function):
         ctx.bk_d = bk_d
         ctx.wide = wide
         ctx.pdtypes = (gamma.dtype, beta.dtype)
+        ctx.pg, ctx.n_rows = pg, n_rows
         return z
 
     @staticmethod
@@ -558,9 +568,18 @@ class _ConvBnAct(torch.autograd.Function):
         dgamma = torch.empty(c, dtype=torch.float32, device=dev)
         dbeta = torch.empty(c, dtype=torch.float32, device=dev)
         ws = _bn_ws(c, dev)
-        _lib.check(lib.y5_bn_act_bwd(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(), invstd.data_ptr(),
-                                     g32.data_ptr(), b32.data_ptr(), 1 if act else 0, dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(),
-                                     _st(dev)), "bn_act_bwd")
+        if ctx.pg is None:
+            _lib.check(lib.y5_bn_act_bwd(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(), invstd.data_ptr(),
+                                         g32.data_ptr(), b32.data_ptr(), 1 if act else 0, dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(),
+                                         _st(dev)), "bn_act_bwd")
+        else:  # SyncBatchNorm: dgamma / dbeta stay this rank's sums (DDP averages them); dy uses the sums of every rank over N
+            _lib.check(lib.y5_bn_act_bwd_reduce(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                                invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), 1 if act else 0, dgamma.data_ptr(),
+                                                dbeta.data_ptr(), ws.data_ptr(), _st(dev)), "bn_act_bwd_reduce")
+            _all_reduce(ws[: 2 * c], ctx.pg)
+            _lib.check(lib.y5_bn_act_bwd_apply(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                               invstd.data_ptr(), g32.data_ptr(), 1 if act else 0, ws.data_ptr(), ctx.n_rows.data_ptr(),
+                                               _st(dev)), "bn_act_bwd_apply")
         def wgrad():
             g = stem_wgrad_wide(x, dy) if ctx.wide else conv_wgrad(x, dy, ke, se, pe)
             if stem:  # (O,16,3,3) gradient of the space-to-depth filter -> (O,3,6,6)
@@ -577,7 +596,7 @@ class _ConvBnAct(torch.autograd.Function):
             dx = conv_dgrad(dy, None, k, s, p, (x.shape[2], x.shape[3]), wp_dgrad=wp_dg, cin=x.shape[1], block_k=ctx.bk_d)
         dres = dz_in if ctx.needs_input_grad[6] else None  # z = residual + act(bn(y)): the shortcut's gradient is dz itself
         return (dx, dw, dgamma.to(ctx.pdtypes[0]), dbeta.to(ctx.pdtypes[1]), None, None, dres, None, None, None, None, None,
-                None, None, None)
+                None, None, None, None)
 
 
 class _ConvBias(torch.autograd.Function):
@@ -631,6 +650,32 @@ def train_dtype(model) -> torch.dtype:
     return dt
 
 
+def _all_reduce(t: torch.Tensor, pg) -> None:
+    """SUM all-reduce of a slice of BN sums, ordered on the calling stream like the kernels around it"""
+    import torch.distributed as dist
+
+    dist.all_reduce(t, group=pg)
+
+
+def bn_process_group(bn):
+    """The group a torch.nn.SyncBatchNorm reduces over in training -- `bn.process_group` or WORLD -- when torch.distributed is
+    initialised and that group has more than one rank; else None (plain BatchNorm2d, and every other BatchNorm, never syncs)."""
+    if not isinstance(bn, torch.nn.SyncBatchNorm):
+        return None
+    import torch.distributed as dist
+
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    pg = bn.process_group or dist.group.WORLD
+    return pg if dist.get_world_size(pg) > 1 else None
+
+
+def bn_sync_group(bn):
+    """torch.nn.SyncBatchNorm's rule for when it syncs: in training mode, with bn_process_group(bn) set.  Otherwise the layer
+    is plain batch norm and takes the BatchNorm2d path, launch for launch."""
+    return bn_process_group(bn) if bn.training else None
+
+
 def conv_module(m, x, stem: int = 0, residual=None):  # stem: 0 no, 1 space-to-depth 3x3x16, 2 wide-pixel 3x1x48
     bn = getattr(m, "bn", None)
     if bn is None:
@@ -648,7 +693,7 @@ def conv_module(m, x, stem: int = 0, residual=None):  # stem: 0 no, 1 space-to-d
         bn.num_batches_tracked += 1
     mom = bn.momentum if bn.momentum is not None else 0.1
     return _ConvBnAct.apply(x, m.conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, residual, k, s, p, act, float(bn.eps),
-                            float(mom), training, stem)
+                            float(mom), training, stem, bn_sync_group(bn))
 
 
 class _Upsample2x(torch.autograd.Function):

@@ -203,8 +203,9 @@ class _FusedOptimizer(torch.optim.Optimizer):
         contiguous fp32 arena (y5_grad_pack, one launch), all-reduces the arena with ONE NCCL call (average over ranks, like
         DDP) and updates from the averaged arena.  No autograd hooks, buckets or copy-backs, and nothing but the all-reduce
         itself touches the link.  `model` must be the plain module (not wrapped in DistributedDataParallel); gradient
-        accumulation needs no `no_sync()`: ranks only talk inside `fused_step`.  BatchNorm statistics stay per rank (the
-        reference does not use SyncBatchNorm unless asked)."""
+        accumulation needs no `no_sync()`: ranks only talk inside `fused_step`.  BatchNorm statistics stay per rank unless the
+        model was converted with torch.nn.SyncBatchNorm.convert_sync_batchnorm (train.py --sync-bn): those layers all-reduce
+        their batch statistics and BN gradients over their process group inside the forward and backward."""
         import torch.distributed as dist
 
         name = type(self).__name__
@@ -508,11 +509,12 @@ def smart_optimizer(model, name="Adam", lr=0.001, momentum=0.9, decay=1e-5):
     if name not in ("SGD", "Adam", "AdamW"):
         raise NotImplementedError(f"y5b200: optimizer {name} is outside the hot path (train.py offers SGD, Adam and AdamW)")
     g = [], [], []
+    bn = tuple(v for k, v in nn.__dict__.items() if "Norm" in k)  # every torch.nn normalisation layer, SyncBatchNorm included
     for v in model.modules():
         for p_name, p in v.named_parameters(recurse=False):
             if p_name == "bias":
                 g[2].append(p)
-            elif p_name == "weight" and isinstance(v, (nn.BatchNorm1d, nn.BatchNorm2d, nn.BatchNorm3d, nn.LayerNorm, nn.GroupNorm)):
+            elif p_name == "weight" and isinstance(v, bn):
                 g[1].append(p)
             else:
                 g[0].append(p)
@@ -570,6 +572,12 @@ class GraphedTrainStep:
         world = optimizer._dp[1] if optimizer._dp is not None else 1
 
         from .. import train_ops
+
+        syncing = [n for n, m in model.named_modules() if train_ops.bn_process_group(m) is not None]
+        if syncing:
+            raise NotImplementedError(f"GraphedTrainStep: {len(syncing)} SyncBatchNorm layers (first: {syncing[0]}) all-reduce their batch "
+                                      "statistics inside the forward and backward, which this step does not capture; train such a model "
+                                      "with the eager step, or convert it back to BatchNorm2d")
 
         def step():
             with torch.autocast("cuda", dtype=amp_dtype):
