@@ -155,11 +155,14 @@ void y5_detect_plan_destroy(y5_detect_plan* plan);
  * models/yolov5s.yaml:20 becomes a 3x3/s1/p1 conv over 16 channels.  Replaces the `im.half(); im /= 255` of
  * detect.py:206-208 / val.py:259-262 plus the layout change.  h, w even.  `out_row_px` (0 = w/2) is the number of
  * 16-channel cells per output row of the buffer and `out_x_off` the cell where each row starts: the engine keeps one
- * zero cell left and right of every row so the stem conv can read 3 neighbouring cells as one 48-channel pixel. */
+ * zero cell left and right of every row so the stem conv can read 3 neighbouring cells as one 48-channel pixel.
+ * `out` must be 16-byte aligned (Y5_E_INVALID otherwise). */
 int y5_stem_s2d(const void* img, int32_t img_dtype, void* out, int32_t out_dtype, int32_t batch, int32_t h, int32_t w,
                 int32_t out_row_px, int32_t out_x_off, void* stream);
 /* SPPF pooling (models/common.py:338-340): reads view x (c channels), writes maxpool5, maxpool5^2 (=9x9),
- * maxpool5^3 (=13x13) into three views (usually channel slices 1..3 of the buffer whose slice 0 is x). */
+ * maxpool5^3 (=13x13) into three views (usually channel slices 1..3 of the buffer whose slice 0 is x).  A NaN in a
+ * window makes its maximum NaN, as F.max_pool2d does.  y5_sppf_pool, y5_upsample2x and y5_copy_view move 16-byte
+ * vectors: every view must be 16-byte aligned with pitch >= c (Y5_E_INVALID otherwise), c and pitches multiples of 8. */
 int y5_sppf_pool(const void* x, int32_t x_pitch, void* y1, void* y2, void* y3, int32_t y_pitch, int32_t batch, int32_t h,
                  int32_t w, int32_t c, int32_t ksize, int32_t dtype, void* stream);
 /* nn.Upsample(scale_factor=2, mode='nearest') written straight into a (concat) view. */

@@ -45,20 +45,21 @@ def test_single_layers_vs_oracle(cuda, dtype):
     torch.manual_seed(0)
     tol = 3e-3 if dtype == torch.float16 else 2.5e-2
     x = torch.rand(2, 64, 20, 20) * 2 - 1
-    xq = x.to(dtype).float()
+    x60 = torch.rand(2, 64, 60, 60) * 2 - 1  # 3600 pixels per plane: SPPF's direct pooling kernel
     cases = [
-        (Conv(64, 128, 3, 2), lambda sd, t: model_ref.conv_block(sd, "model.0", t, 3, 2)),
-        (Bottleneck(64, 64, True, e=1.0), lambda sd, t: model_ref.bottleneck(sd, "model.0", t, True, False)),
-        (C3(64, 64, 2), lambda sd, t: model_ref.c3(sd, "model.0", t, 2, True, False)),
-        (C3(64, 128, 1, False), lambda sd, t: model_ref.c3(sd, "model.0", t, 1, False, False)),
-        (SPPF(64, 64, 5), lambda sd, t: model_ref.sppf(sd, "model.0", t, 5, False)),
+        (Conv(64, 128, 3, 2), lambda sd, t: model_ref.conv_block(sd, "model.0", t, 3, 2), x),
+        (Bottleneck(64, 64, True, e=1.0), lambda sd, t: model_ref.bottleneck(sd, "model.0", t, True, False), x),
+        (C3(64, 64, 2), lambda sd, t: model_ref.c3(sd, "model.0", t, 2, True, False), x),
+        (C3(64, 128, 1, False), lambda sd, t: model_ref.c3(sd, "model.0", t, 1, False, False), x),
+        (SPPF(64, 64, 5), lambda sd, t: model_ref.sppf(sd, "model.0", t, 5, False), x),
+        (SPPF(64, 64, 5), lambda sd, t: model_ref.sppf(sd, "model.0", t, 5, False), x60),
     ]
-    for i, (layer, ref_fn) in enumerate(cases):
+    for i, (layer, ref_fn, xi) in enumerate(cases):
         _randomize_bn(layer, i)
         layer.eval()
         with torch.no_grad():
-            ref = ref_fn(_sd_of(layer), xq)
-        got = layer.to(cuda, dtype)(x.to(cuda, dtype)).float().cpu()
+            ref = ref_fn(_sd_of(layer), xi.to(dtype).float())
+        got = layer.to(cuda, dtype)(xi.to(cuda, dtype)).float().cpu()
         err = float((got - ref).abs().max() / ref.abs().max())
         assert got.shape == ref.shape and err < tol, (type(layer).__name__, err)
 

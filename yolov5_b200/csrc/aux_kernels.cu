@@ -1,7 +1,8 @@
 // HBM-bound data-movement kernels of the forward path: stem space-to-depth (+ u8 -> fp16 /255), SPPF pooling,
 // 2x nearest upsample into a concat slice, strided view copy, NHWC -> NCHW export.
 // All of them move 16-byte vectors (8 fp16/bf16 channels) per thread with the channel index fastest, so a warp
-// touches 512 contiguous bytes.  max() on fp16/bf16 bit patterns is done in fp32 (exact).
+// touches 512 contiguous bytes.  max() on fp16/bf16 bit patterns is done in fp32 (exact).  SPPF's max propagates NaN the way
+// F.max_pool2d does: a NaN anywhere in a window makes that window's maximum NaN.
 #include "../../include/y5b200.h"
 #include "common.cuh"
 #include "host_util.h"
@@ -54,13 +55,15 @@ __global__ void stem_s2d_kernel(const T* __restrict__ img, uint4* __restrict__ o
 // Chained stride-1 max pools compose: y2 is the (2k-1)-window max, y3 the (3k-2)-window max of x, so all three
 // come from one pass over the 13x13 neighbourhood (k=5).  One thread per (pixel, 8-channel vector).
 // ---------------------------------------------------------------------------------------------------------------------
+// max that keeps NaN (fmaxf returns the other operand): once acc is NaN, 'v > acc' is false and acc stays NaN
+__device__ __forceinline__ float max_nan(float acc, float v) { return (v > acc || v != v) ? v : acc; }
 __device__ __forceinline__ void vmax8(float (&acc)[8], const uint4& v, bool bf16) {
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const float2 t = unpack2(w[j], bf16);
-        acc[2 * j] = fmaxf(acc[2 * j], t.x);
-        acc[2 * j + 1] = fmaxf(acc[2 * j + 1], t.y);
+        acc[2 * j] = max_nan(acc[2 * j], t.x);
+        acc[2 * j + 1] = max_nan(acc[2 * j + 1], t.y);
     }
 }
 __device__ __forceinline__ uint4 pack8(const float (&f)[8], bool bf16) {
@@ -110,17 +113,17 @@ __global__ void sppf_pool_kernel(const uint16_t* __restrict__ x, int x_pitch, ui
 // Shared-memory version: one CTA per (image, 8-channel vector).  The H x W plane of that vector sits in smem
 // (uint4 per pixel) and each k x k / stride-1 max-pool is done separably (row max then column max), three times in a
 // row exactly as the reference chains them; y1, y2, y3 are written as they are produced.  Reads each input element
-// once from HBM and writes 3 outputs: the algorithmic minimum.
+// once from HBM and writes 3 outputs: the algorithmic minimum.  __hmax2_nan, not __hmax2, so NaN propagates.
 __device__ __forceinline__ uint4 max8(const uint4& a, const uint4& b, bool bf16) {
     const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
     uint32_t o[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         if (bf16) {
-            __nv_bfloat162 r = __hmax2(*reinterpret_cast<const __nv_bfloat162*>(&aw[j]), *reinterpret_cast<const __nv_bfloat162*>(&bw[j]));
+            __nv_bfloat162 r = __hmax2_nan(*reinterpret_cast<const __nv_bfloat162*>(&aw[j]), *reinterpret_cast<const __nv_bfloat162*>(&bw[j]));
             o[j] = *reinterpret_cast<uint32_t*>(&r);
         } else {
-            __half2 r = __hmax2(*reinterpret_cast<const __half2*>(&aw[j]), *reinterpret_cast<const __half2*>(&bw[j]));
+            __half2 r = __hmax2_nan(*reinterpret_cast<const __half2*>(&aw[j]), *reinterpret_cast<const __half2*>(&bw[j]));
             o[j] = *reinterpret_cast<uint32_t*>(&r);
         }
     }
@@ -234,6 +237,8 @@ static int check_launch(const char* what) {
     return 0;
 }
 static bool half_dtype(int d) { return d == Y5_F16 || d == Y5_BF16; }
+// a view the kernels read or write in 16-byte vectors: aligned base, pitch covering its channels
+static bool vec_view(const void* p, int pitch, int c) { return !(reinterpret_cast<uintptr_t>(p) & 15) && pitch >= c; }
 
 extern "C" Y5_API int y5_stem_s2d(const void* img, int32_t img_dtype, void* out, int32_t out_dtype, int32_t batch, int32_t h, int32_t w,
                                   int32_t out_row_px, int32_t out_x_off, void* stream) {
@@ -241,6 +246,7 @@ extern "C" Y5_API int y5_stem_s2d(const void* img, int32_t img_dtype, void* out,
     if (out_x_off < 0 || out_x_off + w / 2 > row_px) return set_error(Y5_E_INVALID, "stem_s2d: output row pitch/offset do not cover the row");
     if (!img || !out || batch <= 0 || h <= 0 || w <= 0 || (h & 1) || (w & 1)) return set_error(Y5_E_INVALID, "stem_s2d: bad arguments (h, w must be even)");
     if (!half_dtype(out_dtype)) return set_error(Y5_E_UNSUPPORTED, "stem_s2d: output dtype must be fp16/bf16");
+    if (reinterpret_cast<uintptr_t>(out) & 15) return set_error(Y5_E_INVALID, "stem_s2d: output must be 16-byte aligned");
     const long long total = static_cast<long long>(batch) * (h / 2) * (w / 2);
     const int threads = 256, grid = grid_for(total, threads);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -260,6 +266,8 @@ extern "C" Y5_API int y5_sppf_pool(const void* x, int32_t x_pitch, void* y1, voi
                             int32_t w, int32_t c, int32_t ksize, int32_t dtype, void* stream) {
     if (!x || !y1 || !y2 || !y3 || batch <= 0 || h <= 0 || w <= 0 || c <= 0) return set_error(Y5_E_INVALID, "sppf_pool: bad arguments");
     if (c % 8 || x_pitch % 8 || y_pitch % 8 || !half_dtype(dtype) || !(ksize & 1)) return set_error(Y5_E_UNSUPPORTED, "sppf_pool: c/pitch %% 8, odd k, fp16/bf16 only");
+    if (!vec_view(x, x_pitch, c) || !vec_view(y1, y_pitch, c) || !vec_view(y2, y_pitch, c) || !vec_view(y3, y_pitch, c))
+        return set_error(Y5_E_INVALID, "sppf_pool: views must be 16-byte aligned with pitch >= c");
     const size_t smem = static_cast<size_t>(2) * h * w * sizeof(uint4);
     if (smem <= 96 * 1024 && static_cast<long long>(batch) * (c / 8) < 0x7fffffff) {
         if (ensure_dyn_smem(reinterpret_cast<const void*>(sppf_pool_smem_kernel), 96 * 1024) != cudaSuccess)
@@ -281,6 +289,7 @@ extern "C" Y5_API int y5_upsample2x(const void* x, int32_t x_pitch, void* y, int
                              int32_t dtype, void* stream) {
     if (!x || !y || batch <= 0 || h <= 0 || w <= 0 || c <= 0) return set_error(Y5_E_INVALID, "upsample2x: bad arguments");
     if (c % 8 || x_pitch % 8 || y_pitch % 8 || !half_dtype(dtype)) return set_error(Y5_E_UNSUPPORTED, "upsample2x: c/pitch %% 8, fp16/bf16 only");
+    if (!vec_view(x, x_pitch, c) || !vec_view(y, y_pitch, c)) return set_error(Y5_E_INVALID, "upsample2x: views must be 16-byte aligned with pitch >= c");
     const long long total = static_cast<long long>(batch) * 4 * h * w * (c / 8);
     const int threads = 256, grid = grid_for(total, threads);
     launch_pdl(upsample2x_kernel, grid, dim3(threads), 0, static_cast<cudaStream_t>(stream), static_cast<const uint16_t*>(x), x_pitch,
@@ -292,6 +301,7 @@ extern "C" Y5_API int y5_copy_view(const void* x, int32_t x_pitch, void* y, int3
                             void* stream) {
     if (!x || !y || pixels <= 0 || c <= 0) return set_error(Y5_E_INVALID, "copy_view: bad arguments");
     if (c % 8 || x_pitch % 8 || y_pitch % 8 || !half_dtype(dtype)) return set_error(Y5_E_UNSUPPORTED, "copy_view: c/pitch %% 8, fp16/bf16 only");
+    if (!vec_view(x, x_pitch, c) || !vec_view(y, y_pitch, c)) return set_error(Y5_E_INVALID, "copy_view: views must be 16-byte aligned with pitch >= c");
     const long long total = pixels * (c / 8);
     const int threads = 256, grid = grid_for(total, threads);
     launch_pdl(copy_view_kernel, grid, dim3(threads), 0, static_cast<cudaStream_t>(stream), static_cast<const uint16_t*>(x), x_pitch,
