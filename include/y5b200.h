@@ -82,8 +82,8 @@ typedef struct y5_conv_desc {
     int64_t in_n_stride;  /* elements between images (0 = in_h * in_y_stride) */
     int32_t a_mode;       /* activation fetch: 0 auto, 1 force TMA-im2col, 2 force shifted-patch (stride-1 only) */
     int32_t reserved;     /* flags, 0 in normal use.  Tuning / tests: bit 3 (8) staged epilogue (each warpgroup's block goes
-                             through shared memory and leaves as 16-byte row segments), bit 4 (16) forces the default direct
-                             register stores; bit 7 (128) the wide patch fetch (one patch copy per channel chunk
+                             through shared memory and leaves as 16-byte row segments), bit 4 (16) forces direct register
+                             stores instead of the default TMA epilogue; bit 7 (128) the wide patch fetch (one patch copy per channel chunk
                              feeds every tap of a stride-1 k x k conv with 64-channel chunks), bit 5 (32) vetoes it; with a
                              forced block_n also bit 1 (2) = 256-row tiles (block_n 128), bit 2 (4) = CTA pairs (2-CTA cluster),
                              bits 8.. = cluster size (2|4): the CTAs of a cluster split every weight tile and TMA-multicast it */
@@ -110,6 +110,7 @@ struct y5_conv_plan_info {
     int32_t epi;                  /* epilogue: 0 conv, 1 Detect head */
     int32_t a_stages, b_stages;   /* shared-memory pipeline depth */
     int32_t grid;                 /* CTAs launched (persistent, at most one per SM) */
+    int32_t tma_epi;              /* epilogue through shared memory: residual TMA-loaded, output TMA-stored */
 };
 int y5_conv_plan_info(const y5_conv_plan* plan, struct y5_conv_plan_info* info);
 /* one-shot convenience: create + run + destroy (tests) */

@@ -54,13 +54,29 @@ for _ in range(reps):
     for i, (s, e) in enumerate(evs):
         acc[i] += s.elapsed_time(e) / reps
 tot = sum(acc)
+
+
+def plan_cols(op):
+    """tile (rows x cols), pipeline stages a/b and the epilogue (tma | direct) of a conv launch"""
+    if op.fn is not prog.lib.y5_conv_plan_run:
+        return ""
+    info = _lib.PlanInfo()
+    _lib.check(prog.lib.y5_conv_plan_info(op.args[0], C.byref(info)), "conv_plan_info")
+    return f"{128 * info.mt:>4d}x{info.block_n:<4d} {info.a_stages}/{info.b_stages} {'tma' if info.tma_epi else 'direct'}"
+
+
+# floors: NVIDIA's H100 SXM data-sheet rates (989 TFLOP/s dense fp16/bf16, 3.35 TB/s HBM3), not measured ones
+props = torch.cuda.get_device_properties(dev)
+smi = os.popen("nvidia-smi --query-gpu=power.limit,clocks.max.sm --format=csv,noheader -i 0").read().strip()
+print(f"{props.name} ({smi})")
 print(f"{name} bs={bs} {size} {dt}: fixed ops {tot:.3f} ms ({len(prog.ops)} launches)")
-print(f"{'op':28s} {'M':>8s} {'N':>5s} {'K':>5s} {'us':>8s} {'GB/s':>7s} {'TF/s':>6s}  hbm-bound us")
+print(f"{'op':28s} {'M':>8s} {'N':>5s} {'K':>5s} {'us':>8s} {'GB/s':>7s} {'TF/s':>6s} {'tensor-floor':>12s} {'hbm-floor':>9s}  tile      st  epilogue")
 for i, op in enumerate(prog.ops):
     md = meta.get(i)
     if md:
         us = acc[i] * 1e3
-        print(f"{md['name']:28s} {md['M']:8d} {md['N']:5d} {md['K']:5d} {us:8.1f} {md['bytes'] / us / 1e3:7.0f} {md['flops'] / us / 1e6:6.1f}  {md['bytes'] / 6569e3:8.1f}")
+        print(f"{md['name']:28s} {md['M']:8d} {md['N']:5d} {md['K']:5d} {us:8.1f} {md['bytes'] / us / 1e3:7.0f} {md['flops'] / us / 1e6:6.1f} "
+              f"{md['flops'] / 989e6:12.1f} {md['bytes'] / 3350e3:9.1f}  {plan_cols(op)}")
     else:
         print(f"{op.name:28s} {'':8s} {'':5s} {'':5s} {acc[i] * 1e3:8.1f}")
 # Detect-head GEMMs (they run outside the captured graph: fresh output tensors per call)
@@ -81,7 +97,7 @@ for _ in range(reps):
 for i, sh in enumerate(prog.det_shapes):
     mrows = sh[0] * sh[2] * sh[3]
     byt = 2 * (mrows * prog.outs[[17, 20, 23][i]].c + 2 * mrows * sh[1] * sh[4]) if len(prog.outs) > 23 else 0
-    print(f"{'detect.' + str(i):28s} {mrows:8d} {sh[1] * sh[4]:5d} {'':5s} {hacc[i] * 1e3:8.1f} {byt / max(hacc[i], 1e-9) / 1e6:7.0f} {'':6s}  {byt / 6569e3:8.1f}")
+    print(f"{'detect.' + str(i):28s} {mrows:8d} {sh[1] * sh[4]:5d} {'':5s} {hacc[i] * 1e3:8.1f} {byt / max(hacc[i], 1e-9) / 1e6:7.0f} {'':6s} {'':12s} {byt / 3350e3:9.1f}")
 print(f"fixed ops + head {tot + sum(hacc):.3f} ms")
 # head + stem timing
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -60,6 +60,7 @@ class PlanInfo(C.Structure):
         ("block_k", C.c_int32), ("block_n", C.c_int32), ("mt", C.c_int32), ("cluster", C.c_int32),
         ("patch_pw", C.c_int32), ("b_grouped", C.c_int32), ("staged", C.c_int32), ("opt", C.c_int32), ("epi", C.c_int32),
         ("a_stages", C.c_int32), ("b_stages", C.c_int32), ("grid", C.c_int32),
+        ("tma_epi", C.c_int32),
     ]
 
     def as_dict(self) -> dict:

@@ -183,6 +183,15 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

@@ -19,9 +19,11 @@
 // MMA + epilogue: two consumer warpgroups.  Warpgroup w owns rows [64w, 64w + 64) of every 128-row sub-tile and issues
 // wgmma m64 x BLOCK_N x k16 (fp32 accumulators in registers) for them; after the tile's last K block it applies the
 // folded-BN bias -> SiLU -> (+ residual) -> fp16/bf16 and stores straight from the registers to the NHWC (slice) view.
-// Epilogue stores: by default each thread stores its 4-byte pairs straight from the registers; on request each warpgroup stages
-// its packed 64 x BLOCK_N block in shared memory and writes whole 16-byte row segments instead.  Residual words are loaded in
-// batches ahead of the stores (the residual may alias the output, so loads interleaved with stores would serialise).
+// Epilogue stores: by default the tile is staged in shared memory in swizzled 64-row boxes, with its residual TMA-loaded there by
+// the producer warp, and leaves by TMA bulk stores (the TMA unit clips the tails).  Direct mode (reserved bit 16, and plans where
+// the staging block does not fit or costs too much): each thread stores its 4-byte pairs straight from the registers, with the
+// residual words loaded in batches ahead of the stores (the residual may alias the output, so interleaving would serialise); the
+// OPT instantiation can instead stage each warpgroup's block and write whole 16-byte row segments.
 // Tiles: MT sub-tiles of 128 rows x BLOCK_N with MT * BLOCK_N <= 256 (128 accumulator registers per thread), so one weight
 // tile feeds MT sub-tiles and narrow layers do as much work per barrier round as wide ones.
 // Clusters (2 or 4 CTAs along M): the CTAs of a cluster work on different M super-tiles of the SAME N tile in lock-step, each
@@ -76,6 +78,7 @@ struct ConvParams {
     int patch_pw;               // > 0: wide patch mode, patch row pitch in pixels (8*MT + 8); one A copy per channel chunk feeds kh*kw taps
     int cluster_n;              // CTAs per cluster (1, 2, 4): weight tiles are split between them and multicast
     uint32_t stg_bytes;         // EPI 0: shared-memory staging of the epilogue (0 = direct stores)
+    int tma_epi;                // EPI 0, default instantiation: the tile is staged in smem (residual TMA-loaded into it) and TMA-stored
     uint32_t b_sub_bytes;       // bytes of one weight tile inside a (possibly grouped) stage
     float rcp_per_img, rcp_tiles_x, rcp_HoWo, rcp_Wo;  // reciprocals for fdiv(): exact small-integer division in ~7 instructions
     int a_stages, b_stages;
@@ -111,12 +114,12 @@ __host__ __device__ inline SmemLayout smem_layout(int epi, int no, int bias_n, i
     o = (o + 1023) & ~1023u;
     L.off_out = o;
     if (epi == 1) o += 4 * ((kBlockM * no * 2 + 1023) & ~1023u);  // head: 2 sets x {raw, decoded} blocks [128][no], global layout
-    else o += stg_bytes;                                            // EPI 0 staged stores: one [64 rows][BLOCK_N] block per consumer warpgroup
+    else o += stg_bytes;                                            // EPI 0 staging: per warpgroup [64 rows][BLOCK_N] (staged) or the tile (TMA)
     L.off_bias = o;
     o += ((bias_n + 3) & ~3) * 4;
     o = (o + 7) & ~7u;
     L.off_bars = o;
-    o += 4 * kMaxStages * 8;
+    o += (4 * kMaxStages + 2) * 8;  // A / B rings, then the TMA epilogue's res_full / stg_free pair
     L.total = o;
     return L;
 }
@@ -130,6 +133,31 @@ __device__ __forceinline__ int fdiv(int n, int d, float rd) {
     if (r >= d) ++q;
     else if (r < 0) --q;
     return q;
+}
+
+// TMA epilogue: a warpgroup's 64 rows of a sub-tile are kNB boxes of [64 rows][kCols columns] with kRB-byte rows and the TMA
+// swizzle of that row size (64 or 128 bytes), placed [warpgroup][sub-tile][box] in the staging block.
+template <int BLOCK_N>
+struct EpiBox {
+    static constexpr int kRB = BLOCK_N * 2 < 128 ? BLOCK_N * 2 : 128;
+    static constexpr int kCols = kRB / 2;
+    static constexpr int kNB = BLOCK_N / kCols;
+    static constexpr uint32_t kBytes = 64u * kRB;
+};
+struct EpiOrigin {
+    int x, y, img;  // 2-D map: y = first row; PATCH (4-D map): first pixel x, y of image img
+};
+// where warpgroup wg's 64 rows of sub-tile mt start in the output / residual map; a PATCH box is [min(tw, 64)] x [max(64 / tw, 1)]
+// pixels.  Rows past M, pixels past Wo / Ho and sub-tiles past the last one land out of bounds: the TMA unit clips the stores and
+// zero-fills the loads.
+__device__ __forceinline__ EpiOrigin epi_origin(const ConvParams& p, int mt, int wg) {
+    if (p.a_mode != A_PATCH) return {0, mt * kBlockM + 64 * wg, 0};
+    const int per_img = p.tiles_x * p.tiles_y;
+    const int img = fdiv(mt, per_img, p.rcp_per_img);
+    const int rem = mt - img * per_img;
+    const int ty = fdiv(rem, p.tiles_x, p.rcp_tiles_x);
+    const int x = (rem - ty * p.tiles_x) * p.tw, y = ty * p.th;
+    return p.tw > 64 ? EpiOrigin{x + 64 * wg, y, img} : EpiOrigin{x, y + wg * (64 / p.tw), img};
 }
 
 // One K block (KS k16 steps) for all MT sub-tiles as one wgmma batch: fence, KS * MT back-to-back wgmmas, commit.  Nothing
@@ -153,9 +181,12 @@ __device__ __forceinline__ void mma_batch(float (&acc)[MT][BLOCK_N / 2], uint32_
 // BF16: activation / weight dtype (bf16 or fp16), fixed per instantiation so the MMA batches and the epilogue carry no dtype branch.
 template <int BLOCK_N, int EPI, int MT, bool OPT, bool BF16>
 __global__ void __launch_bounds__(kThreads, 1)
-conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
+conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+                 const __grid_constant__ CUtensorMap tmR, const ConvParams p) {
     static_assert(MT * BLOCK_N <= 256, "accumulators: at most 128 fp32 registers per consumer thread");
     constexpr int kAcc = BLOCK_N / 2;  // accumulator registers per sub-tile and thread (64 x BLOCK_N over a warpgroup)
+    using Box = EpiBox<BLOCK_N>;
+    const bool tma_epi = EPI == 0 && !OPT && p.tma_epi;
 
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -167,6 +198,11 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint64_t* a_empty = a_full + kMaxStages;
     uint64_t* b_full = a_empty + kMaxStages;
     uint64_t* b_empty = b_full + kMaxStages;
+    // TMA epilogue: the producer fills the staging block with a tile's residual (or just arrives, without one) on res_full once the
+    // previous tile's bulk stores have finished reading it (stg_free, one arrival per consumer warpgroup)
+    uint64_t* res_full = b_empty + kMaxStages;
+    uint64_t* stg_free = res_full + 1;
+    uint8_t* stg = smem + L.off_out;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -181,6 +217,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             mbar_init(&a_empty[s], kConsumers);  // one arrival per consumer warpgroup
             mbar_init(&b_full[s], 1);
             mbar_init(&b_empty[s], kConsumers * csize);  // multicast stages: released by the consumers of every CTA of the cluster
+        }
+        mbar_init(res_full, 1);
+        mbar_init(stg_free, kConsumers);
+        if (tma_epi) {
+            tma_prefetch_desc(&tmO);
+            if (p.res) tma_prefetch_desc(&tmR);
         }
         fence_barrier_init();
     }
@@ -219,7 +261,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         // ===================================== TMA producer =====================================
         // the whole warp runs the loop with warp-uniform state; one elected lane issues the copies
         int as = 0, bs = 0;
-        uint32_t aph = 0, bph = 0;
+        uint32_t aph = 0, bph = 0, sph = 0;
         for (int tile = tile0; tile < num_tiles; tile += tile_step) {
             const int ms = (tile / nn) * csize + static_cast<int>(crank);
             const int n0 = (tile - (tile / nn) * nn) * BLOCK_N;
@@ -293,6 +335,30 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     for (int s = 0; s < p.kw; ++s)
                         for (int cc = 0; cc < p.c_chunks; ++cc) issue_group(cc, s, r);
             }
+            // the tile's residual, after its last K block: by then the consumers have started this tile (its first batch frees the
+            // staging block of the previous one), so the wait rarely blocks and the copy lands while the tile's MMAs run
+            if (tma_epi) {
+                mbar_wait(stg_free, sph ^ 1);
+                if (elect_one()) {
+                    if (p.res) {
+                        mbar_arrive_expect_tx(res_full, p.stg_bytes);
+#pragma unroll 1
+                        for (int i = 0; i < kConsumers * MT; ++i) {
+                            const EpiOrigin o = epi_origin(p, ms * MT + i % MT, i / MT);
+#pragma unroll
+                            for (int b = 0; b < Box::kNB; ++b) {
+                                uint8_t* dst = stg + (i * Box::kNB + b) * Box::kBytes;
+                                if (patch) tma_load_4d(&tmR, res_full, dst, n0 + b * Box::kCols, o.x, o.y, o.img);
+                                else tma_load_2d(&tmR, res_full, dst, n0 + b * Box::kCols, o.y);
+                            }
+                        }
+                    } else {
+                        mbar_arrive(res_full);
+                    }
+                }
+                __syncwarp();
+                sph ^= 1;
+            }
         }
     } else if (warp >= 4) {
     // ===================================== MMA + epilogue (warpgroups 1, 2) =====================================
@@ -315,7 +381,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int per_img = p.tiles_x * p.tiles_y;
     const int tw_shift = patch ? __ffs(p.tw) - 1 : 0;
     int as = 0, bs = 0, head_set = 0;
-    uint32_t aph = 0, bph = 0;
+    uint32_t aph = 0, bph = 0, rph = 0;
     float acc[MT][kAcc];
 #pragma unroll
     for (int mi = 0; mi < MT; ++mi)
@@ -366,6 +432,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
                 for (int mi = 0; mi < MT; ++mi) fence_regs(acc[mi]);
                 if (g | j) release_pending();  // the tile's first batch: everything before it was released at the previous tile's end
+                else if (tma_epi && signal && tile != tile0) {
+                    // the previous tile's bulk stores have read the staging block (waited for under this batch): the producer may
+                    // load this tile's residual into it
+                    tma_store_wait_read0();
+                    mbar_arrive(stg_free);
+                }
                 pend_as = as;
                 pend_a_last = j == grp - 1;
                 pend_bs = bs;
@@ -385,7 +457,18 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (EPI == 0) {
             const bool staged = OPT && p.stg_bytes != 0;
             const uint32_t stg_pitch = BLOCK_N * 2 + 16;  // +16 bytes: the fragment's 8 rows x 4 column pairs hit 32 distinct banks
-            uint8_t* stg = smem + L.off_out + wg * 64 * stg_pitch;
+            uint8_t* stg_wg = stg + wg * 64 * stg_pitch;
+            // TMA epilogue: shared address of the word of column pair (8 j + ccol) of row half h of sub-tile mi in its swizzled box
+            // (16-byte chunk index XOR the row's offset bits 7.., as the TMA unit lays it out; the fragment's 8 rows x 4 column pairs
+            // hit 32 distinct banks).  The thread's row base and XOR term are laundered per tile, so the compiler does not hoist
+            // every word address out of the tile loop and hold them next to the accumulators.
+            constexpr int kChunks = Box::kRB / 16;
+            uint32_t stg_row = smem_u32(stg) + wg * MT * Box::kNB * Box::kBytes + (wrow - wg * 64) * Box::kRB + ccol * 2;
+            uint32_t stg_swz = ((((wrow - wg * 64) * Box::kRB) >> 7) & (kChunks - 1)) << 4;
+            asm volatile("" : "+r"(stg_row), "+r"(stg_swz));
+            auto stg_word = [&](int mi, int h, int j) -> uint32_t {
+                return stg_row + (mi * Box::kNB + j / kChunks) * Box::kBytes + h * 8 * Box::kRB + (((j % kChunks) << 4) ^ stg_swz);
+            };
             // global output pixel of row `row` of sub-tile `mt`, -1 outside the output
             auto pixel_of = [&](int mt, int row) -> long long {
                 if (patch) {  // image + origin of the th x tw block
@@ -407,82 +490,122 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             constexpr float kTail = BF16 ? 8.0f : 4.0f;  // silu_from_half is faithful down to -kTail (see common.cuh)
             constexpr int kRows = 2 * MT, kWords = (OPT ? 128 : 256) / BLOCK_N;
             constexpr int kBatch = kWords < 1 ? 1 : (kWords < kRows ? kWords : kRows);
+            // TMA epilogue: the residual words (zero outside the output) are in the staging block and the tile is written there; no
+            // global access and no bounds test per element, the TMA unit clips the stores
             const bool has_res = p.res != nullptr;
+            if (tma_epi) {
+                mbar_wait(res_full, rph);
+                rph ^= 1;
+            }
+            // the two store paths as separate straight-line code: run-time tests of the path inside the unrolled loops made ptxas spill
+            auto rows = [&](auto tma_path) {
+                constexpr bool TMA = decltype(tma_path)::value;
 #pragma unroll
-            for (int q0 = 0; q0 < kRows; q0 += kBatch) {
-                uint32_t rv[kBatch][BLOCK_N / 8];
-                long long gp[kBatch];  // output pixel of each row half of the batch, -1 outside the output
+                for (int q0 = 0; q0 < kRows; q0 += kBatch) {
+                    uint32_t rv[kBatch][BLOCK_N / 8];
+                    long long gp[kBatch];  // output pixel of each row half of the batch, -1 outside the output
 #pragma unroll
-                for (int q = 0; q < kBatch; ++q) gp[q] = pixel_of(ms * MT + (q0 + q) / 2, wrow + 8 * ((q0 + q) & 1));
-                if (has_res) {
+                    for (int q = 0; q < kBatch; ++q) gp[q] = TMA ? 0 : pixel_of(ms * MT + (q0 + q) / 2, wrow + 8 * ((q0 + q) & 1));
+                    if (has_res && TMA) {
+#pragma unroll
+                        for (int q = 0; q < kBatch; ++q)
+#pragma unroll
+                            for (int j = 0; j < BLOCK_N / 8; ++j) rv[q][j] = ld_shared_u32(stg_word((q0 + q) / 2, (q0 + q) & 1, j));
+                    } else if (has_res) {
+#pragma unroll
+                        for (int q = 0; q < kBatch; ++q) {
+                            const uint16_t* rp = reinterpret_cast<const uint16_t*>(p.res) + (gp[q] < 0 ? 0 : gp[q] * p.res_pitch) + n0 + ccol;
+#pragma unroll
+                            for (int j = 0; j < BLOCK_N / 8; ++j)
+                                rv[q][j] = (gp[q] >= 0 && n0 + 8 * j < p.N) ? *reinterpret_cast<const uint32_t*>(rp + 8 * j) : 0u;
+                        }
+                    }
 #pragma unroll
                     for (int q = 0; q < kBatch; ++q) {
-                        const uint16_t* rp = reinterpret_cast<const uint16_t*>(p.res) + (gp[q] < 0 ? 0 : gp[q] * p.res_pitch) + n0 + ccol;
+                        const int mi = (q0 + q) / 2, h = (q0 + q) & 1;  // sub-tile, row half
+                        const int mt = ms * MT + mi;
+                        const int row = wrow + 8 * h;
+                        const long long gpix = gp[q];
+                        if (gpix >= 0 || staged) {
+                            uint16_t* op = reinterpret_cast<uint16_t*>(p.out) + gpix * p.out_pitch + n0 + ccol;
+                            uint8_t* sp = stg_wg + (row - wg * 64) * stg_pitch + ccol * 2;
+                            float hmin = 0.0f;  // smallest SiLU input / 2 of the row half
+                            // the row half's 8-column groups: bias -> SiLU -> + residual -> pack -> store.  TAIL: the pass that recomputes
+                            // the SiLU inputs below -kTail with silu_tail (silu_from_half is not faithful there) and stores the row again
+                            auto row_half = [&](auto tail_pass) {
+                                constexpr bool TAIL = decltype(tail_pass)::value;
 #pragma unroll
-                        for (int j = 0; j < BLOCK_N / 8; ++j)
-                            rv[q][j] = (gp[q] >= 0 && n0 + 8 * j < p.N) ? *reinterpret_cast<const uint32_t*>(rp + 8 * j) : 0u;
+                                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                                    if (n0 + 8 * j >= p.N) continue;  // N % 8 == 0: an 8-column group is all in or all out
+                                    const float2 b = *reinterpret_cast<const float2*>(sBias + n0 + 8 * j + ccol);
+                                    const float a0 = acc[mi][4 * j + 2 * h], a1 = acc[mi][4 * j + 2 * h + 1];
+                                    float f0, f1;
+                                    if (p.act) {  // b holds bias / 2 (see the preload)
+                                        const float h0 = fmaf(a0, 0.5f, b.x), h1 = fmaf(a1, 0.5f, b.y);  // exactly fp32(acc + bias) / 2
+                                        f0 = silu_from_half(h0);
+                                        f1 = silu_from_half(h1);
+                                        if (TAIL) {
+                                            if (h0 < -0.5f * kTail) f0 = silu_tail(2.0f * h0);
+                                            if (h1 < -0.5f * kTail) f1 = silu_tail(2.0f * h1);
+                                        } else {
+                                            hmin = fminf(hmin, fminf(h0, h1));
+                                        }
+                                    } else {
+                                        f0 = a0 + b.x;
+                                        f1 = a1 + b.y;
+                                    }
+                                    if (has_res && gpix >= 0) {
+                                        const float2 t = unpack2(rv[q][j], bf16);
+                                        f0 += t.x;
+                                        f1 += t.y;
+                                    }
+                                    if (TMA) st_shared_u32(stg_word(mi, h, j), pack2(f0, f1, bf16));
+                                    else if (staged) *reinterpret_cast<uint32_t*>(sp + 16 * j) = pack2(f0, f1, bf16);
+                                    else *reinterpret_cast<uint32_t*>(op + 8 * j) = pack2(f0, f1, bf16);
+                                }
+                            };
+                            row_half(std::false_type{});
+                            // inputs below -kTail are rare: one vote per row half, and only the warps holding some take the second pass
+                            // (the residual comes from the registers, so an in-place residual stays right)
+                            if (p.act && __any_sync(__activemask(), hmin < -0.5f * kTail)) row_half(std::true_type{});
+                        }
+                        if (staged && h == 1) {  // the sub-tile is complete: the warpgroup's 64 rows leave as whole 16-byte row segments
+                            named_bar_sync(2 + wg, 128);
+                            constexpr int kSeg = BLOCK_N / 8;
+                            for (int i = threadIdx.x & 127; i < 64 * kSeg; i += 128) {
+                                const int lrow = i / kSeg, c = i - lrow * kSeg;
+                                const long long gp = pixel_of(mt, wg * 64 + lrow);
+                                if (gp >= 0 && n0 + 8 * c < p.N)
+                                    *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + gp * p.out_pitch + n0 + 8 * c) =
+                                        *reinterpret_cast<const uint4*>(stg_wg + lrow * stg_pitch + c * 16);
+                            }
+                            named_bar_sync(2 + wg, 128);  // the staging block is rewritten by the next sub-tile / tile
+                        }
                     }
                 }
+            };
+            if (tma_epi) rows(std::true_type{});
+            else rows(std::false_type{});
+            if (tma_epi) {
+                // the warpgroup's rows are in the staging block: make them visible to the async proxy, then one thread stores them and
+                // goes on to the next tile; it waits for the stores to have read the block under the next tile's first MMA batch
+                fence_proxy_async_smem();
+                named_bar_sync(2 + wg, 128);
+                if (signal) {
+#pragma unroll 1
+                    for (int mi = 0; mi < MT; ++mi) {
+                        const EpiOrigin o = epi_origin(p, ms * MT + mi, wg);
 #pragma unroll
-                for (int q = 0; q < kBatch; ++q) {
-                    const int mi = (q0 + q) / 2, h = (q0 + q) & 1;  // sub-tile, row half
-                    const int mt = ms * MT + mi;
-                    const int row = wrow + 8 * h;
-                    const long long gpix = gp[q];
-                    if (gpix >= 0 || staged) {
-                        uint16_t* op = reinterpret_cast<uint16_t*>(p.out) + gpix * p.out_pitch + n0 + ccol;
-                        uint8_t* sp = stg + (row - wg * 64) * stg_pitch + ccol * 2;
-                        float hmin = 0.0f;  // smallest SiLU input / 2 of the row half
-                        // the row half's 8-column groups: bias -> SiLU -> + residual -> pack -> store.  TAIL: the pass that recomputes
-                        // the SiLU inputs below -kTail with silu_tail (silu_from_half is not faithful there) and stores the row again
-                        auto row_half = [&](auto tail_pass) {
-                            constexpr bool TAIL = decltype(tail_pass)::value;
-#pragma unroll
-                            for (int j = 0; j < BLOCK_N / 8; ++j) {
-                                if (n0 + 8 * j >= p.N) continue;  // N % 8 == 0: an 8-column group is all in or all out
-                                const float2 b = *reinterpret_cast<const float2*>(sBias + n0 + 8 * j + ccol);
-                                const float a0 = acc[mi][4 * j + 2 * h], a1 = acc[mi][4 * j + 2 * h + 1];
-                                float f0, f1;
-                                if (p.act) {  // b holds bias / 2 (see the preload)
-                                    const float h0 = fmaf(a0, 0.5f, b.x), h1 = fmaf(a1, 0.5f, b.y);  // exactly fp32(acc + bias) / 2
-                                    f0 = silu_from_half(h0);
-                                    f1 = silu_from_half(h1);
-                                    if (TAIL) {
-                                        if (h0 < -0.5f * kTail) f0 = silu_tail(2.0f * h0);
-                                        if (h1 < -0.5f * kTail) f1 = silu_tail(2.0f * h1);
-                                    } else {
-                                        hmin = fminf(hmin, fminf(h0, h1));
-                                    }
-                                } else {
-                                    f0 = a0 + b.x;
-                                    f1 = a1 + b.y;
-                                }
-                                if (has_res && gpix >= 0) {
-                                    const float2 t = unpack2(rv[q][j], bf16);
-                                    f0 += t.x;
-                                    f1 += t.y;
-                                }
-                                if (staged) *reinterpret_cast<uint32_t*>(sp + 16 * j) = pack2(f0, f1, bf16);
-                                else *reinterpret_cast<uint32_t*>(op + 8 * j) = pack2(f0, f1, bf16);
-                            }
-                        };
-                        row_half(std::false_type{});
-                        // inputs below -kTail are rare: one vote per row half, and only the warps holding some take the second pass
-                        // (the residual comes from the registers, so an in-place residual stays right)
-                        if (p.act && __any_sync(__activemask(), hmin < -0.5f * kTail)) row_half(std::true_type{});
-                    }
-                    if (staged && h == 1) {  // the sub-tile is complete: the warpgroup's 64 rows leave as whole 16-byte row segments
-                        named_bar_sync(2 + wg, 128);
-                        constexpr int kSeg = BLOCK_N / 8;
-                        for (int i = threadIdx.x & 127; i < 64 * kSeg; i += 128) {
-                            const int lrow = i / kSeg, c = i - lrow * kSeg;
-                            const long long gp = pixel_of(mt, wg * 64 + lrow);
-                            if (gp >= 0 && n0 + 8 * c < p.N)
-                                *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + gp * p.out_pitch + n0 + 8 * c) =
-                                    *reinterpret_cast<const uint4*>(stg + lrow * stg_pitch + c * 16);
+                        for (int b = 0; b < Box::kNB; ++b) {
+                            const uint8_t* src = stg + ((wg * MT + mi) * Box::kNB + b) * Box::kBytes;
+                            if (patch) tma_store_4d(&tmO, src, n0 + b * Box::kCols, o.x, o.y, o.img);
+                            else tma_store_2d(&tmO, src, n0 + b * Box::kCols, o.y);
                         }
-                        named_bar_sync(2 + wg, 128);  // the staging block is rewritten by the next sub-tile / tile
                     }
+                    tma_store_commit();
+                    // the next layer reads this output (under PDL, as soon as this grid completes): the CTA's last stores are complete
+                    // before it exits.  (Placed here: the same wait after the tile loop made ptxas serialise the wgmmas and spill.)
+                    if (tile + tile_step >= num_tiles) tma_store_wait_all();
                 }
             }
         } else {
@@ -630,13 +753,13 @@ int pick_block_n(int out_c, int64_t m_rows) {
 }
 
 template <int BN, int EPI, int MT, bool OPT>
-cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const ConvParams& p, int grid, int cluster, uint32_t smem,
-                        cudaStream_t st) {
+cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const CUtensorMap& r, const ConvParams& p,
+                        int grid, int cluster, uint32_t smem, cudaStream_t st) {
     auto* kernel = p.is_bf16 ? conv_gemm_kernel<BN, EPI, MT, OPT, true> : conv_gemm_kernel<BN, EPI, MT, OPT, false>;
     const cudaError_t attr_err = ensure_dyn_smem(reinterpret_cast<const void*>(kernel), 227 * 1024);
     if (attr_err != cudaSuccess) return attr_err;
     count_launch();
-    if (cluster == 1) return launch_pdl(kernel, dim3(grid), dim3(kThreads), smem, st, a, b, p);
+    if (cluster == 1) return launch_pdl(kernel, dim3(grid), dim3(kThreads), smem, st, a, b, o, r, p);
     static const bool pdl = [] { const char* e = getenv("Y5_PDL"); return !(e && e[0] == '0'); }();
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid);
@@ -652,11 +775,12 @@ cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const ConvPa
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 2 : 1;
-    return cudaLaunchKernelEx(&cfg, kernel, a, b, p);
+    return cudaLaunchKernelEx(&cfg, kernel, a, b, o, r, p);
 }
 
 struct PlanCommon {
     CUtensorMap tmA, tmB;
+    CUtensorMap tmO, tmR;  // TMA epilogue: output and residual views
     ConvParams p;
     int block_n, epi, mt, grid, cluster;
     uint32_t smem_bytes;
@@ -700,23 +824,24 @@ int finish_plan(PlanCommon& pc, int block_n, int epi, int mt, int cluster = 1) {
 }
 
 // the optional modes run in the OPT instantiation (see conv_gemm_kernel)
-bool plan_opt(const PlanCommon& pc) { return pc.cluster > 1 || pc.p.patch_pw > 0 || pc.p.stg_bytes > 0; }
+bool plan_staged(const PlanCommon& pc) { return pc.p.stg_bytes > 0 && !pc.p.tma_epi; }
+bool plan_opt(const PlanCommon& pc) { return pc.cluster > 1 || pc.p.patch_pw > 0 || plan_staged(pc); }
 
 int run_plan(const PlanCommon& pc, cudaStream_t st) {
     cudaError_t e = cudaErrorInvalidValue;
     const int key = (plan_opt(pc) ? 100000 : 0) + pc.epi * 10000 + pc.block_n * 10 + pc.mt;
     switch (key) {
-        case 324: e = launch_conv<32, 0, 4, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 642: e = launch_conv<64, 0, 2, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 1281: e = launch_conv<128, 0, 1, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 1282: e = launch_conv<128, 0, 2, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 2561: e = launch_conv<256, 0, 1, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 11281: e = launch_conv<kHeadN, 1, 1, false>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 100324: e = launch_conv<32, 0, 4, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 100642: e = launch_conv<64, 0, 2, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 101281: e = launch_conv<128, 0, 1, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 101282: e = launch_conv<128, 0, 2, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 102561: e = launch_conv<256, 0, 1, true>(pc.tmA, pc.tmB, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 324: e = launch_conv<32, 0, 4, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 642: e = launch_conv<64, 0, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 1281: e = launch_conv<128, 0, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 1282: e = launch_conv<128, 0, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 2561: e = launch_conv<256, 0, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 11281: e = launch_conv<kHeadN, 1, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 100324: e = launch_conv<32, 0, 4, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 100642: e = launch_conv<64, 0, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 101281: e = launch_conv<128, 0, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 101282: e = launch_conv<128, 0, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 102561: e = launch_conv<256, 0, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
         default: return set_error(Y5_E_UNSUPPORTED, "conv: no kernel for block_n %d mt %d epi %d", pc.block_n, pc.mt, pc.epi);
     }
     if (e != cudaSuccess) return set_error(int(e), "conv_gemm launch failed: %s", cudaGetErrorString(e));
@@ -741,6 +866,23 @@ Geo geometry(const y5_conv_desc* d) {
     g.Ho = (d->in_h + 2 * g.pad_h - g.kh) / d->stride + 1;
     g.Wo = (d->in_w + 2 * g.pad_w - g.kw) / d->stride + 1;
     return g;
+}
+
+// TMA epilogue view of the output or the residual (EpiBox boxes, the swizzle of their row size): 2-D [M rows][N] for LINEAR and
+// IM2COL tiles, 4-D (N, Wo, Ho, batch) for PATCH tiles
+int encode_epi_map(CUtensorMap* map, int dtype, const void* base, int pitch, const ConvParams& p, int batch, int bn, const char* what) {
+    const int rb = bn * 2 < 128 ? bn * 2 : 128;
+    const cuuint64_t px = static_cast<cuuint64_t>(pitch) * 2;
+    if (p.a_mode == A_PATCH) {
+        cuuint64_t dims[4] = {(cuuint64_t)p.N, (cuuint64_t)p.Wo, (cuuint64_t)p.Ho, (cuuint64_t)batch};
+        cuuint64_t str[3] = {px, px * p.Wo, px * p.HoWo};
+        cuuint32_t box[4] = {(cuuint32_t)(rb / 2), (cuuint32_t)(p.tw < 64 ? p.tw : 64), (cuuint32_t)(p.tw < 64 ? 64 / p.tw : 1), 1};
+        return encode_tiled(map, dtype, base, 4, dims, str, box, swizzle_for_row_bytes(rb), what);
+    }
+    cuuint64_t dims[2] = {(cuuint64_t)p.N, (cuuint64_t)p.M};
+    cuuint64_t str[1] = {px};
+    cuuint32_t box[2] = {(cuuint32_t)(rb / 2), 64};
+    return encode_tiled(map, dtype, base, 2, dims, str, box, swizzle_for_row_bytes(rb), what);
 }
 
 }  // namespace
@@ -902,13 +1044,27 @@ extern "C" Y5_API int y5_conv_plan_create(const y5_conv_desc* d, y5_conv_plan** 
         e = encode_tiled(&pc.tmB, d->dtype, d->weight, 2, dims, str, box, sw, "B");
     }
     if (e) { delete plan; return e; }
-    // epilogue stores: direct from the registers unless reserved bit 3 (8) asks for staged 16-byte row segments (bit 4, 16, forces
-    // direct).  Direct is the default: staging takes up to 66 KB (256-wide tiles) from the pipeline stages and has not been measured
-    // faster.  Staging falls back to direct when the blocks do not fit next to the pipeline stages.
-    p.stg_bytes = ((d->reserved & 8) && !(d->reserved & 16)) ? static_cast<uint32_t>(kConsumers * 64 * (bn * 2 + 16)) : 0u;
+    // Epilogue stores.  Default: the TMA epilogue (the tile staged in shared memory with its residual TMA-loaded there, then TMA
+    // bulk stores).  Reserved bit 4 (16) forces direct stores from the registers; bit 3 (8) asks for the staged 16-byte row segments
+    // of the OPT instantiation, whose optional modes (clusters, wide patch) also keep direct stores.  Either staging falls back to
+    // direct stores when its block does not fit next to the pipeline stages.
+    // The staging block costs the 128 x 256 tiles a pipeline stage (4 -> 3): on the stride-2 IM2COL convs, whose K loops are long and
+    // whose epilogue is a small share of the tile, that measured 4-7 % slower per layer (yolov5l, H100), so they keep direct stores.
+    const bool opt_modes = cl_sel > 1 || p.patch_pw > 0 || (d->reserved & 8);
+    const bool stages_first = p.a_mode == A_IM2COL && bn == 256;
+    if (!(d->reserved & 16) && !opt_modes && !stages_first) {
+        p.tma_epi = 1;
+        p.stg_bytes = static_cast<uint32_t>(mt_sel * bn * 256);  // the whole tile: MT sub-tiles x 128 rows x bn columns
+        e = encode_epi_map(&pc.tmO, d->dtype, d->out, d->out_pitch, p, d->batch, bn, "output");
+        if (!e && d->residual) e = encode_epi_map(&pc.tmR, d->dtype, d->residual, d->res_pitch, p, d->batch, bn, "residual");
+        if (e) { delete plan; return e; }
+    } else if ((d->reserved & 8) && !(d->reserved & 16)) {
+        p.stg_bytes = static_cast<uint32_t>(kConsumers * 64 * (bn * 2 + 16));
+    }
     int e2 = finish_plan(pc, bn, 0, mt_sel, cl_sel);
     if (e2 && p.stg_bytes) {
         p.stg_bytes = 0;
+        p.tma_epi = 0;
         e2 = finish_plan(pc, bn, 0, mt_sel, cl_sel);
     }
     if (e2) { delete plan; return e2; }
@@ -935,7 +1091,8 @@ extern "C" Y5_API int y5_conv_plan_info(const y5_conv_plan* plan, struct y5_conv
     out->cluster = pc.cluster;
     out->patch_pw = p.patch_pw;
     out->b_grouped = p.b_grouped;
-    out->staged = p.stg_bytes > 0;
+    out->staged = plan_staged(pc);
+    out->tma_epi = p.tma_epi;
     out->opt = plan_opt(pc);
     out->epi = pc.epi;
     out->a_stages = p.a_stages;
