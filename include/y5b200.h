@@ -129,12 +129,14 @@ typedef struct y5_detect_desc {
     const void* in;
     int32_t in_pitch;
     int32_t batch, ny, nx, in_c;
-    const void* weight;   /* packed [na*128][cin_pad]: anchor a in rows [128a, 128a + no), the rest zero */
-    const float* bias;    /* fp32 [na*128], laid out like the weight rows */
+    const void* weight;   /* packed [na*npad][cin_pad], npad = 128 * ceil(no / 128): anchor a in rows [a*npad, a*npad + no),
+                             the rest zero (npad = 128 while no <= 128) */
+    const float* bias;    /* fp32 [na*npad], laid out like the weight rows */
     void* raw;
     void* z;
     int32_t z_rows, z_row0;
-    int32_t na, no, nc;   /* no = 5 + nc + nm; columns >= 5+nc (mask coefficients) are passed through un-sigmoided */
+    int32_t na, no, nc;   /* no = 5 + nc + nm <= 8192, nc <= 4096 (Y5_E_UNSUPPORTED beyond); columns >= 5+nc (mask
+                             coefficients) are passed through un-sigmoided */
     float stride;         /* pixels per cell of this level */
     float anchor_wh[8];   /* na x (w,h) in PIXELS (= anchors * stride), na <= 4 */
     int32_t dtype;

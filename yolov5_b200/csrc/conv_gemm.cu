@@ -29,8 +29,10 @@
 // Clusters (2 or 4 CTAs along M): the CTAs of a cluster work on different M super-tiles of the SAME N tile in lock-step, each
 // fetches 1/csize of every weight tile and TMA-multicasts it to all of them, so the L2 -> smem weight traffic per CTA drops by
 // the cluster size.  A weight stage is free again only when the consumers of every CTA of the cluster have released it.
-// Detect head (EPI=1): N tile == one anchor; raw logits and decoded predictions are staged in smem in the exact
-// global layout and copied out with 16-byte vectors.
+// Detect head (EPI=1): an anchor's `no` outputs are tpa = ceil(no / 128) N tiles (weights packed npad = 128 * tpa rows per anchor).
+// no <= 128 (one tile per anchor): raw logits and decoded predictions are staged in smem in the exact global layout and copied out
+// with 16-byte vectors.  Wider heads stage [128 rows][128 columns] blocks and copy each row segment to its column offset, with 16-,
+// 4- or 2-byte stores as `no` and the output alignment allow, and read their bias per tile instead of preloading it.
 // Mainloop: one K block of a tile is one wgmma batch (block_k / 16 k16 steps x MT sub-tiles, issued back to back; the dtype is a
 // template parameter, the step count a per-block switch into unrolled batches).  One batch stays in flight: after issuing batch i a
 // consumer waits (wgmma.wait_group 1) only for batch i-1 and then releases the stages i-1 was the last reader of, so the tensor
@@ -61,7 +63,12 @@ constexpr int kConsumers = 2;                          // MMA + epilogue warpgro
 constexpr int kConsumerThreads = 128 * kConsumers;
 constexpr int kThreads = 128 + kConsumerThreads;       // warpgroup 0: TMA producer (warp 0 only)
 constexpr int kMaxStages = 8;
-constexpr int kHeadN = 128;                 // head GEMM: one anchor per 128-wide N tile (no <= 128)
+constexpr int kHeadN = 128;                 // head GEMM: N tile width; an anchor takes ceil(no / 128) of them
+constexpr int kHeadMaxNo = 8192;            // head outputs per anchor (5 + nc + nm), with nc <= kHeadMaxNc
+constexpr int kHeadMaxNc = 4096;            // classes: the NMS / AP class limit
+
+// head staging: [128 rows][cols] per block, cols = no for one N tile per anchor (the global layout), else one 128-column tile
+__host__ __device__ inline int head_stage_cols(int no) { return no < kHeadN ? no : kHeadN; }
 
 enum AMode { A_LINEAR = 0, A_IM2COL = 1, A_PATCH = 2 };
 
@@ -85,7 +92,7 @@ struct ConvParams {
     uint32_t a_sub_bytes, a_stage_bytes, b_stage_bytes;
     int is_bf16, act;
     const float* bias;
-    int bias_n;                 // floats preloaded into smem
+    int bias_n;                 // floats preloaded into smem (0: a wide head reads each tile's bias from global memory)
     // EPI 0
     void* out;
     int out_pitch;
@@ -113,7 +120,7 @@ __host__ __device__ inline SmemLayout smem_layout(int epi, int no, int bias_n, i
     o += b_stages * b_bytes;
     o = (o + 1023) & ~1023u;
     L.off_out = o;
-    if (epi == 1) o += 4 * ((kBlockM * no * 2 + 1023) & ~1023u);  // head: 2 sets x {raw, decoded} blocks [128][no], global layout
+    if (epi == 1) o += 4 * ((kBlockM * head_stage_cols(no) * 2 + 1023) & ~1023u);  // head: 2 sets x {raw, decoded} blocks
     else o += stg_bytes;                                            // EPI 0 staging: per warpgroup [64 rows][BLOCK_N] (staged) or the tile (TMA)
     L.off_bias = o;
     o += ((bias_n + 3) & ~3) * 4;
@@ -609,49 +616,109 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 }
             }
         } else {
-            // ---- Detect head (models/yolo.py:95-113): N tile `nt` == anchor.  The accumulators give the raw logits AND the
-            // decoded predictions, written into two smem blocks laid out exactly like their global destinations ([128 pixels][no]
-            // contiguous per anchor), one barrier of the consumer warpgroups, then 16-byte vector copy-out.  Two staging sets
+            // ---- Detect head (models/yolo.py:95-113): N tile `nt` is tile nt % tpa of anchor nt / tpa, its output columns
+            // [c0, c0 + 128).  The accumulators give the raw logits AND the decoded predictions, written into two smem blocks, one
+            // barrier of the consumer warpgroups, then the copy-out.  One tile per anchor (no <= 128): the blocks are laid out exactly
+            // like their global destinations ([128 pixels][no] contiguous per anchor) and leave as 16-byte vectors.  Wider heads: the
+            // blocks are [128 pixels][128 columns] and every row segment goes to column c0 of its pixel's row.  Two staging sets
             // alternate per tile, so the barrier of tile i+1 also fences the reuse of tile i-1's set.
-            const uint32_t blk = (kBlockM * p.no * 2 + 1023) & ~1023u;
+            const int no = p.no;
+            const int tpa = (no + kHeadN - 1) / kHeadN;
+            const int scols = head_stage_cols(no);
+            const uint32_t blk = (kBlockM * scols * 2 + 1023) & ~1023u;
             const int set = head_set;
             head_set ^= 1;
             uint16_t* stage_raw = reinterpret_cast<uint16_t*>(smem + L.off_out + (2 * set) * blk);
             uint16_t* stage_z = reinterpret_cast<uint16_t*>(smem + L.off_out + (2 * set + 1) * blk);
-            const int no = p.no;
-            const int a = nt;
+            const int a = tpa == 1 ? nt : nt / tpa;  // (no integer division on the one-tile path)
+            const int c0 = (nt - a * tpa) * kHeadN;
+            const int ncol = min(kHeadN, no - c0);  // columns of the anchor's outputs in this tile
             const float aw = p.anchor_wh[a * 2], ah = p.anchor_wh[a * 2 + 1];
             const int m0 = ms * kBlockM;
             const int rows_here = min(kBlockM, p.M - m0);
+            // the two staging paths as separate straight-line code (a run-time test of the path inside the unrolled loop slowed the
+            // one-tile head by 9 %, measured on yolov5l's nc = 80 levels).  WIDE: the tile's bias is read from global memory once
+            // (bias_n == 0), columns are offset by c0 and only the anchor's first tile holds the box columns.
+            auto stage = [&](auto wide_path) {
+                constexpr bool WIDE = decltype(wide_path)::value;
+                float bcol[BLOCK_N / 8][2];
+                if (WIDE) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = wrow + 8 * h;
-                const int m = m0 + row;
-                int gx = 0, gy = 0;
-                if (m < p.M) { const int pix = m - fdiv(m, p.HoWo, p.rcp_HoWo) * p.HoWo; gy = fdiv(pix, p.nx, p.rcp_Wo); gx = pix - gy * p.nx; }
-                const float fgx = static_cast<float>(gx) - 0.5f, fgy = static_cast<float>(gy) - 0.5f;
+                    for (int j = 0; j < BLOCK_N / 8; ++j)
 #pragma unroll
-                for (int j = 0; j < BLOCK_N / 8; ++j) {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int o = 8 * j + ccol + e;
-                        if (o >= no) continue;
-                        const float x = acc[0][4 * j + 2 * h + e] + sBias[n0 + o];
-                        float d = x;
-                        if (o < 5 + p.nc) {
-                            const float sg = sigmoid_f(x);
-                            if (o == 0) d = (sg * 2.0f + fgx) * p.det_stride;
-                            else if (o == 1) d = (sg * 2.0f + fgy) * p.det_stride;
-                            else if (o == 2) { const float u = sg * 2.0f; d = u * u * aw; }
-                            else if (o == 3) { const float u = sg * 2.0f; d = u * u * ah; }
-                            else d = sg;
+                        for (int e = 0; e < 2; ++e) {
+                            const int o = 8 * j + ccol + e;
+                            bcol[j][e] = o < ncol ? __ldg(p.bias + n0 + o) : 0.0f;
                         }
-                        stage_raw[row * no + o] = pack1(x, bf16);
-                        stage_z[row * no + o] = pack1(d, bf16);
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = wrow + 8 * h;
+                    const int m = m0 + row;
+                    int gx = 0, gy = 0;
+                    if (m < p.M && (!WIDE || c0 == 0)) {
+                        const int pix = m - fdiv(m, p.HoWo, p.rcp_HoWo) * p.HoWo;
+                        gy = fdiv(pix, p.nx, p.rcp_Wo);
+                        gx = pix - gy * p.nx;
+                    }
+                    const float fgx = static_cast<float>(gx) - 0.5f, fgy = static_cast<float>(gy) - 0.5f;
+#pragma unroll
+                    for (int j = 0; j < BLOCK_N / 8; ++j) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int o = 8 * j + ccol + e;  // column in the tile
+                            if (o >= (WIDE ? ncol : no)) continue;
+                            const int oc = WIDE ? c0 + o : o;  // column of the anchor's outputs
+                            const float x = acc[0][4 * j + 2 * h + e] + (WIDE ? bcol[j][e] : sBias[n0 + o]);
+                            float d = x;
+                            if (oc < 5 + p.nc) {
+                                const float sg = sigmoid_f(x);
+                                if (oc == 0) d = (sg * 2.0f + fgx) * p.det_stride;
+                                else if (oc == 1) d = (sg * 2.0f + fgy) * p.det_stride;
+                                else if (oc == 2) { const float u = sg * 2.0f; d = u * u * aw; }
+                                else if (oc == 3) { const float u = sg * 2.0f; d = u * u * ah; }
+                                else d = sg;
+                            }
+                            const int si = row * (WIDE ? kHeadN : no) + o;
+                            stage_raw[si] = pack1(x, bf16);
+                            stage_z[si] = pack1(d, bf16);
+                        }
                     }
                 }
-            }
+            };
+            if (tpa > 1) stage(std::true_type{});
+            else stage(std::false_type{});
             named_bar_sync(1, kConsumerThreads);
+            if (tpa > 1) {
+                // wide head: row r of the block is ncol elements at column c0 of global row (b, a, pix) of raw and (b, z_row0 + a
+                // HoWo + pix) of z.  16-byte vectors when no % 8 == 0 (c0 is a multiple of 128, so every segment is then aligned),
+                // 4-byte words when no is even, else half-words.
+#pragma unroll 1
+                for (int which = 0; which < 2; ++which) {
+                    uint16_t* base = reinterpret_cast<uint16_t*>(which == 0 ? p.raw : p.z);
+                    const uint16_t* src = which == 0 ? stage_raw : stage_z;
+                    auto copy = [&](auto vec) {
+                        constexpr int V = decltype(vec)::value;  // elements per store
+                        using T = std::conditional_t<V == 8, uint4, std::conditional_t<V == 2, uint32_t, uint16_t>>;
+                        const int segs = ncol / V;
+                        // one warp per row: the row's destination is computed once, the lanes store its segment
+                        for (int r = ct >> 5; r < rows_here; r += kConsumerThreads / 32) {
+                            const int m = m0 + r;
+                            const int b = fdiv(m, p.HoWo, p.rcp_HoWo), pix = m - b * p.HoWo;
+                            const long long grow = which == 0 ? (static_cast<long long>(b) * p.na + a) * p.HoWo + pix
+                                                              : static_cast<long long>(b) * p.z_rows + p.z_row0 + static_cast<long long>(a) * p.HoWo + pix;
+                            T* d = reinterpret_cast<T*>(base + grow * no + c0);
+                            const T* s = reinterpret_cast<const T*>(src + r * kHeadN);
+                            for (int c = lane; c < segs; c += 32) d[c] = s[c];
+                        }
+                    };
+                    const uintptr_t ba = reinterpret_cast<uintptr_t>(base);
+                    if ((no & 7) == 0 && (ba & 15) == 0) copy(std::integral_constant<int, 8>{});
+                    else if ((no & 1) == 0 && (ba & 3) == 0) copy(std::integral_constant<int, 2>{});
+                    else copy(std::integral_constant<int, 1>{});
+                }
+                continue;
+            }
             // copy out: for each image the tile touches, rows [r_lo, r_hi) are one contiguous global block per output
             const int b_lo = fdiv(m0, p.HoWo, p.rcp_HoWo), b_hi = fdiv(m0 + rows_here - 1, p.HoWo, p.rcp_HoWo);
             for (int b = b_lo; b <= b_hi; ++b) {
@@ -794,8 +861,9 @@ int finish_plan(PlanCommon& pc, int block_n, int epi, int mt, int cluster = 1) {
     p.a_stage_bytes = mt * p.a_sub_bytes;
     if (p.patch_pw > 0) p.a_stage_bytes = static_cast<uint32_t>(p.th + p.kh - 1) * p.patch_pw * p.block_k * 2;  // one shared patch per stage
     p.num_m_super = (p.num_m_tiles + mt - 1) / mt;
-    p.num_n_tiles = epi == 1 ? p.na : (p.N + block_n - 1) / block_n;
-    p.bias_n = p.num_n_tiles * block_n;
+    p.num_n_tiles = (p.N + block_n - 1) / block_n;  // head: na * ceil(no / 128), p.N being the padded na * npad rows
+    // a wide head reads each tile's bias in the epilogue: na * npad floats would not fit beside the staging at the class limit
+    p.bias_n = (epi == 1 && p.no > kHeadN) ? 0 : p.num_n_tiles * block_n;
     const uint32_t budget = 225 * 1024 - 1024;
     const bool patch = p.a_mode == A_PATCH;
     int a_st = 0, b_st = 0;
@@ -1132,8 +1200,9 @@ extern "C" Y5_API int y5_detect_plan_create(const y5_detect_desc* d, y5_detect_p
     *out = nullptr;
     if (!d || !d->in || !d->weight || !d->bias || !d->raw || !d->z) return set_error(Y5_E_INVALID, "detect: null pointer");
     if (d->dtype != Y5_F16 && d->dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "detect: dtype must be fp16/bf16");
-    if (d->na < 1 || d->na > 4 || d->no < 6 || d->no > kHeadN || d->nc < 1 || 5 + d->nc > d->no)
-        return set_error(Y5_E_UNSUPPORTED, "detect: na %d no %d nc %d unsupported (no <= %d, na <= 4)", d->na, d->no, d->nc, kHeadN);
+    if (d->na < 1 || d->na > 4 || d->no < 6 || d->no > kHeadMaxNo || d->nc < 1 || d->nc > kHeadMaxNc || 5 + d->nc > d->no)
+        return set_error(Y5_E_UNSUPPORTED, "detect: na %d no %d nc %d unsupported (no <= %d, nc <= %d, na <= 4)", d->na, d->no, d->nc,
+                         kHeadMaxNo, kHeadMaxNc);
     if (d->in_pitch < d->in_c || d->in_pitch % 8 || !aligned16(d->in) || !aligned16(d->weight))
         return set_error(Y5_E_INVALID, "detect: bad input view");
     const int64_t M64 = static_cast<int64_t>(d->batch) * d->ny * d->nx;
@@ -1144,7 +1213,7 @@ extern "C" Y5_API int y5_detect_plan_create(const y5_detect_desc* d, y5_detect_p
     std::memset(&pc.p, 0, sizeof(pc.p));
     ConvParams& p = pc.p;
     p.M = static_cast<int>(M64);
-    p.N = d->na * kHeadN;  // weights / bias are packed with every anchor padded to kHeadN rows
+    p.N = d->na * kHeadN * ((d->no + kHeadN - 1) / kHeadN);  // weights / bias are packed with every anchor padded to npad rows
     p.kh = p.kw = 1;
     p.Ho = d->ny; p.Wo = d->nx; p.HoWo = d->ny * d->nx;
     p.rcp_HoWo = 1.0f / static_cast<float>(p.HoWo);

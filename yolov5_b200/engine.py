@@ -26,6 +26,10 @@ from . import _lib
 from ._lib import ConvDesc, DetectDesc
 
 BN_EPS_DEFAULT = 1e-3
+# Detect head GEMM (conv_gemm.cu): an anchor's no = 5 + nc + nm outputs are ceil(no / HEAD_N) N tiles of HEAD_N columns
+HEAD_N = 128
+HEAD_MAX_NO = 8192  # kHeadMaxNo
+HEAD_MAX_NC = 4096  # kHeadMaxNc: the NMS / AP class limit
 
 
 class View:
@@ -344,23 +348,24 @@ class Program:
 
     def lower_detect(self, m, xs: list[View], name):
         na, no, nc = m.na, m.no, m.nc
+        if no > HEAD_MAX_NO or nc > HEAD_MAX_NC:
+            raise NotImplementedError(f"y5b200: Detect with no={no} nc={nc}: the head takes no <= {HEAD_MAX_NO} outputs per anchor "
+                                      f"and nc <= {HEAD_MAX_NC} classes")
+        npad = -(-no // HEAD_N) * HEAD_N  # rows per anchor in the packed weights: ceil(no / 128) N tiles
         self.z_rows = sum(na * v.h * v.w for v in xs)
         self.det_shapes = [(self.B, na, v.h, v.w, no) for v in xs]
         row0 = 0
         for i, v in enumerate(xs):
             conv = m.m[i]
-            HEAD_N = 128  # kHeadN in conv_gemm.cu: one anchor per 128-wide N tile
-            if no > HEAD_N:
-                raise NotImplementedError(f"y5b200: Detect with no={no} > {HEAD_N} outputs per anchor")
-            # every anchor's `no` rows padded to HEAD_N: one fold_pack launch per anchor (weights + bias, no BatchNorm)
+            # every anchor's `no` rows padded to npad: one fold_pack launch per anchor (weights + bias, no BatchNorm)
             bk = C.c_int32(self.block_k(v.c, na * no, self.B * v.h * v.w))
             ipad = (v.c + bk.value - 1) // bk.value * bk.value
-            wp = torch.empty(na * HEAD_N, 1, 1, ipad, dtype=self.dtype, device=self.device)
-            bias = torch.empty(na * HEAD_N, dtype=torch.float32, device=self.device)
+            wp = torch.empty(na * npad, 1, 1, ipad, dtype=self.dtype, device=self.device)
+            bias = torch.empty(na * npad, dtype=torch.float32, device=self.device)
             w4 = conv.weight.detach().contiguous().view(na, no, v.c, 1, 1)
             b2 = conv.bias.detach().contiguous().view(na, no)
             for a_i in range(na):
-                self.fold_pack_into([(w4[a_i], b2[a_i], None)], wp, bias, a_i * HEAD_N, ipad, pad_rows_to=HEAD_N)
+                self.fold_pack_into([(w4[a_i], b2[a_i], None)], wp, bias, a_i * npad, ipad, pad_rows_to=npad)
             self._keep += [wp, bias, w4, b2]
             d = DetectDesc()
             d.inp, d.in_pitch = v.ptr, v.pitch
