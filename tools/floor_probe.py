@@ -11,7 +11,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from yolov5_b200 import _lib
-from yolov5_b200.engine import pack_weight
+from yolov5_b200.engine import ConvInput, conv_desc, pack_weight
 
 
 def plan_for(dev, dtype, M, cin, cout, k):
@@ -25,10 +25,7 @@ def plan_for(dev, dtype, M, cin, cout, k):
     w = torch.randn(cout, cin, k, k) / (cin * k * k) ** 0.5
     wp = pack_weight(w, bk.value, dtype).to(dev)
     b = torch.zeros(cout, device=dev)
-    d = _lib.ConvDesc()
-    d.inp, d.in_pitch, d.batch, d.in_h, d.in_w, d.in_c = x.data_ptr(), cin, 1, H, W, cin
-    d.weight, d.bias, d.out, d.out_pitch, d.out_c = wp.data_ptr(), b.data_ptr(), y.data_ptr(), cout, cout
-    d.ksize, d.stride, d.pad, d.act, d.dtype, d.block_k = k, 1, k // 2, 1, _lib.dtype_code(dtype), bk.value
+    d = conv_desc(ConvInput(x.data_ptr(), cin, 1, H, W, cin), wp, b, bk.value, y.data_ptr(), cout, k, 1, k // 2, True, dtype)
     plan = C.c_void_p()
     _lib.check(lib.y5_conv_plan_create(C.byref(d), C.byref(plan)))
     return plan, (x, y, wp, b)

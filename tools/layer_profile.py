@@ -18,24 +18,26 @@ size = int(sys.argv[3]) if len(sys.argv) > 3 else 640
 dt = {"fp16": torch.float16, "bf16": torch.bfloat16}[sys.argv[4] if len(sys.argv) > 4 else "fp16"]
 dev = torch.device("cuda:0")
 
-# record per-conv metadata by wrapping Program.conv
+# record per-conv metadata by wrapping Program.emit_conv
 meta = {}
-_orig = engine.Program.conv
+_orig = engine.Program.emit_conv
 
 
-def conv(self, x, out, w, b, k, s, p, act, residual=None, name="conv", virt=None, packed=None):
+def emit_conv(self, d, name, keep):
     n0 = len(self.ops)
-    _orig(self, x, out, w, b, k, s, p, act, residual, name, virt, packed)
-    m = self.B * out.h * out.w
-    if virt is None:
-        cin, kk, in_el = x.c, k * k, self.B * x.h * x.w * x.c
-    else:  # stem: count the real 6x6x3 filter and the image
+    _orig(self, d, name, keep)
+    k, s, n = d.ksize, d.stride, d.out_c
+    kw, pad_w = (d.kw, d.pad_w) if d.kw else (k, d.pad)
+    m = d.batch * ((d.in_h + 2 * d.pad - k) // s + 1) * ((d.in_w + 2 * pad_w - kw) // s + 1)
+    if d.in_x_stride:  # stem: count the real 6x6x3 filter and the image
         cin, kk, in_el = 3, 36, self.B * self.H * self.W * 3
-    meta[n0] = dict(name=name, M=m, N=out.c, K=cin * kk, k=k, s=s, flops=2 * m * out.c * cin * kk,
-                    bytes=2 * (in_el + m * out.c) + 2 * out.c * cin * kk + (2 * m * out.c if residual is not None else 0))
+    else:
+        cin, kk, in_el = d.in_c, k * k, d.batch * d.in_h * d.in_w * d.in_c
+    meta[n0] = dict(name=name, M=m, N=n, K=cin * kk, k=k, s=s, flops=2 * m * n * cin * kk,
+                    bytes=2 * (in_el + m * n) + 2 * n * cin * kk + (2 * m * n if d.residual else 0))
 
 
-engine.Program.conv = conv
+engine.Program.emit_conv = emit_conv
 torch.manual_seed(0)
 m = DetectionModel(name).to(dev, dt).eval()
 x = torch.rand(bs, 3, size, size, device=dev).to(dt)

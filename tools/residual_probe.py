@@ -14,7 +14,7 @@ sys.path.insert(0, ROOT)
 import torch
 
 from yolov5_b200 import _lib
-from yolov5_b200.engine import pack_weight
+from yolov5_b200.engine import ConvInput, conv_desc, pack_weight
 
 # (model, batch, dtype, [(map size, c_)]) -- the 3x3 c_ -> c_ m{j}.cv2 convs of backbone layers 2, 4, 6 and 8
 SHAPES = [("yolov5l", 64, torch.bfloat16, [(160, 64), (80, 128), (40, 256), (20, 512)]),
@@ -70,14 +70,8 @@ def main():
             bias = torch.zeros(c, dtype=torch.float32, device=dev)
             plans = {}
             for v in VARIANTS:
-                d = _lib.ConvDesc()
-                d.inp, d.in_pitch = x.data_ptr(), c
-                d.batch, d.in_h, d.in_w, d.in_c = bs, hw, hw, c
-                d.weight, d.bias = wp.data_ptr(), bias.data_ptr()
-                d.out, d.out_pitch, d.out_c = cat.data_ptr(), 2 * c, c
-                d.residual, d.res_pitch = {"none": (None, 0), "separate": (sep.data_ptr(), 2 * c), "in-place": (cat.data_ptr(), 2 * c)}[v]
-                d.ksize, d.stride, d.pad = 3, 1, 1
-                d.act, d.dtype, d.block_k = _lib.ACT_SILU, _lib.dtype_code(dt), bk.value
+                res = {"none": (None, 0), "separate": (sep.data_ptr(), 2 * c), "in-place": (cat.data_ptr(), 2 * c)}[v]
+                d = conv_desc(ConvInput(x.data_ptr(), c, bs, hw, hw, c), wp, bias, bk.value, cat.data_ptr(), 2 * c, 3, 1, 1, True, dt, *res)
                 plan = C.c_void_p()
                 _lib.check(lib.y5_conv_plan_create(C.byref(d), C.byref(plan)), "plan")
                 plans[v] = plan

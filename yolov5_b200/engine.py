@@ -19,11 +19,12 @@ from __future__ import annotations
 import ctypes as C
 import math
 import os
+from collections import namedtuple
 
 import torch
 
 from . import _lib
-from ._lib import ConvDesc, DetectDesc
+from ._lib import ConvDesc, DetectDesc, WgradDesc
 
 BN_EPS_DEFAULT = 1e-3
 # Detect head GEMM (conv_gemm.cu): an anchor's no = 5 + nc + nm outputs are ceil(no / HEAD_N) N tiles of HEAD_N columns
@@ -95,6 +96,88 @@ def stem_weight_s2d(w: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def stem_weight_wide(w3: torch.Tensor) -> torch.Tensor:
+    """(O,16,3,3) space-to-depth stem filter -> the (O,48,3,1) filter of its wide-pixel form: [o][s*16+c][r][0] = w3[o][c][r][s]."""
+    return w3.permute(0, 3, 1, 2).reshape(w3.shape[0], 48, 3, 1)
+
+
+def stem_weight_narrow(wv: torch.Tensor) -> torch.Tensor:
+    """Inverse of stem_weight_wide: (O,48,3,1) -> (O,16,3,3), a view."""
+    return wv.view(wv.shape[0], 3, 16, 3).permute(0, 2, 3, 1)
+
+
+def stem_buffer(b: int, h: int, w: int, dtype: torch.dtype, device) -> torch.Tensor:
+    """Zeroed [B][H/2][W/2 + 2][16] buffer for the space-to-depth cells of a (B,3,H,W) image, with one zero cell at each end
+    of a row (stem_geom reads them as padding); stem_s2d writes the inner cells only."""
+    return torch.zeros(b, h // 2, w // 2 + 2, 16, dtype=dtype, device=device)
+
+
+def stem_s2d(img: torch.Tensor, out: torch.Tensor) -> None:
+    """y5_stem_s2d of a (B,3,H,W) image into `out`, NHWC [B][H/2][row][16]: a stem_buffer (row W/2 + 2, cells from x = 1) or a
+    dense one (row W/2)."""
+    b, _, h, w = img.shape
+    row = out.shape[2]
+    img = img.contiguous()
+    _lib.check(_lib.lib().y5_stem_s2d(img.data_ptr(), _lib.dtype_code(img.dtype), out.data_ptr(), _lib.dtype_code(out.dtype), b, h, w, row,
+                                      (row - w // 2) // 2, C.c_void_p(_lib.stream_ptr(out.device))), "stem_s2d")
+
+
+_block_k_cache: dict = {}
+
+
+def block_k(cin: int, cout: int, m_rows: int) -> int:
+    """y5_conv_pick's K block for a cin -> cout conv over m_rows output pixels (weights are packed to it)."""
+    key = (cin, cout, m_rows)
+    v = _block_k_cache.get(key)
+    if v is None:  # a pure function of the shape: one library call per distinct layer shape
+        bk = C.c_int32()
+        _lib.check(_lib.lib().y5_conv_pick(cin, cout, m_rows, C.byref(bk), None), "conv_pick")
+        v = _block_k_cache[key] = bk.value
+    return v
+
+
+# The input-view fields of y5_conv_desc and y5_wgrad_desc (include/y5b200.h): an NHWC view of in_c channels at element pointer
+# `inp`, in_pitch elements per pixel.  The optional ones (0: the plain case) describe the strided views of stem_geom.
+ConvInput = namedtuple("ConvInput", "inp in_pitch batch in_h in_w in_c kw pad_w in_x_stride in_y_stride in_n_stride", defaults=(0,) * 5)
+
+
+def stem_geom(buf: torch.Tensor, wide: bool) -> ConvInput:
+    """The stem conv's input over a stem_buffer: a 3x3/s1/p1 conv of the 16-channel cells.  Three horizontally adjacent cells are
+    contiguous, so the wide form reads overlapping 48-channel "wide pixels" (x stride 16) from the left padding cell on with a
+    3x1 filter and no horizontal padding: 3 taps of K=48 instead of 9 of K=16.  The narrow form is the 3x3x16 view of the cells."""
+    b, h2, row, _ = buf.shape
+    geom = dict(in_pitch=16, batch=b, in_h=h2, in_w=row - 2, in_x_stride=16, in_y_stride=row * 16, in_n_stride=h2 * row * 16)
+    if wide:
+        return ConvInput(inp=buf.data_ptr(), in_c=48, kw=1, pad_w=0, **geom)
+    return ConvInput(inp=buf.data_ptr() + 16 * buf.element_size(), in_c=16, kw=3, pad_w=1, **geom)
+
+
+def conv_desc(x: ConvInput, wp: torch.Tensor, bias: torch.Tensor, bk: int, out: int, out_pitch: int, k: int, s: int, p: int,
+              act: bool, dtype: torch.dtype, residual: int | None = None, res_pitch: int = 0) -> ConvDesc:
+    """y5_conv_desc of out = act(conv(x, w) + bias [+ residual]).  wp: w packed [cout][k][kw][cin_pad] for K block bk (pack_weight,
+    fold_pack); bias: fp32 [cout]; out / residual: element pointers of NHWC views with their pitches."""
+    d = ConvDesc()
+    d.inp, d.in_pitch, d.batch, d.in_h, d.in_w, d.in_c, d.kw, d.pad_w, d.in_x_stride, d.in_y_stride, d.in_n_stride = x
+    d.weight, d.bias = wp.data_ptr(), bias.data_ptr()
+    d.out, d.out_pitch, d.out_c = out, out_pitch, wp.shape[0]
+    d.residual, d.res_pitch = residual, res_pitch
+    d.ksize, d.stride, d.pad = k, s, p
+    d.act = _lib.ACT_SILU if act else _lib.ACT_NONE
+    d.dtype, d.block_k = _lib.dtype_code(dtype), bk
+    return d
+
+
+def wgrad_desc(x: ConvInput, dy: int, dy_pitch: int, dw: torch.Tensor, k: int, s: int, p: int, dtype: torch.dtype) -> WgradDesc:
+    """y5_wgrad_desc of the fp32 weight gradient dw ([cout][k][kw][cin], KRSC) of a conv over x, from dy (element pointer, pitch)."""
+    d = WgradDesc()
+    d.inp, d.in_pitch, d.batch, d.in_h, d.in_w, d.in_c, d.kw, d.pad_w, d.in_x_stride, d.in_y_stride, d.in_n_stride = x
+    d.dout, d.dout_pitch, d.out_c = dy, dy_pitch, dw.shape[0]
+    d.dweight = dw.data_ptr()
+    d.ksize, d.stride, d.pad = k, s, p
+    d.dtype = _lib.dtype_code(dtype)
+    return d
+
+
 class _Op:
     """One launch: (function, ctypes args...) bound at plan time; run(stream) issues it."""
 
@@ -139,18 +222,13 @@ class Program:
         return View(self.new_buf(h, w, c), 0, c)
 
     # ------------------------------------------------------------------ op emitters
-    def block_k(self, cin: int, cout: int, m_rows: int) -> int:
-        bk = C.c_int32()
-        _lib.check(self.lib.y5_conv_pick(cin, cout, m_rows, C.byref(bk), None), "conv_pick")
-        return bk.value
-
     def fold_pack(self, parts, m_rows: int):
         """Folded + packed weights of one GEMM from module parameters, one y5_fold_pack launch per part (no ATen arithmetic).
         parts: list of (weight (O,I,kh,kw) tensor, conv bias | None, bn | None); several parts stack along the output channels
         (C3's cv1 | cv2).  Returns (packed [sum O][kh][kw][I_pad] in the activation dtype, fp32 bias [sum O], block_k)."""
         cin, kh, kw = parts[0][0].shape[1:]
         cout = sum(w.shape[0] for w, _, _ in parts)
-        bk = self.block_k(cin, cout, m_rows)
+        bk = block_k(cin, cout, m_rows)
         ipad = (cin + bk - 1) // bk * bk
         wp = torch.empty(cout, kh, kw, ipad, dtype=self.dtype, device=self.device)
         bias = torch.empty(cout, dtype=torch.float32, device=self.device)
@@ -188,58 +266,31 @@ class Program:
             self._keep += keep  # the launch is asynchronous: temporaries must outlive it
             row0 += rows
 
-    def conv(self, x: View, out: View, w_fp32, b_fp32, k: int, s: int, p: int, act: bool,
-             residual: View | None = None, name: str = "conv", virt=None, packed=None):
-        """Emit one fused conv.  Weights come either as fp32 tensors (w_fp32 OIHW already folded, b_fp32) that are packed here,
-        or pre-packed by fold_pack: packed = (wp, bias, block_k, cin).  `virt` (stem only) = dict(ptr, in_c, in_w, in_h, x_stride,
-        y_stride, n_stride, kw, pad_w): a strided "wide pixel" view of the input and a non-square filter, see y5_conv_desc in
-        include/y5b200.h."""
-        cout = out.c
-        if virt is None:
-            cin, in_h, in_w, kw = x.c, x.h, x.w, k
-            ho, wo = (x.h + 2 * p - k) // s + 1, (x.w + 2 * p - k) // s + 1
-        else:
-            cin, in_h, in_w, kw = virt["in_c"], virt["in_h"], virt["in_w"], virt["kw"]
-            ho, wo = (in_h + 2 * p - k) // s + 1, (in_w + 2 * virt["pad_w"] - kw) // s + 1
-        assert (ho, wo) == (out.h, out.w), (name, ho, wo, out.h, out.w)
-        m_rows = self.B * ho * wo
-        bk, bn = C.c_int32(), C.c_int32()
-        bn.value = int(os.environ.get("Y5_FORCE_BLOCK_N", "0"))  # 0: the library's tile cost model decides (block_n, MT)
-        if packed is None:
-            assert w_fp32.shape == (cout, cin, k, kw), (w_fp32.shape, cout, cin, k, kw)
-            bk.value = self.block_k(cin, cout, m_rows)
-            wp = pack_weight(w_fp32, bk.value, self.dtype)
-            bias = b_fp32.to(torch.float32).contiguous()
-        else:
-            wp, bias, bk.value, pc = packed
-            assert pc == cin and wp.shape[0] == cout and wp.shape[1:3] == (k, kw), (name, wp.shape, cout, cin, k, kw)
-        self._keep += [wp, bias]
-        d = ConvDesc()
-        if virt is None:
-            d.inp, d.in_pitch = x.ptr, x.pitch
-        else:
-            d.inp, d.in_pitch = virt["ptr"], virt["x_stride"]
-            d.in_x_stride, d.in_y_stride, d.in_n_stride = virt["x_stride"], virt["y_stride"], virt["n_stride"]
-            d.kw, d.pad_w = kw, virt["pad_w"]
-        d.batch, d.in_h, d.in_w, d.in_c = self.B, in_h, in_w, cin
-        d.weight, d.bias = wp.data_ptr(), bias.data_ptr()
-        d.out, d.out_pitch, d.out_c = out.ptr, out.pitch, cout
-        d.residual = residual.ptr if residual is not None else None
-        d.res_pitch = residual.pitch if residual is not None else 0
-        d.ksize, d.stride, d.pad = k, s, p
-        d.act = _lib.ACT_SILU if act else _lib.ACT_NONE
-        d.dtype, d.block_k, d.block_n = self.dt_code, bk.value, bn.value
+    def emit_conv(self, d: ConvDesc, name: str, keep):
+        """Plan the conv of descriptor d and append its launch; `keep` (its weights and bias) lives as long as the program."""
+        self._keep += keep
+        d.block_n = int(os.environ.get("Y5_FORCE_BLOCK_N", "0"))  # 0: the library's tile cost model decides (block_n, MT)
         d.a_mode = int(os.environ.get("Y5_FORCE_A_MODE", "0"))
-        if d.a_mode == 2 and s != 1:
+        if d.a_mode == 2 and d.stride != 1:
             d.a_mode = 0
         plan = C.c_void_p()
         _lib.check(self.lib.y5_conv_plan_create(C.byref(d), C.byref(plan)), f"conv_plan_create[{name}]")
         self._plans.append((self.lib.y5_conv_plan_destroy, plan))
         self.ops.append(_Op(name, self.lib.y5_conv_plan_run, (plan,)))
-        if virt is None:
-            self.flops += 2 * m_rows * cout * cin * k * k
-            self.act_bytes += 2 * (self.B * x.h * x.w * x.c + m_rows * cout)
-            self.weight_bytes += 2 * cout * cin * k * k
+
+    def conv(self, x: View, out: View, packed, k: int, s: int, p: int, act: bool, residual: View | None = None, name: str = "conv"):
+        """Emit one fused conv of view x into view out; packed = (wp, bias, block_k) as fold_pack returns them."""
+        wp, bias, bk = packed
+        ho, wo = (x.h + 2 * p - k) // s + 1, (x.w + 2 * p - k) // s + 1
+        cout, cin = out.c, x.c
+        assert (ho, wo) == (out.h, out.w) and wp.shape == (cout, k, k, -(-cin // bk) * bk), (name, ho, wo, out.h, out.w, wp.shape, cin)
+        res = (residual.ptr, residual.pitch) if residual is not None else (None, 0)
+        d = conv_desc(ConvInput(x.ptr, x.pitch, self.B, x.h, x.w, cin), wp, bias, bk, out.ptr, out.pitch, k, s, p, act, self.dtype, *res)
+        self.emit_conv(d, name, (wp, bias))
+        m_rows = self.B * ho * wo
+        self.flops += 2 * m_rows * cout * cin * k * k
+        self.act_bytes += 2 * (self.B * x.h * x.w * cin + m_rows * cout)
+        self.weight_bytes += 2 * cout * cin * k * k
 
     def conv_module(self, m, x: View, out: View, residual: View | None = None, name="conv"):
         """m: models.common.Conv (conv + bn + act) in its fused or unfused state."""
@@ -250,8 +301,8 @@ class Program:
         if m.conv.groups != 1 or m.conv.dilation[0] != 1:
             raise NotImplementedError("y5b200: grouped / dilated convolutions are outside the YOLOv5 n..x hot path")
         ho, wo = (x.h + 2 * p - k) // s + 1, (x.w + 2 * p - k) // s + 1
-        wp, bias, bk = self.fold_pack([(m.conv.weight, m.conv.bias, getattr(m, "bn", None))], self.B * ho * wo)
-        self.conv(x, out, None, None, k, s, p, act, residual, name, packed=(wp, bias, bk, x.c))
+        packed = self.fold_pack([(m.conv.weight, m.conv.bias, getattr(m, "bn", None))], self.B * ho * wo)
+        self.conv(x, out, packed, k, s, p, act, residual, name)
 
     def out_hw(self, m, x: View):
         k, s, p = m.conv.kernel_size[0], m.conv.stride[0], m.conv.padding[0]
@@ -268,28 +319,23 @@ class Program:
             if self.H % 2 or self.W % 2:
                 raise ValueError("y5b200: image height and width must be even")
             h2, w2 = self.H // 2, self.W // 2
-            # space-to-depth buffer with one zero cell left and right of every row: [B][h2][w2+2][16]
-            s2d_buf = torch.zeros(self.B, h2, w2 + 2, 16, dtype=self.dtype, device=self.device)
-            self._keep.append(s2d_buf)
-            self.stem_in = s2d_buf
+            self.stem_in = stem_buffer(self.B, self.H, self.W, self.dtype, self.device)
             w, b = fold_conv_bn(m.conv, getattr(m, "bn", None))
             out = out or self.new_view(h2, w2, m.conv.out_channels)
             w3 = stem_weight_s2d(w)  # (O,16,3,3): 3x3/s1/p1 over the 16-channel cells
             act = isinstance(m.act, torch.nn.SiLU)
-            # 3 horizontally adjacent cells are contiguous in memory (48 channels): run the stem as a 3x1 conv over
-            # overlapping 48-channel "wide pixels" (x stride 16 elements) -> 3 taps of K=48 instead of 9 taps of K=16
-            wv = w3.permute(0, 3, 1, 2).reshape(w3.shape[0], 48, 3, 1)  # [o][s*16+c][r][0] = w3[o][c][r][s]
-            virt = dict(ptr=s2d_buf.data_ptr(), in_c=48, in_w=w2, in_h=h2, x_stride=16, y_stride=(w2 + 2) * 16,
-                        n_stride=h2 * (w2 + 2) * 16, kw=1, pad_w=0)
-            n_before = len(self.ops)
+
+            def stem_conv(wide: bool, form: str):
+                wv = stem_weight_wide(w3) if wide else w3
+                bk = block_k(wv.shape[1], wv.shape[0], self.B * h2 * w2)
+                wp = pack_weight(wv, bk, self.dtype)
+                d = conv_desc(stem_geom(self.stem_in, wide), wp, b, bk, out.ptr, out.pitch, 3, 1, 1, act, self.dtype)
+                self.emit_conv(d, f"{name}(s2d {form})", (wp, b))
+
             try:
-                self.conv(None, out, wv, b, 3, 1, 1, act, None, name + "(s2d 3x1x48)", virt=virt)
-            except RuntimeError:
-                # driver refused the overlapping-stride tensor map: plain 3x3 over 16-channel cells of the padded buffer
-                del self.ops[n_before:]
-                virt = dict(ptr=s2d_buf.data_ptr() + 16 * s2d_buf.element_size(), in_c=16, in_w=w2, in_h=h2, x_stride=16,
-                            y_stride=(w2 + 2) * 16, n_stride=h2 * (w2 + 2) * 16, kw=3, pad_w=1)
-                self.conv(None, out, w3, b, 3, 1, 1, act, None, name + "(s2d 3x3x16)", virt=virt)
+                stem_conv(True, "3x1x48")
+            except RuntimeError:  # driver refused the overlapping-stride tensor map: plain 3x3 over the padded buffer's cells
+                stem_conv(False, "3x3x16")
             cout = m.conv.out_channels
             self.flops += 2 * self.B * h2 * w2 * cout * 3 * 36
             self.act_bytes += 2 * (self.B * self.H * self.W * 3 + self.B * h2 * w2 * cout)
@@ -304,9 +350,9 @@ class Program:
         c_ = m.cv1.conv.out_channels
         cat = self.new_view(x.h, x.w, 2 * c_)
         # cv1 | cv2 stacked along the output channels: one GEMM, result is already the concat layout
-        wp, bias, bk = self.fold_pack([(m.cv1.conv.weight, m.cv1.conv.bias, getattr(m.cv1, "bn", None)),
-                                       (m.cv2.conv.weight, m.cv2.conv.bias, getattr(m.cv2, "bn", None))], self.B * x.h * x.w)
-        self.conv(x, cat, None, None, 1, 1, 0, True, None, f"{name}.cv1|cv2", packed=(wp, bias, bk, x.c))
+        packed = self.fold_pack([(m.cv1.conv.weight, m.cv1.conv.bias, getattr(m.cv1, "bn", None)),
+                                 (m.cv2.conv.weight, m.cv2.conv.bias, getattr(m.cv2, "bn", None))], self.B * x.h * x.w)
+        self.conv(x, cat, packed, 1, 1, 0, True, None, f"{name}.cv1|cv2")
         a = cat.slice(0, c_)
         if len(m.m):
             tmp = self.new_view(x.h, x.w, c_)
@@ -358,8 +404,8 @@ class Program:
         for i, v in enumerate(xs):
             conv = m.m[i]
             # every anchor's `no` rows padded to npad: one fold_pack launch per anchor (weights + bias, no BatchNorm)
-            bk = C.c_int32(self.block_k(v.c, na * no, self.B * v.h * v.w))
-            ipad = (v.c + bk.value - 1) // bk.value * bk.value
+            bk = block_k(v.c, na * no, self.B * v.h * v.w)
+            ipad = (v.c + bk - 1) // bk * bk
             wp = torch.empty(na * npad, 1, 1, ipad, dtype=self.dtype, device=self.device)
             bias = torch.empty(na * npad, dtype=torch.float32, device=self.device)
             w4 = conv.weight.detach().contiguous().view(na, no, v.c, 1, 1)
@@ -381,7 +427,7 @@ class Program:
             anc = (m.anchors[i].detach().float().cpu() * stride).reshape(-1).tolist()
             for q in range(8):
                 d.anchor_wh[q] = anc[q] if q < len(anc) else 0.0
-            d.dtype, d.block_k = self.dt_code, bk.value
+            d.dtype, d.block_k = self.dt_code, bk
             plan = C.c_void_p()
             _lib.check(self.lib.y5_detect_plan_create(C.byref(d), C.byref(plan)), f"detect_plan_create[{name}.{i}]")
             self._plans.append((self.lib.y5_detect_plan_destroy, plan))
@@ -405,13 +451,13 @@ class Program:
         lin = m.linear
         nc, cin = lin.weight.shape
         ncpad = _pad8(nc)
-        bk = self.block_k(cin, ncpad, self.B)
+        bk = block_k(cin, ncpad, self.B)
         ipad = (cin + bk - 1) // bk * bk
         wp = torch.empty(ncpad, 1, 1, ipad, dtype=self.dtype, device=self.device)
         bias = torch.empty(ncpad, dtype=torch.float32, device=self.device)
         self.fold_pack_into([(lin.weight.view(nc, cin, 1, 1), lin.bias, None)], wp, bias, 0, ipad, pad_rows_to=ncpad)
         out = self.new_view(1, 1, ncpad)
-        self.conv(pooled, out, None, None, 1, 1, 0, False, None, f"{name}.linear", packed=(wp, bias, bk, cin))
+        self.conv(pooled, out, (wp, bias, bk), 1, 1, 0, False, None, f"{name}.linear")
         self.cls_view = View(out.buf, 0, nc)
 
     # ------------------------------------------------------------------ builders
@@ -559,11 +605,8 @@ class Program:
     def _run_body(self, img: torch.Tensor, use_graph: bool) -> int:
         """stem space-to-depth of `img`, then the fixed part (graph replay); returns the stream pointer."""
         assert img.is_cuda and img.shape == (self.B, 3, self.H, self.W), (img.shape, (self.B, 3, self.H, self.W))
-        if not img.is_contiguous():
-            img = img.contiguous()
+        stem_s2d(img, self.stem_in)
         st = _lib.stream_ptr(self.device)
-        _lib.check(self.lib.y5_stem_s2d(img.data_ptr(), _lib.dtype_code(img.dtype), self.stem_in.data_ptr(), self.dt_code, self.B,
-                                        self.H, self.W, self.W // 2 + 2, 1, C.c_void_p(st)), "stem_s2d")
         if use_graph and os.environ.get("Y5_NO_GRAPH") != "1":
             if self.graph is None:
                 self.capture()

@@ -27,8 +27,9 @@ import os
 import torch
 
 from . import _lib
-from ._lib import ConvDesc, WgradDesc
-from .engine import pack_weight
+from .engine import (ConvInput, conv_desc, pack_weight, stem_buffer, stem_geom, stem_s2d, stem_weight_narrow, stem_weight_wide,
+                     wgrad_desc)
+from .engine import block_k as _block_k  # the shared, cached y5_conv_pick lookup
 
 
 def _st(dev):
@@ -69,19 +70,6 @@ def _zero_bias(n: int, device) -> torch.Tensor:
     if t is None:
         t = _zero_bias_cache[key] = torch.zeros(n, dtype=torch.float32, device=device)
     return t
-
-
-_block_k_cache: dict = {}
-
-
-def _block_k(cin: int, cout: int, m_rows: int) -> int:
-    key = (cin, cout, m_rows)
-    v = _block_k_cache.get(key)
-    if v is None:  # a pure function of the shape: one library call per distinct layer shape, not two per layer per step
-        bk = C.c_int32()
-        _lib.check(_lib.lib().y5_conv_pick(cin, cout, m_rows, C.byref(bk), None), "conv_pick")
-        v = _block_k_cache[key] = bk.value
-    return v
 
 
 def pack_weights(w: torch.Tensor, dtype: torch.dtype, m_rows: int, want_fwd: bool = True, want_dgrad: bool = False):
@@ -223,22 +211,14 @@ def conv_packed(x: torch.Tensor, x_pitch: int, wp: torch.Tensor, block_k: int, b
                 act: bool = False) -> torch.Tensor:
     """y = act(conv(x, w) + bias) through y5_conv_bn_silu_fwd.  x: (B,Cin,H,W) NHWC view with row pitch x_pitch; wp: K-major
     packed weights [cout][k][k][cin_pad]."""
-    lib = _lib.lib()
     b, cin, h, w = x.shape
     ho, wo = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
     if cin % 8 or cout % 8:
         raise NotImplementedError(f"y5b200: training convs need channel counts that are multiples of 8 (got {cin} -> {cout})")
     bias32 = _zero_bias(cout, x.device) if bias32 is None else bias32
     y = _empty_cl(b, cout, ho, wo, x.dtype, x.device)
-    d = ConvDesc()
-    d.inp, d.in_pitch = x.data_ptr(), x_pitch
-    d.batch, d.in_h, d.in_w, d.in_c = b, h, w, cin
-    d.weight, d.bias = wp.data_ptr(), bias32.data_ptr()
-    d.out, d.out_pitch, d.out_c = y.data_ptr(), cout, cout
-    d.ksize, d.stride, d.pad = k, s, p
-    d.act = _lib.ACT_SILU if act else _lib.ACT_NONE
-    d.dtype, d.block_k, d.block_n = _lib.dtype_code(x.dtype), block_k, 0
-    _lib.check(lib.y5_conv_bn_silu_fwd(C.byref(d), _st(x.device)), "conv fprop/dgrad")
+    d = conv_desc(ConvInput(x.data_ptr(), x_pitch, b, h, w, cin), wp, bias32, block_k, y.data_ptr(), cout, k, s, p, act, x.dtype)
+    _lib.check(_lib.lib().y5_conv_bn_silu_fwd(C.byref(d), _st(x.device)), "conv fprop/dgrad")
     return y
 
 
@@ -278,20 +258,13 @@ def conv_dgrad(dy: torch.Tensor, w_oihw: torch.Tensor | None, k: int, s: int, p:
 
 def conv_wgrad(x: torch.Tensor, dy: torch.Tensor, k: int, s: int, p: int) -> torch.Tensor:
     """fp32 dW (Cout,Cin,k,k) of y = conv(x, w) from NHWC views of x and dy."""
-    lib = _lib.lib()
     x, xp = _nhwc(x)
     dy, dp = _nhwc(dy)
     b, cin, h, w = x.shape
     cout = dy.shape[1]
     dw = torch.empty(cout, k, k, cin, dtype=torch.float32, device=x.device)
-    d = WgradDesc()
-    d.inp, d.in_pitch = x.data_ptr(), xp
-    d.batch, d.in_h, d.in_w, d.in_c = b, h, w, cin
-    d.dout, d.dout_pitch, d.out_c = dy.data_ptr(), dp, cout
-    d.dweight = dw.data_ptr()
-    d.ksize, d.stride, d.pad = k, s, p
-    d.dtype, d.accumulate = _lib.dtype_code(x.dtype), 0
-    _lib.check(lib.y5_conv_wgrad(C.byref(d), _st(x.device)), "conv_wgrad")
+    d = wgrad_desc(ConvInput(x.data_ptr(), xp, b, h, w, cin), dy.data_ptr(), dp, dw, k, s, p, x.dtype)
+    _lib.check(_lib.lib().y5_conv_wgrad(C.byref(d), _st(x.device)), "conv_wgrad")
     if k == 1:
         return dw.view(cout, cin, 1, 1)  # KRSC == OIHW for 1x1 filters
     return dw.permute(0, 3, 1, 2).contiguous()  # gradients must be laid out like the parameter (DDP buckets, optimizers)
@@ -304,51 +277,25 @@ def stem_wide_enabled() -> bool:
     return os.environ.get("Y5_TRAIN_STEM_WIDE", "1") != "0"
 
 
-def _wide_geom(buf: torch.Tensor):
-    b, h2, wp, _ = buf.shape  # (B, H/2, W/2 + 2, 16): one zero cell left and right of every row
-    return b, h2, wp - 2, dict(x=16, y=wp * 16, n=h2 * wp * 16)
-
-
 def stem_conv_wide(buf: torch.Tensor, w3: torch.Tensor) -> torch.Tensor:
-    """y = conv3x3/s1/p1(s2d image, w3) evaluated as a 3x1 conv over 48-channel wide pixels.  w3: (O,16,3,3)."""
-    lib = _lib.lib()
-    b, h2, w2, st = _wide_geom(buf)
+    """y = conv3x3/s1/p1(s2d image, w3) evaluated as a 3x1 conv over 48-channel wide pixels.  buf: stem_buffer; w3: (O,16,3,3)."""
+    x = stem_geom(buf, wide=True)
     o = w3.shape[0]
-    wv = w3.detach().float().permute(0, 3, 1, 2).reshape(o, 48, 3, 1)  # [o][s*16+c][r][0] = w3[o][c][r][s]
-    bk = _block_k(48, o, b * h2 * w2)
-    wp = pack_weight(wv, bk, buf.dtype)
-    y = _empty_cl(b, o, h2, w2, buf.dtype, buf.device)
-    d = ConvDesc()
-    d.inp, d.in_pitch = buf.data_ptr(), 16
-    d.in_x_stride, d.in_y_stride, d.in_n_stride = st["x"], st["y"], st["n"]
-    d.kw, d.pad_w = 1, 0
-    d.batch, d.in_h, d.in_w, d.in_c = b, h2, w2, 48
-    d.weight, d.bias = wp.data_ptr(), _zero_bias(o, buf.device).data_ptr()
-    d.out, d.out_pitch, d.out_c = y.data_ptr(), o, o
-    d.ksize, d.stride, d.pad = 3, 1, 1
-    d.act, d.dtype, d.block_k, d.block_n = _lib.ACT_NONE, _lib.dtype_code(buf.dtype), bk, 0
-    _lib.check(lib.y5_conv_bn_silu_fwd(C.byref(d), _st(buf.device)), "stem conv (wide pixels)")
+    bk = _block_k(48, o, x.batch * x.in_h * x.in_w)
+    wp = pack_weight(stem_weight_wide(w3.detach().float()), bk, buf.dtype)
+    y = _empty_cl(x.batch, o, x.in_h, x.in_w, buf.dtype, buf.device)
+    d = conv_desc(x, wp, _zero_bias(o, buf.device), bk, y.data_ptr(), o, 3, 1, 1, False, buf.dtype)
+    _lib.check(_lib.lib().y5_conv_bn_silu_fwd(C.byref(d), _st(buf.device)), "stem conv (wide pixels)")
     return y
 
 
 def stem_wgrad_wide(buf: torch.Tensor, dy: torch.Tensor) -> torch.Tensor:
-    """fp32 gradient of the (O,16,3,3) space-to-depth stem filter from the padded image buffer and dy (B,O,H/2,W/2)."""
-    lib = _lib.lib()
-    b, h2, w2, st = _wide_geom(buf)
+    """fp32 gradient of the (O,16,3,3) space-to-depth stem filter from the stem_buffer and dy (B,O,H/2,W/2)."""
     dy, dp = _nhwc(dy)
-    o = dy.shape[1]
-    dw = torch.empty(o, 3, 1, 48, dtype=torch.float32, device=buf.device)
-    d = WgradDesc()
-    d.inp, d.in_pitch = buf.data_ptr(), 16
-    d.in_x_stride, d.in_y_stride, d.in_n_stride = st["x"], st["y"], st["n"]
-    d.kw, d.pad_w = 1, 0
-    d.batch, d.in_h, d.in_w, d.in_c = b, h2, w2, 48
-    d.dout, d.dout_pitch, d.out_c = dy.data_ptr(), dp, o
-    d.dweight = dw.data_ptr()
-    d.ksize, d.stride, d.pad = 3, 1, 1
-    d.dtype, d.accumulate = _lib.dtype_code(buf.dtype), 0
-    _lib.check(lib.y5_conv_wgrad(C.byref(d), _st(buf.device)), "stem wgrad (wide pixels)")
-    return dw.view(o, 3, 3, 16).permute(0, 3, 1, 2)  # [o][r][s][c] -> (O,16,3,3)
+    dw = torch.empty(dy.shape[1], 3, 1, 48, dtype=torch.float32, device=buf.device)
+    d = wgrad_desc(stem_geom(buf, wide=True), dy.data_ptr(), dp, dw, 3, 1, 1, buf.dtype)
+    _lib.check(_lib.lib().y5_conv_wgrad(C.byref(d), _st(buf.device)), "stem wgrad (wide pixels)")
+    return stem_weight_narrow(dw.permute(0, 3, 1, 2))  # KRSC -> (O,48,3,1) -> (O,16,3,3)
 
 
 _stem_idx_cache: dict = {}
@@ -819,20 +766,17 @@ def _classify(m, x):
 
 
 def stem_input(img: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
-    """(B,3,H,W) uint8 / float image -> (B,16,H/2,W/2) channels_last space-to-depth tensor (12 channels used)."""
-    lib = _lib.lib()
+    """(B,3,H,W) uint8 / float image -> its space-to-depth cells (12 of 16 channels used): a stem_buffer for the wide-pixel stem,
+    else a (B,16,H/2,W/2) channels_last tensor."""
     b, c, h, w = img.shape
     if c != 3 or h % 2 or w % 2:
         raise ValueError(f"y5b200: expected a (B,3,even,even) image batch, got {tuple(img.shape)}")
-    img = img.contiguous()
-    if stem_wide_enabled():  # (B, H/2, W/2 + 2, 16) NHWC with a zero cell at both ends of every row
-        out = torch.zeros(b, h // 2, w // 2 + 2, 16, dtype=dtype, device=img.device)
-        _lib.check(lib.y5_stem_s2d(img.data_ptr(), _lib.dtype_code(img.dtype), out.data_ptr(), _lib.dtype_code(dtype), b, h, w, w // 2 + 2, 1,
-                                   _st(img.device)), "stem_s2d")
+    if stem_wide_enabled():
+        out = stem_buffer(b, h, w, dtype, img.device)
+        stem_s2d(img, out)
         return out
     out = _empty_cl(b, 16, h // 2, w // 2, dtype, img.device)
-    _lib.check(lib.y5_stem_s2d(img.data_ptr(), _lib.dtype_code(img.dtype), out.data_ptr(), _lib.dtype_code(dtype), b, h, w, w // 2, 0,
-                               _st(img.device)), "stem_s2d")
+    stem_s2d(img, out.permute(0, 2, 3, 1))
     return out
 
 
