@@ -41,6 +41,7 @@ extern "C" {
 
 #define Y5_ACT_NONE 0
 #define Y5_ACT_SILU 1
+#define Y5_ACT_LEAKY 2 /* v > 0 ? v : slope * v in fp32 (nn.LeakyReLU(slope); nn.ReLU is slope 0), slope passed next to the code */
 
 int y5_version(void);
 const char* y5_last_error(void);
@@ -48,7 +49,8 @@ const char* y5_last_error(void);
 int64_t y5_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Fused Conv2d(bias=False) + folded BatchNorm + SiLU (+ residual add), implicit GEMM on wgmma tensor cores.
+ * Fused Conv2d(bias=False) + folded BatchNorm + SiLU or LeakyReLU / ReLU (+ residual add), implicit GEMM on wgmma tensor cores.
+ * The activation (desc.act, desc.act_slope) acts on fp32(acc + bias); the residual is added in fp32 and the sum rounded once.
  * Replaces: models/common.py:86-92 Conv.forward / forward_fuse (conv -> bn -> act), utils/torch_utils.py:224-254
  * (BN fold, done once by the caller when packing), models/common.py:181 Bottleneck's `x + ...` (residual),
  * and, through out pitch/offset, the torch.cat of models/common.py:246,340,453.
@@ -68,7 +70,7 @@ typedef struct y5_conv_desc {
     const void* residual; /* optional: same shape as out; may alias out (in-place add) */
     int32_t res_pitch;
     int32_t ksize, stride, pad;
-    int32_t act;          /* Y5_ACT_* */
+    int32_t act;          /* Y5_ACT_NONE | Y5_ACT_SILU | Y5_ACT_LEAKY (with act_slope) */
     int32_t dtype;        /* Y5_F16 | Y5_BF16 */
     int32_t block_k;      /* 16|32|64, or 0 = y5_conv_pick's choice; must match the weight packing */
     int32_t block_n;      /* 32|64|128|256, or 0 = auto */
@@ -87,6 +89,7 @@ typedef struct y5_conv_desc {
                              feeds every tap of a stride-1 k x k conv with 64-channel chunks), bit 5 (32) vetoes it; with a
                              forced block_n also bit 1 (2) = 256-row tiles (block_n 128), bit 2 (4) = CTA pairs (2-CTA cluster),
                              bits 8.. = cluster size (2|4): the CTAs of a cluster split every weight tile and TMA-multicast it */
+    float act_slope;      /* Y5_ACT_LEAKY: negative slope (finite; 0 = ReLU).  Ignored for the other activations */
 } y5_conv_desc;
 
 /* Tiling the library will use for a conv: block_k decides the weight packing (cin_pad = ceil(in_c/block_k)*block_k). */
@@ -107,7 +110,7 @@ struct y5_conv_plan_info {
     int32_t b_grouped;            /* patch: the kh weight tiles of a (chunk, horizontal tap) group share one stage */
     int32_t staged;               /* epilogue stores go through shared memory (else straight from the registers) */
     int32_t opt;                  /* runs the kernel instantiation with the optional modes compiled in */
-    int32_t epi;                  /* epilogue: 0 conv, 1 Detect head */
+    int32_t epi;                  /* epilogue: 0 conv (SiLU or none), 1 Detect head, 2 conv with LeakyReLU / ReLU */
     int32_t a_stages, b_stages;   /* shared-memory pipeline depth */
     int32_t grid;                 /* CTAs launched (persistent, at most one per SM) */
     int32_t tma_epi;              /* epilogue through shared memory: residual TMA-loaded, output TMA-stored */
@@ -298,7 +301,8 @@ int64_t y5_bn_workspace_bytes(int32_t channels);
 /* per-channel sum and sum of squares of a [rows][channels] view, accumulated into workspace (fp64) */
 int y5_bn_stats(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace,
                 void* stream);
-/* z = act(gamma * (y - mean) * invstd + beta), act: Y5_ACT_NONE | Y5_ACT_SILU; z may be a channel-slice view.
+/* z = act(gamma * (y - mean) * invstd + beta), act: Y5_ACT_NONE | Y5_ACT_SILU (LeakyReLU: the _ex forms below); z may be a
+ * channel-slice view.
  * sums != NULL (training): mean / invstd (biased variance + eps) are first derived from the y5_bn_stats workspace and
  * WRITTEN to mean / invstd, and running_mean / running_var (nullable) are updated like nn.BatchNorm2d does (momentum,
  * unbiased variance).  sums == NULL (eval): mean / invstd are inputs.  residual != NULL adds a view of the same shape
@@ -337,6 +341,24 @@ int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const void* dz, int32_t
 int y5_bn_act_bwd_apply(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
                         int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
                         const float* gamma, int32_t act, const void* sums, const void* count, void* stream);
+/* Four of the passes above with the activation's parameter after `act` (y5_bn_act_bwd_apply takes Y5_ACT_LEAKY as it is: it only
+ * reads the parked du): `slope` is the negative slope of
+ * Y5_ACT_LEAKY (finite; 0 = ReLU) and is ignored for Y5_ACT_NONE / Y5_ACT_SILU, so act = NONE | SILU computes exactly what the
+ * entry points without the suffix compute.  LeakyReLU, with t = bn(y) rounded to the activation dtype as above:
+ *   forward:  z = round(t > 0 ? t : slope * t)                       (fp32 product; + residual as above)
+ *   backward: du = round(t > 0 ? dz : dz * slope)                    (torch's leaky_relu_backward), parked in dy like SiLU's */
+int y5_bn_act_fwd_ex(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
+                     float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope, const void* sums, float eps,
+                     float momentum, float* running_mean, float* running_var, const void* residual, int32_t res_pitch, void* stream);
+int y5_bn_act_bwd_ex(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
+                     int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                     int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream);
+int y5_bn_act_fwd_sync_ex(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
+                          float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope, const void* sums, float eps,
+                          float momentum, float* running_mean, float* running_var, const void* residual, int32_t res_pitch, void* stream);
+int y5_bn_act_bwd_reduce_ex(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                            int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
+                            const float* gamma, const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream);
 /* out[c] = sum over rows of y[row][c] (fp32) */
 int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, float* out, void* workspace,
                void* stream);

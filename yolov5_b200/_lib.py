@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("Y5B200_LIB") or os.path.join(_HERE, "liby5b200.so")  # env override: A/B experiments only
 
 Y5_F16, Y5_BF16, Y5_F32, Y5_U8 = 0, 1, 2, 3
-ACT_NONE, ACT_SILU = 0, 1
+ACT_NONE, ACT_SILU, ACT_LEAKY = 0, 1, 2  # include/y5b200.h Y5_ACT_*
 
 _DTYPE = {torch.float16: Y5_F16, torch.bfloat16: Y5_BF16, torch.float32: Y5_F32, torch.uint8: Y5_U8}
 
@@ -37,7 +37,7 @@ class ConvDesc(C.Structure):
         ("act", C.c_int32), ("dtype", C.c_int32), ("block_k", C.c_int32), ("block_n", C.c_int32),
         ("kw", C.c_int32), ("pad_w", C.c_int32),
         ("in_x_stride", C.c_int64), ("in_y_stride", C.c_int64), ("in_n_stride", C.c_int64),
-        ("a_mode", C.c_int32), ("reserved", C.c_int32),
+        ("a_mode", C.c_int32), ("reserved", C.c_int32), ("act_slope", C.c_float),
     ]
 
 
@@ -221,6 +221,10 @@ SIGNATURES = {
     "y5_bn_act_fwd_sync": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _F, _F, _P, _P, _P, _I32, _P]),
     "y5_bn_act_bwd_reduce": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _P, _P, _P]),
     "y5_bn_act_bwd_apply": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _I32, _P, _P, _P]),
+    "y5_bn_act_fwd_ex": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _F, _F, _P, _P, _P, _I32, _P]),
+    "y5_bn_act_bwd_ex": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P]),
+    "y5_bn_act_fwd_sync_ex": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _F, _F, _P, _P, _P, _I32, _P]),
+    "y5_bn_act_bwd_reduce_ex": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P]),
     "y5_weight_pack": (_I32, [_P, _I32, _I32, _I32, _I32, _P, _I32, _P, _I32, _I32, _P]),
     "y5_weight_pack_chunk_elems": (_I32, []),
     "y5_weight_pack_multi": (_I32, [_P, _P, _P, _I32, _I32, _P]),

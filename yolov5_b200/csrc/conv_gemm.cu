@@ -18,7 +18,7 @@
 // have separate mbarrier rings because one A patch feeds kh B tiles (PATCH mode: the kh tiles of a group may share one stage).
 // MMA + epilogue: two consumer warpgroups.  Warpgroup w owns rows [64w, 64w + 64) of every 128-row sub-tile and issues
 // wgmma m64 x BLOCK_N x k16 (fp32 accumulators in registers) for them; after the tile's last K block it applies the
-// folded-BN bias -> SiLU -> (+ residual) -> fp16/bf16 and stores straight from the registers to the NHWC (slice) view.
+// folded-BN bias -> SiLU or LeakyReLU -> (+ residual) -> fp16/bf16 and stores straight from the registers to the NHWC (slice) view.
 // Epilogue stores: by default the tile is staged in shared memory in swizzled 64-row boxes, with its residual TMA-loaded there by
 // the producer warp, and leaves by TMA bulk stores (the TMA unit clips the tails).  Direct mode (reserved bit 16, and plans where
 // the staging block does not fit or costs too much): each thread stores its 4-byte pairs straight from the registers, with the
@@ -29,6 +29,8 @@
 // Clusters (2 or 4 CTAs along M): the CTAs of a cluster work on different M super-tiles of the SAME N tile in lock-step, each
 // fetches 1/csize of every weight tile and TMA-multicasts it to all of them, so the L2 -> smem weight traffic per CTA drops by
 // the cluster size.  A weight stage is free again only when the consumers of every CTA of the cluster have released it.
+// EPI=2 is the conv epilogue with LeakyReLU (ReLU: slope 0) in place of SiLU: an instantiation of its own, so the SiLU / linear
+// instantiations (EPI=0) compile to exactly the code they had without it.
 // Detect head (EPI=1): an anchor's `no` outputs are tpa = ceil(no / 128) N tiles (weights packed npad = 128 * tpa rows per anchor).
 // no <= 128 (one tile per anchor): raw logits and decoded predictions are staged in smem in the exact global layout and copied out
 // with 16-byte vectors.  Wider heads stage [128 rows][128 columns] blocks and copy each row segment to its column offset, with 16-,
@@ -45,6 +47,7 @@
 //
 // Replaces reference models/common.py:86-92 (Conv), :181 (Bottleneck add), :246/:340/:453 (cat, via strided
 // output views) and models/yolo.py:95-113 (Detect level).
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -90,7 +93,7 @@ struct ConvParams {
     float rcp_per_img, rcp_tiles_x, rcp_HoWo, rcp_Wo;  // reciprocals for fdiv(): exact small-integer division in ~7 instructions
     int a_stages, b_stages;
     uint32_t a_sub_bytes, a_stage_bytes, b_stage_bytes;
-    int is_bf16, act;
+    int is_bf16, act;           // act: SiLU (EPI 0)
     const float* bias;
     int bias_n;                 // floats preloaded into smem (0: a wide head reads each tile's bias from global memory)
     // EPI 0
@@ -104,6 +107,9 @@ struct ConvParams {
     int na, no, nc, nx, z_rows, z_row0;
     float det_stride;
     float anchor_wh[8];
+    // EPI 2 (conv with LeakyReLU / ReLU): v > 0 ? v : slope * v on v = fp32(acc + bias).  Last, so the other instantiations read
+    // their parameters at the offsets they always had
+    float slope;
 };
 
 struct SmemLayout {
@@ -191,9 +197,11 @@ __global__ void __launch_bounds__(kThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
                  const __grid_constant__ CUtensorMap tmR, const ConvParams p) {
     static_assert(MT * BLOCK_N <= 256, "accumulators: at most 128 fp32 registers per consumer thread");
+    constexpr bool kConv = EPI != 1;   // EPI 0 and 2: the conv epilogue
+    constexpr bool kLeaky = EPI == 2;  // ... with LeakyReLU instead of SiLU / none
     constexpr int kAcc = BLOCK_N / 2;  // accumulator registers per sub-tile and thread (64 x BLOCK_N over a warpgroup)
     using Box = EpiBox<BLOCK_N>;
-    const bool tma_epi = EPI == 0 && !OPT && p.tma_epi;
+    const bool tma_epi = kConv && !OPT && p.tma_epi;
 
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -237,7 +245,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = threadIdx.x - 128; i < p.bias_n; i += kConsumerThreads) {
             // SiLU layers keep HALF the bias: the epilogue forms h = (acc + b) / 2 with one FMA and silu = h + h * tanh(h)
             const float b = i < p.N ? __ldg(p.bias + i) : 0.0f;
-            sBias[i] = (EPI == 0 && p.act) ? 0.5f * b : b;
+            sBias[i] = (kConv && p.act) ? 0.5f * b : b;
         }
     __syncthreads();
     if (csize > 1) cluster_sync_all();  // peers' barriers are initialised before anyone multicasts into them or arrives on them
@@ -461,7 +469,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int mi = 0; mi < MT; ++mi) fence_regs(acc[mi]);
         release_pending();
 
-        if (EPI == 0) {
+        if (kConv) {
             const bool staged = OPT && p.stg_bytes != 0;
             const uint32_t stg_pitch = BLOCK_N * 2 + 16;  // +16 bytes: the fragment's 8 rows x 4 column pairs hit 32 distinct banks
             uint8_t* stg_wg = stg + wg * 64 * stg_pitch;
@@ -560,6 +568,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                                     } else {
                                         f0 = a0 + b.x;
                                         f1 = a1 + b.y;
+                                        if (kLeaky) {
+                                            f0 = f0 > 0.0f ? f0 : p.slope * f0;
+                                            f1 = f1 > 0.0f ? f1 : p.slope * f1;
+                                        }
                                     }
                                     if (has_res && gpix >= 0) {
                                         const float2 t = unpack2(rv[q][j], bf16);
@@ -753,7 +765,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 __global__ void conv_direct_kernel(const uint16_t* __restrict__ in, long long xs, long long ys, long long ns, int B, int H,
                                    int W, int Cin, const uint16_t* __restrict__ w, int cin_pad, const float* __restrict__ bias,
                                    uint16_t* out, int out_pitch, int Cout, const uint16_t* res, int res_pitch, int kh, int kw,
-                                   int stride, int pad_h, int pad_w, int Ho, int Wo, int act, int bf16) {
+                                   int stride, int pad_h, int pad_w, int Ho, int Wo, int act, float slope, int bf16) {
     const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
     const long long total = static_cast<long long>(B) * Ho * Wo * Cout;
     if (idx >= total) return;
@@ -775,7 +787,8 @@ __global__ void conv_direct_kernel(const uint16_t* __restrict__ in, long long xs
         }
     }
     float x = acc + bias[n];
-    if (act) x = x / (1.0f + expf(-x));
+    if (act == Y5_ACT_SILU) x = x / (1.0f + expf(-x));
+    else if (act == Y5_ACT_LEAKY) x = x > 0.0f ? x : slope * x;
     if (res) x += unpack1(res[m * res_pitch + n], bf16);
     out[m * out_pitch + n] = pack1(x, bf16);
 }
@@ -910,6 +923,17 @@ int run_plan(const PlanCommon& pc, cudaStream_t st) {
         case 101281: e = launch_conv<128, 0, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
         case 101282: e = launch_conv<128, 0, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
         case 102561: e = launch_conv<256, 0, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        // conv with LeakyReLU (EPI 2)
+        case 20324: e = launch_conv<32, 2, 4, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 20642: e = launch_conv<64, 2, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 21281: e = launch_conv<128, 2, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 21282: e = launch_conv<128, 2, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 22561: e = launch_conv<256, 2, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 120324: e = launch_conv<32, 2, 4, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 120642: e = launch_conv<64, 2, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 121281: e = launch_conv<128, 2, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 121282: e = launch_conv<128, 2, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 122561: e = launch_conv<256, 2, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
         default: return set_error(Y5_E_UNSUPPORTED, "conv: no kernel for block_n %d mt %d epi %d", pc.block_n, pc.mt, pc.epi);
     }
     if (e != cudaSuccess) return set_error(int(e), "conv_gemm launch failed: %s", cudaGetErrorString(e));
@@ -981,6 +1005,9 @@ static int validate_conv(const y5_conv_desc* d) {
     if (!aligned16(d->in) || !aligned16(d->out) || !aligned16(d->weight) || (d->residual && !aligned16(d->residual)))
         return set_error(Y5_E_INVALID, "conv: pointers must be 16-byte aligned");
     if (d->residual && (d->res_pitch < d->out_c || d->res_pitch % 8)) return set_error(Y5_E_INVALID, "conv: bad residual pitch");
+    if (d->act != Y5_ACT_NONE && d->act != Y5_ACT_SILU && d->act != Y5_ACT_LEAKY)
+        return set_error(Y5_E_UNSUPPORTED, "conv: activation code %d unsupported", d->act);
+    if (d->act == Y5_ACT_LEAKY && !std::isfinite(d->act_slope)) return set_error(Y5_E_INVALID, "conv: LeakyReLU slope must be finite");
     const int kw = d->kw ? d->kw : d->ksize, pw = d->kw ? d->pad_w : d->pad;
     if (d->ksize < 1 || d->ksize > 7 || kw < 1 || kw > 7 || d->stride < 1 || d->stride > 8 || d->pad < 0 || d->pad > d->ksize || pw < 0 ||
         pw > kw)
@@ -1043,7 +1070,8 @@ extern "C" Y5_API int y5_conv_plan_create(const y5_conv_desc* d, y5_conv_plan** 
     p.stride = d->stride;
     p.pad_h = g.pad_h; p.pad_w = g.pad_w;
     p.is_bf16 = d->dtype == Y5_BF16;
-    p.act = d->act;
+    p.act = d->act == Y5_ACT_SILU;
+    p.slope = d->act_slope;
     p.bias = d->bias;
     p.out = d->out;
     p.out_pitch = d->out_pitch;
@@ -1129,11 +1157,12 @@ extern "C" Y5_API int y5_conv_plan_create(const y5_conv_desc* d, y5_conv_plan** 
     } else if ((d->reserved & 8) && !(d->reserved & 16)) {
         p.stg_bytes = static_cast<uint32_t>(kConsumers * 64 * (bn * 2 + 16));
     }
-    int e2 = finish_plan(pc, bn, 0, mt_sel, cl_sel);
+    const int epi = d->act == Y5_ACT_LEAKY ? 2 : 0;
+    int e2 = finish_plan(pc, bn, epi, mt_sel, cl_sel);
     if (e2 && p.stg_bytes) {
         p.stg_bytes = 0;
         p.tma_epi = 0;
-        e2 = finish_plan(pc, bn, 0, mt_sel, cl_sel);
+        e2 = finish_plan(pc, bn, epi, mt_sel, cl_sel);
     }
     if (e2) { delete plan; return e2; }
     *out = plan;
@@ -1188,7 +1217,7 @@ extern "C" Y5_API int y5_conv_direct_fwd(const y5_conv_desc* d, void* stream) {
     conv_direct_kernel<<<static_cast<unsigned>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const uint16_t*>(d->in), g.xs, g.ys, g.ns, d->batch, d->in_h, d->in_w, d->in_c, static_cast<const uint16_t*>(d->weight),
         cin_pad, d->bias, static_cast<uint16_t*>(d->out), d->out_pitch, d->out_c, static_cast<const uint16_t*>(d->residual), d->res_pitch,
-        g.kh, g.kw, d->stride, g.pad_h, g.pad_w, g.Ho, g.Wo, d->act, d->dtype == Y5_BF16);
+        g.kh, g.kw, d->stride, g.pad_h, g.pad_w, g.Ho, g.Wo, d->act, d->act_slope, d->dtype == Y5_BF16);
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(int(e), "conv_direct launch failed: %s", cudaGetErrorString(e));

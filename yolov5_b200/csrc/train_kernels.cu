@@ -8,6 +8,7 @@
 // Numerics follow the reference under torch.autocast: BN math in fp32 on the low-precision conv output, its result
 // rounded to the activation dtype, SiLU on that rounded value, gradients rounded to the activation dtype between ops.
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 
@@ -177,8 +178,8 @@ __global__ void col_sum_finalize_kernel(const double* __restrict__ ws, int chann
 
 // Per-channel constants of the three passes live in shared memory:
 //   a = invstd*gamma, b = beta - mean*a           -> t = round(y*a + b) is the BN output
-//   forward : z = silu(t)
-//   reduce  : xh = y*is + m2 (m2 = -mean*invstd);  du = dz*silu'(t);  sum du, sum du*xh
+//   forward : z = silu(t)  or  leaky(t) = t > 0 ? t : slope*t
+//   reduce  : xh = y*is + m2 (m2 = -mean*invstd);  du = dz*act'(t);  sum du, sum du*xh
 //   apply   : dy = du*a + y*c1 + c0  with c1 = -invstd*(dgamma/rows)*a,  c0 = -(dbeta/rows + m2*dgamma/rows)*a
 // which is (du - dbeta/rows - xh*dgamma/rows)*gamma*invstd written so that four constants per channel suffice; keeping
 // them out of registers lets 3-4 blocks share an SM.  Layout: two float2 tables indexed [channel-in-group * cgx + group] --
@@ -191,13 +192,17 @@ struct ChanTables {
 };
 __device__ __forceinline__ int chan_slot(int i, int cgx) { return (i & 7) * cgx + (i >> 3); }  // i = channel inside the block's span
 
-__device__ __forceinline__ float act_bwd(float dz, float t, int act, bool bf16) {
-    if (!act) return dz;
+// du = dz * act'(t) rounded to the activation dtype.  LeakyReLU: torch's leaky_relu_backward (t > 0 ? dz : dz * slope)
+template <int ACT>
+__device__ __forceinline__ float act_bwd(float dz, float t, float slope, bool bf16) {
+    if (ACT == Y5_ACT_NONE) return dz;
+    if (ACT == Y5_ACT_LEAKY) return round_lowp(t > 0.0f ? dz : dz * slope, bf16);
     const float sg = __fdividef(1.0f, 1.0f + __expf(-t));
     return round_lowp(dz * sg * (1.0f + t * (1.0f - sg)), bf16);
 }
 
-template <bool RES>
+// LEAKY: z = t > 0 ? t : slope * t (a template parameter, so the SiLU / linear instantiations carry none of it)
+template <bool RES, bool LEAKY>
 __global__ void __launch_bounds__(kRedThreads, RES ? 3 : 4) bn_act_fwd_kernel(const void* __restrict__ y, int y_pitch, void* __restrict__ z, int z_pitch,
                                                                     long long rows, int channels, int bf16, int act, int cgx, int rpb,
                                                                     float* __restrict__ mean, float* __restrict__ invstd,
@@ -205,7 +210,8 @@ __global__ void __launch_bounds__(kRedThreads, RES ? 3 : 4) bn_act_fwd_kernel(co
                                                                     const double* __restrict__ sums, const double* __restrict__ count,
                                                                     double inv_rows, double unbias, float eps,
                                                                     float momentum, float* __restrict__ running_mean,
-                                                                    float* __restrict__ running_var, const void* __restrict__ res, int res_pitch) {
+                                                                    float* __restrict__ running_var, const void* __restrict__ res, int res_pitch,
+                                                                    float slope) {
     griddep_wait();  // PDL: the predecessor kernel has completed and flushed beyond this point
     griddep_launch_dependents();
     if (count) {  // SyncBN: the row count N of all ranks, summed with the column sums; the same double arithmetic as the host's
@@ -270,8 +276,9 @@ __global__ void __launch_bounds__(kRedThreads, RES ? 3 : 4) bn_act_fwd_kernel(co
                 for (int i = 0; i < 8; ++i) {
                     const float2 k = kt[i * cgx];
                     const float t = round_lowp(fmaf(v[i], k.x, k.y), b);
-                    v[i] = act ? __fdividef(t, 1.0f + __expf(-t)) : t;
-                    if (RES) v[i] = round_lowp(v[i], b) + q[i];  // z = x + SiLU(BN(y)), each term rounded like the reference's add
+                    if (LEAKY) v[i] = t > 0.0f ? t : slope * t;
+                    else v[i] = act ? __fdividef(t, 1.0f + __expf(-t)) : t;
+                    if (RES) v[i] = round_lowp(v[i], b) + q[i];  // z = x + act(BN(y)), each term rounded like the reference's add
                 }
                 st16(z, rr * z_pitch + cg * 8, pack8(v, b));
             }
@@ -282,13 +289,13 @@ __global__ void __launch_bounds__(kRedThreads, RES ? 3 : 4) bn_act_fwd_kernel(co
 // U rows in flight per thread.  This pass is bound by its instruction stream (exp + reciprocal + ~18 more per element), not by
 // HBM: the constants of a channel pair are read once per loop trip and used for all U rows, and the loop nest is
 // channel-pair-major so that nothing but the raw 16-byte words of the U rows stays live across it.
-template <int U, bool BF16, bool ACT>
+template <int U, bool BF16, int ACT>
 __global__ void __launch_bounds__(kRedThreads, U == 4 ? 2 : 3) bn_act_bwd_reduce_kernel(const void* __restrict__ y, int y_pitch, const void* __restrict__ dz,
                                                                            int dz_pitch, long long rows, int channels,
                                                                            int cgx, int rpb, const float* __restrict__ mean,
                                                                            const float* __restrict__ invstd, const float* __restrict__ gamma,
                                                                            const float* __restrict__ beta, double* __restrict__ ws,
-                                                                           void* __restrict__ du_out, int du_pitch) {
+                                                                           void* __restrict__ du_out, int du_pitch, float slope) {
     griddep_wait();  // PDL: the predecessor kernel has completed and flushed beyond this point
     griddep_launch_dependents();
     __shared__ ChanTables tab;
@@ -344,7 +351,7 @@ __global__ void __launch_bounds__(kRedThreads, U == 4 ? 2 : 3) bn_act_bwd_reduce
                             const uint32_t gw[4] = {gv[u].x, gv[u].y, gv[u].z, gv[u].w};
                             const float2 yy = unpack2(yw[p], b), gg = unpack2(gw[p], b);
                             const float t0 = round_lowp(fmaf(yy.x, ab0.x, ab0.y), b), t1 = round_lowp(fmaf(yy.y, ab1.x, ab1.y), b);
-                            const float du0 = act_bwd(gg.x, t0, ACT, b), du1 = act_bwd(gg.y, t1, ACT, b);
+                            const float du0 = act_bwd<ACT>(gg.x, t0, slope, b), du1 = act_bwd<ACT>(gg.y, t1, slope, b);
                             acc[0][2 * p] += du0;
                             acc[0][2 * p + 1] += du1;
                             acc[1][2 * p] = fmaf(du0, fmaf(yy.x, cd0.x, cd0.y), acc[1][2 * p]);
@@ -663,6 +670,13 @@ using namespace y5;
 
 extern "C" Y5_API int64_t y5_bn_workspace_bytes(int32_t channels) { return static_cast<int64_t>(channels) * 2 * sizeof(double); }
 
+// the activation of a BN pass: Y5_ACT_NONE | Y5_ACT_SILU | Y5_ACT_LEAKY with a finite slope
+static int check_act(const char* what, int32_t act, float slope) {
+    if (act != Y5_ACT_NONE && act != Y5_ACT_SILU && act != Y5_ACT_LEAKY) return set_error(Y5_E_UNSUPPORTED, "%s: activation code %d unsupported", what, act);
+    if (act == Y5_ACT_LEAKY && !std::isfinite(slope)) return set_error(Y5_E_INVALID, "%s: LeakyReLU slope must be finite", what);
+    return 0;
+}
+
 // check_view with the operand named after the entry point ("bn_act_fwd y")
 static int check_operand(const char* what, const char* operand, const void* p, int pitch, int channels) {
     char name[64];
@@ -687,9 +701,10 @@ static int bn_stats_launch(const char* what, const void* y, int32_t pitch, int64
 }
 
 static int bn_act_fwd_launch(const char* what, const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
-                             float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, const void* sums, bool sync,
-                             float eps, float momentum, float* running_mean, float* running_var, const void* residual, int32_t res_pitch,
-                             void* stream) {
+                             float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope, const void* sums,
+                             bool sync, float eps, float momentum, float* running_mean, float* running_var, const void* residual,
+                             int32_t res_pitch, void* stream) {
+    if (int e = check_act(what, act, slope)) return e;
     if (int e = check_operand(what, "y", y, y_pitch, channels)) return e;
     if (int e = check_operand(what, "z", z, z_pitch, channels)) return e;
     if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "%s: dtype must be fp16 or bf16", what);
@@ -701,10 +716,13 @@ static int bn_act_fwd_launch(const char* what, const void* y, int32_t y_pitch, v
     const double unbias = rows > 1 ? static_cast<double>(rows) / static_cast<double>(rows - 1) : 1.0;
     const double* s = static_cast<const double*>(sums);
     count_launch();
-    launch_pdl(residual ? bn_act_fwd_kernel<true> : bn_act_fwd_kernel<false>, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream), 
+    const bool leaky = act == Y5_ACT_LEAKY;
+    auto* kernel = residual ? (leaky ? bn_act_fwd_kernel<true, true> : bn_act_fwd_kernel<true, false>)
+                            : (leaky ? bn_act_fwd_kernel<false, true> : bn_act_fwd_kernel<false, false>);
+    launch_pdl(kernel, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream),
         y, y_pitch, z, z_pitch, rows, channels, dtype == Y5_BF16, act, g.cgx, g.rpb, mean, invstd, gamma, beta, s,
         sync ? s + 2 * static_cast<int64_t>(channels) : static_cast<const double*>(nullptr), inv_rows, unbias, eps, momentum,
-        running_mean, running_var, residual, res_pitch);
+        running_mean, running_var, residual, res_pitch, slope);
     return launch_status(what);
 }
 
@@ -718,23 +736,24 @@ static int bn_bwd_check(const char* what, const void* y, int32_t y_pitch, const 
     return 0;
 }
 
-// reduce pass: du = dz * act'(t) and its two column sums into the workspace.  SiLU layers: du is left in the dy buffer and the
-// apply pass finishes it in place; linear layers have du == dz
+// reduce pass: du = dz * act'(t) and its two column sums into the workspace.  SiLU and LeakyReLU layers: du is left in the dy
+// buffer and the apply pass finishes it in place; linear layers have du == dz
 static void bn_bwd_reduce_launch(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
                                  int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, const float* beta,
-                                 int32_t act, void* workspace, cudaStream_t st) {
+                                 int32_t act, float slope, void* workspace, cudaStream_t st) {
     static const int red_u = env_int("Y5_BN_RED_U", 4);
     const RowGeom g = row_geom(channels, rows, true, red_u == 2 ? 3 : 2);
     using RedFn = void (*)(const void*, int, const void*, int, long long, int, int, int, const float*, const float*, const float*, const float*,
-                           double*, void*, int);
-    static const RedFn table[2][2][2] = {
-        {{bn_act_bwd_reduce_kernel<4, false, false>, bn_act_bwd_reduce_kernel<4, false, true>},
-         {bn_act_bwd_reduce_kernel<4, true, false>, bn_act_bwd_reduce_kernel<4, true, true>}},
-        {{bn_act_bwd_reduce_kernel<2, false, false>, bn_act_bwd_reduce_kernel<2, false, true>},
-         {bn_act_bwd_reduce_kernel<2, true, false>, bn_act_bwd_reduce_kernel<2, true, true>}}};
-    launch_pdl(table[red_u == 2 ? 1 : 0][dtype == Y5_BF16 ? 1 : 0][act ? 1 : 0], row_grid(g, channels, rows), dim3(kRedThreads), 0, st, y, y_pitch, dz,
+                           double*, void*, int, float);
+    constexpr int N = Y5_ACT_NONE, S = Y5_ACT_SILU, L = Y5_ACT_LEAKY;
+    static const RedFn table[2][2][3] = {
+        {{bn_act_bwd_reduce_kernel<4, false, N>, bn_act_bwd_reduce_kernel<4, false, S>, bn_act_bwd_reduce_kernel<4, false, L>},
+         {bn_act_bwd_reduce_kernel<4, true, N>, bn_act_bwd_reduce_kernel<4, true, S>, bn_act_bwd_reduce_kernel<4, true, L>}},
+        {{bn_act_bwd_reduce_kernel<2, false, N>, bn_act_bwd_reduce_kernel<2, false, S>, bn_act_bwd_reduce_kernel<2, false, L>},
+         {bn_act_bwd_reduce_kernel<2, true, N>, bn_act_bwd_reduce_kernel<2, true, S>, bn_act_bwd_reduce_kernel<2, true, L>}}};
+    launch_pdl(table[red_u == 2 ? 1 : 0][dtype == Y5_BF16 ? 1 : 0][act], row_grid(g, channels, rows), dim3(kRedThreads), 0, st, y, y_pitch, dz,
                dz_pitch, rows, channels, g.cgx, g.rpb, mean, invstd, gamma, beta, static_cast<double*>(workspace),
-               act ? dy : static_cast<void*>(nullptr), dy_pitch);
+               act ? dy : static_cast<void*>(nullptr), dy_pitch, slope);
 }
 
 // apply pass: dy from du and the column sums (count == NULL: divided by this call's rows); dgamma / dbeta written when non-NULL
@@ -770,53 +789,100 @@ extern "C" Y5_API int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int
     return launch_status("col_sum");
 }
 
+static int bn_act_bwd_impl(const char* what, const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                           int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
+                           const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream) {
+    if (int e = check_act(what, act, slope)) return e;
+    if (int e = bn_bwd_check(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace)) return e;
+    if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "%s: bad argument", what);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    count_launch(2);
+    bn_bwd_reduce_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope, workspace, st);
+    bn_bwd_apply_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, act, static_cast<const double*>(workspace),
+                        nullptr, dgamma, dbeta, st);
+    return launch_status(what);
+}
+
+static int bn_act_bwd_reduce_impl(const char* what, const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                                  int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
+                                  const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream) {
+    if (int e = check_act(what, act, slope)) return e;
+    if (int e = bn_bwd_check(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace)) return e;
+    if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "%s: bad argument", what);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    count_launch(2);
+    bn_bwd_reduce_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope, workspace, st);
+    launch_pdl(bn_affine_grad_kernel, dim3((channels + 127) / 128), dim3(128), 0, st, static_cast<const double*>(workspace), static_cast<int>(channels),
+               dgamma, dbeta);
+    return launch_status(what);
+}
+
 extern "C" Y5_API int y5_bn_act_fwd(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
                                     float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, const void* sums,
                                     float eps, float momentum, float* running_mean, float* running_var, const void* residual,
                                     int32_t res_pitch, void* stream) {
-    return bn_act_fwd_launch("bn_act_fwd", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, sums, false, eps, momentum,
-                             running_mean, running_var, residual, res_pitch, stream);
+    return bn_act_fwd_launch("bn_act_fwd", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, 0.0f, sums, false, eps,
+                             momentum, running_mean, running_var, residual, res_pitch, stream);
+}
+
+extern "C" Y5_API int y5_bn_act_fwd_ex(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
+                                       float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope, const void* sums,
+                                       float eps, float momentum, float* running_mean, float* running_var, const void* residual,
+                                       int32_t res_pitch, void* stream) {
+    return bn_act_fwd_launch("bn_act_fwd_ex", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope, sums, false, eps,
+                             momentum, running_mean, running_var, residual, res_pitch, stream);
 }
 
 extern "C" Y5_API int y5_bn_act_fwd_sync(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
                                          float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, const void* sums,
                                          float eps, float momentum, float* running_mean, float* running_var, const void* residual,
                                          int32_t res_pitch, void* stream) {
-    return bn_act_fwd_launch("bn_act_fwd_sync", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, sums, true, eps,
+    return bn_act_fwd_launch("bn_act_fwd_sync", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, 0.0f, sums, true, eps,
                              momentum, running_mean, running_var, residual, res_pitch, stream);
+}
+
+extern "C" Y5_API int y5_bn_act_fwd_sync_ex(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels,
+                                            int32_t dtype, float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope,
+                                            const void* sums, float eps, float momentum, float* running_mean, float* running_var,
+                                            const void* residual, int32_t res_pitch, void* stream) {
+    return bn_act_fwd_launch("bn_act_fwd_sync_ex", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope, sums, true,
+                             eps, momentum, running_mean, running_var, residual, res_pitch, stream);
 }
 
 extern "C" Y5_API int y5_bn_act_bwd(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
                                     int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
                                     const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace, void* stream) {
-    if (int e = bn_bwd_check("bn_act_bwd", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace)) return e;
-    if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "bn_act_bwd: bad argument");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    count_launch(2);
-    bn_bwd_reduce_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, workspace, st);
-    bn_bwd_apply_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, act, static_cast<const double*>(workspace),
-                        nullptr, dgamma, dbeta, st);
-    return launch_status("bn_act_bwd");
+    return bn_act_bwd_impl("bn_act_bwd", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, 0.0f, dgamma,
+                           dbeta, workspace, stream);
+}
+
+extern "C" Y5_API int y5_bn_act_bwd_ex(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
+                                       int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
+                                       const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream) {
+    return bn_act_bwd_impl("bn_act_bwd_ex", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope,
+                           dgamma, dbeta, workspace, stream);
 }
 
 extern "C" Y5_API int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
                                            int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
                                            const float* gamma, const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace,
                                            void* stream) {
-    if (int e = bn_bwd_check("bn_act_bwd_reduce", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace))
-        return e;
-    if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "bn_act_bwd_reduce: bad argument");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    count_launch(2);
-    bn_bwd_reduce_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, workspace, st);
-    launch_pdl(bn_affine_grad_kernel, dim3((channels + 127) / 128), dim3(128), 0, st, static_cast<const double*>(workspace), static_cast<int>(channels),
-               dgamma, dbeta);
-    return launch_status("bn_act_bwd_reduce");
+    return bn_act_bwd_reduce_impl("bn_act_bwd_reduce", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act,
+                                  0.0f, dgamma, dbeta, workspace, stream);
+}
+
+extern "C" Y5_API int y5_bn_act_bwd_reduce_ex(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                                              int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
+                                              const float* gamma, const float* beta, int32_t act, float slope, float* dgamma, float* dbeta,
+                                              void* workspace, void* stream) {
+    return bn_act_bwd_reduce_impl("bn_act_bwd_reduce_ex", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta,
+                                  act, slope, dgamma, dbeta, workspace, stream);
 }
 
 extern "C" Y5_API int y5_bn_act_bwd_apply(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
                                           int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
                                           const float* gamma, int32_t act, const void* sums, const void* count, void* stream) {
+    if (int e = check_act("bn_act_bwd_apply", act, 0.0f)) return e;
     if (int e = bn_bwd_check("bn_act_bwd_apply", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, sums)) return e;
     if (!count) return set_error(Y5_E_INVALID, "bn_act_bwd_apply: bad argument");
     count_launch();

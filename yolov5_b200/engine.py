@@ -8,7 +8,7 @@ What the reference does layer by layer through torch.nn (models/yolo.py:160-170 
   * C3's cv1 and cv2 (same input, models/common.py:246) run as ONE GEMM with stacked output channels that lands
     directly in the C3's concat buffer; each Bottleneck's residual add (models/common.py:181) is the epilogue of its
     3x3 conv, in place; SPPF's three pools are one kernel; Upsample writes into its Concat slice;
-  * Conv = conv + folded BN + SiLU in one wgmma implicit-GEMM kernel (weights are folded/packed once, here);
+  * Conv = conv + folded BN + SiLU / (Leaky)ReLU in one wgmma implicit-GEMM kernel (weights are folded/packed once, here);
   * the Detect/Segment head levels run the GEMM with the decode epilogue and write fresh output tensors each call;
   * the whole fixed part is captured in a CUDA graph and replayed.
 
@@ -136,6 +136,20 @@ def block_k(cin: int, cout: int, m_rows: int) -> int:
     return v
 
 
+def act_spec(act: torch.nn.Module) -> tuple[int, float]:
+    """(Y5_ACT_* code, negative slope) of a Conv's activation module: SiLU, Identity, ReLU (LeakyReLU with slope 0) or LeakyReLU
+    with a finite slope.  Any other activation raises NotImplementedError with its name."""
+    if isinstance(act, torch.nn.SiLU):
+        return _lib.ACT_SILU, 0.0
+    if isinstance(act, torch.nn.Identity):
+        return _lib.ACT_NONE, 0.0
+    if isinstance(act, torch.nn.ReLU):
+        return _lib.ACT_LEAKY, 0.0
+    if isinstance(act, torch.nn.LeakyReLU) and math.isfinite(act.negative_slope):
+        return _lib.ACT_LEAKY, float(act.negative_slope)
+    raise NotImplementedError(f"y5b200: activation {act!r} (SiLU, ReLU, LeakyReLU and Identity are built)")
+
+
 # The input-view fields of y5_conv_desc and y5_wgrad_desc (include/y5b200.h): an NHWC view of in_c channels at element pointer
 # `inp`, in_pitch elements per pixel.  The optional ones (0: the plain case) describe the strided views of stem_geom.
 ConvInput = namedtuple("ConvInput", "inp in_pitch batch in_h in_w in_c kw pad_w in_x_stride in_y_stride in_n_stride", defaults=(0,) * 5)
@@ -153,16 +167,17 @@ def stem_geom(buf: torch.Tensor, wide: bool) -> ConvInput:
 
 
 def conv_desc(x: ConvInput, wp: torch.Tensor, bias: torch.Tensor, bk: int, out: int, out_pitch: int, k: int, s: int, p: int,
-              act: bool, dtype: torch.dtype, residual: int | None = None, res_pitch: int = 0) -> ConvDesc:
+              act: bool | tuple[int, float], dtype: torch.dtype, residual: int | None = None, res_pitch: int = 0) -> ConvDesc:
     """y5_conv_desc of out = act(conv(x, w) + bias [+ residual]).  wp: w packed [cout][k][kw][cin_pad] for K block bk (pack_weight,
-    fold_pack); bias: fp32 [cout]; out / residual: element pointers of NHWC views with their pitches."""
+    fold_pack); bias: fp32 [cout]; out / residual: element pointers of NHWC views with their pitches; act: an act_spec pair, or a
+    bool for SiLU / none."""
     d = ConvDesc()
     d.inp, d.in_pitch, d.batch, d.in_h, d.in_w, d.in_c, d.kw, d.pad_w, d.in_x_stride, d.in_y_stride, d.in_n_stride = x
     d.weight, d.bias = wp.data_ptr(), bias.data_ptr()
     d.out, d.out_pitch, d.out_c = out, out_pitch, wp.shape[0]
     d.residual, d.res_pitch = residual, res_pitch
     d.ksize, d.stride, d.pad = k, s, p
-    d.act = _lib.ACT_SILU if act else _lib.ACT_NONE
+    d.act, d.act_slope = act if isinstance(act, tuple) else (_lib.ACT_SILU if act else _lib.ACT_NONE, 0.0)
     d.dtype, d.block_k = _lib.dtype_code(dtype), bk
     return d
 
@@ -278,8 +293,9 @@ class Program:
         self._plans.append((self.lib.y5_conv_plan_destroy, plan))
         self.ops.append(_Op(name, self.lib.y5_conv_plan_run, (plan,)))
 
-    def conv(self, x: View, out: View, packed, k: int, s: int, p: int, act: bool, residual: View | None = None, name: str = "conv"):
-        """Emit one fused conv of view x into view out; packed = (wp, bias, block_k) as fold_pack returns them."""
+    def conv(self, x: View, out: View, packed, k: int, s: int, p: int, act, residual: View | None = None, name: str = "conv"):
+        """Emit one fused conv of view x into view out; packed = (wp, bias, block_k) as fold_pack returns them; act as conv_desc
+        takes it."""
         wp, bias, bk = packed
         ho, wo = (x.h + 2 * p - k) // s + 1, (x.w + 2 * p - k) // s + 1
         cout, cin = out.c, x.c
@@ -295,9 +311,7 @@ class Program:
     def conv_module(self, m, x: View, out: View, residual: View | None = None, name="conv"):
         """m: models.common.Conv (conv + bn + act) in its fused or unfused state."""
         k, s, p = m.conv.kernel_size[0], m.conv.stride[0], m.conv.padding[0]
-        act = isinstance(m.act, torch.nn.SiLU)
-        if not act and not isinstance(m.act, torch.nn.Identity):
-            raise NotImplementedError(f"y5b200: activation {type(m.act).__name__} (only SiLU / Identity are built)")
+        act = act_spec(m.act)
         if m.conv.groups != 1 or m.conv.dilation[0] != 1:
             raise NotImplementedError("y5b200: grouped / dilated convolutions are outside the YOLOv5 n..x hot path")
         ho, wo = (x.h + 2 * p - k) // s + 1, (x.w + 2 * p - k) // s + 1
@@ -323,7 +337,7 @@ class Program:
             w, b = fold_conv_bn(m.conv, getattr(m, "bn", None))
             out = out or self.new_view(h2, w2, m.conv.out_channels)
             w3 = stem_weight_s2d(w)  # (O,16,3,3): 3x3/s1/p1 over the 16-channel cells
-            act = isinstance(m.act, torch.nn.SiLU)
+            act = act_spec(m.act)
 
             def stem_conv(wide: bool, form: str):
                 wv = stem_weight_wide(w3) if wide else w3
@@ -349,10 +363,15 @@ class Program:
     def lower_c3(self, m, x: View, out: View | None, name):
         c_ = m.cv1.conv.out_channels
         cat = self.new_view(x.h, x.w, 2 * c_)
-        # cv1 | cv2 stacked along the output channels: one GEMM, result is already the concat layout
-        packed = self.fold_pack([(m.cv1.conv.weight, m.cv1.conv.bias, getattr(m.cv1, "bn", None)),
-                                 (m.cv2.conv.weight, m.cv2.conv.bias, getattr(m.cv2, "bn", None))], self.B * x.h * x.w)
-        self.conv(x, cat, packed, 1, 1, 0, True, None, f"{name}.cv1|cv2")
+        act = act_spec(m.cv1.act)
+        if act == act_spec(m.cv2.act):
+            # cv1 | cv2 stacked along the output channels: one GEMM, result is already the concat layout
+            packed = self.fold_pack([(m.cv1.conv.weight, m.cv1.conv.bias, getattr(m.cv1, "bn", None)),
+                                     (m.cv2.conv.weight, m.cv2.conv.bias, getattr(m.cv2, "bn", None))], self.B * x.h * x.w)
+            self.conv(x, cat, packed, 1, 1, 0, act, None, f"{name}.cv1|cv2")
+        else:  # different activations: one GEMM each, into the two halves of the concat
+            self.conv_module(m.cv1, x, cat.slice(0, c_), None, f"{name}.cv1")
+            self.conv_module(m.cv2, x, cat.slice(c_, c_), None, f"{name}.cv2")
         a = cat.slice(0, c_)
         if len(m.m):
             tmp = self.new_view(x.h, x.w, c_)

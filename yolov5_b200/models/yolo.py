@@ -66,8 +66,9 @@ def parse_model(d, ch):
     """Model dict -> (nn.Sequential, save list); same scaling rules as reference models/yolo.py:375-458."""
     anchors, nc, gd, gw = d["anchors"], d["nc"], d["depth_multiple"], d["width_multiple"]
     ch_mul = d.get("channel_multiple") or 8
-    if d.get("activation"):
-        raise NotImplementedError("y5b200: custom activations are outside the hot path (SiLU only)")
+    act = d.get("activation")
+    if act:  # e.g. "nn.LeakyReLU(0.1)" (models/hub/yolov5s-LeakyReLU.yaml): every Conv built from here on uses it
+        Conv.default_act = eval(act, {"nn": nn, "torch": torch})
     na = (len(anchors[0]) // 2) if isinstance(anchors, list) else anchors
     no = na * (nc + 5)
     layers, save, c2 = [], [], ch[-1]

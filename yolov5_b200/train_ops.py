@@ -1,4 +1,5 @@
-"""Training-mode execution of the hot path: Conv = SiLU(BN_batchstats(conv(x))) forward and backward on liby5b200.
+"""Training-mode execution of the hot path: Conv = act(BN_batchstats(conv(x))) forward and backward on liby5b200, act = SiLU,
+LeakyReLU / ReLU or none.
 
 Reference: models/common.py:86-88 (Conv.forward), :181 (Bottleneck), :246 (C3), :338-340 (SPPF), :453 (Concat),
 models/yolo.py:95-98 (Detect in training returns the raw (B,na,ny,nx,no) maps), :160-170 (_forward_once routing);
@@ -6,7 +7,7 @@ train.py:401-410 (autocast forward, scaled backward).
 
 What runs where
   * every convolution (forward, data gradient, weight gradient), BatchNorm batch statistics / normalise / backward and
-    SiLU forward / backward: liby5b200 kernels (wgmma implicit GEMMs + HBM-bound passes), wrapped in
+    activation forward / backward: liby5b200 kernels (wgmma implicit GEMMs + HBM-bound passes), wrapped in
     torch.autograd.Function so gradients land in the ordinary ``.grad`` of the nn.Parameters (DDP's bucketed NCCL
     all-reduce -- smart_DDP -- works unchanged); a torch.nn.SyncBatchNorm that syncs (bn_sync_group) all-reduces its column
     sums between the split BN passes (train.py --sync-bn);
@@ -27,7 +28,7 @@ import os
 import torch
 
 from . import _lib
-from .engine import (ConvInput, conv_desc, pack_weight, stem_buffer, stem_geom, stem_s2d, stem_weight_narrow, stem_weight_wide,
+from .engine import (ConvInput, act_spec, conv_desc, pack_weight, stem_buffer, stem_geom, stem_s2d, stem_weight_narrow, stem_weight_wide,
                      wgrad_desc)
 from .engine import block_k as _block_k  # the shared, cached y5_conv_pick lookup
 
@@ -418,7 +419,8 @@ def _wgrad_async(dev, fn, keep):
 
 
 class _ConvBnAct(torch.autograd.Function):
-    """z = act(BN(conv(x, w)))  with batch statistics (training) or running statistics (eval inside a training graph)."""
+    """z = act(BN(conv(x, w)))  with batch statistics (training) or running statistics (eval inside a training graph); act is
+    engine.act_spec's (code, slope) pair."""
 
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, residual, k, s, p, act, eps, momentum, training, stem, pg=None):
@@ -457,7 +459,7 @@ class _ConvBnAct(torch.autograd.Function):
         b, c, ho, wo = y.shape
         rows = b * ho * wo
         code = _lib.dtype_code(y.dtype)
-        fwd_fn, n_rows = lib.y5_bn_act_fwd, None
+        fwd_fn, n_rows = lib.y5_bn_act_fwd_ex, None
         if training:
             mean = torch.empty(c, dtype=torch.float32, device=dev)
             invstd = torch.empty(c, dtype=torch.float32, device=dev)
@@ -472,7 +474,7 @@ class _ConvBnAct(torch.autograd.Function):
                 _lib.check(lib.y5_bn_stats_sync(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats_sync")
                 _all_reduce(ws[: 2 * c + 1], pg)
                 n_rows = ws[2 * c : 2 * c + 1].clone()  # N for the backward: the arena is cleared by the next forward
-                fwd_fn = lib.y5_bn_act_fwd_sync
+                fwd_fn = lib.y5_bn_act_fwd_sync_ex
             sums = ws.data_ptr()
         else:
             mean = running_mean.float().contiguous()
@@ -482,7 +484,7 @@ class _ConvBnAct(torch.autograd.Function):
         z = torch.empty_like(y)
         res, resp = (None, 0) if residual is None else _nhwc(residual)
         _lib.check(fwd_fn(y.data_ptr(), c, z.data_ptr(), c, rows, c, code, mean.data_ptr(), invstd.data_ptr(), g32.data_ptr(),
-                          b32.data_ptr(), 1 if act else 0, sums, eps, momentum, rm.data_ptr() if rm is not None else None,
+                          b32.data_ptr(), *act, sums, eps, momentum, rm.data_ptr() if rm is not None else None,
                           rv.data_ptr() if rv is not None else None, res.data_ptr() if res is not None else None, resp,
                           _st(dev)), "bn_act_fwd")
         if training:
@@ -516,16 +518,16 @@ class _ConvBnAct(torch.autograd.Function):
         dbeta = torch.empty(c, dtype=torch.float32, device=dev)
         ws = _bn_ws(c, dev)
         if ctx.pg is None:
-            _lib.check(lib.y5_bn_act_bwd(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(), invstd.data_ptr(),
-                                         g32.data_ptr(), b32.data_ptr(), 1 if act else 0, dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(),
-                                         _st(dev)), "bn_act_bwd")
+            _lib.check(lib.y5_bn_act_bwd_ex(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                            invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(), dbeta.data_ptr(),
+                                            ws.data_ptr(), _st(dev)), "bn_act_bwd")
         else:  # SyncBatchNorm: dgamma / dbeta stay this rank's sums (DDP averages them); dy uses the sums of every rank over N
-            _lib.check(lib.y5_bn_act_bwd_reduce(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
-                                                invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), 1 if act else 0, dgamma.data_ptr(),
-                                                dbeta.data_ptr(), ws.data_ptr(), _st(dev)), "bn_act_bwd_reduce")
+            _lib.check(lib.y5_bn_act_bwd_reduce_ex(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                                   invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(),
+                                                   dbeta.data_ptr(), ws.data_ptr(), _st(dev)), "bn_act_bwd_reduce")
             _all_reduce(ws[: 2 * c], ctx.pg)
             _lib.check(lib.y5_bn_act_bwd_apply(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
-                                               invstd.data_ptr(), g32.data_ptr(), 1 if act else 0, ws.data_ptr(), ctx.n_rows.data_ptr(),
+                                               invstd.data_ptr(), g32.data_ptr(), act[0], ws.data_ptr(), ctx.n_rows.data_ptr(),
                                                _st(dev)), "bn_act_bwd_apply")
         def wgrad():
             g = stem_wgrad_wide(x, dy) if ctx.wide else conv_wgrad(x, dy, ke, se, pe)
@@ -627,9 +629,7 @@ def conv_module(m, x, stem: int = 0, residual=None):  # stem: 0 no, 1 space-to-d
     bn = getattr(m, "bn", None)
     if bn is None:
         raise RuntimeError("y5b200: cannot train a fused model (Conv without BatchNorm); build it unfused")
-    act = isinstance(m.act, torch.nn.SiLU)
-    if not act and not isinstance(m.act, torch.nn.Identity):
-        raise NotImplementedError(f"y5b200: activation {type(m.act).__name__}")
+    act = act_spec(m.act)
     if m.conv.groups != 1 or m.conv.dilation[0] != 1:
         raise NotImplementedError("y5b200: grouped / dilated convolutions are outside the YOLOv5 n..x hot path")
     k, s, p = m.conv.kernel_size[0], m.conv.stride[0], m.conv.padding[0]
