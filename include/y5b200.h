@@ -756,6 +756,24 @@ int y5_ap_per_class(const uint8_t* tp, const uint8_t* tp2, int64_t tp_img_stride
                     int32_t rows_per_image, int32_t niou, const float* target_cls, int32_t nt, const double* grid, double eps,
                     void* workspace, int64_t workspace_bytes, double* out, int32_t* meta, void* stream);
 
+/* Fused multi-head softmax attention (nn.MultiheadAttention's core with dropout 0, as the C3TR transformer layers run it):
+ * per image b and head h, O = softmax(scale * Q K^T) V over `seq` tokens.  Token l of image b is row b*seq + l of each view;
+ * head h owns the channels [h*head_dim, (h+1)*head_dim) of q, k, v (rows of `qkv_pitch` elements, e.g. the Q | K | V channel
+ * slices of one (batch*seq, 3c) buffer) and of o (rows of `o_pitch`).  Other channels are neither read nor written.
+ * head_dim 32, 64, 96, 128 or 160 (Y5_E_UNSUPPORTED otherwise); dtype Y5_F16 | Y5_BF16; any seq >= 1.  q, k, v, o 16-byte
+ * aligned, pitches multiples of 8 and >= heads*head_dim (Y5_E_INVALID otherwise).  Products in fp32, online softmax in fp32,
+ * O rounded once.  lse (optional, 4-byte aligned): the natural logsumexp of every row's scaled logits, [batch][heads][seq]
+ * fp32, which y5_attention_bwd needs.  No L x L tensor is written; no allocation, no synchronisation. */
+int y5_attention_fwd(const void* q, const void* k, const void* v, int32_t qkv_pitch, void* o, int32_t o_pitch, float* lse, int32_t batch,
+                     int32_t seq, int32_t heads, int32_t head_dim, float scale, int32_t dtype, void* stream);
+/* Its backward: dq, dk, dv (rows of `dqkv_pitch`, head channels as above) from q, k, v, o, dout (rows of `dout_pitch`) and the
+ * forward's lse.  P is recomputed tile by tile from lse; delta is a workspace of batch*heads*seq fp32 (the row sums of
+ * dout * o).  Same argument rules as y5_attention_fwd; every pointer is required.  Three launches, no atomics: the result
+ * repeats bit for bit. */
+int y5_attention_bwd(const void* q, const void* k, const void* v, int32_t qkv_pitch, const void* o, int32_t o_pitch, const void* dout,
+                     int32_t dout_pitch, const float* lse, float* delta, void* dq, void* dk, void* dv, int32_t dqkv_pitch, int32_t batch,
+                     int32_t seq, int32_t heads, int32_t head_dim, float scale, int32_t dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

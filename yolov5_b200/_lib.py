@@ -263,6 +263,8 @@ SIGNATURES = {
     "y5_cross_entropy": (_I32, [_P, _I32, _I32, _I32, _I64, _P, _F, _P, _P, _I64, _P, _P, _P]),
     "y5_ap_workspace_bytes": (_I64, [_I32, _I32, _I32, _I32, _I32]),
     "y5_ap_per_class": (_I32, [_P, _P, _I64, _I32, _P, _P, _I64, _I32, _P, _I32, _I32, _I32, _P, _I32, _P, C.c_double, _P, _I64, _P, _P, _P]),
+    "y5_attention_fwd": (_I32, [_P, _P, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _F, _I32, _P]),
+    "y5_attention_bwd": (_I32, [_P, _P, _P, _I32, _P, _I32, _P, _I32, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _F, _I32, _P]),
 }
 
 AP_META = 5  # include/y5b200.h Y5_AP_META

@@ -35,6 +35,7 @@ SOURCES = {
     "aug_kernels.cu": ["-fmad=false"],
     "seg_aug_kernels.cu": ["-fmad=false"],
     "cls_kernels.cu": [],
+    "attention.cu": [],
     "ap_metrics.cu": ["-fmad=false"],
 }
 

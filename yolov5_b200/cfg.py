@@ -6,6 +6,9 @@ scaling multiples.  Here the topology is data in code so the engine needs no fil
 ``model_cfg`` returns a dict with exactly the keys ``yaml.safe_load`` yields for the reference
 files (pinned by tests/test_cfg_golden.py against a digest taken from the reference YAMLs).
 A user-supplied ``*.yaml`` path is still accepted by ``DetectionModel`` (see models/yolo.py).
+
+``yolov5s-transformer`` (reference models/hub/yolov5s-transformer.yaml) is yolov5s with a C3TR in place of the backbone's last
+C3 (layer 8); it is a built-in name too, pinned by tests/test_transformer_cpu.py against a digest of that YAML.
 """
 from __future__ import annotations
 
@@ -61,10 +64,15 @@ def model_names() -> list[str]:
 
 
 def model_cfg(name: str) -> dict:
-    """Return the model dict for ``yolov5s`` / ``yolov5l.yaml`` / ``models/segment/yolov5x-seg.yaml`` ..."""
+    """Return the model dict for ``yolov5s`` / ``yolov5l.yaml`` / ``models/segment/yolov5x-seg.yaml`` /
+    ``models/hub/yolov5s-transformer.yaml`` ..."""
     stem = Path(str(name)).name
     if stem.endswith(".yaml"):
         stem = stem[: -len(".yaml")]
+    if stem == "yolov5s-transformer":
+        cfg = model_cfg("yolov5s")
+        cfg["backbone"][8][2] = "C3TR"  # [-1, 3, C3TR, [1024]]: layer 8, the backbone's last C3
+        return cfg
     seg = stem.endswith("-seg")
     key = stem[: -len("-seg")] if seg else stem
     if not (key.startswith("yolov5") and key[6:] in _SCALES):

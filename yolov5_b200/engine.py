@@ -25,6 +25,7 @@ import torch
 
 from . import _lib
 from ._lib import ConvDesc, DetectDesc, WgradDesc
+from .models.common import TransformerBlock, transformer_spec
 
 BN_EPS_DEFAULT = 1e-3
 # Detect head GEMM (conv_gemm.cu): an anchor's no = 5 + nc + nm outputs are ceil(no / HEAD_N) N tiles of HEAD_N columns
@@ -373,14 +374,50 @@ class Program:
             self.conv_module(m.cv1, x, cat.slice(0, c_), None, f"{name}.cv1")
             self.conv_module(m.cv2, x, cat.slice(c_, c_), None, f"{name}.cv2")
         a = cat.slice(0, c_)
-        if len(m.m):
-            tmp = self.new_view(x.h, x.w, c_)
-        for j, bt in enumerate(m.m):
-            self.conv_module(bt.cv1, a, tmp, None, f"{name}.m{j}.cv1")
-            self.conv_module(bt.cv2, tmp, a, a if bt.add else None, f"{name}.m{j}.cv2")  # in-place residual add
+        if isinstance(m.m, TransformerBlock):  # C3TR
+            self.lower_transformer(m.m, a, f"{name}.m")
+        else:
+            if len(m.m):
+                tmp = self.new_view(x.h, x.w, c_)
+            for j, bt in enumerate(m.m):
+                self.conv_module(bt.cv1, a, tmp, None, f"{name}.m{j}.cv1")
+                self.conv_module(bt.cv2, tmp, a, a if bt.add else None, f"{name}.m{j}.cv2")  # in-place residual add
         out = out or self.new_view(x.h, x.w, m.cv3.conv.out_channels)
         self.conv_module(m.cv3, cat, out, None, f"{name}.cv3")
         return out
+
+    def lower_transformer(self, tb, a: View, name):
+        """C3TR's TransformerBlock (reference models/common.py:115-161) over the H*W tokens of view `a`, in place: its result
+        lands in `a` (the C3's concat slice).  Per layer, with the projections folded in fp32 here, as BatchNorm is:
+          qkv = x [in_q q | in_k k | in_v v]^T + in_proj_bias      one GEMM with 3c outputs
+          o   = y5_attention_fwd(qkv)                              per image and head, softmax(q k^T / sqrt(dh)) v
+          x   = o out_proj^T + out_proj.bias + x                   the residual rides the GEMM epilogue
+          x   = x (fc2 fc1)^T + x                                  fc2 . fc1 folded into one GEMM
+        after the position embedding x = a linear^T + linear.bias + a."""
+        heads, dh = transformer_spec(tb, training=False)
+        c, m_rows, es = a.c, self.B * a.h * a.w, self.dtype.itemsize
+
+        def packed(w, b):
+            return self.fold_pack([(w.reshape(w.shape[0], w.shape[1], 1, 1), b, None)], m_rows)
+
+        x = self.new_view(a.h, a.w, c)
+        qkv, o, y = self.new_view(a.h, a.w, 3 * c), self.new_view(a.h, a.w, c), self.new_view(a.h, a.w, c)
+        self.conv(a, x, packed(tb.linear.weight, tb.linear.bias), 1, 1, 0, False, a, f"{name}.linear")
+        seq = a.h * a.w
+        for j, layer in enumerate(tb.tr):
+            ma, nm = layer.ma, f"{name}.tr{j}"
+            wi = ma.in_proj_weight.detach().float()
+            w_qkv = torch.cat([wi[i * c : (i + 1) * c] @ lin.weight.detach().float() for i, lin in enumerate((layer.q, layer.k, layer.v))])
+            self.conv(x, qkv, packed(w_qkv, ma.in_proj_bias.detach().float()), 1, 1, 0, False, None, f"{nm}.qkv")
+            self.ops.append(_Op(f"{nm}.attn", self.lib.y5_attention_fwd, (qkv.ptr, qkv.ptr + c * es, qkv.ptr + 2 * c * es, qkv.pitch, o.ptr,
+                                                                         o.pitch, None, self.B, seq, heads, dh, dh ** -0.5, self.dt_code)))
+            self.flops += 4 * self.B * heads * seq * seq * dh
+            self.act_bytes += 2 * self.B * seq * 4 * c
+            self.conv(o, y, packed(ma.out_proj.weight, ma.out_proj.bias), 1, 1, 0, False, x, f"{nm}.out_proj")
+            w_fc = layer.fc2.weight.detach().float() @ layer.fc1.weight.detach().float()
+            self.conv(y, a if j == len(tb.tr) - 1 else x, packed(w_fc, None), 1, 1, 0, False, y, f"{nm}.fc2.fc1")
+        if not len(tb.tr):
+            self.copy_into(x, a, f"{name}.copy")
 
     def lower_sppf(self, m, x: View, out: View | None, name):
         c_ = m.cv1.conv.out_channels

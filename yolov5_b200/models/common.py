@@ -1,5 +1,5 @@
 """Layer zoo of the hot path with the reference's class names, constructor signatures, attribute names and
-state_dict keys (reference models/common.py:62-92,164-181,230-246,318-340,443-453,1104-1140), so checkpoints and
+state_dict keys (reference models/common.py:62-92,115-181,230-270,318-340,443-453,1104-1140), so checkpoints and
 state_dicts move between the two unchanged.  The modules only *hold* parameters: executing one (``forward``) lowers it
 to liby5b200 kernels through yolov5_b200.engine.Program (eval) or yolov5_b200.train_ops (training: batch-statistics
 BatchNorm, autograd) -- there is no torch.nn convolution behind them and CPU tensors are rejected.
@@ -137,6 +137,78 @@ class C3(_EngineLayer):
         self.cv2 = Conv(c1, c_, 1, 1)
         self.cv3 = Conv(2 * c_, c2, 1)
         self.m = nn.Sequential(*(Bottleneck(c_, c_, shortcut, g, e=1.0) for _ in range(n)))
+
+
+class TransformerLayer(nn.Module):
+    """x = ma(q(x), k(x), v(x)) + x;  x = fc2(fc1(x)) + x  (no LayerNorm, no activation).  `ma` is a real nn.MultiheadAttention
+    because it holds the in- and out-projection parameters under the reference's keys; its forward never runs: the layer is
+    lowered inside C3TR (engine: folded GEMMs around y5_attention_fwd; training: train_ops)."""
+
+    def __init__(self, c, num_heads):
+        super().__init__()
+        self.q = nn.Linear(c, c, bias=False)
+        self.k = nn.Linear(c, c, bias=False)
+        self.v = nn.Linear(c, c, bias=False)
+        self.ma = nn.MultiheadAttention(embed_dim=c, num_heads=num_heads)
+        self.fc1 = nn.Linear(c, c, bias=False)
+        self.fc2 = nn.Linear(c, c, bias=False)
+
+    def forward(self, x):
+        raise RuntimeError("y5b200: TransformerLayer runs inside C3TR (GEMMs and y5_attention kernels)")
+
+
+class TransformerBlock(nn.Module):
+    """Learnable position embedding p + linear(p) followed by `num_layers` TransformerLayers over the H*W tokens of each image.
+    `conv` exists only when c1 != c2 (as in the reference); no model dict builds that case and the engine refuses it."""
+
+    def __init__(self, c1, c2, num_heads, num_layers):
+        super().__init__()
+        self.conv = None
+        if c1 != c2:
+            self.conv = Conv(c1, c2)
+        self.linear = nn.Linear(c2, c2)  # learnable position embedding
+        self.tr = nn.Sequential(*(TransformerLayer(c2, num_heads) for _ in range(num_layers)))
+        self.c2 = c2
+
+    def forward(self, x):
+        raise RuntimeError("y5b200: TransformerBlock runs inside C3TR (GEMMs and y5_attention kernels)")
+
+
+ATTN_HEAD_DIMS = (32, 64, 96, 128, 160)  # the head dims y5_attention_fwd / _bwd are built for
+
+
+def transformer_spec(tb: TransformerBlock, training: bool) -> tuple[int, int]:
+    """(heads, head dim) of a TransformerBlock the kernels run; NotImplementedError naming any other configuration."""
+    if tb.conv is not None:
+        raise NotImplementedError("y5b200: TransformerBlock with c1 != c2 (its input Conv) is not built; C3TR never creates one")
+    heads = dh = None
+    for j, layer in enumerate(tb.tr):
+        ma = layer.ma
+        if not isinstance(ma, nn.MultiheadAttention):
+            raise NotImplementedError(f"y5b200: TransformerLayer {j}: attention module {type(ma).__name__}")
+        if (not ma._qkv_same_embed_dim or ma.batch_first or ma.bias_k is not None or ma.add_zero_attn or ma.in_proj_bias is None
+                or ma.out_proj.bias is None or ma.embed_dim != tb.c2):
+            raise NotImplementedError(f"y5b200: TransformerLayer {j}: nn.MultiheadAttention configuration (kdim/vdim != embed_dim, "
+                                      "batch_first, add_bias_kv, add_zero_attn or no bias) outside nn.MultiheadAttention(c, heads)")
+        if ma.head_dim not in ATTN_HEAD_DIMS:
+            raise NotImplementedError(f"y5b200: attention head dim {ma.head_dim} (built: {ATTN_HEAD_DIMS})")
+        if training and ma.dropout > 0:
+            raise NotImplementedError(f"y5b200: attention dropout {ma.dropout} in training (its mask cannot follow torch's RNG)")
+        if heads is not None and (ma.num_heads, ma.head_dim) != (heads, dh):
+            raise NotImplementedError("y5b200: TransformerLayers with different head counts in one block")
+        heads, dh = ma.num_heads, ma.head_dim
+    if tb.linear.bias is None:
+        raise NotImplementedError("y5b200: TransformerBlock position embedding without bias")
+    return heads, dh
+
+
+class C3TR(C3):
+    """C3 whose `m` is a TransformerBlock(c_, c_, 4, n) (reference models/common.py:261-270)."""
+
+    def __init__(self, c1, c2, n=1, shortcut=True, g=1, e=0.5):
+        super().__init__(c1, c2, n, shortcut, g, e)
+        c_ = int(c2 * e)
+        self.m = TransformerBlock(c_, c_, 4, n)
 
 
 class SPPF(_EngineLayer):

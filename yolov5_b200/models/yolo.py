@@ -19,7 +19,7 @@ import torch
 from torch import nn
 
 from ..cfg import model_cfg
-from .common import (C3, SPPF, Bottleneck, Classify, Concat, Conv, Proto, _cached_program, _drop_engine_cache, _lib_on,  # noqa: F401
+from .common import (C3, C3TR, SPPF, Bottleneck, Classify, Concat, Conv, Proto, _cached_program, _drop_engine_cache, _lib_on,  # noqa: F401
                      _param_version)
 
 
@@ -58,7 +58,7 @@ class Segment(Detect):
         self.proto = Proto(ch[0], self.npr, self.nm)
 
 
-_MODULES = {"Conv": Conv, "C3": C3, "SPPF": SPPF, "Bottleneck": Bottleneck, "Concat": Concat, "nn.Upsample": nn.Upsample,
+_MODULES = {"Conv": Conv, "C3": C3, "C3TR": C3TR, "SPPF": SPPF, "Bottleneck": Bottleneck, "Concat": Concat, "nn.Upsample": nn.Upsample,
             "Detect": Detect, "Segment": Segment}
 
 
@@ -80,12 +80,12 @@ def parse_model(d, ch):
             m = _MODULES[m]
         args = [names.get(a, a) if isinstance(a, str) else a for a in args]
         n = n_ = max(round(n * gd), 1) if n > 1 else n
-        if m in (Conv, Bottleneck, SPPF, C3):
+        if m in (Conv, Bottleneck, SPPF, C3, C3TR):
             c1, c2 = ch[f], args[0]
             if c2 != no:
                 c2 = make_divisible(c2 * gw, ch_mul)
             args = [c1, c2, *args[1:]]
-            if m is C3:
+            if m in (C3, C3TR):
                 args.insert(2, n)
                 n = 1
         elif m is Concat:

@@ -583,6 +583,96 @@ class _ConvBias(torch.autograd.Function):
         return dx, dw.to(ctx.wdtype), db[:cout].to(ctx.bdtype)
 
 
+class _Linear(torch.autograd.Function):
+    """y = x W^T (+ bias) (+ residual) over the pixels of an NHWC (B,C,H,W) view: a 1x1 conv on the conv kernels, the residual
+    added in its epilogue.  Backward: y5_conv_wgrad, the data-gradient conv and y5_col_sum, as _ConvBias does."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual):
+        x, xp = _nhwc(x)
+        b, cin, h, w = x.shape
+        cout = weight.shape[0]
+        wp, _, bk, _ = pack_weights(weight.view(cout, cin, 1, 1), x.dtype, b * h * w)
+        bias32 = _zero_bias(cout, x.device) if bias is None else bias.detach().float().contiguous()
+        res, resp = (None, 0) if residual is None else _nhwc(residual)
+        y = _empty_cl(b, cout, h, w, x.dtype, x.device)
+        d = conv_desc(ConvInput(x.data_ptr(), xp, b, h, w, cin), wp, bias32, bk, y.data_ptr(), cout, 1, 1, 0, False, x.dtype,
+                      res.data_ptr() if res is not None else None, resp)
+        _lib.check(_lib.lib().y5_conv_bn_silu_fwd(C.byref(d), _st(x.device)), "linear")
+        ctx.save_for_backward(x, weight)
+        ctx.has_bias = bias is not None
+        ctx.dtypes = (weight.dtype, bias.dtype if bias is not None else None)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy_in):
+        x, weight = ctx.saved_tensors
+        b, cin, h, w = x.shape
+        cout = weight.shape[0]
+        dy, dp = _nhwc(dy_in if dy_in.dtype == x.dtype else dy_in.to(x.dtype))
+        dw = conv_wgrad(x, dy, 1, 1, 0).view(cout, cin).to(ctx.dtypes[0])
+        db = None
+        if ctx.has_bias:
+            db = torch.empty(cout, dtype=torch.float32, device=x.device)
+            _lib.check(_lib.lib().y5_col_sum(dy.data_ptr(), dp, b * h * w, cout, _lib.dtype_code(dy.dtype), db.data_ptr(),
+                                             _bn_ws(cout, x.device).data_ptr(), _st(x.device)), "col_sum")
+            db = db.to(ctx.dtypes[1])
+        dx = conv_dgrad(dy, weight.view(cout, cin, 1, 1), 1, 1, 0, (h, w)) if ctx.needs_input_grad[0] else None
+        return dx, dw, db, (dy_in if ctx.needs_input_grad[3] else None)
+
+
+class _Attention(torch.autograd.Function):
+    """Per image and head, softmax(q k^T / sqrt(dh)) v over the H*W tokens of NHWC (B,c,H,W) views (y5_attention_fwd, which
+    saves the row logsumexp); the backward recomputes P from it (y5_attention_bwd) and returns dq, dk, dv as channel slices
+    of one (B,3c,H,W) buffer."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, heads, dh):
+        q, k, v = (_cl(t) for t in (q, k, v))
+        b, c, h, w = q.shape
+        seq, dev = h * w, q.device
+        o = _empty_cl(b, c, h, w, q.dtype, dev)
+        lse = torch.empty(b * heads * seq, dtype=torch.float32, device=dev)
+        _lib.check(_lib.lib().y5_attention_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), c, o.data_ptr(), c, lse.data_ptr(), b, seq, heads, dh,
+                                               dh ** -0.5, _lib.dtype_code(q.dtype), _st(dev)), "attention_fwd")
+        ctx.save_for_backward(q, k, v, o, lse)
+        ctx.cfg = (heads, dh)
+        return o
+
+    @staticmethod
+    def backward(ctx, do):
+        q, k, v, o, lse = ctx.saved_tensors
+        heads, dh = ctx.cfg
+        b, c, h, w = q.shape
+        seq, dev = h * w, q.device
+        do = _cl(do if do.dtype == q.dtype else do.to(q.dtype))
+        dqkv = _empty_cl(b, 3 * c, h, w, q.dtype, dev)
+        delta = torch.empty(b * heads * seq, dtype=torch.float32, device=dev)
+        p, es = dqkv.data_ptr(), dqkv.element_size()
+        _lib.check(_lib.lib().y5_attention_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), c, o.data_ptr(), c, do.data_ptr(), c, lse.data_ptr(),
+                                               delta.data_ptr(), p, p + c * es, p + 2 * c * es, 3 * c, b, seq, heads, dh, dh ** -0.5,
+                                               _lib.dtype_code(q.dtype), _st(dev)), "attention_bwd")
+        return dqkv[:, :c], dqkv[:, c : 2 * c], dqkv[:, 2 * c :], None, None
+
+
+def _transformer(tb, x):
+    """TransformerBlock (reference models/common.py:115-161) in training: nothing is folded, so every Linear, the in- and
+    out-projections and the position embedding get their own gradients."""
+    from .models.common import transformer_spec
+
+    heads, dh = transformer_spec(tb, training=True)
+    c = tb.c2
+    x = _Linear.apply(x, tb.linear.weight, tb.linear.bias, x)  # p + linear(p)
+    for layer in tb.tr:
+        ma = layer.ma
+        wi, bi = ma.in_proj_weight, ma.in_proj_bias
+        q, k, v = (_Linear.apply(_Linear.apply(x, lin.weight, None, None), wi[i * c : (i + 1) * c], bi[i * c : (i + 1) * c], None)
+                   for i, lin in enumerate((layer.q, layer.k, layer.v)))
+        x = _Linear.apply(_Attention.apply(q, k, v, heads, dh), ma.out_proj.weight, ma.out_proj.bias, x)
+        x = _Linear.apply(_Linear.apply(x, layer.fc1.weight, None, None), layer.fc2.weight, None, x)
+    return x
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # module-level training forward
 # ---------------------------------------------------------------------------------------------------------------------
@@ -788,6 +878,8 @@ def _run(m, x, dt):
         return conv_module(m, x)
     if isinstance(m, mc.Bottleneck):  # the shortcut add rides on cv2's normalise+activate pass
         return conv_module(m.cv2, conv_module(m.cv1, x), residual=x if m.add else None)
+    if isinstance(m, mc.C3TR):
+        return conv_module(m.cv3, _Concat.apply(_transformer(m.m, conv_module(m.cv1, x)), conv_module(m.cv2, x)))
     if isinstance(m, mc.C3):
         a = conv_module(m.cv1, x)
         for bt in m.m:
