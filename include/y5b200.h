@@ -165,6 +165,11 @@ void y5_detect_plan_destroy(y5_detect_plan* plan);
  * `out` must be 16-byte aligned (Y5_E_INVALID otherwise). */
 int y5_stem_s2d(const void* img, int32_t img_dtype, void* out, int32_t out_dtype, int32_t batch, int32_t h, int32_t w,
                 int32_t out_row_px, int32_t out_x_off, void* stream);
+/* Input of a first layer that is not the v6 stem (models/hub/yolov3*.yaml start with Conv(3, c, 3, 1)): NCHW image (dtypes
+ * as y5_stem_s2d) -> dense NHWC [batch][h][w][out_c] in out_dtype (fp16/bf16), channels 0..2 the image and 3..out_c-1
+ * zero.  out_c a multiple of 8; `out` 16-byte aligned. */
+int y5_image_nhwc(const void* img, int32_t img_dtype, void* out, int32_t out_dtype, int32_t batch, int32_t h, int32_t w,
+                  int32_t out_c, void* stream);
 /* SPPF pooling (models/common.py:338-340): reads view x (c channels), writes maxpool5, maxpool5^2 (=9x9),
  * maxpool5^3 (=13x13) into three views (usually channel slices 1..3 of the buffer whose slice 0 is x).  A NaN in a
  * window makes its maximum NaN, as F.max_pool2d does.  y5_sppf_pool, y5_upsample2x and y5_copy_view move 16-byte
@@ -392,6 +397,25 @@ int64_t y5_sppf_bwd_workspace_bytes(int32_t batch, int32_t h, int32_t w, int32_t
 int y5_sppf_pool_bwd(const void* cat, int32_t cat_pitch, const void* dcat, int32_t dcat_pitch, void* da, int32_t da_pitch,
                      int32_t batch, int32_t h, int32_t w, int32_t c, int32_t ksize, int32_t dtype, void* workspace,
                      void* stream);
+/* Max-pools of the YOLOv3 models over NHWC views (x: h x w, c channels), dtype Y5_F16 | Y5_BF16 | Y5_F32:
+ *   Y5_POOL_K2S2       nn.MaxPool2d(2, 2, 0): y is (h/2) x (w/2)
+ *   Y5_POOL_K2S1_ZPAD  nn.ZeroPad2d((0, 1, 0, 1)) then nn.MaxPool2d(2, 1, 0): y is h x w; the pad cells hold 0
+ * A NaN in a window makes its maximum NaN.  The backward writes dx: each window's gradient goes to its first maximum in
+ * row-major window order (a NaN takes it from earlier cells), as torch's max_pool2d backward does; a window whose maximum
+ * is a pad cell routes nowhere.  Views are 16-byte aligned, c and pitches multiples of 8 (Y5_E_INVALID / Y5_E_UNSUPPORTED). */
+#define Y5_POOL_K2S2 0
+#define Y5_POOL_K2S1_ZPAD 1
+int y5_maxpool2d(const void* x, int32_t x_pitch, void* y, int32_t y_pitch, int32_t batch, int32_t h, int32_t w, int32_t c,
+                 int32_t mode, int32_t dtype, void* stream);
+int y5_maxpool2d_bwd(const void* x, int32_t x_pitch, const void* dy, int32_t dy_pitch, void* dx, int32_t dx_pitch, int32_t batch,
+                     int32_t h, int32_t w, int32_t c, int32_t mode, int32_t dtype, void* stream);
+/* backward of SPP's pools + concat (models/common.py SPP): cat = [a, mp_k(a), mp_2k-1(a), mp_3k-2(a)] (the y5_sppf_pool
+ * buffer), dcat its gradient (4 slices of c channels).  da = dcat[0] + each window's gradient routed to the first maximum
+ * of that window of `a` (torch's tie rule, unlike y5_sppf_pool_bwd's chain through the intermediate pools), summed in fp32
+ * and rounded once.  dtype Y5_F16 | Y5_BF16 | Y5_F32; workspace: y5_spp_bwd_workspace_bytes, 16-byte aligned. */
+int64_t y5_spp_bwd_workspace_bytes(int32_t batch, int32_t h, int32_t w, int32_t c);
+int y5_spp_pool_bwd(const void* a, int32_t a_pitch, const void* dcat, int32_t dcat_pitch, void* da, int32_t da_pitch,
+                    int32_t batch, int32_t h, int32_t w, int32_t c, int32_t ksize, int32_t dtype, void* workspace, void* stream);
 /* y[n, 2i, 2j, :] = x[n, i, j, :], other pixels of the (2h, 2w) output zero */
 int y5_zero_stuff2x(const void* x, int32_t x_pitch, void* y, int32_t y_pitch, int32_t batch, int32_t h, int32_t w,
                     int32_t c, int32_t dtype, void* stream);

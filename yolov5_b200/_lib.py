@@ -15,6 +15,7 @@ LIB_PATH = os.environ.get("Y5B200_LIB") or os.path.join(_HERE, "liby5b200.so")  
 
 Y5_F16, Y5_BF16, Y5_F32, Y5_U8 = 0, 1, 2, 3
 ACT_NONE, ACT_SILU, ACT_LEAKY = 0, 1, 2  # include/y5b200.h Y5_ACT_*
+POOL_K2S2, POOL_K2S1_ZPAD = 0, 1  # include/y5b200.h Y5_POOL_*
 
 _DTYPE = {torch.float16: Y5_F16, torch.bfloat16: Y5_BF16, torch.float32: Y5_F32, torch.uint8: Y5_U8}
 
@@ -265,6 +266,11 @@ SIGNATURES = {
     "y5_ap_per_class": (_I32, [_P, _P, _I64, _I32, _P, _P, _I64, _I32, _P, _I32, _I32, _I32, _P, _I32, _P, C.c_double, _P, _I64, _P, _P, _P]),
     "y5_attention_fwd": (_I32, [_P, _P, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _F, _I32, _P]),
     "y5_attention_bwd": (_I32, [_P, _P, _P, _I32, _P, _I32, _P, _I32, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _F, _I32, _P]),
+    "y5_image_nhwc": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _P]),
+    "y5_maxpool2d": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
+    "y5_maxpool2d_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
+    "y5_spp_bwd_workspace_bytes": (_I64, [_I32, _I32, _I32, _I32]),
+    "y5_spp_pool_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P]),
 }
 
 AP_META = 5  # include/y5b200.h Y5_AP_META

@@ -36,6 +36,7 @@ SOURCES = {
     "seg_aug_kernels.cu": ["-fmad=false"],
     "cls_kernels.cu": [],
     "attention.cu": [],
+    "pool_kernels.cu": [],
     "ap_metrics.cu": ["-fmad=false"],
 }
 

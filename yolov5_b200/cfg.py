@@ -59,6 +59,36 @@ def _topology(head_module: str, head_args: list) -> tuple[list, list]:
     return backbone, head
 
 
+_YOLOV3 = ("yolov3", "yolov3-spp", "yolov3-tiny")
+
+
+def _yolov3(name: str) -> dict:
+    """Reference models/hub/yolov3.yaml, yolov3-spp.yaml and yolov3-tiny.yaml as yaml.safe_load returns them."""
+    conv = lambda c, k=1, s=1: [-1, 1, "Conv", [c, k, s]]  # noqa: E731
+    up = [-1, 1, "nn.Upsample", ["None", 2, "nearest"]]
+    if name == "yolov3-tiny":
+        pool = [-1, 1, "nn.MaxPool2d", [2, 2, 0]]
+        backbone = []
+        for c in (16, 32, 64, 128, 256):
+            backbone += [conv(c, 3, 1), copy.deepcopy(pool)]
+        backbone += [conv(512, 3, 1), [-1, 1, "nn.ZeroPad2d", [[0, 1, 0, 1]]], [-1, 1, "nn.MaxPool2d", [2, 1, 0]]]
+        head = [conv(1024, 3, 1), conv(256, 1, 1), conv(512, 3, 1), [-2, 1, "Conv", [128, 1, 1]], copy.deepcopy(up),
+                [[-1, 8], 1, "Concat", [1]], conv(256, 3, 1), [[19, 15], 1, "Detect", ["nc", "anchors"]]]
+        anchors = [[10, 14, 23, 27, 37, 58], [81, 82, 135, 169, 344, 319]]
+    else:
+        backbone = [conv(32, 3, 1), conv(64, 3, 2), [-1, 1, "Bottleneck", [64]]]
+        for c, n in ((128, 2), (256, 8), (512, 8), (1024, 4)):
+            backbone += [conv(c, 3, 2), [-1, n, "Bottleneck", [c]]]
+        p5 = [-1, 1, "SPP", [512, [5, 9, 13]]] if name == "yolov3-spp" else conv(512, 1, 1)
+        head = [[-1, 1, "Bottleneck", [1024, False]], p5, conv(1024, 3, 1), conv(512, 1, 1), conv(1024, 3, 1),
+                [-2, 1, "Conv", [256, 1, 1]], copy.deepcopy(up), [[-1, 8], 1, "Concat", [1]], [-1, 1, "Bottleneck", [512, False]],
+                [-1, 1, "Bottleneck", [512, False]], conv(256, 1, 1), conv(512, 3, 1), [-2, 1, "Conv", [128, 1, 1]], copy.deepcopy(up),
+                [[-1, 6], 1, "Concat", [1]], [-1, 1, "Bottleneck", [256, False]], [-1, 2, "Bottleneck", [256, False]],
+                [[27, 22, 15], 1, "Detect", ["nc", "anchors"]]]
+        anchors = copy.deepcopy(_ANCHORS)
+    return {"nc": 80, "depth_multiple": 1.0, "width_multiple": 1.0, "anchors": anchors, "backbone": backbone, "head": head}
+
+
 def model_names() -> list[str]:
     return [f"yolov5{k}" for k in _SCALES] + [f"yolov5{k}-seg" for k in _SCALES]
 
@@ -73,6 +103,8 @@ def model_cfg(name: str) -> dict:
         cfg = model_cfg("yolov5s")
         cfg["backbone"][8][2] = "C3TR"  # [-1, 3, C3TR, [1024]]: layer 8, the backbone's last C3
         return cfg
+    if stem in _YOLOV3:
+        return _yolov3(stem)
     seg = stem.endswith("-seg")
     key = stem[: -len("-seg")] if seg else stem
     if not (key.startswith("yolov5") and key[6:] in _SCALES):

@@ -51,6 +51,28 @@ __global__ void stem_s2d_kernel(const T* __restrict__ img, uint4* __restrict__ o
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// plain first layer (models/hub/yolov3*.yaml: Conv(3, c, 3, 1)): NCHW image -> NHWC [B][H][W][out_c], channels 0..2 the
+// image, the rest zero, so the conv GEMM reads it as an out_c-channel map.  One thread per (pixel, 8-channel vector).
+// ---------------------------------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void image_nhwc_kernel(const T* __restrict__ img, uint4* __restrict__ out, int B, int H, int W, int cv, int bf16) {
+    const long long total = static_cast<long long>(B) * H * W * cv;
+    for (long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
+         idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const int c8 = static_cast<int>(idx % cv);
+        const long long pix = idx / cv;
+        uint4 o = make_uint4(0, 0, 0, 0);
+        if (c8 == 0) {
+            const long long hw = static_cast<long long>(H) * W, n = pix / hw, p = pix - n * hw;
+            const T* src = img + n * 3 * hw + p;
+            o.x = pack2(load_px<T>(src), load_px<T>(src + hw), bf16);
+            o.y = pack2(load_px<T>(src + 2 * hw), 0.0f, bf16);
+        }
+        out[idx] = o;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // SPPF: y1 = maxpool_k(x), y2 = maxpool_k(y1), y3 = maxpool_k(y2) with stride 1, pad k/2 (implicit -inf padding).
 // Chained stride-1 max pools compose: y2 is the (2k-1)-window max, y3 the (3k-2)-window max of x, so all three
 // come from one pass over the 13x13 neighbourhood (k=5).  One thread per (pixel, 8-channel vector).
@@ -260,6 +282,27 @@ extern "C" Y5_API int y5_stem_s2d(const void* img, int32_t img_dtype, void* out,
         default: return set_error(Y5_E_UNSUPPORTED, "stem_s2d: image dtype %d", img_dtype);
     }
     return check_launch("stem_s2d");
+}
+
+extern "C" Y5_API int y5_image_nhwc(const void* img, int32_t img_dtype, void* out, int32_t out_dtype, int32_t batch, int32_t h, int32_t w,
+                                    int32_t out_c, void* stream) {
+    if (!img || !out || batch <= 0 || h <= 0 || w <= 0 || out_c < 8 || out_c % 8) return set_error(Y5_E_INVALID, "image_nhwc: bad arguments (out_c a multiple of 8)");
+    if (!half_dtype(out_dtype)) return set_error(Y5_E_UNSUPPORTED, "image_nhwc: output dtype must be fp16/bf16");
+    if (reinterpret_cast<uintptr_t>(out) & 15) return set_error(Y5_E_INVALID, "image_nhwc: output must be 16-byte aligned");
+    const int cv = out_c / 8;
+    const long long total = static_cast<long long>(batch) * h * w * cv;
+    const int threads = 256, grid = grid_for(total, threads);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int bf = out_dtype == Y5_BF16;
+    uint4* o = static_cast<uint4*>(out);
+    switch (img_dtype) {
+        case Y5_U8: image_nhwc_kernel<uint8_t><<<grid, threads, 0, st>>>(static_cast<const uint8_t*>(img), o, batch, h, w, cv, bf); break;
+        case Y5_F16: image_nhwc_kernel<__half><<<grid, threads, 0, st>>>(static_cast<const __half*>(img), o, batch, h, w, cv, bf); break;
+        case Y5_BF16: image_nhwc_kernel<__nv_bfloat16><<<grid, threads, 0, st>>>(static_cast<const __nv_bfloat16*>(img), o, batch, h, w, cv, bf); break;
+        case Y5_F32: image_nhwc_kernel<float><<<grid, threads, 0, st>>>(static_cast<const float*>(img), o, batch, h, w, cv, bf); break;
+        default: return set_error(Y5_E_UNSUPPORTED, "image_nhwc: image dtype %d", img_dtype);
+    }
+    return check_launch("image_nhwc");
 }
 
 extern "C" Y5_API int y5_sppf_pool(const void* x, int32_t x_pitch, void* y1, void* y2, void* y3, int32_t y_pitch, int32_t batch, int32_t h,

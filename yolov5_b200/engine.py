@@ -25,7 +25,7 @@ import torch
 
 from . import _lib
 from ._lib import ConvDesc, DetectDesc, WgradDesc
-from .models.common import TransformerBlock, transformer_spec
+from .models.common import TransformerBlock, pool_modes, spp_kernel, transformer_spec
 
 BN_EPS_DEFAULT = 1e-3
 # Detect head GEMM (conv_gemm.cu): an anchor's no = 5 + nc + nm outputs are ceil(no / HEAD_N) N tiles of HEAD_N columns
@@ -123,6 +123,22 @@ def stem_s2d(img: torch.Tensor, out: torch.Tensor) -> None:
                                       (row - w // 2) // 2, C.c_void_p(_lib.stream_ptr(out.device))), "stem_s2d")
 
 
+IMAGE_C = 16  # channels of the NHWC image buffer of a plain first layer (3 used), a count the conv GEMM takes, as the stem's cells
+
+
+def image_nhwc(img: torch.Tensor, out: torch.Tensor) -> None:
+    """y5_image_nhwc of a (B,3,H,W) image into `out`, a dense NHWC [B][H][W][c] buffer: channels 0..2 the image, the rest zero."""
+    b, _, h, w = img.shape
+    img = img.contiguous()
+    _lib.check(_lib.lib().y5_image_nhwc(img.data_ptr(), _lib.dtype_code(img.dtype), out.data_ptr(), _lib.dtype_code(out.dtype), b, h, w,
+                                        out.shape[3], C.c_void_p(_lib.stream_ptr(out.device))), "image_nhwc")
+
+
+def pad_image_weight(w: torch.Tensor) -> torch.Tensor:
+    """(O,3,k,k) filter of a plain first layer -> (O,IMAGE_C,k,k), zero for the image buffer's padding channels."""
+    return torch.nn.functional.pad(w, (0, 0, 0, 0, 0, IMAGE_C - w.shape[1]))
+
+
 _block_k_cache: dict = {}
 
 
@@ -135,6 +151,12 @@ def block_k(cin: int, cout: int, m_rows: int) -> int:
         _lib.check(_lib.lib().y5_conv_pick(cin, cout, m_rows, C.byref(bk), None), "conv_pick")
         v = _block_k_cache[key] = bk.value
     return v
+
+
+def is_v6_stem(m) -> bool:
+    """The YOLOv5 v6 stem Conv(3, c, 6, 2, 2), which runs as a 3x3 conv over the image's 2x2 space-to-depth cells."""
+    c = m.conv
+    return c.kernel_size[0] == 6 and c.stride[0] == 2 and c.padding[0] == 2 and c.in_channels == 3
 
 
 def act_spec(act: torch.nn.Module) -> tuple[int, float]:
@@ -328,9 +350,17 @@ class Program:
         from .models.common import Conv  # noqa: F401
 
         k, s, p, cin = m.conv.kernel_size[0], m.conv.stride[0], m.conv.padding[0], m.conv.in_channels
-        if isinstance(x, torch.Tensor):  # network input (B,3,H,W) NCHW: stem path
-            if not (k == 6 and s == 2 and p == 2 and cin == 3):
-                raise NotImplementedError("y5b200: the first layer must be the YOLOv5 v6 stem Conv(3, c, 6, 2, 2)")
+        if isinstance(x, torch.Tensor) and not is_v6_stem(m):  # network input, plain Conv(3, c, k, s): over the NHWC image buffer
+            if cin != 3 or m.conv.groups != 1 or m.conv.dilation[0] != 1:
+                raise NotImplementedError(f"y5b200: the first layer must be a plain Conv(3, c, k, s) or the v6 stem, got {m.conv!r}")
+            self.image_in = torch.zeros(self.B, self.H, self.W, IMAGE_C, dtype=self.dtype, device=self.device)
+            x = View(self.image_in, 0, IMAGE_C)
+            ho, wo = self.out_hw(m, x)
+            out = out or self.new_view(ho, wo, m.conv.out_channels)
+            packed = self.fold_pack([(pad_image_weight(m.conv.weight.detach()), m.conv.bias, getattr(m, "bn", None))], self.B * ho * wo)
+            self.conv(x, out, packed, k, s, p, act_spec(m.act), None, name)
+            return out
+        if isinstance(x, torch.Tensor):  # network input (B,3,H,W) NCHW: v6 stem path
             if self.H % 2 or self.W % 2:
                 raise ValueError("y5b200: image height and width must be even")
             h2, w2 = self.H // 2, self.W // 2
@@ -419,9 +449,11 @@ class Program:
         if not len(tb.tr):
             self.copy_into(x, a, f"{name}.copy")
 
-    def lower_sppf(self, m, x: View, out: View | None, name):
+    def lower_sppf(self, m, x: View, out: View | None, name, k: int | None = None):
+        """SPPF, or SPP with pools (k, 2k-1, 3k-2) (k given): both are cv2(cat(a, mp_k(a), mp_k^2(a), mp_k^3(a))), a = cv1(x)."""
         c_ = m.cv1.conv.out_channels
-        k = m.m.kernel_size if isinstance(m.m.kernel_size, int) else m.m.kernel_size[0]
+        if k is None:
+            k = m.m.kernel_size if isinstance(m.m.kernel_size, int) else m.m.kernel_size[0]
         cat = self.new_view(x.h, x.w, 4 * c_)
         s0, s1, s2, s3 = (cat.slice(i * c_, c_) for i in range(4))
         self.conv_module(m.cv1, x, s0, None, f"{name}.cv1")
@@ -429,6 +461,15 @@ class Program:
                             (s0.ptr, s0.pitch, s1.ptr, s2.ptr, s3.ptr, cat.pitch, self.B, x.h, x.w, c_, k, self.dt_code)))
         out = out or self.new_view(x.h, x.w, m.cv2.conv.out_channels)
         self.conv_module(m.cv2, cat, out, None, f"{name}.cv2")
+        return out
+
+    def lower_pool(self, x: View, out: View | None, mode: int, name):
+        """nn.MaxPool2d(2, 2, 0), or the nn.ZeroPad2d((0, 1, 0, 1)) + nn.MaxPool2d(2, 1, 0) pair, as one y5_maxpool2d launch."""
+        ho, wo = (x.h // 2, x.w // 2) if mode == _lib.POOL_K2S2 else (x.h, x.w)
+        out = out or self.new_view(ho, wo, x.c)
+        assert (out.h, out.w, out.c) == (ho, wo, x.c), name
+        self.ops.append(_Op(name, self.lib.y5_maxpool2d, (x.ptr, x.pitch, out.ptr, out.pitch, self.B, x.h, x.w, x.c, mode, self.dt_code)))
+        self.act_bytes += 2 * self.B * (x.h * x.w + ho * wo) * x.c
         return out
 
     def lower_upsample(self, m, x: View, out: View | None, name):
@@ -523,6 +564,7 @@ class Program:
 
         mod = self.module
         self.stem_in = None
+        self.image_in = None
         self.proto_view = None
         self.cls_view = None
         self.single_out = None
@@ -543,6 +585,8 @@ class Program:
             return self.lower_c3(m, x, out, name)
         if isinstance(m, mc.SPPF):
             return self.lower_sppf(m, x, out, name)
+        if isinstance(m, mc.SPP):
+            return self.lower_sppf(m, x, out, name, k=spp_kernel(m))
         if isinstance(m, mc.Bottleneck):
             tmp = self.new_view(x.h, x.w, m.cv1.conv.out_channels)
             self.conv_module(m.cv1, x, tmp, None, f"{name}.cv1")
@@ -565,6 +609,7 @@ class Program:
 
         layers = list(model.model)
         n = len(layers)
+        pools = pool_modes(layers, model.save)
         # pass 1: symbolic (c, h, w) of every layer output
         shp = []
         for i, m in enumerate(layers):
@@ -616,8 +661,13 @@ class Program:
                     off += v.c
                 outs[i] = cat
                 continue
-            xin = (torch.empty(0) if i == 0 else outs[i - 1]) if f == -1 else outs[f]
-            outs[i] = self._lower(m, xin, assigned.get(i), name)
+            xin = (torch.empty(0) if i == 0 else outs[i - 1]) if f == -1 else outs[f % i]  # f < 0 counts back from layer i
+            if isinstance(m, torch.nn.ZeroPad2d):  # runs inside the max-pool after it (pool_modes checked the pair)
+                outs[i] = xin
+            elif isinstance(m, torch.nn.MaxPool2d):
+                outs[i] = self.lower_pool(xin, assigned.get(i), pools[i], name)
+            else:
+                outs[i] = self._lower(m, xin, assigned.get(i), name)
         self.outs = outs
 
     def _shape_of(self, m, src):
@@ -630,8 +680,18 @@ class Program:
             return (m.conv.out_channels, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1)
         if isinstance(m, mc.C3):
             return (m.cv3.conv.out_channels, src[1], src[2])
-        if isinstance(m, mc.SPPF):
+        if isinstance(m, (mc.SPPF, mc.SPP, mc.Bottleneck)):
             return (m.cv2.conv.out_channels, src[1], src[2])
+        if isinstance(m, torch.nn.Sequential):
+            for sub in m:
+                src = self._shape_of(sub, src)
+            return src
+        if isinstance(m, torch.nn.ZeroPad2d):
+            left, right, top, bottom = m.padding
+            return (src[0], src[1] + top + bottom, src[2] + left + right)
+        if isinstance(m, torch.nn.MaxPool2d):  # a form pool_modes accepted: (2, 2, 0) or (2, 1, 0)
+            s = m.stride if isinstance(m.stride, int) else m.stride[0]
+            return (src[0], (src[1] - 2) // s + 1, (src[2] - 2) // s + 1)
         if isinstance(m, torch.nn.Upsample):
             return (src[0], src[1] * 2, src[2] * 2)
         if isinstance(m, mc.Concat):
@@ -661,7 +721,10 @@ class Program:
     def _run_body(self, img: torch.Tensor, use_graph: bool) -> int:
         """stem space-to-depth of `img`, then the fixed part (graph replay); returns the stream pointer."""
         assert img.is_cuda and img.shape == (self.B, 3, self.H, self.W), (img.shape, (self.B, 3, self.H, self.W))
-        stem_s2d(img, self.stem_in)
+        if self.image_in is not None:
+            image_nhwc(img, self.image_in)
+        else:
+            stem_s2d(img, self.stem_in)
         st = _lib.stream_ptr(self.device)
         if use_graph and os.environ.get("Y5_NO_GRAPH") != "1":
             if self.graph is None:
@@ -710,7 +773,8 @@ class Program:
         return y
 
     def launches_per_forward(self) -> int:
-        n = len(self.ops) + len(self.head_ops) + (1 if self.stem_in is not None else 0) + (1 if self.proto_view is not None else 0)
+        n = len(self.ops) + len(self.head_ops) + (1 if self.stem_in is not None or self.image_in is not None else 0)
+        n += 1 if self.proto_view is not None else 0
         return n + (1 if self.cls_view is not None else 0)
 
     def __del__(self):

@@ -220,6 +220,78 @@ class SPPF(_EngineLayer):
         self.m = nn.MaxPool2d(kernel_size=k, stride=1, padding=k // 2)
 
 
+class SPP(_EngineLayer):
+    """Spatial pyramid pooling of yolov3-spp (reference models/common.py SPP): cv2(cat(x, mp_k0(x), mp_k1(x), mp_k2(x))) with
+    x = cv1(input) and stride-1 'same' max-pools.  The engine runs k = (k, 2k-1, 3k-2) -- the default (5, 9, 13) -- because
+    those pools are SPPF's chain mp_k, mp_k^2, mp_k^3 exactly; spp_kernel refuses any other k."""
+
+    def __init__(self, c1, c2, k=(5, 9, 13)):
+        super().__init__()
+        c_ = c1 // 2
+        self.cv1 = Conv(c1, c_, 1, 1)
+        self.cv2 = Conv(c_ * (len(k) + 1), c2, 1, 1)
+        self.m = nn.ModuleList([nn.MaxPool2d(kernel_size=x, stride=1, padding=x // 2) for x in k])
+
+
+def _pool_arg(v):
+    return v if isinstance(v, int) else (v[0] if len(set(v)) == 1 else None)
+
+
+def maxpool_form(m: nn.MaxPool2d) -> tuple[int, int, int] | None:
+    """(kernel, stride, padding) of a square, undilated nn.MaxPool2d without ceil_mode / return_indices, else None."""
+    k, s, p, d = (_pool_arg(m.kernel_size), _pool_arg(m.stride if m.stride is not None else m.kernel_size), _pool_arg(m.padding),
+                  _pool_arg(m.dilation))
+    if None in (k, s, p) or d != 1 or m.ceil_mode or m.return_indices:
+        return None
+    return k, s, p
+
+
+def spp_kernel(m: SPP) -> int:
+    """SPPF kernel size k of an SPP whose pools are stride-1 'same' max-pools of sizes (k, 2k-1, 3k-2), k odd; NotImplementedError
+    naming the configuration otherwise."""
+    forms = [maxpool_form(p) if isinstance(p, nn.MaxPool2d) else None for p in m.m]
+    if len(forms) == 3 and None not in forms:
+        k = forms[0][0]
+        if k % 2 and forms == [(k, 1, k // 2), (2 * k - 1, 1, k - 1), (3 * k - 2, 1, 3 * (k // 2))]:
+            return k
+    raise NotImplementedError(f"y5b200: SPP pools {[p for p in m.m]} (built: three stride-1 'same' max-pools of sizes k, 2k-1, 3k-2, "
+                              "k odd, such as (5, 9, 13))")
+
+
+def pool_mode(m: nn.MaxPool2d, pad: nn.ZeroPad2d | None) -> int:
+    """y5_maxpool2d mode of nn.MaxPool2d(2, 2, 0), or of nn.ZeroPad2d((0, 1, 0, 1)) followed by nn.MaxPool2d(2, 1, 0) (yolov3-tiny);
+    NotImplementedError naming any other pool or pad."""
+    from .. import _lib
+
+    form = maxpool_form(m)
+    if pad is None and form == (2, 2, 0):
+        return _lib.POOL_K2S2
+    if pad is not None and form == (2, 1, 0):
+        if tuple(pad.padding) == (0, 1, 0, 1):
+            return _lib.POOL_K2S1_ZPAD
+        raise NotImplementedError(f"y5b200: {pad!r} before a max-pool (built: nn.ZeroPad2d((0, 1, 0, 1)))")
+    raise NotImplementedError(f"y5b200: {m!r}{' after ' + repr(pad) if pad is not None else ''} (built: nn.MaxPool2d(2, 2, 0), and "
+                              "nn.MaxPool2d(2, 1, 0) after nn.ZeroPad2d((0, 1, 0, 1)); no ceil_mode, dilation or return_indices)")
+
+
+def pool_modes(layers, save) -> dict[int, int]:
+    """y5_maxpool2d mode of every nn.MaxPool2d in a model's layer list.  Checks, before anything runs, that each nn.ZeroPad2d
+    feeds only the max-pool right after it (the pair runs as one kernel, so nothing else may read the padded map) and that
+    every SPP has pools the engine builds; NotImplementedError naming the layer otherwise."""
+    modes = {}
+    for i, m in enumerate(layers):
+        if isinstance(m, nn.ZeroPad2d):
+            nxt = layers[i + 1] if i + 1 < len(layers) else None
+            if not (isinstance(nxt, nn.MaxPool2d) and nxt.f == -1) or i in save:
+                raise NotImplementedError(f"y5b200: layer {i} {m!r} must feed only an nn.MaxPool2d(2, 1, 0) right after it")
+        elif isinstance(m, nn.MaxPool2d):
+            pad = layers[i - 1] if i > 0 and m.f == -1 and isinstance(layers[i - 1], nn.ZeroPad2d) else None
+            modes[i] = pool_mode(m, pad)
+        elif isinstance(m, SPP):
+            spp_kernel(m)
+    return modes
+
+
 class Concat(nn.Module):
     """Channel concatenation.  Inside a model it costs nothing (producers write into slices of one buffer); called on
     its own it has no arithmetic to offload and simply concatenates."""

@@ -19,8 +19,8 @@ import torch
 from torch import nn
 
 from ..cfg import model_cfg
-from .common import (C3, C3TR, SPPF, Bottleneck, Classify, Concat, Conv, Proto, _cached_program, _drop_engine_cache, _lib_on,  # noqa: F401
-                     _param_version)
+from .common import (C3, C3TR, SPP, SPPF, Bottleneck, Classify, Concat, Conv, Proto, _cached_program, _drop_engine_cache,  # noqa: F401
+                     _lib_on, _param_version)
 
 
 def make_divisible(x, divisor):
@@ -58,8 +58,8 @@ class Segment(Detect):
         self.proto = Proto(ch[0], self.npr, self.nm)
 
 
-_MODULES = {"Conv": Conv, "C3": C3, "C3TR": C3TR, "SPPF": SPPF, "Bottleneck": Bottleneck, "Concat": Concat, "nn.Upsample": nn.Upsample,
-            "Detect": Detect, "Segment": Segment}
+_MODULES = {"Conv": Conv, "C3": C3, "C3TR": C3TR, "SPP": SPP, "SPPF": SPPF, "Bottleneck": Bottleneck, "Concat": Concat,
+            "nn.Upsample": nn.Upsample, "nn.MaxPool2d": nn.MaxPool2d, "nn.ZeroPad2d": nn.ZeroPad2d, "Detect": Detect, "Segment": Segment}
 
 
 def parse_model(d, ch):
@@ -76,11 +76,11 @@ def parse_model(d, ch):
     for i, (f, n, m, args) in enumerate(d["backbone"] + d["head"]):
         if isinstance(m, str):
             if m not in _MODULES:
-                raise NotImplementedError(f"y5b200: module '{m}' is outside the engine's hot path (models n/s/m/l/x[-seg])")
+                raise NotImplementedError(f"y5b200: module '{m}' is outside the engine's hot path (models n/s/m/l/x[-seg], yolov3[-spp|-tiny])")
             m = _MODULES[m]
         args = [names.get(a, a) if isinstance(a, str) else a for a in args]
         n = n_ = max(round(n * gd), 1) if n > 1 else n
-        if m in (Conv, Bottleneck, SPPF, C3, C3TR):
+        if m in (Conv, Bottleneck, SPP, SPPF, C3, C3TR):
             c1, c2 = ch[f], args[0]
             if c2 != no:
                 c2 = make_divisible(c2 * gw, ch_mul)
@@ -131,6 +131,9 @@ def _layer_strides(model: nn.Sequential) -> list[float]:
             r = r * m.conv.stride[0]
         elif isinstance(m, nn.Upsample):
             r = r / float(m.scale_factor)
+        elif isinstance(m, nn.MaxPool2d):
+            s = m.stride if m.stride is not None else m.kernel_size
+            r = r * (s if isinstance(s, int) else s[0])
         red.append(r)
     return []
 

@@ -28,8 +28,8 @@ import os
 import torch
 
 from . import _lib
-from .engine import (ConvInput, act_spec, conv_desc, pack_weight, stem_buffer, stem_geom, stem_s2d, stem_weight_narrow, stem_weight_wide,
-                     wgrad_desc)
+from .engine import (IMAGE_C, ConvInput, act_spec, conv_desc, image_nhwc, is_v6_stem, pack_weight, pad_image_weight, stem_buffer, stem_geom,
+                     stem_s2d, stem_weight_narrow, stem_weight_wide, wgrad_desc)
 from .engine import block_k as _block_k  # the shared, cached y5_conv_pick lookup
 
 
@@ -426,7 +426,9 @@ class _ConvBnAct(torch.autograd.Function):
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, residual, k, s, p, act, eps, momentum, training, stem, pg=None):
         lib = _lib.lib()
         dev = x.device
-        if stem:  # x is already the 16-channel space-to-depth image; weight is the (O,3,6,6) stem filter
+        if stem == STEM_IMAGE:  # x is the image_input buffer; weight is the (O,3,k,k) filter, zero-padded to its channels
+            w_eff, ke, se, pe = pad_image_weight(weight.detach()), k, s, p
+        elif stem:  # x is already the 16-channel space-to-depth image; weight is the (O,3,6,6) stem filter
             fwd_idx, _ = _stem_index(dev)
             wf = weight.detach().flatten(1)
             w_eff = torch.cat((wf, wf.new_zeros(wf.shape[0], 1)), 1)[:, fwd_idx].view(-1, 16, 3, 3)
@@ -531,7 +533,9 @@ class _ConvBnAct(torch.autograd.Function):
                                                _st(dev)), "bn_act_bwd_apply")
         def wgrad():
             g = stem_wgrad_wide(x, dy) if ctx.wide else conv_wgrad(x, dy, ke, se, pe)
-            if stem:  # (O,16,3,3) gradient of the space-to-depth filter -> (O,3,6,6)
+            if stem == STEM_IMAGE:  # the image buffer's padding channels carry no filter taps
+                g = g[:, : weight.shape[1]].contiguous()
+            elif stem:  # (O,16,3,3) gradient of the space-to-depth filter -> (O,3,6,6)
                 _, inv_idx = _stem_index(dev)
                 g = g.reshape(g.shape[0], -1)[:, inv_idx].view(weight.shape)
             return g.to(weight.dtype)
@@ -715,16 +719,24 @@ def bn_sync_group(bn):
     return bn_process_group(bn) if bn.training else None
 
 
-def conv_module(m, x, stem: int = 0, residual=None):  # stem: 0 no, 1 space-to-depth 3x3x16, 2 wide-pixel 3x1x48
+STEM_IMAGE = 3  # conv_module(stem=...): a plain first layer over the image_input buffer
+
+
+def _check_conv(m, stem: int = 0):
+    if m.conv.groups != 1 or m.conv.dilation[0] != 1:
+        raise NotImplementedError("y5b200: grouped / dilated convolutions are outside the YOLOv5 n..x hot path")
+    k, s, p = m.conv.kernel_size[0], m.conv.stride[0], m.conv.padding[0]
+    if stem in (0, STEM_IMAGE) and (k, s, p) not in ((1, 1, 0), (3, 1, 1), (3, 2, 1)):
+        raise NotImplementedError(f"y5b200: training conv k{k} s{s} p{p}")
+    return k, s, p
+
+
+def conv_module(m, x, stem: int = 0, residual=None):  # stem: 0 no, 1 space-to-depth 3x3x16, 2 wide-pixel 3x1x48, STEM_IMAGE
     bn = getattr(m, "bn", None)
     if bn is None:
         raise RuntimeError("y5b200: cannot train a fused model (Conv without BatchNorm); build it unfused")
     act = act_spec(m.act)
-    if m.conv.groups != 1 or m.conv.dilation[0] != 1:
-        raise NotImplementedError("y5b200: grouped / dilated convolutions are outside the YOLOv5 n..x hot path")
-    k, s, p = m.conv.kernel_size[0], m.conv.stride[0], m.conv.padding[0]
-    if not stem and (k, s, p) not in ((1, 1, 0), (3, 1, 1), (3, 2, 1)):
-        raise NotImplementedError(f"y5b200: training conv k{k} s{s} p{p}")
+    k, s, p = _check_conv(m, stem)
     training = bn.training
     if training and bn.track_running_stats and bn.num_batches_tracked is not None:
         bn.num_batches_tracked += 1
@@ -785,6 +797,51 @@ class _SppfPoolCat(torch.autograd.Function):
         _lib.check(lib.y5_sppf_pool_bwd(cat.data_ptr(), c4, dcat.data_ptr(), dp, da.data_ptr(), c, b, h, w, c, ctx.k, _lib.dtype_code(cat.dtype),
                                         ws.data_ptr(), _st(cat.device)), "sppf_pool_bwd")
         return da, None
+
+
+class _SppPoolCat(_SppfPoolCat):
+    """cat(a, mp_k(a), mp_2k-1(a), mp_3k-2(a)) of SPP: the forward is SPPF's (the pools compose exactly); the backward routes each
+    pool's gradient to the first maximum of its own window of `a` (y5_spp_pool_bwd), as torch does, not through SPPF's chain."""
+
+    @staticmethod
+    def backward(ctx, dcat):
+        lib = _lib.lib()
+        (cat,) = ctx.saved_tensors
+        b, c4, h, w = cat.shape
+        c = c4 // 4
+        dcat, dp = _nhwc(dcat)
+        da = _empty_cl(b, c, h, w, cat.dtype, cat.device)
+        ws = torch.empty(lib.y5_spp_bwd_workspace_bytes(b, h, w, c), dtype=torch.uint8, device=cat.device)
+        _lib.check(lib.y5_spp_pool_bwd(cat.data_ptr(), c4, dcat.data_ptr(), dp, da.data_ptr(), c, b, h, w, c, ctx.k, _lib.dtype_code(cat.dtype),
+                                       ws.data_ptr(), _st(cat.device)), "spp_pool_bwd")
+        return da, None
+
+
+class _MaxPool(torch.autograd.Function):
+    """nn.MaxPool2d(2, 2, 0), or nn.ZeroPad2d((0, 1, 0, 1)) + nn.MaxPool2d(2, 1, 0) (mode: y5_maxpool2d's), forward and backward."""
+
+    @staticmethod
+    def forward(ctx, x, mode):
+        x, xp = _nhwc(x)
+        b, c, h, w = x.shape
+        ho, wo = (h // 2, w // 2) if mode == _lib.POOL_K2S2 else (h, w)
+        y = _empty_cl(b, c, ho, wo, x.dtype, x.device)
+        _lib.check(_lib.lib().y5_maxpool2d(x.data_ptr(), xp, y.data_ptr(), c, b, h, w, c, mode, _lib.dtype_code(x.dtype), _st(x.device)),
+                   "maxpool2d")
+        ctx.save_for_backward(x)
+        ctx.cfg = (xp, mode)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        xp, mode = ctx.cfg
+        b, c, h, w = x.shape
+        dy, dp = _nhwc(dy if dy.dtype == x.dtype else dy.to(x.dtype))
+        dx = _empty_cl(b, c, h, w, x.dtype, x.device)
+        _lib.check(_lib.lib().y5_maxpool2d_bwd(x.data_ptr(), xp, dy.data_ptr(), dp, dx.data_ptr(), c, b, h, w, c, mode, _lib.dtype_code(x.dtype),
+                                               _st(x.device)), "maxpool2d_bwd")
+        return dx, None
 
 
 class _Concat(torch.autograd.Function):
@@ -855,6 +912,16 @@ def _classify(m, x):
     return y.reshape(y.shape[0], -1)[:, :nc]
 
 
+def image_input(img: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """(B,3,H,W) uint8 / float image -> a (B,IMAGE_C,H,W) channels_last tensor, channels 3.. zero: the input of a plain first layer."""
+    b, c, h, w = img.shape
+    if c != 3:
+        raise ValueError(f"y5b200: expected a (B,3,H,W) image batch, got {tuple(img.shape)}")
+    out = _empty_cl(b, IMAGE_C, h, w, dtype, img.device)
+    image_nhwc(img, out.permute(0, 2, 3, 1))
+    return out
+
+
 def stem_input(img: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
     """(B,3,H,W) uint8 / float image -> its space-to-depth cells (12 of 16 channels used): a stem_buffer for the wide-pixel stem,
     else a (B,16,H/2,W/2) channels_last tensor."""
@@ -888,6 +955,8 @@ def _run(m, x, dt):
     if isinstance(m, mc.SPPF):
         k = m.m.kernel_size if isinstance(m.m.kernel_size, int) else m.m.kernel_size[0]
         return conv_module(m.cv2, _SppfPoolCat.apply(conv_module(m.cv1, x), k))
+    if isinstance(m, mc.SPP):
+        return conv_module(m.cv2, _SppPoolCat.apply(conv_module(m.cv1, x), mc.spp_kernel(m)))
     if isinstance(m, torch.nn.Upsample):
         if float(m.scale_factor) != 2.0 or m.mode != "nearest":
             raise NotImplementedError("y5b200: only nn.Upsample(scale_factor=2, mode='nearest')")
@@ -924,9 +993,12 @@ def forward_train(model, img: torch.Tensor):
     dt = train_dtype(model)
     layers = list(model.model)
     first = layers[0]
-    if not (isinstance(first, mc.Conv) and first.conv.kernel_size[0] == 6 and first.conv.stride[0] == 2 and first.conv.padding[0] == 2
-            and first.conv.in_channels == 3):
-        raise NotImplementedError("y5b200: the first layer must be the YOLOv5 v6 stem Conv(3, c, 6, 2, 2)")
+    if not (isinstance(first, mc.Conv) and first.conv.in_channels == 3):
+        raise NotImplementedError("y5b200: the first layer must be a Conv reading the 3-channel image")
+    stem = is_v6_stem(first)
+    if not stem:
+        _check_conv(first, STEM_IMAGE)
+    pools = mc.pool_modes(layers, model.save)  # every refusal before the first launch
     # every op below picks its dtype explicitly; autocast's own casting rules must not touch the glue ops
     global _cur_plan
     with torch.autocast("cuda", enabled=False):
@@ -938,12 +1010,17 @@ def forward_train(model, img: torch.Tensor):
             ys = []
             x = None
             for i, m in enumerate(layers):
-                if i == 0:
+                if i == 0 and stem:
                     x = conv_module(m, stem_input(img, dt), stem=2 if stem_wide_enabled() else 1)
+                elif i == 0:
+                    x = conv_module(m, image_input(img, dt), stem=STEM_IMAGE)
                 else:
                     if m.f != -1:
                         x = ys[m.f] if isinstance(m.f, int) else [x if j == -1 else ys[j] for j in m.f]
-                    x = _run(m, x, dt)
+                    if isinstance(m, torch.nn.MaxPool2d):
+                        x = _MaxPool.apply(x, pools[i])
+                    elif not isinstance(m, torch.nn.ZeroPad2d):  # a ZeroPad2d runs inside the max-pool after it
+                        x = _run(m, x, dt)
                 ys.append(x if i in model.save else None)
         finally:
             _cur_plan = None
