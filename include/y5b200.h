@@ -798,6 +798,27 @@ int y5_attention_bwd(const void* q, const void* k, const void* v, int32_t qkv_pi
                      int32_t dout_pitch, const float* lse, float* delta, void* dq, void* dk, void* dv, int32_t dqkv_pitch, int32_t batch,
                      int32_t seq, int32_t heads, int32_t head_dim, float scale, int32_t dtype, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Depthwise 5x5 / stride 1 / pad 2 conv of GhostConv's cheap half (models/common.py GhostConv.cv2 = Conv(c_, c_, 5, 1, None, c_))
+ * over NHWC views of c channels (h x w), dtype Y5_F16 | Y5_BF16.
+ *   weight : [c][5][5] in the activation dtype (the (c, 1, 5, 5) filter, y5_fold_pack with in_c = in_c_pad = 1), BN folded in
+ *   bias   : fp32 [c] or NULL
+ * y5_dwconv_fwd: y = act(fp32(sum of the 25 taps) + bias) + residual, the activation and residual as in y5_conv_desc, rounded
+ * once.  flip != 0 rotates the taps 180 degrees: with bias NULL and Y5_ACT_NONE that is the data gradient dx of the conv from
+ * dy = x, and `residual` adds another gradient of x in the same pass.  x_out (optional) receives x + x_res (x_res optional) at
+ * every pixel: GhostBottleneck's first concat half, or a copy of x.  y may alias residual and x_out may alias x_res (in-place
+ * adds); x may alias no output.  residual, x_res, x_out: NULL or views like x.
+ * y5_dwconv_wgrad: fp32 dweight [c][5][5] = sum over (n, y, x) of x[n, y+ky-2, x+kx-2, c] * dy[n, y, x, c] (dweight is
+ * overwritten).  The partial sums are added with fp32 atomics, so the last bits depend on scheduling (as y5_conv_wgrad).
+ * Y5_E_INVALID for: ksize != 5 or stride != 1, c not a positive multiple of 8, a pitch < c or not a multiple of 8, a view not
+ * 16-byte aligned, weight / bias / dweight not 4-byte aligned. */
+int y5_dwconv_fwd(const void* x, int32_t x_pitch, const void* weight, const float* bias, void* y, int32_t y_pitch, const void* residual,
+                  int32_t res_pitch, const void* x_res, int32_t x_res_pitch, void* x_out, int32_t x_out_pitch, int32_t batch, int32_t h,
+                  int32_t w, int32_t c, int32_t ksize, int32_t stride, int32_t act, float act_slope, int32_t flip, int32_t dtype,
+                  void* stream);
+int y5_dwconv_wgrad(const void* x, int32_t x_pitch, const void* dy, int32_t dy_pitch, float* dweight, int32_t batch, int32_t h, int32_t w,
+                    int32_t c, int32_t ksize, int32_t stride, int32_t dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

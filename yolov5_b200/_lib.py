@@ -271,6 +271,9 @@ SIGNATURES = {
     "y5_maxpool2d_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "y5_spp_bwd_workspace_bytes": (_I64, [_I32, _I32, _I32, _I32]),
     "y5_spp_pool_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P]),
+    "y5_dwconv_fwd": (_I32, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _F, _I32,
+                             _I32, _P]),
+    "y5_dwconv_wgrad": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
 }
 
 AP_META = 5  # include/y5b200.h Y5_AP_META

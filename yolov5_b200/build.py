@@ -37,6 +37,7 @@ SOURCES = {
     "cls_kernels.cu": [],
     "attention.cu": [],
     "pool_kernels.cu": [],
+    "dwconv.cu": [],
     "ap_metrics.cu": ["-fmad=false"],
 }
 

@@ -9,6 +9,8 @@ A user-supplied ``*.yaml`` path is still accepted by ``DetectionModel`` (see mod
 
 ``yolov5s-transformer`` (reference models/hub/yolov5s-transformer.yaml) is yolov5s with a C3TR in place of the backbone's last
 C3 (layer 8); it is a built-in name too, pinned by tests/test_transformer_cpu.py against a digest of that YAML.
+``yolov5s-ghost`` (reference models/hub/yolov5s-ghost.yaml) is yolov5s built from GhostConv and C3Ghost; ``model_cfg`` accepts
+it, pinned by tests/test_ghost_cpu.py, but it is not one of ``model_names()``.
 """
 from __future__ import annotations
 
@@ -89,6 +91,18 @@ def _yolov3(name: str) -> dict:
     return {"nc": 80, "depth_multiple": 1.0, "width_multiple": 1.0, "anchors": anchors, "backbone": backbone, "head": head}
 
 
+def _ghost() -> dict:
+    """Reference models/hub/yolov5s-ghost.yaml as yaml.safe_load returns it: yolov5s with every stride-2 Conv and the head's 1x1
+    Convs as GhostConv, and every C3 as C3Ghost."""
+    cfg = model_cfg("yolov5s")
+    for row in cfg["backbone"] + cfg["head"]:
+        if row[2] == "C3":
+            row[2] = "C3Ghost"
+        elif row[2] == "Conv" and row[3] != [64, 6, 2, 2]:  # all but the stem
+            row[2] = "GhostConv"
+    return cfg
+
+
 def model_names() -> list[str]:
     return [f"yolov5{k}" for k in _SCALES] + [f"yolov5{k}-seg" for k in _SCALES]
 
@@ -105,6 +119,8 @@ def model_cfg(name: str) -> dict:
         return cfg
     if stem in _YOLOV3:
         return _yolov3(stem)
+    if stem == "yolov5s-ghost":
+        return _ghost()
     seg = stem.endswith("-seg")
     key = stem[: -len("-seg")] if seg else stem
     if not (key.startswith("yolov5") and key[6:] in _SCALES):

@@ -5,6 +5,8 @@ What the reference does layer by layer through torch.nn (models/yolo.py:160-170 
 
   * every activation is a channel-slice VIEW of a pre-allocated NHWC buffer; a Concat's inputs are allocated inside
     the Concat's buffer, so torch.cat (models/common.py:246,340,453) disappears;
+  * GhostConv's cv1 writes the first half of its output and the depthwise 5x5 conv (y5_dwconv_fwd) reads it and writes the
+    second half; a GhostBottleneck's residual rides the depthwise kernel, which writes both halves of the C3's slice in place;
   * C3's cv1 and cv2 (same input, models/common.py:246) run as ONE GEMM with stacked output channels that lands
     directly in the C3's concat buffer; each Bottleneck's residual add (models/common.py:181) is the epilogue of its
     3x3 conv, in place; SPPF's three pools are one kernel; Upsample writes into its Concat slice;
@@ -25,7 +27,8 @@ import torch
 
 from . import _lib
 from ._lib import ConvDesc, DetectDesc, WgradDesc
-from .models.common import TransformerBlock, pool_modes, spp_kernel, transformer_spec
+from .models.common import (C3Ghost, TransformerBlock, check_grouped_convs, ghost_bottleneck_convs, ghost_dw_channels, pool_modes, spp_kernel,
+                            transformer_spec)
 
 BN_EPS_DEFAULT = 1e-3
 # Detect head GEMM (conv_gemm.cu): an anchor's no = 5 + nc + nm outputs are ceil(no / HEAD_N) N tiles of HEAD_N columns
@@ -406,6 +409,10 @@ class Program:
         a = cat.slice(0, c_)
         if isinstance(m.m, TransformerBlock):  # C3TR
             self.lower_transformer(m.m, a, f"{name}.m")
+        elif isinstance(m, C3Ghost):
+            scratch = None
+            for j, bt in enumerate(m.m):
+                scratch = self.lower_ghost_bottleneck(bt, a, a, f"{name}.m{j}", scratch)
         else:
             if len(m.m):
                 tmp = self.new_view(x.h, x.w, c_)
@@ -415,6 +422,53 @@ class Program:
         out = out or self.new_view(x.h, x.w, m.cv3.conv.out_channels)
         self.conv_module(m.cv3, cat, out, None, f"{name}.cv3")
         return out
+
+    def dwconv(self, m, x: View, out: View, residual: View | None = None, x_out: View | None = None, x_res: View | None = None,
+               name: str = "dwconv"):
+        """GhostConv.cv2 (depthwise 5x5 conv + folded BN + act) of view x into view out on y5_dwconv_fwd, + residual; x_out
+        (optional) receives x + x_res in the same launch.  The weights are y5_fold_pack's [c][5][5][1] packing."""
+        c = x.c
+        wp = torch.empty(c, 5, 5, 1, dtype=self.dtype, device=self.device)
+        bias = torch.empty(c, dtype=torch.float32, device=self.device)
+        self.fold_pack_into([(m.conv.weight, m.conv.bias, getattr(m, "bn", None))], wp, bias, 0, 1)
+        self._keep += [wp, bias]
+        code, slope = act_spec(m.act)
+
+        def view(v):
+            return (v.ptr, v.pitch) if v is not None else (None, 0)
+
+        self.ops.append(_Op(name, self.lib.y5_dwconv_fwd, (x.ptr, x.pitch, wp.data_ptr(), bias.data_ptr(), out.ptr, out.pitch, *view(residual),
+                                                           *view(x_res), *view(x_out), self.B, x.h, x.w, c, 5, 1, code, slope, 0, self.dt_code)))
+        pix = self.B * x.h * x.w
+        self.flops += 2 * 25 * pix * c
+        self.act_bytes += 2 * pix * c * (2 + (residual is not None) + (x_out is not None) + (x_res is not None))
+        self.weight_bytes += 2 * 25 * c
+
+    def lower_ghost(self, m, x: View, out: View | None, name):
+        """GhostConv: cv1 on the conv GEMM straight into out[:, :c_], the depthwise conv from that slice into out[:, c_:]."""
+        c_ = ghost_dw_channels(m)
+        ho, wo = self.out_hw(m.cv1, x)
+        out = out or self.new_view(ho, wo, 2 * c_)
+        y = out.slice(0, c_)
+        self.conv_module(m.cv1, x, y, None, f"{name}.cv1")
+        self.dwconv(m.cv2, y, out.slice(c_, c_), name=f"{name}.cv2")
+        return out
+
+    def lower_ghost_bottleneck(self, m, x: View, out: View | None, name, scratch=None):
+        """GhostBottleneck (s=1): out = cat(u, dw(u)) + x with u = g2.cv1(g1(x)).  g1 writes a scratch view t, g2.cv1 writes u to
+        a second one, and one y5_dwconv_fwd launch writes both halves of out: u + x[:, :c] and dw(u) + b + x[:, c:].  out may be x
+        itself (C3Ghost's concat slice, in place).  Returns the scratch views (t, u) for the next bottleneck of the chain."""
+        g1, g2 = ghost_bottleneck_convs(m)
+        c1_, c2_ = ghost_dw_channels(g1), ghost_dw_channels(g2)
+        if 2 * c2_ != x.c:
+            raise NotImplementedError(f"y5b200: GhostBottleneck {x.c} -> {2 * c2_} channels (its identity shortcut needs c1 == c2)")
+        t, u = scratch or (self.new_view(x.h, x.w, 2 * c1_), self.new_view(x.h, x.w, c2_))
+        self.lower_ghost(g1, x, t, f"{name}.conv.0")
+        self.conv_module(g2.cv1, t, u, None, f"{name}.conv.2.cv1")
+        out = out or self.new_view(x.h, x.w, x.c)
+        self.dwconv(g2.cv2, u, out.slice(c2_, c2_), residual=x.slice(c2_, c2_), x_out=out.slice(0, c2_), x_res=x.slice(0, c2_),
+                    name=f"{name}.conv.2.cv2")
+        return t, u
 
     def lower_transformer(self, tb, a: View, name):
         """C3TR's TransformerBlock (reference models/common.py:115-161) over the H*W tokens of view `a`, in place: its result
@@ -563,6 +617,7 @@ class Program:
         from .models import yolo as my
 
         mod = self.module
+        check_grouped_convs(mod)  # every refusal of a grouped conv before the first launch
         self.stem_in = None
         self.image_in = None
         self.proto_view = None
@@ -587,6 +642,12 @@ class Program:
             return self.lower_sppf(m, x, out, name)
         if isinstance(m, mc.SPP):
             return self.lower_sppf(m, x, out, name, k=spp_kernel(m))
+        if isinstance(m, mc.GhostConv):
+            return self.lower_ghost(m, x, out, name)
+        if isinstance(m, mc.GhostBottleneck):
+            out = out or self.new_view(x.h, x.w, x.c)
+            self.lower_ghost_bottleneck(m, x, out, name)
+            return out
         if isinstance(m, mc.Bottleneck):
             tmp = self.new_view(x.h, x.w, m.cv1.conv.out_channels)
             self.conv_module(m.cv1, x, tmp, None, f"{name}.cv1")
@@ -682,6 +743,12 @@ class Program:
             return (m.cv3.conv.out_channels, src[1], src[2])
         if isinstance(m, (mc.SPPF, mc.SPP, mc.Bottleneck)):
             return (m.cv2.conv.out_channels, src[1], src[2])
+        if isinstance(m, mc.GhostConv):
+            c, h, w = src
+            k, s, p = m.cv1.conv.kernel_size[0], m.cv1.conv.stride[0], m.cv1.conv.padding[0]
+            return (2 * m.cv1.conv.out_channels, (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1)
+        if isinstance(m, mc.GhostBottleneck):  # the stride-1 form (check_grouped_convs refused the other)
+            return (2 * m.conv[2].cv1.conv.out_channels, src[1], src[2])
         if isinstance(m, torch.nn.Sequential):
             for sub in m:
                 src = self._shape_of(sub, src)

@@ -211,6 +211,78 @@ class C3TR(C3):
         self.m = TransformerBlock(c_, c_, 4, n)
 
 
+class GhostConv(_EngineLayer):
+    """cat(y, cv2(y)) with y = cv1(x) (reference models/common.py GhostConv): cv2 is the depthwise 5x5 conv Conv(c_, c_, 5, 1,
+    None, c_), which runs on y5_dwconv_fwd.  Not a Conv subclass, as in the reference, so isinstance tests and state_dict keys
+    (cv1.*, cv2.*) behave the same."""
+
+    def __init__(self, c1, c2, k=1, s=1, g=1, act=True):
+        super().__init__()
+        c_ = c2 // 2
+        self.cv1 = Conv(c1, c_, k, s, None, g, act=act)
+        self.cv2 = Conv(c_, c_, 5, 1, None, c_, act=act)
+
+
+class GhostBottleneck(_EngineLayer):
+    """conv(x) + x with conv = GhostConv(c1, c2 // 2) -> Identity -> GhostConv(c2 // 2, c2, act=False) (reference models/common.py
+    GhostBottleneck).  The stride-2 form puts a depthwise k x k conv in both branches; it is built here for its state_dict keys
+    (the reference's DWConv holds conv / bn / act like Conv), and the engine refuses it: no reference model dict uses it."""
+
+    def __init__(self, c1, c2, k=3, s=1):
+        super().__init__()
+        c_ = c2 // 2
+        self.conv = nn.Sequential(GhostConv(c1, c_, 1, 1), Conv(c_, c_, k, s, g=c_, act=False) if s == 2 else nn.Identity(),
+                                  GhostConv(c_, c2, 1, 1, act=False))
+        self.shortcut = (nn.Sequential(Conv(c1, c1, k, s, g=c1, act=False), Conv(c1, c2, 1, 1, act=False)) if s == 2 else nn.Identity())
+
+
+class C3Ghost(C3):
+    """C3 whose `m` is a chain of GhostBottleneck(c_, c_) (reference models/common.py C3Ghost).  Like the reference it ignores
+    `shortcut`: every GhostBottleneck adds its input."""
+
+    def __init__(self, c1, c2, n=1, shortcut=True, g=1, e=0.5):
+        super().__init__(c1, c2, n, shortcut, g, e)
+        c_ = int(c2 * e)
+        self.m = nn.Sequential(*(GhostBottleneck(c_, c_) for _ in range(n)))
+
+
+def ghost_dw_channels(m: GhostConv) -> int:
+    """Channel count of a GhostConv's depthwise half when y5_dwconv runs it: Conv2d(c, c, 5, 1, 2, groups=c) with c a multiple
+    of 8; NotImplementedError naming the configuration otherwise."""
+    d = m.cv2.conv
+    c = d.in_channels
+    if not (d.out_channels == c == d.groups and tuple(d.kernel_size) == (5, 5) and tuple(d.stride) == (1, 1)
+            and tuple(d.padding) == (2, 2) and tuple(d.dilation) == (1, 1)):
+        raise NotImplementedError(f"y5b200: GhostConv.cv2 {d!r} (built: the depthwise Conv2d(c, c, 5, 1, 2, groups=c))")
+    if c % 8:
+        raise NotImplementedError(f"y5b200: GhostConv with a depthwise conv of {c} channels (built: multiples of 8)")
+    if m.cv1.conv.out_channels != c:
+        raise NotImplementedError(f"y5b200: GhostConv whose cv1 gives {m.cv1.conv.out_channels} channels to a {c}-channel cv2")
+    return c
+
+
+def ghost_bottleneck_convs(m: GhostBottleneck) -> tuple[GhostConv, GhostConv]:
+    """The two GhostConvs of a stride-1 GhostBottleneck; NotImplementedError for the stride-2 form."""
+    if not (isinstance(m.conv[1], nn.Identity) and isinstance(m.shortcut, nn.Identity)):
+        raise NotImplementedError("y5b200: GhostBottleneck(s=2) (built: the stride-1 form that C3Ghost uses)")
+    return m.conv[0], m.conv[2]
+
+
+def check_grouped_convs(root: nn.Module) -> None:
+    """Refuse, before anything runs, every grouped convolution the kernels do not build: any GhostBottleneck other than the
+    stride-1 form, any GhostConv whose cv2 is not the 5x5 depthwise conv, and every other Conv2d with groups != 1."""
+    built = set()
+    for name, m in root.named_modules():
+        if isinstance(m, GhostBottleneck):
+            ghost_bottleneck_convs(m)
+        elif isinstance(m, GhostConv):
+            ghost_dw_channels(m)
+            built.add(id(m.cv2.conv))
+    for name, m in root.named_modules():
+        if isinstance(m, nn.Conv2d) and m.groups != 1 and id(m) not in built:
+            raise NotImplementedError(f"y5b200: grouped convolution '{name}' {m!r} (built: only GhostConv's depthwise 5x5 conv)")
+
+
 class SPPF(_EngineLayer):
     def __init__(self, c1, c2, k=5):
         super().__init__()

@@ -19,8 +19,8 @@ import torch
 from torch import nn
 
 from ..cfg import model_cfg
-from .common import (C3, C3TR, SPP, SPPF, Bottleneck, Classify, Concat, Conv, Proto, _cached_program, _drop_engine_cache,  # noqa: F401
-                     _lib_on, _param_version)
+from .common import (C3, C3TR, SPP, SPPF, Bottleneck, C3Ghost, Classify, Concat, Conv, GhostBottleneck, GhostConv, Proto,  # noqa: F401
+                     _cached_program, _drop_engine_cache, _lib_on, _param_version)
 
 
 def make_divisible(x, divisor):
@@ -59,7 +59,8 @@ class Segment(Detect):
 
 
 _MODULES = {"Conv": Conv, "C3": C3, "C3TR": C3TR, "SPP": SPP, "SPPF": SPPF, "Bottleneck": Bottleneck, "Concat": Concat,
-            "nn.Upsample": nn.Upsample, "nn.MaxPool2d": nn.MaxPool2d, "nn.ZeroPad2d": nn.ZeroPad2d, "Detect": Detect, "Segment": Segment}
+            "nn.Upsample": nn.Upsample, "nn.MaxPool2d": nn.MaxPool2d, "nn.ZeroPad2d": nn.ZeroPad2d, "Detect": Detect, "Segment": Segment,
+            "GhostConv": GhostConv, "GhostBottleneck": GhostBottleneck, "C3Ghost": C3Ghost}
 
 
 def parse_model(d, ch):
@@ -76,16 +77,17 @@ def parse_model(d, ch):
     for i, (f, n, m, args) in enumerate(d["backbone"] + d["head"]):
         if isinstance(m, str):
             if m not in _MODULES:
-                raise NotImplementedError(f"y5b200: module '{m}' is outside the engine's hot path (models n/s/m/l/x[-seg], yolov3[-spp|-tiny])")
+                raise NotImplementedError(f"y5b200: module '{m}' is outside the engine's hot path (models n/s/m/l/x[-seg], yolov3[-spp|-tiny], "
+                                          "yolov5s-ghost)")
             m = _MODULES[m]
         args = [names.get(a, a) if isinstance(a, str) else a for a in args]
         n = n_ = max(round(n * gd), 1) if n > 1 else n
-        if m in (Conv, Bottleneck, SPP, SPPF, C3, C3TR):
+        if m in (Conv, Bottleneck, SPP, SPPF, C3, C3TR, GhostConv, GhostBottleneck, C3Ghost):
             c1, c2 = ch[f], args[0]
             if c2 != no:
                 c2 = make_divisible(c2 * gw, ch_mul)
             args = [c1, c2, *args[1:]]
-            if m in (C3, C3TR):
+            if m in (C3, C3TR, C3Ghost):
                 args.insert(2, n)
                 n = 1
         elif m is Concat:
@@ -129,6 +131,8 @@ def _layer_strides(model: nn.Sequential) -> list[float]:
         r = red[f if isinstance(f, int) else f[0]] if red else 1
         if isinstance(m, Conv):
             r = r * m.conv.stride[0]
+        elif isinstance(m, GhostConv):  # its stride sits in cv1 (yolov5s-ghost downsamples with GhostConv(c, 3, 2))
+            r = r * m.cv1.conv.stride[0]
         elif isinstance(m, nn.Upsample):
             r = r / float(m.scale_factor)
         elif isinstance(m, nn.MaxPool2d):

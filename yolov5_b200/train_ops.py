@@ -13,7 +13,8 @@ What runs where
     sums between the split BN passes (train.py --sync-bn);
   * the glue between convolutions is liby5b200 too: channel concat = strided slice copies whose backward is a set of
     views, 2x nearest upsample and its 2x2-sum backward, SPPF's pooling chain and its arg-max backward, the Bottleneck
-    shortcut as a residual operand of cv2's normalise+activate pass.  What is left to torch autograd is bookkeeping: the
+    shortcut as a residual operand of cv2's normalise+activate pass, GhostConv's depthwise half and its concat in one pass
+    (y5_dwconv_fwd / y5_dwconv_wgrad).  What is left to torch autograd is bookkeeping: the
     graph itself, summing gradients of tensors with several consumers, the (B,na,ny,nx,no) permute of the head output.
     Activations are channels_last, so every op reads and writes the same NHWC bytes and no layout conversion exists.
 
@@ -24,6 +25,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import weakref
 
 import torch
 
@@ -418,13 +420,80 @@ def _wgrad_async(dev, fn, keep):
     return out
 
 
+def _bn_act_fwd(y, z_ptr: int, z_pitch: int, gamma, beta, running_mean, running_var, res: tuple, act, eps, momentum, training, pg):
+    """z = act(BN(y)) + residual for the raw conv output y (dense NHWC): batch statistics in training (SyncBatchNorm's all-reduced
+    ones when pg is set), running statistics otherwise.  z: element pointer and pitch of the output view; res: (pointer or None,
+    pitch).  Returns (mean, invstd, gamma, beta as fp32, the all-rank row count or None) for _bn_act_bwd."""
+    lib = _lib.lib()
+    dev = y.device
+    b, c, ho, wo = y.shape
+    rows = b * ho * wo
+    code = _lib.dtype_code(y.dtype)
+    fwd_fn, n_rows = lib.y5_bn_act_fwd_ex, None
+    if training:
+        mean = torch.empty(c, dtype=torch.float32, device=dev)
+        invstd = torch.empty(c, dtype=torch.float32, device=dev)
+        # the kernel updates fp32 running statistics in place; a model cast to fp16/bf16 goes through fp32 copies
+        rm = running_mean if running_mean is None or running_mean.dtype == torch.float32 else running_mean.float()
+        rv = running_var if running_var is None or running_var.dtype == torch.float32 else running_var.float()
+        if pg is None:
+            ws = _bn_ws(c, dev)
+            _lib.check(lib.y5_bn_stats(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats")
+        else:  # SyncBatchNorm: [column sums | row count] of every rank in one all-reduce, then the statistics of all rows
+            ws = _arena.take(2 * c + 1, dev)
+            _lib.check(lib.y5_bn_stats_sync(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats_sync")
+            _all_reduce(ws[: 2 * c + 1], pg)
+            n_rows = ws[2 * c : 2 * c + 1].clone()  # N for the backward: the arena is cleared by the next forward
+            fwd_fn = lib.y5_bn_act_fwd_sync_ex
+        sums = ws.data_ptr()
+    else:
+        mean = running_mean.float().contiguous()
+        invstd = torch.rsqrt(running_var.float() + eps)
+        rm = rv = sums = None
+    g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
+    _lib.check(fwd_fn(y.data_ptr(), c, z_ptr, z_pitch, rows, c, code, mean.data_ptr(), invstd.data_ptr(), g32.data_ptr(),
+                      b32.data_ptr(), *act, sums, eps, momentum, rm.data_ptr() if rm is not None else None,
+                      rv.data_ptr() if rv is not None else None, res[0], res[1], _st(dev)), "bn_act_fwd")
+    if training:
+        if rm is not running_mean:
+            running_mean.copy_(rm)
+        if rv is not running_var:
+            running_var.copy_(rv)
+    return mean, invstd, g32, b32, n_rows
+
+
+def _bn_act_bwd(y, dz_ptr: int, dz_pitch: int, mean, invstd, g32, b32, act, pg, n_rows):
+    """Backward of _bn_act_fwd in training: (dy like y, fp32 dgamma, fp32 dbeta) from the gradient view dz (pointer, pitch)."""
+    lib = _lib.lib()
+    dev = y.device
+    b, c, ho, wo = y.shape
+    rows = b * ho * wo
+    code = _lib.dtype_code(y.dtype)
+    dy = torch.empty_like(y)
+    dgamma = torch.empty(c, dtype=torch.float32, device=dev)
+    dbeta = torch.empty(c, dtype=torch.float32, device=dev)
+    ws = _bn_ws(c, dev)
+    if pg is None:
+        _lib.check(lib.y5_bn_act_bwd_ex(y.data_ptr(), c, dz_ptr, dz_pitch, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                        invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(), dbeta.data_ptr(),
+                                        ws.data_ptr(), _st(dev)), "bn_act_bwd")
+    else:  # SyncBatchNorm: dgamma / dbeta stay this rank's sums (DDP averages them); dy uses the sums of every rank over N
+        _lib.check(lib.y5_bn_act_bwd_reduce_ex(y.data_ptr(), c, dz_ptr, dz_pitch, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                               invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(),
+                                               dbeta.data_ptr(), ws.data_ptr(), _st(dev)), "bn_act_bwd_reduce")
+        _all_reduce(ws[: 2 * c], pg)
+        _lib.check(lib.y5_bn_act_bwd_apply(y.data_ptr(), c, dz_ptr, dz_pitch, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                           invstd.data_ptr(), g32.data_ptr(), act[0], ws.data_ptr(), n_rows.data_ptr(),
+                                           _st(dev)), "bn_act_bwd_apply")
+    return dy, dgamma, dbeta
+
+
 class _ConvBnAct(torch.autograd.Function):
     """z = act(BN(conv(x, w)))  with batch statistics (training) or running statistics (eval inside a training graph); act is
     engine.act_spec's (code, slope) pair."""
 
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, residual, k, s, p, act, eps, momentum, training, stem, pg=None):
-        lib = _lib.lib()
         dev = x.device
         if stem == STEM_IMAGE:  # x is the image_input buffer; weight is the (O,3,k,k) filter, zero-padded to its channels
             w_eff, ke, se, pe = pad_image_weight(weight.detach()), k, s, p
@@ -458,42 +527,11 @@ class _ConvBnAct(torch.autograd.Function):
                 if _cur_plan is not None and not stem and _cur_plan.dtype == x.dtype and isinstance(weight, torch.nn.Parameter):
                     _cur_plan.register(weight, wp, wp_dg, wp.shape[3], wp_dg.shape[3] if wp_dg is not None else 0, bk_f, bk_d)
             y = conv_packed(x, xp, wp, bk_f, None, w_eff.shape[0], ke, se, pe, act=False)
-        b, c, ho, wo = y.shape
-        rows = b * ho * wo
-        code = _lib.dtype_code(y.dtype)
-        fwd_fn, n_rows = lib.y5_bn_act_fwd_ex, None
-        if training:
-            mean = torch.empty(c, dtype=torch.float32, device=dev)
-            invstd = torch.empty(c, dtype=torch.float32, device=dev)
-            # the kernel updates fp32 running statistics in place; a model cast to fp16/bf16 goes through fp32 copies
-            rm = running_mean if running_mean is None or running_mean.dtype == torch.float32 else running_mean.float()
-            rv = running_var if running_var is None or running_var.dtype == torch.float32 else running_var.float()
-            if pg is None:
-                ws = _bn_ws(c, dev)
-                _lib.check(lib.y5_bn_stats(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats")
-            else:  # SyncBatchNorm: [column sums | row count] of every rank in one all-reduce, then the statistics of all rows
-                ws = _arena.take(2 * c + 1, dev)
-                _lib.check(lib.y5_bn_stats_sync(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats_sync")
-                _all_reduce(ws[: 2 * c + 1], pg)
-                n_rows = ws[2 * c : 2 * c + 1].clone()  # N for the backward: the arena is cleared by the next forward
-                fwd_fn = lib.y5_bn_act_fwd_sync_ex
-            sums = ws.data_ptr()
-        else:
-            mean = running_mean.float().contiguous()
-            invstd = torch.rsqrt(running_var.float() + eps)
-            rm = rv = sums = None
-        g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
         z = torch.empty_like(y)
-        res, resp = (None, 0) if residual is None else _nhwc(residual)
-        _lib.check(fwd_fn(y.data_ptr(), c, z.data_ptr(), c, rows, c, code, mean.data_ptr(), invstd.data_ptr(), g32.data_ptr(),
-                          b32.data_ptr(), *act, sums, eps, momentum, rm.data_ptr() if rm is not None else None,
-                          rv.data_ptr() if rv is not None else None, res.data_ptr() if res is not None else None, resp,
-                          _st(dev)), "bn_act_fwd")
-        if training:
-            if rm is not running_mean:
-                running_mean.copy_(rm)
-            if rv is not running_var:
-                running_var.copy_(rv)
+        res = (None, 0) if residual is None else _nhwc(residual)
+        mean, invstd, g32, b32, n_rows = _bn_act_fwd(y, z.data_ptr(), y.shape[1], gamma, beta, running_mean, running_var,
+                                                     (res[0].data_ptr() if res[0] is not None else None, res[1]), act, eps, momentum,
+                                                     training, pg)
         ctx.save_for_backward(x, weight, y, mean, invstd, g32, b32, wp_dg)
         ctx.cfg = (k, s, p, act, training, stem, ke, se, pe)
         ctx.bk_d = bk_d
@@ -504,33 +542,15 @@ class _ConvBnAct(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dz):
-        lib = _lib.lib()
         x, weight, y, mean, invstd, g32, b32, wp_dg = ctx.saved_tensors
         k, s, p, act, training, stem, ke, se, pe = ctx.cfg
         if not training:
             raise NotImplementedError("y5b200: backward through eval-mode BatchNorm")
         dev = y.device
-        b, c, ho, wo = y.shape
-        rows = b * ho * wo
-        code = _lib.dtype_code(y.dtype)
         dz_in = dz
         dz, dzp = _nhwc(dz if dz.dtype == y.dtype else dz.to(y.dtype))
-        dy = torch.empty_like(y)
-        dgamma = torch.empty(c, dtype=torch.float32, device=dev)
-        dbeta = torch.empty(c, dtype=torch.float32, device=dev)
-        ws = _bn_ws(c, dev)
-        if ctx.pg is None:
-            _lib.check(lib.y5_bn_act_bwd_ex(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
-                                            invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(), dbeta.data_ptr(),
-                                            ws.data_ptr(), _st(dev)), "bn_act_bwd")
-        else:  # SyncBatchNorm: dgamma / dbeta stay this rank's sums (DDP averages them); dy uses the sums of every rank over N
-            _lib.check(lib.y5_bn_act_bwd_reduce_ex(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
-                                                   invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(),
-                                                   dbeta.data_ptr(), ws.data_ptr(), _st(dev)), "bn_act_bwd_reduce")
-            _all_reduce(ws[: 2 * c], ctx.pg)
-            _lib.check(lib.y5_bn_act_bwd_apply(y.data_ptr(), c, dz.data_ptr(), dzp, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
-                                               invstd.data_ptr(), g32.data_ptr(), act[0], ws.data_ptr(), ctx.n_rows.data_ptr(),
-                                               _st(dev)), "bn_act_bwd_apply")
+        dy, dgamma, dbeta = _bn_act_bwd(y, dz.data_ptr(), dzp, mean, invstd, g32, b32, act, ctx.pg, ctx.n_rows)
+
         def wgrad():
             g = stem_wgrad_wide(x, dy) if ctx.wide else conv_wgrad(x, dy, ke, se, pe)
             if stem == STEM_IMAGE:  # the image buffer's padding channels carry no filter taps
@@ -550,6 +570,88 @@ class _ConvBnAct(torch.autograd.Function):
         dres = dz_in if ctx.needs_input_grad[6] else None  # z = residual + act(bn(y)): the shortcut's gradient is dz itself
         return (dx, dw, dgamma.to(ctx.pdtypes[0]), dbeta.to(ctx.pdtypes[1]), None, None, dres, None, None, None, None, None,
                 None, None, None, None)
+
+
+class _GhostDw(torch.autograd.Function):
+    """GhostConv's second half with its concat in training: out = cat(y + res[:, :c], act(BN(dw(y))) + res[:, c:]), dw the depthwise
+    5x5 conv of GhostConv.cv2 and res an optional (B,2c,H,W) residual (GhostBottleneck's input).  One y5_dwconv_fwd launch writes
+    the raw dw(y) and the first half; the BN passes of _ConvBnAct write the second half.  Backward: the BN backward gives d_raw,
+    the same kernel with the taps rotated gives dy = dw^T(d_raw) + dout[:, :c] in one pass, and y5_dwconv_wgrad the weight
+    gradient (on the side stream, as _ConvBnAct's)."""
+
+    @staticmethod
+    def forward(ctx, y, weight, gamma, beta, running_mean, running_var, residual, act, eps, momentum, training, pg=None):
+        lib = _lib.lib()
+        y, yp = _nhwc(y)
+        b, c, h, w = y.shape
+        dev, code = y.device, _lib.dtype_code(y.dtype)
+        wp = torch.empty(c, 5, 5, 1, dtype=y.dtype, device=dev)  # [c][5][5]: the fp32 master filter rounded once
+        wm = weight.detach().contiguous()
+        _lib.check(lib.y5_weight_pack(wm.data_ptr(), _lib.dtype_code(wm.dtype), c, 1, 5, wp.data_ptr(), 1, None, 0, code, _st(dev)),
+                   "weight_pack (depthwise)")
+        out = _empty_cl(b, 2 * c, h, w, y.dtype, dev)
+        raw = _empty_cl(b, c, h, w, y.dtype, dev)
+        res, rp = (None, 0) if residual is None else _nhwc(residual)
+        es = out.element_size()
+        _lib.check(lib.y5_dwconv_fwd(y.data_ptr(), yp, wp.data_ptr(), None, raw.data_ptr(), c, None, 0, res.data_ptr() if res is not None else None,
+                                     rp, out.data_ptr(), 2 * c, b, h, w, c, 5, 1, _lib.ACT_NONE, 0.0, 0, code, _st(dev)), "dwconv_fwd")
+        mean, invstd, g32, b32, n_rows = _bn_act_fwd(raw, out.data_ptr() + c * es, 2 * c, gamma, beta, running_mean, running_var,
+                                                     (res.data_ptr() + c * es if res is not None else None, rp), act, eps, momentum,
+                                                     training, pg)
+        ctx.save_for_backward(y, weight, raw, mean, invstd, g32, b32, wp)
+        ctx.cfg = (act, training, pg, n_rows, gamma.dtype, beta.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = _lib.lib()
+        y, weight, raw, mean, invstd, g32, b32, wp = ctx.saved_tensors
+        act, training, pg, n_rows, gdt, bdt = ctx.cfg
+        if not training:
+            raise NotImplementedError("y5b200: backward through eval-mode BatchNorm")
+        b, c, h, w = y.shape
+        dev, code = y.device, _lib.dtype_code(y.dtype)
+        dout_in = dout
+        dout, dp = _nhwc(dout if dout.dtype == y.dtype else dout.to(y.dtype))
+        es = dout.element_size()
+        d_raw, dgamma, dbeta = _bn_act_bwd(raw, dout.data_ptr() + c * es, dp, mean, invstd, g32, b32, act, pg, n_rows)
+        yp = _nhwc(y)[1]
+
+        def wgrad():
+            dw = torch.empty(c, 1, 5, 5, dtype=torch.float32, device=dev)
+            _lib.check(lib.y5_dwconv_wgrad(y.data_ptr(), yp, d_raw.data_ptr(), c, dw.data_ptr(), b, h, w, c, 5, 1, code, _st(dev)),
+                       "dwconv_wgrad")
+            return dw.to(weight.dtype)
+
+        dw = _wgrad_async(dev, wgrad, (y, d_raw)) if (_async_wgrad and weight.grad is None) else wgrad()
+        dy = None
+        if ctx.needs_input_grad[0]:
+            dy = _empty_cl(b, c, h, w, y.dtype, dev)
+            _lib.check(lib.y5_dwconv_fwd(d_raw.data_ptr(), c, wp.data_ptr(), None, dy.data_ptr(), c, dout.data_ptr(), dp, None, 0, None, 0,
+                                         b, h, w, c, 5, 1, _lib.ACT_NONE, 0.0, 1, code, _st(dev)), "dwconv_fwd (data gradient)")
+        dres = dout_in if ctx.needs_input_grad[6] else None  # out = ... + residual: the residual's gradient is dout itself
+        return dy, dw, dgamma.to(gdt), dbeta.to(bdt), None, None, dres, None, None, None, None, None
+
+
+def dwconv_module(m, y, residual=None):
+    """GhostConv.cv2 (depthwise conv + BN + act) on y, concatenated after y, + residual: _GhostDw with conv_module's BN rules."""
+    bn = getattr(m, "bn", None)
+    if bn is None:
+        raise RuntimeError("y5b200: cannot train a fused model (Conv without BatchNorm); build it unfused")
+    act = act_spec(m.act)
+    if bn.training and bn.track_running_stats and bn.num_batches_tracked is not None:
+        bn.num_batches_tracked += 1
+    mom = bn.momentum if bn.momentum is not None else 0.1
+    return _GhostDw.apply(y, m.conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, residual, act, float(bn.eps), float(mom),
+                          bn.training, bn_sync_group(bn))
+
+
+def _ghost(m, x, residual=None):
+    """GhostConv: cat(y, cv2(y)) + residual with y = cv1(x)."""
+    from .models.common import ghost_dw_channels
+
+    ghost_dw_channels(m)
+    return dwconv_module(m.cv2, conv_module(m.cv1, x), residual)
 
 
 class _ConvBias(torch.autograd.Function):
@@ -945,6 +1047,11 @@ def _run(m, x, dt):
         return conv_module(m, x)
     if isinstance(m, mc.Bottleneck):  # the shortcut add rides on cv2's normalise+activate pass
         return conv_module(m.cv2, conv_module(m.cv1, x), residual=x if m.add else None)
+    if isinstance(m, mc.GhostConv):
+        return _ghost(m, x)
+    if isinstance(m, mc.GhostBottleneck):  # cat(u, dw(u)) + x with u = g2.cv1(g1(x)): the add rides the depthwise pass, as in eval
+        g1, g2 = mc.ghost_bottleneck_convs(m)
+        return _ghost(g2, _ghost(g1, x), residual=x)
     if isinstance(m, mc.C3TR):
         return conv_module(m.cv3, _Concat.apply(_transformer(m.m, conv_module(m.cv1, x)), conv_module(m.cv2, x)))
     if isinstance(m, mc.C3):
@@ -985,6 +1092,9 @@ def _run(m, x, dt):
     raise NotImplementedError(f"y5b200: module {type(m).__name__} is outside the engine's hot path")
 
 
+_grouped_checked: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()  # model -> ids of the layer list check_grouped_convs passed
+
+
 def forward_train(model, img: torch.Tensor):
     """Training-mode DetectionModel / SegmentationModel forward: list of raw (B,na,ny,nx,no) maps (Segment: (list, proto)),
     differentiable w.r.t. every parameter."""
@@ -999,6 +1109,10 @@ def forward_train(model, img: torch.Tensor):
     if not stem:
         _check_conv(first, STEM_IMAGE)
     pools = mc.pool_modes(layers, model.save)  # every refusal before the first launch
+    key = tuple(map(id, layers))  # the walk over every module costs ~0.5 ms: once per layer list (the lowerings check again)
+    if _grouped_checked.get(model) != key:
+        mc.check_grouped_convs(model)
+        _grouped_checked[model] = key
     # every op below picks its dtype explicitly; autocast's own casting rules must not touch the glue ops
     global _cur_plan
     with torch.autocast("cuda", enabled=False):
