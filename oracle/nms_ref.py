@@ -95,12 +95,16 @@ def non_max_suppression(
     dtype: str = "fp32",
     return_index: bool = False,
     labels=(),
+    max_nms: int = 30000,
 ):
     """prediction: (B, N, 5+nc+nm) fp32 array holding values exactly representable in ``dtype``.
 
     ``labels`` (autolabelling, reference :706-712): per image an (m,5) array [cls, x, y, w, h]; its rows are appended to the
     image's candidates with obj = class score = 1.  The reference's ``torch.cat((x, v), 0)`` with an fp32 ``v`` promotes that
     image's rows to fp32, so everything after the first objectness test (:686) runs in fp32 for such an image.
+
+    ``max_nms`` is the reference's hard-coded cap on the candidates that reach the greedy pass (:691); it is a keyword here
+    so that the cut can be checked on small inputs.
 
     Returns a list of B fp32 arrays (n_i, 6+nm) = [x1,y1,x2,y2,conf,cls,(masks)]; with ``return_index`` also the
     list of int64 arrays of candidate ids ``row*nc + cls`` of the kept detections (the integer result).
@@ -110,7 +114,7 @@ def non_max_suppression(
     bs, _, no = pred.shape
     nc = no - nm - 5
     mi = 5 + nc
-    max_wh, max_nms = 7680.0, 30000
+    max_wh = 7680.0
     multi_label = multi_label and nc > 1
     thr = round_to(np.float32(conf_thres), dtype)  # python scalar is rounded to the tensor dtype before comparing
     outs, idxs = [], []

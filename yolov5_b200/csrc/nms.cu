@@ -110,12 +110,14 @@ __device__ __forceinline__ int for_each_candidate(const NmsArgs& a, int b, int s
             float best = -INFINITY;
             int bj = 0x7fffffff;
             int r = 0;
+            bool nan = false;  // torch.max propagates NaN: a row with any NaN product has a NaN best score and is dropped
             if (has) {
                 r = row0 + static_cast<int>(rl);
                 const long long rb = img_base + static_cast<long long>(r) * a.no;
                 const float obj = ld_elem(a.pred, rb + 4, a.dtype);
                 for (int j = sl; j < a.nc; j += 8) {
                     const float conf = rnd(__fmul_rn(ld_elem(a.pred, rb + 5 + j, a.dtype), obj), a.dtype);
+                    nan |= isnan(conf);
                     if (bj == 0x7fffffff || conf > best) { best = conf; bj = j; }
                 }
             }
@@ -123,9 +125,10 @@ __device__ __forceinline__ int for_each_candidate(const NmsArgs& a, int b, int s
             for (int o = 4; o > 0; o >>= 1) {  // reduce inside the 8-lane group
                 const float ob = __shfl_xor_sync(0xffffffffu, best, o);
                 const int oj = __shfl_xor_sync(0xffffffffu, bj, o);
+                nan |= __shfl_xor_sync(0xffffffffu, static_cast<int>(nan), o) != 0;
                 if (oj != 0x7fffffff && (bj == 0x7fffffff || ob > best || (ob == best && oj < bj))) { best = ob; bj = oj; }
             }
-            const bool okrow = has && bj != 0x7fffffff && best > a.thr && class_allowed(cls_mask, bj);
+            const bool okrow = has && !nan && bj != 0x7fffffff && best > a.thr && class_allowed(cls_mask, bj);
             const bool ok = okrow && sl == 0;
             const unsigned m = __ballot_sync(0xffffffffu, ok);
             f(ok, best, static_cast<unsigned>(r) * a.nc + (okrow ? bj : 0), count, m);
