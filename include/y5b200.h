@@ -135,8 +135,6 @@ typedef struct y5_detect_desc {
     const void* weight;   /* packed [na*npad][cin_pad], npad = 128 * ceil(no / 128): anchor a in rows [a*npad, a*npad + no),
                              the rest zero (npad = 128 while no <= 128) */
     const float* bias;    /* fp32 [na*npad], laid out like the weight rows */
-    void* raw;
-    void* z;
     int32_t z_rows, z_row0;
     int32_t na, no, nc;   /* no = 5 + nc + nm <= 8192, nc <= 4096 (Y5_E_UNSUPPORTED beyond); columns >= 5+nc (mask
                              coefficients) are passed through un-sigmoided */
@@ -147,9 +145,8 @@ typedef struct y5_detect_desc {
 } y5_detect_desc;
 typedef struct y5_detect_plan y5_detect_plan;
 int y5_detect_plan_create(const y5_detect_desc* desc, y5_detect_plan** plan);
-int y5_detect_plan_run(const y5_detect_plan* plan, void* stream);
-/* same plan, outputs redirected to freshly allocated tensors of the same shapes (the reference returns new tensors
- * from every forward; the input side of the plan stays bound to the engine's static buffers) */
+/* runs the plan into the outputs given per call (the reference returns new tensors from every forward; the input side
+ * of the plan stays bound to the engine's static buffers) */
 int y5_detect_plan_run_to(const y5_detect_plan* plan, void* raw, void* z, void* stream);
 void y5_detect_plan_destroy(y5_detect_plan* plan);
 
@@ -231,10 +228,8 @@ typedef struct y5_loss_params {
 } y5_loss_params;
 int64_t y5_loss_workspace_bytes(const y5_loss_params* p);
 /* matches: per level, int32 count + rows (b, a, gj, gi, cls) int64 and tbox fp32 live in the workspace; the
- * build_targets result can be read back with y5_loss_read_targets for parity tests */
-int y5_loss_fwd_bwd(const y5_loss_params* p, const void* const* pl, const float* targets, const float* anchors,
-                    float* out_loss, void* const* grad, void* workspace, int64_t workspace_bytes, void* stream);
-/* same, with the upstream gradient of the loss read from DEVICE memory: grad[l] = d(out_loss[0])/dp * p->grad_scale *
+ * build_targets result can be read back with y5_loss_read_targets for parity tests.
+ * The upstream gradient of the loss is read from DEVICE memory: grad[l] = d(out_loss[0])/dp * p->grad_scale *
  * (*grad_scale_dev), multiplied in fp32 BEFORE the result is rounded to the prediction dtype -- what autograd does for
  * `scaler.scale(loss).backward()` (train.py:410): a GradScaler factor of 65536 (x WORLD_SIZE) neither overflows fp16 on
  * the way nor flushes small objectness gradients to zero.  grad_scale_dev may be NULL (= 1).  Targets whose image index
@@ -299,71 +294,56 @@ typedef struct y5_wgrad_desc {
 } y5_wgrad_desc;
 int y5_conv_wgrad(const y5_wgrad_desc* d, void* stream);
 
+/* Training BatchNorm + activation, in five passes:
+ *   forward:  y5_bn_stats (column sums) -> y5_bn_act_fwd (normalise + activate)
+ *   backward: y5_bn_act_bwd (reduce + apply), or, split for SyncBatchNorm, y5_bn_act_bwd_reduce -> y5_bn_act_bwd_apply
+ * act: Y5_ACT_NONE | Y5_ACT_SILU | Y5_ACT_LEAKY; `slope` is the negative slope of Y5_ACT_LEAKY (finite; 0 = ReLU) and is
+ * ignored otherwise.  LeakyReLU, with t = bn(y) rounded to the activation dtype:
+ *   forward:  z = round(t > 0 ? t : slope * t)                       (fp32 product; + residual as below)
+ *   backward: du = round(t > 0 ? dz : dz * slope)                    (torch's leaky_relu_backward), parked in dy like SiLU's
+ * SyncBatchNorm (torch.nn.SyncBatchNorm in training under torch.distributed) adds the column sums of every rank with the
+ * caller's SUM all-reduce between passes.  Its forward workspace is 2 * channels + 1 doubles, ZERO on entry; slot 2 * channels
+ * is the row count:
+ *   forward:  y5_bn_stats(count = ws + 2C) -> all-reduce ws[0 .. 2C] -> y5_bn_act_fwd(sums = ws, count = ws + 2C)
+ *   backward: y5_bn_act_bwd_reduce -> all-reduce ws[0 .. 2C) -> y5_bn_act_bwd_apply(count = the forward's N)
+ * `count` points at one fp64 row count, or is NULL for plain BatchNorm, where `rows` is the whole batch (y5_bn_act_bwd_apply
+ * requires it; y5_bn_act_fwd takes it only with `sums`).  y5_bn_stats adds `rows` to *count; y5_bn_act_fwd and
+ * y5_bn_act_bwd_apply divide by the N it holds instead of `rows`, and y5_bn_act_fwd's running_var takes the unbiased factor
+ * N / (N - 1).  Without the all-reduce, the SyncBatchNorm passes compute exactly what the plain ones compute. */
 /* workspace of y5_bn_stats / y5_bn_act_bwd / y5_col_sum: 2 * channels doubles.  For y5_bn_stats and y5_bn_act_bwd it
  * must be ZERO on entry and is left dirty (callers carve it from one arena cleared once per step); y5_col_sum clears
  * its own. */
 int64_t y5_bn_workspace_bytes(int32_t channels);
 /* per-channel sum and sum of squares of a [rows][channels] view, accumulated into workspace (fp64) */
 int y5_bn_stats(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace,
-                void* stream);
-/* z = act(gamma * (y - mean) * invstd + beta), act: Y5_ACT_NONE | Y5_ACT_SILU (LeakyReLU: the _ex forms below); z may be a
- * channel-slice view.
+                double* count, void* stream);
+/* z = act(gamma * (y - mean) * invstd + beta); z may be a channel-slice view.
  * sums != NULL (training): mean / invstd (biased variance + eps) are first derived from the y5_bn_stats workspace and
  * WRITTEN to mean / invstd, and running_mean / running_var (nullable) are updated like nn.BatchNorm2d does (momentum,
  * unbiased variance).  sums == NULL (eval): mean / invstd are inputs.  residual != NULL adds a view of the same shape
  * after the activation (Bottleneck shortcut, models/common.py:181); its gradient is dz itself. */
 int y5_bn_act_fwd(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels,
-                  int32_t dtype, float* mean, float* invstd, const float* gamma, const float* beta, int32_t act,
-                  const void* sums, float eps, float momentum, float* running_mean, float* running_var,
+                  int32_t dtype, float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope,
+                  const void* sums, const void* count, float eps, float momentum, float* running_mean, float* running_var,
                   const void* residual, int32_t res_pitch, void* stream);
 /* given dz: dy (gradient w.r.t. the conv output), dgamma, dbeta (fp32, overwritten).  Two launches: the reduce pass forms
- * du = dz * act'(bn(y)) and its two column sums and, for Y5_ACT_SILU, parks du in the dy buffer; the apply pass turns it into dy
- * in place.  dy may alias dz (every element is read before it is written) but not y. */
+ * du = dz * act'(bn(y)) and its two column sums and, for Y5_ACT_SILU / Y5_ACT_LEAKY, parks du in the dy buffer; the apply
+ * pass turns it into dy in place.  dy may alias dz (every element is read before it is written) but not y. */
 int y5_bn_act_bwd(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
                   int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
-                  const float* gamma, const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace,
-                  void* stream);
-/* SyncBatchNorm (torch.nn.SyncBatchNorm in training under torch.distributed): the same passes split where the column sums
- * of every rank must be added, with the caller's SUM all-reduce in between.  The workspace is 2 * channels + 1 doubles,
- * ZERO on entry; slot 2 * channels is the row count.
- * Forward:  y5_bn_stats_sync (y5_bn_stats that also adds `rows` to ws[2C]) -> all-reduce ws[0 .. 2C] -> y5_bn_act_fwd_sync
- *           (y5_bn_act_fwd in training mode, `sums` required, dividing by the global N = sums[2C] instead of `rows`;
- *           running_var takes the unbiased factor N / (N - 1)).
- * Backward: y5_bn_act_bwd_reduce (the reduce pass of y5_bn_act_bwd; writes THIS rank's dgamma / dbeta and, for
- *           Y5_ACT_SILU, leaves du in dy) -> all-reduce ws[0 .. 2C) -> y5_bn_act_bwd_apply (the apply pass with the summed
- *           `sums` and `count` -> the forward's N, one double; dgamma / dbeta untouched).
- * Without the all-reduce, the pairs compute exactly what y5_bn_stats + y5_bn_act_fwd and y5_bn_act_bwd compute. */
-int y5_bn_stats_sync(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace,
-                     void* stream);
-int y5_bn_act_fwd_sync(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels,
-                       int32_t dtype, float* mean, float* invstd, const float* gamma, const float* beta, int32_t act,
-                       const void* sums, float eps, float momentum, float* running_mean, float* running_var,
-                       const void* residual, int32_t res_pitch, void* stream);
+                  const float* gamma, const float* beta, int32_t act, float slope, float* dgamma, float* dbeta,
+                  void* workspace, void* stream);
+/* the reduce pass of y5_bn_act_bwd: the column sums into the workspace, THIS rank's dgamma / dbeta from them and, for
+ * Y5_ACT_SILU / Y5_ACT_LEAKY, du left in dy */
 int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
                          int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
-                         const float* gamma, const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace,
-                         void* stream);
+                         const float* gamma, const float* beta, int32_t act, float slope, float* dgamma, float* dbeta,
+                         void* workspace, void* stream);
+/* the apply pass of y5_bn_act_bwd with the all-reduced `sums` and `count` (required); dgamma / dbeta untouched.  It only
+ * reads the parked du, so it takes no slope. */
 int y5_bn_act_bwd_apply(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
                         int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
                         const float* gamma, int32_t act, const void* sums, const void* count, void* stream);
-/* Four of the passes above with the activation's parameter after `act` (y5_bn_act_bwd_apply takes Y5_ACT_LEAKY as it is: it only
- * reads the parked du): `slope` is the negative slope of
- * Y5_ACT_LEAKY (finite; 0 = ReLU) and is ignored for Y5_ACT_NONE / Y5_ACT_SILU, so act = NONE | SILU computes exactly what the
- * entry points without the suffix compute.  LeakyReLU, with t = bn(y) rounded to the activation dtype as above:
- *   forward:  z = round(t > 0 ? t : slope * t)                       (fp32 product; + residual as above)
- *   backward: du = round(t > 0 ? dz : dz * slope)                    (torch's leaky_relu_backward), parked in dy like SiLU's */
-int y5_bn_act_fwd_ex(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
-                     float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope, const void* sums, float eps,
-                     float momentum, float* running_mean, float* running_var, const void* residual, int32_t res_pitch, void* stream);
-int y5_bn_act_bwd_ex(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
-                     int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, const float* beta,
-                     int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream);
-int y5_bn_act_fwd_sync_ex(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
-                          float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope, const void* sums, float eps,
-                          float momentum, float* running_mean, float* running_var, const void* residual, int32_t res_pitch, void* stream);
-int y5_bn_act_bwd_reduce_ex(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
-                            int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
-                            const float* gamma, const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream);
 /* out[c] = sum over rows of y[row][c] (fp32) */
 int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, float* out, void* workspace,
                void* stream);

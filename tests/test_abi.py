@@ -17,10 +17,10 @@ def _declared():
     return sorted(set(re.findall(r"\b(y5_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_header_declares_the_boundary():
+def test_header_declares_the_entry_points():
     names = _declared()
     for must in ("y5_conv_plan_create", "y5_conv_plan_run", "y5_detect_plan_create", "y5_stem_s2d", "y5_sppf_pool",
-                 "y5_upsample2x", "y5_nms_batched", "y5_box_iou", "y5_loss_fwd_bwd", "y5_last_error"):
+                 "y5_upsample2x", "y5_nms_batched", "y5_box_iou", "y5_loss_fwd_bwd_scaled", "y5_last_error"):
         assert must in names
 
 
@@ -43,13 +43,13 @@ def test_library_is_sm90a_with_wgmma_and_tma(built_lib):
         assert mnemonic in wg, mnemonic
 
 
-def test_wgrad_and_bn_argument_validation_without_gpu(built_lib):
+def test_wgrad_and_bn_pass_argument_validation_without_gpu(built_lib):
     lib = built_lib
     d = _lib.WgradDesc()
     assert lib.y5_conv_wgrad(ctypes.byref(d), None) == -1 and b"null" in lib.y5_last_error()
     assert lib.y5_bn_workspace_bytes(64) == 64 * 2 * 8
     assert lib.y5_sppf_bwd_workspace_bytes(2, 20, 20, 128) == 3 * 2 * 20 * 20 * 128 * 4
-    assert lib.y5_bn_stats(None, 64, 10, 64, _lib.Y5_F16, None, None) == -1
+    assert lib.y5_bn_stats(None, 64, 10, 64, _lib.Y5_F16, None, None, None) == -1
     assert lib.y5_weight_pack(None, _lib.Y5_F32, 8, 8, 1, None, 8, None, 8, _lib.Y5_F16, None) == -1
     assert lib.y5_weight_pack_chunk_elems() > 0
     assert lib.y5_weight_pack_multi(None, None, None, 3, _lib.Y5_F16, None) == -1 and lib.y5_weight_pack_multi(None, None, None, 0, _lib.Y5_F16, None) == 0
@@ -77,9 +77,9 @@ def test_pre_post_optimizer_argument_validation_without_gpu(built_lib):
     assert lib.y5_loss_fwd_bwd_scaled(None, None, None, None, None, None, None, None, 0, None) == -1
 
 
-def test_argument_validation_without_gpu(built_lib):
+def test_abi_version_and_argument_validation_without_gpu(built_lib):
     lib = built_lib
-    assert lib.y5_version() == 1
+    assert lib.y5_version() == 2
     d = _lib.ConvDesc()  # all null
     plan = ctypes.c_void_p()
     assert lib.y5_conv_plan_create(ctypes.byref(d), ctypes.byref(plan)) == -1  # Y5_E_INVALID

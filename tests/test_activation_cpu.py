@@ -98,7 +98,7 @@ def test_act_spec_and_refusals(restore_act):
         train_ops.conv_module(m.model[0], torch.zeros(1, 3, 32, 32), stem=2)
 
 
-def test_abi_activation_code_and_entry_points(built_lib):
+def test_abi_activation_code_and_slope_argument(built_lib):
     src = open(HEADER).read()
     codes = dict(re.findall(r"#define (Y5_ACT_\w+) (\d+)", src))
     assert {k: int(v) for k, v in codes.items()} == {"Y5_ACT_NONE": _lib.ACT_NONE, "Y5_ACT_SILU": _lib.ACT_SILU, "Y5_ACT_LEAKY": _lib.ACT_LEAKY}
@@ -107,11 +107,12 @@ def test_abi_activation_code_and_entry_points(built_lib):
     P = None
     # the activation is checked before anything touches the device: a bad code or a non-finite slope is refused on any machine
     args = (P, 64, P, 64, 10, 64, _lib.Y5_F16, P, P, P, P)
-    tail = (P, 1e-3, 0.03, P, P, P, 0, P)
-    assert lib.y5_bn_act_fwd_ex(*args, 3, 0.0, *tail) == -2 and b"activation code 3" in lib.y5_last_error()
-    assert lib.y5_bn_act_fwd_ex(*args, _lib.ACT_LEAKY, float("nan"), *tail) == -1 and b"slope" in lib.y5_last_error()
-    assert lib.y5_bn_act_fwd_sync_ex(*args, _lib.ACT_LEAKY, float("inf"), *tail) == -1
+    tail = (P, P, 1e-3, 0.03, P, P, P, 0, P)
+    sync_tail = (P, 4096, *tail[2:])  # a non-NULL row count: SyncBatchNorm's forward
+    assert lib.y5_bn_act_fwd(*args, 3, 0.0, *tail) == -2 and b"activation code 3" in lib.y5_last_error()
+    assert lib.y5_bn_act_fwd(*args, _lib.ACT_LEAKY, float("nan"), *tail) == -1 and b"slope" in lib.y5_last_error()
+    assert lib.y5_bn_act_fwd(*args, _lib.ACT_LEAKY, float("inf"), *sync_tail) == -1 and b"slope" in lib.y5_last_error()
     bargs = (P, 64, P, 64, P, 64, 10, 64, _lib.Y5_F16, P, P, P, P)
-    assert lib.y5_bn_act_bwd_ex(*bargs, 7, 0.0, P, P, P, P) == -2
-    assert lib.y5_bn_act_bwd_reduce_ex(*bargs, _lib.ACT_LEAKY, float("nan"), P, P, P, P) == -1
-    assert lib.y5_bn_act_bwd_ex(*bargs, _lib.ACT_LEAKY, 0.1, P, P, P, P) == -1 and b"null" in lib.y5_last_error().lower()
+    assert lib.y5_bn_act_bwd(*bargs, 7, 0.0, P, P, P, P) == -2
+    assert lib.y5_bn_act_bwd_reduce(*bargs, _lib.ACT_LEAKY, float("nan"), P, P, P, P) == -1
+    assert lib.y5_bn_act_bwd(*bargs, _lib.ACT_LEAKY, 0.1, P, P, P, P) == -1 and b"null" in lib.y5_last_error().lower()

@@ -361,13 +361,10 @@ class Head:
         wp, bp = _pack_head(w, bias, na, self.no, block_k, dtype)
         self.wp, self.bp = wp.to(dev), bp.to(dev)
         self.anchors = ANCHORS[:na] * stride / 8
-        dummy = torch.empty(8, dtype=dtype, device=dev)
-        self.keep = dummy
         d = _lib.DetectDesc()
         d.inp, d.in_pitch = self.ibuf.data_ptr() + off * self.ibuf.element_size(), pitch
         d.batch, d.ny, d.nx, d.in_c = B, ny, nx, cin
         d.weight, d.bias = self.wp.data_ptr(), self.bp.data_ptr()
-        d.raw, d.z = dummy.data_ptr(), dummy.data_ptr()  # outputs are bound per run, as the engine does
         d.z_rows, d.z_row0 = self.z_rows, z_row0
         d.na, d.no, d.nc = na, self.no, nc
         d.stride = stride

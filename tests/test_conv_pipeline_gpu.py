@@ -168,7 +168,6 @@ def _detect_case(dev, dtype, B, ny, nx, cin, na=3, nc=80, stride=16.0, seed=2):
     d.inp, d.in_pitch = xin.data_ptr(), cin
     d.batch, d.ny, d.nx, d.in_c = B, ny, nx, cin
     d.weight, d.bias = wp.data_ptr(), bias.data_ptr()
-    d.raw, d.z = raw_out.data_ptr(), z_out.data_ptr()
     d.z_rows, d.z_row0 = na * ny * nx, 0
     d.na, d.no, d.nc = na, no, nc
     d.stride = stride
@@ -178,7 +177,8 @@ def _detect_case(dev, dtype, B, ny, nx, cin, na=3, nc=80, stride=16.0, seed=2):
     plan = C.c_void_p()
     _lib.check(lib.y5_detect_plan_create(C.byref(d), C.byref(plan)), "detect_plan_create")
     try:
-        _lib.check(lib.y5_detect_plan_run(plan, C.c_void_p(_lib.stream_ptr(dev))), "detect")
+        _lib.check(lib.y5_detect_plan_run_to(plan, C.c_void_p(raw_out.data_ptr()), C.c_void_p(z_out.data_ptr()),
+                                             C.c_void_p(_lib.stream_ptr(dev))), "detect")
         torch.cuda.synchronize()
     finally:
         lib.y5_detect_plan_destroy(plan)
@@ -191,7 +191,7 @@ def _detect_case(dev, dtype, B, ny, nx, cin, na=3, nc=80, stride=16.0, seed=2):
     (64, 13, 13, 256),  # M = 10816 (84.5 tiles) x 3 anchors: several tiles per CTA, 4 K blocks each
     (5, 7, 9, 64),      # M = 315, one K block per tile
 ])
-def test_detect_head(cuda, dtype, case):
+def test_detect_head_run_to(cuda, dtype, case):
     raw, raw_ref, z, z_ref = _detect_case(cuda, dtype, *case)
     assert rel_err(raw, raw_ref) < TOL[dtype], (case, "raw", rel_err(raw, raw_ref))
     assert rel_err(z, z_ref) < TOL[dtype], (case, "z", rel_err(z, z_ref))

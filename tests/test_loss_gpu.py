@@ -1,4 +1,4 @@
-"""GPU: ComputeLoss (y5_loss_fwd_bwd) vs the oracle: build_targets bit-exact (int64 indices, order, fp32 tbox);
+"""GPU: ComputeLoss (y5_loss_fwd_bwd_scaled) vs the oracle: build_targets bit-exact (int64 indices, order, fp32 tbox);
 loss / items / gradients within fp32 tolerance (rtol 1e-4) for fp32 logits, 2e-3 for fp16 logits."""
 import os
 

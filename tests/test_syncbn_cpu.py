@@ -99,18 +99,23 @@ def test_graphed_train_step_refuses_a_syncing_model(fake_world):
         GraphedTrainStep(m, None, opt, batch=2, size=64)
 
 
-def test_split_entry_points_check_arguments_without_gpu(built_lib):
+def test_sync_passes_check_arguments_without_gpu(built_lib):
     lib = built_lib
     f16 = _lib.Y5_F16
-    assert lib.y5_bn_stats_sync(None, 64, 10, 64, f16, None, None) == -1 and b"bn_stats_sync" in lib.y5_last_error()
-    assert lib.y5_bn_act_fwd_sync(None, 64, None, 64, 10, 64, f16, None, None, None, None, 1, None, 1e-3, 0.03, None, None, None, 0, None) == -1
-    assert b"bn_act_fwd_sync y" in lib.y5_last_error()
-    assert lib.y5_bn_act_bwd_reduce(None, 64, None, 64, None, 64, 10, 64, f16, None, None, None, None, 1, None, None, None, None) == -1
+    n = 4096  # a non-NULL row count: SyncBatchNorm's forms of the passes
+    assert lib.y5_bn_stats(None, 64, 10, 64, f16, None, n, None) == -1 and b"bn_stats" in lib.y5_last_error()
+    assert lib.y5_bn_act_fwd(None, 64, None, 64, 10, 64, f16, None, None, None, None, 1, 0.0, None, n, 1e-3, 0.03, None, None, None, 0, None) == -1
+    assert b"bn_act_fwd y" in lib.y5_last_error()
+    assert lib.y5_bn_act_bwd_reduce(None, 64, None, 64, None, 64, 10, 64, f16, None, None, None, None, 1, 0.0, None, None, None, None) == -1
     assert b"bn_act_bwd_reduce y" in lib.y5_last_error()
     assert lib.y5_bn_act_bwd_apply(None, 64, None, 64, None, 64, 10, 64, f16, None, None, None, 1, None, None, None) == -1
     assert b"bn_act_bwd_apply y" in lib.y5_last_error()
-    # the existing entry points keep their messages
-    assert lib.y5_bn_act_fwd(None, 64, None, 64, 10, 64, f16, None, None, None, None, 1, None, 1e-3, 0.03, None, None, None, 0, None) == -1
+    # the plain forms
+    assert lib.y5_bn_act_fwd(None, 64, None, 64, 10, 64, f16, None, None, None, None, 1, 0.0, None, None, 1e-3, 0.03, None, None, None, 0, None) == -1
     assert b"bn_act_fwd y" in lib.y5_last_error()
-    assert lib.y5_bn_act_bwd(None, 64, None, 64, None, 64, 10, 64, f16, None, None, None, None, 1, None, None, None, None) == -1
+    assert lib.y5_bn_act_bwd(None, 64, None, 64, None, 64, 10, 64, f16, None, None, None, None, 1, 0.0, None, None, None, None) == -1
     assert b"bn_act_bwd y" in lib.y5_last_error()
+    # a row count needs the column sums it divides: refused before anything is launched (the pointers are never read)
+    p = 4096
+    assert lib.y5_bn_act_fwd(p, 64, p, 64, 10, 64, f16, p, p, p, p, 1, 0.0, None, n, 1e-3, 0.03, None, None, None, 0, None) == -1
+    assert b"bn_act_fwd: count needs the column sums" in lib.y5_last_error()

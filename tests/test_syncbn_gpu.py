@@ -2,8 +2,8 @@
 torch.nn.SyncBatchNorm.convert_sync_batchnorm, reference train.py:268-271).
 
 The defining property: k ranks synchronised on shards of a batch compute what one rank computes on the whole batch.
-  * the split entry points (y5_bn_stats_sync / y5_bn_act_fwd_sync, y5_bn_act_bwd_reduce / y5_bn_act_bwd_apply) with no
-    all-reduce between them give exactly what y5_bn_stats + y5_bn_act_fwd and y5_bn_act_bwd give;
+  * the split passes (y5_bn_stats / y5_bn_act_fwd with a row count, y5_bn_act_bwd_reduce / y5_bn_act_bwd_apply) with no
+    all-reduce between them give exactly what y5_bn_stats + y5_bn_act_fwd without one and y5_bn_act_bwd give;
   * shards of one batch whose workspaces are added (fp64, exact on integer-valued data) stand in for the all-reduce: each
     shard's z / dy are the full batch's rows bit for bit, and so are the running statistics;
   * two processes on one GPU (gloo) train a converted yolov5n like one process on the whole batch;
@@ -72,15 +72,20 @@ class _Layer:
 
 
 def _forward(L, act, sync, rm, rv, ws, eps=EPS):
-    """stats + normalise/activate; returns (z buffer, mean, invstd).  `ws` is the workspace (2C, or 2C + 1 for sync)."""
+    """stats + normalise/activate; returns (z buffer, mean, invstd).  `ws` is the workspace (2C, or 2C + 1 for sync, whose
+    slot 2C is the row count)."""
     lib, code, st = _lib.lib(), _lib.dtype_code(L.dtype), _st(L.dev)
     mean, invstd = torch.empty(L.ch, device=L.dev), torch.empty(L.ch, device=L.dev)
     zbuf, zp, zpitch = _slice(L.rows, L.ch, 16, -7.0, L.dtype, L.dev)
-    stats, fwd = (lib.y5_bn_stats_sync, lib.y5_bn_act_fwd_sync) if sync else (lib.y5_bn_stats, lib.y5_bn_act_fwd)
-    _lib.check(stats(L.yp, L.ypitch, L.rows, L.ch, code, ws.data_ptr(), st), "stats")
+
+    def count(w):
+        return w[2 * L.ch :].data_ptr() if sync else None
+
+    _lib.check(lib.y5_bn_stats(L.yp, L.ypitch, L.rows, L.ch, code, ws.data_ptr(), count(ws), st), "stats")
     return zbuf, zp, zpitch, mean, invstd, lambda sums: _lib.check(
-        fwd(L.yp, L.ypitch, zp, zpitch, L.rows, L.ch, code, mean.data_ptr(), invstd.data_ptr(), L.gamma.data_ptr(), L.beta.data_ptr(), act,
-            sums.data_ptr(), eps, MOM, rm.data_ptr(), rv.data_ptr(), L.rp, L.rpitch, st), "fwd")
+        lib.y5_bn_act_fwd(L.yp, L.ypitch, zp, zpitch, L.rows, L.ch, code, mean.data_ptr(), invstd.data_ptr(), L.gamma.data_ptr(),
+                          L.beta.data_ptr(), act, 0.0, sums.data_ptr(), count(sums), eps, MOM, rm.data_ptr(), rv.data_ptr(), L.rp, L.rpitch,
+                          st), "fwd")
 
 
 def _fused(L, act, rm, rv, eps=EPS):
@@ -93,13 +98,13 @@ def _fused(L, act, rm, rv, eps=EPS):
     dg, db = torch.empty(L.ch, device=L.dev), torch.empty(L.ch, device=L.dev)
     wsb = torch.zeros(2 * L.ch, dtype=torch.float64, device=L.dev)
     _lib.check(lib.y5_bn_act_bwd(L.yp, L.ypitch, L.dzp, L.dzpitch, dyp, dypitch, L.rows, L.ch, code, mean.data_ptr(), invstd.data_ptr(),
-                                 L.gamma.data_ptr(), L.beta.data_ptr(), act, dg.data_ptr(), db.data_ptr(), wsb.data_ptr(), st), "bwd")
+                                 L.gamma.data_ptr(), L.beta.data_ptr(), act, 0.0, dg.data_ptr(), db.data_ptr(), wsb.data_ptr(), st), "bwd")
     torch.cuda.synchronize()
     return dict(z=zbuf, mean=mean, invstd=invstd, rm=rm, rv=rv, dy=dybuf, dgamma=dg, dbeta=db)
 
 
 def _sharded(L, act, bounds, rm0, rv0, eps=EPS):
-    """The sync entry points on the shards [bounds[i], bounds[i+1]) of L, with the all-reduce emulated by adding the shards'
+    """The sync passes on the shards [bounds[i], bounds[i+1]) of L, with the all-reduce emulated by adding the shards'
     workspaces in fp64 (torch.stack(...).sum(0)).  Returns one result dict per shard."""
     lib, code, st = _lib.lib(), _lib.dtype_code(L.dtype), _st(L.dev)
     shards = [L.view(a, b) for a, b in zip(bounds[:-1], bounds[1:])]
@@ -123,7 +128,7 @@ def _sharded(L, act, bounds, rm0, rv0, eps=EPS):
         o["dgamma"], o["dbeta"] = torch.empty(c, device=L.dev), torch.empty(c, device=L.dev)
         ws = torch.zeros(2 * c, dtype=torch.float64, device=L.dev)
         _lib.check(lib.y5_bn_act_bwd_reduce(S.yp, S.ypitch, S.dzp, S.dzpitch, o["dyp"], o["dypitch"], S.rows, c, code, o["mean"].data_ptr(),
-                                            o["invstd"].data_ptr(), L.gamma.data_ptr(), L.beta.data_ptr(), act, o["dgamma"].data_ptr(),
+                                            o["invstd"].data_ptr(), L.gamma.data_ptr(), L.beta.data_ptr(), act, 0.0, o["dgamma"].data_ptr(),
                                             o["dbeta"].data_ptr(), ws.data_ptr(), st), "bwd_reduce")
         bws.append(ws)
     btotal = torch.stack(bws).sum(0)
@@ -171,19 +176,19 @@ def _running(ch, dev, seed):
 @pytest.mark.parametrize("ch,rows,residual", BN_SHAPES)
 @pytest.mark.parametrize("act", [0, 1])
 @pytest.mark.parametrize("dtype", DTYPES)
-def test_split_entry_points_equal_fused(cuda, ch, rows, residual, act, dtype):
+def test_sync_passes_equal_plain(cuda, ch, rows, residual, act, dtype):
     L = _layer(ch, rows, residual, dtype, cuda, ch + rows)
     rm0, rv0 = _running(ch, cuda, rows)
     ref = _fused(L, act, rm0.clone(), rv0.clone())
     (got,) = _sharded(L, act, [0, rows], rm0, rv0)
     for k in ("z", "mean", "invstd", "rm", "rv", "dy", "dgamma", "dbeta"):
-        assert _bits(got[k], ref[k]), (k, "split entry points differ from y5_bn_stats + y5_bn_act_fwd / y5_bn_act_bwd")
+        assert _bits(got[k], ref[k]), (k, "the passes with a row count differ from y5_bn_stats + y5_bn_act_fwd / y5_bn_act_bwd without one")
     _check_views_untouched(L, got)
 
 
 @pytest.mark.parametrize("act", [0, 1])
 @pytest.mark.parametrize("dtype", DTYPES)
-def test_split_entry_points_random_data(cuda, act, dtype):
+def test_sync_passes_random_data(cuda, act, dtype):
     """random data: the fp64 column sums may add in another order, so equal to a few ulps (dy: one activation-dtype ulp)"""
     ch, rows = 80, 10007
     L = _layer(ch, rows, True, dtype, cuda, 5, integer=False)
@@ -198,21 +203,22 @@ def test_split_entry_points_random_data(cuda, act, dtype):
         assert float((a - b).abs().max()) <= ulp * float(b.abs().max()), k
 
 
-def test_split_entry_points_validate_arguments(cuda):
+def test_sync_passes_validate_arguments(cuda):
     lib = _lib.lib()
     y = torch.zeros(16, 8, dtype=torch.float16, device=cuda)
     f = torch.zeros(8, device=cuda)
     ws = torch.zeros(17, dtype=torch.float64, device=cuda)
     p = y.data_ptr()
-    assert lib.y5_bn_stats_sync(p, 8, 16, 8, _lib.Y5_F32, ws.data_ptr(), None) != 0
-    assert lib.y5_bn_stats_sync(p + 2, 8, 16, 8, _lib.Y5_F16, ws.data_ptr(), None) != 0  # misaligned view
-    assert lib.y5_bn_act_fwd_sync(p, 8, p, 8, 16, 8, _lib.Y5_F16, f.data_ptr(), f.data_ptr(), f.data_ptr(), f.data_ptr(), 1, None, EPS, MOM,
-                                  None, None, None, 0, None) != 0  # sums are required
-    assert b"bn_act_fwd_sync" in lib.y5_last_error()
+    n = ws[16:].data_ptr()
+    assert lib.y5_bn_stats(p, 8, 16, 8, _lib.Y5_F32, ws.data_ptr(), n, None) != 0
+    assert lib.y5_bn_stats(p + 2, 8, 16, 8, _lib.Y5_F16, ws.data_ptr(), n, None) != 0  # misaligned view
+    assert lib.y5_bn_act_fwd(p, 8, p, 8, 16, 8, _lib.Y5_F16, f.data_ptr(), f.data_ptr(), f.data_ptr(), f.data_ptr(), 1, 0.0, None, n, EPS, MOM,
+                             None, None, None, 0, None) != 0  # a row count requires the sums
+    assert b"bn_act_fwd" in lib.y5_last_error()
     assert lib.y5_bn_act_bwd_apply(p, 8, p, 8, p, 8, 16, 8, _lib.Y5_F16, f.data_ptr(), f.data_ptr(), f.data_ptr(), 1, ws.data_ptr(), None,
                                    None) != 0  # count is required
-    assert lib.y5_bn_act_bwd_reduce(p, 8, p, 8, p, 8, 16, 8, _lib.Y5_F16, f.data_ptr(), f.data_ptr(), f.data_ptr(), f.data_ptr(), 1, None,
-                                    f.data_ptr(), ws.data_ptr(), None) != 0  # dgamma is required
+    assert lib.y5_bn_act_bwd_reduce(p, 8, p, 8, p, 8, 16, 8, _lib.Y5_F16, f.data_ptr(), f.data_ptr(), f.data_ptr(), f.data_ptr(), 1, 0.0,
+                                    None, f.data_ptr(), ws.data_ptr(), None) != 0  # dgamma is required
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -228,7 +234,7 @@ def _bounds(rows, k):
 @pytest.mark.parametrize("k", [2, 3, 4])
 @pytest.mark.parametrize("ch,rows,residual", [(40, 4099, True), (1280, 3001, False), (80, 10007, True)])
 @pytest.mark.parametrize("dtype", DTYPES)
-def test_emulated_ranks_forward_exact(cuda, k, ch, rows, residual, dtype):
+def test_emulated_rank_shards_forward_exact(cuda, k, ch, rows, residual, dtype):
     """Integer data: every fp64 sum is exact in any order, so the shards' statistics are the full batch's: z rows, mean,
     invstd and the running statistics (1/N and N/(N-1) formed on the device from the summed count) bit for bit.
     dgamma / dbeta are per-shard fp32 sums of non-integer terms: their sum over shards matches to a few fp32 ulps."""
@@ -251,7 +257,7 @@ def test_emulated_ranks_forward_exact(cuda, k, ch, rows, residual, dtype):
 @pytest.mark.parametrize("act,rows", [(0, 10007), (1, 390)])
 @pytest.mark.parametrize("ch", [40, 1280])
 @pytest.mark.parametrize("dtype", DTYPES)
-def test_emulated_ranks_backward_exact(cuda, k, act, rows, ch, dtype):
+def test_emulated_rank_shards_backward_exact(cuda, k, act, rows, ch, dtype):
     """dy needs both backward sums exact whatever the shard boundaries.  Every column holds +1 and -1 equally often and
     eps = 0, so mean = 0, invstd = 1 and x_hat = y exactly; dz is an integer.  Linear layers then sum integers.  SiLU layers
     sum du = round(dz * silu'(t)) with t = +-gamma + beta in [-3, 3]: multiples of 2^-14 below 2^10 in magnitude over 390

@@ -50,7 +50,6 @@ def _desc(dtype, in_ptr, pitch, B, ny, nx, cin, wp, bp, na, no, nc, stride, bloc
     d.inp, d.in_pitch = in_ptr, pitch
     d.batch, d.ny, d.nx, d.in_c = B, ny, nx, cin
     d.weight, d.bias = wp.data_ptr(), bp.data_ptr()
-    d.raw, d.z = wp.data_ptr(), wp.data_ptr()  # outputs are bound per run, as the engine does
     d.z_rows, d.z_row0 = z_rows, z_row0
     d.na, d.no, d.nc = na, no, nc
     d.stride = stride

@@ -54,11 +54,12 @@ def main():
         def st():
             return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
-        t_stats = graph_time(lambda: lib.y5_bn_stats(y.data_ptr(), c, rows, c, code, ws.data_ptr(), st()))
+        t_stats = graph_time(lambda: lib.y5_bn_stats(y.data_ptr(), c, rows, c, code, ws.data_ptr(), None, st()))
         t_fwd = graph_time(lambda: lib.y5_bn_act_fwd(y.data_ptr(), c, z.data_ptr(), c, rows, c, code, mean.data_ptr(), invstd.data_ptr(),
-                                                     gamma.data_ptr(), beta.data_ptr(), 1, None, 1e-3, 0.03, None, None, None, 0, st()))
+                                                     gamma.data_ptr(), beta.data_ptr(), 1, 0.0, None, None, 1e-3, 0.03, None, None, None, 0,
+                                                     st()))
         t_bwd = graph_time(lambda: lib.y5_bn_act_bwd(y.data_ptr(), c, dz.data_ptr(), c, z.data_ptr(), c, rows, c, code, mean.data_ptr(),
-                                                     invstd.data_ptr(), gamma.data_ptr(), beta.data_ptr(), 1, dg.data_ptr(), db.data_ptr(),
+                                                     invstd.data_ptr(), gamma.data_ptr(), beta.data_ptr(), 1, 0.0, dg.data_ptr(), db.data_ptr(),
                                                      ws.data_ptr(), st()))
         nb = rows * c * 2
         print(f"{rows:>9} {c:>4} | {t_stats:7.1f} ({nb / t_stats / 1e3:5.0f}) {t_fwd:7.1f} ({2 * nb / t_fwd / 1e3:5.0f}) {t_bwd:7.1f} ({5 * nb / t_bwd / 1e3:5.0f})",

@@ -47,7 +47,6 @@ class DetectDesc(C.Structure):
         ("inp", C.c_void_p), ("in_pitch", C.c_int32),
         ("batch", C.c_int32), ("ny", C.c_int32), ("nx", C.c_int32), ("in_c", C.c_int32),
         ("weight", C.c_void_p), ("bias", C.c_void_p),
-        ("raw", C.c_void_p), ("z", C.c_void_p),
         ("z_rows", C.c_int32), ("z_row0", C.c_int32),
         ("na", C.c_int32), ("no", C.c_int32), ("nc", C.c_int32),
         ("stride", C.c_float), ("anchor_wh", C.c_float * 8),
@@ -191,7 +190,6 @@ SIGNATURES = {
     "y5_conv_bn_silu_fwd": (_I32, [C.POINTER(ConvDesc), _P]),
     "y5_conv_direct_fwd": (_I32, [C.POINTER(ConvDesc), _P]),
     "y5_detect_plan_create": (_I32, [C.POINTER(DetectDesc), C.POINTER(_P)]),
-    "y5_detect_plan_run": (_I32, [_P, _P]),
     "y5_detect_plan_run_to": (_I32, [_P, _P, _P, _P]),
     "y5_detect_plan_destroy": (None, [_P]),
     "y5_stem_s2d": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
@@ -203,7 +201,6 @@ SIGNATURES = {
     "y5_nms_batched": (_I32, [C.POINTER(NmsParams), _P, _P, _P, _P, _P, _I64, _P]),
     "y5_box_iou": (_I32, [_P, _I32, _P, _I32, _F, _P, _P]),
     "y5_loss_workspace_bytes": (_I64, [C.POINTER(LossParams)]),
-    "y5_loss_fwd_bwd": (_I32, [C.POINTER(LossParams), C.POINTER(_P), _P, _P, _P, C.POINTER(_P), _P, _I64, _P]),
     "y5_loss_read_targets": (_I32, [C.POINTER(LossParams), _P, _I32, _P, _P, _P, _P]),
     "y5_seg_loss_workspace_bytes": (_I64, [C.POINTER(LossParams)]),
     "y5_seg_loss_fwd_bwd_scaled": (_I32, [C.POINTER(LossParams), C.POINTER(_P), _P, _P, _P, _I32, _I64, _I64, _I64, _I64, _I32, _I32, _I32,
@@ -211,21 +208,15 @@ SIGNATURES = {
     "y5_seg_loss_read_targets": (_I32, [C.POINTER(LossParams), _P, _I32, _P, _P, _P, _P]),
     "y5_conv_wgrad": (_I32, [C.POINTER(WgradDesc), _P]),
     "y5_bn_workspace_bytes": (_I64, [_I32]),
-    "y5_bn_stats": (_I32, [_P, _I32, _I64, _I32, _I32, _P, _P]),
-    "y5_bn_act_fwd": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _F, _F, _P, _P, _P, _I32, _P]),
+    "y5_bn_stats": (_I32, [_P, _I32, _I64, _I32, _I32, _P, _P, _P]),
+    "y5_bn_act_fwd": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _P, _F, _F, _P, _P, _P, _I32, _P]),
     "y5_upsample2x_bwd": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "y5_sppf_bwd_workspace_bytes": (_I64, [_I32, _I32, _I32, _I32]),
     "y5_sppf_pool_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P]),
-    "y5_bn_act_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _P, _P, _P]),
+    "y5_bn_act_bwd": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P]),
     "y5_col_sum": (_I32, [_P, _I32, _I64, _I32, _I32, _P, _P, _P]),
-    "y5_bn_stats_sync": (_I32, [_P, _I32, _I64, _I32, _I32, _P, _P]),
-    "y5_bn_act_fwd_sync": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _F, _F, _P, _P, _P, _I32, _P]),
-    "y5_bn_act_bwd_reduce": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _P, _P, _P]),
+    "y5_bn_act_bwd_reduce": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P]),
     "y5_bn_act_bwd_apply": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _I32, _P, _P, _P]),
-    "y5_bn_act_fwd_ex": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _F, _F, _P, _P, _P, _I32, _P]),
-    "y5_bn_act_bwd_ex": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P]),
-    "y5_bn_act_fwd_sync_ex": (_I32, [_P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _F, _F, _P, _P, _P, _I32, _P]),
-    "y5_bn_act_bwd_reduce_ex": (_I32, [_P, _I32, _P, _I32, _P, _I32, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P]),
     "y5_weight_pack": (_I32, [_P, _I32, _I32, _I32, _I32, _P, _I32, _P, _I32, _I32, _P]),
     "y5_weight_pack_chunk_elems": (_I32, []),
     "y5_weight_pack_multi": (_I32, [_P, _P, _P, _I32, _I32, _P]),

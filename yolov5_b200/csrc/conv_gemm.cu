@@ -1227,7 +1227,7 @@ extern "C" Y5_API int y5_conv_direct_fwd(const y5_conv_desc* d, void* stream) {
 extern "C" Y5_API int y5_detect_plan_create(const y5_detect_desc* d, y5_detect_plan** out) {
     if (!out) return set_error(Y5_E_INVALID, "detect: null plan out");
     *out = nullptr;
-    if (!d || !d->in || !d->weight || !d->bias || !d->raw || !d->z) return set_error(Y5_E_INVALID, "detect: null pointer");
+    if (!d || !d->in || !d->weight || !d->bias) return set_error(Y5_E_INVALID, "detect: null pointer");
     if (d->dtype != Y5_F16 && d->dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "detect: dtype must be fp16/bf16");
     if (d->na < 1 || d->na > 4 || d->no < 6 || d->no > kHeadMaxNo || d->nc < 1 || d->nc > kHeadMaxNc || 5 + d->nc > d->no)
         return set_error(Y5_E_UNSUPPORTED, "detect: na %d no %d nc %d unsupported (no <= %d, nc <= %d, na <= 4)", d->na, d->no, d->nc,
@@ -1250,8 +1250,6 @@ extern "C" Y5_API int y5_detect_plan_create(const y5_detect_desc* d, y5_detect_p
     p.stride = 1;
     p.is_bf16 = d->dtype == Y5_BF16;
     p.bias = d->bias;
-    p.raw = d->raw;
-    p.z = d->z;
     p.na = d->na; p.no = d->no; p.nc = d->nc; p.nx = d->nx;
     p.z_rows = d->z_rows; p.z_row0 = d->z_row0;
     p.det_stride = d->stride;
@@ -1278,10 +1276,6 @@ extern "C" Y5_API int y5_detect_plan_create(const y5_detect_desc* d, y5_detect_p
     if (int e2 = finish_plan(pc, kHeadN, 1, 1)) { delete plan; return e2; }
     *out = plan;
     return 0;
-}
-extern "C" Y5_API int y5_detect_plan_run(const y5_detect_plan* plan, void* stream) {
-    if (!plan) return set_error(Y5_E_INVALID, "detect: null plan");
-    return run_plan(plan->pc, static_cast<cudaStream_t>(stream));
 }
 extern "C" Y5_API int y5_detect_plan_run_to(const y5_detect_plan* plan, void* raw, void* z, void* stream) {
     if (!plan || !raw || !z) return set_error(Y5_E_INVALID, "detect: null plan/output");

@@ -124,6 +124,6 @@ int encode_im2col(CUtensorMap* map, int dtype, const void* base, int C, int W, i
 
 }  // namespace y5
 
-extern "C" Y5_API int y5_version(void) { return 1; }
+extern "C" Y5_API int y5_version(void) { return 2; }
 extern "C" Y5_API const char* y5_last_error(void) { return y5::g_err; }
 extern "C" Y5_API int64_t y5_launch_count(void) { return y5::g_launches.load(std::memory_order_relaxed); }

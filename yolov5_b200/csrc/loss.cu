@@ -728,11 +728,6 @@ extern "C" Y5_API int64_t y5_loss_workspace_bytes(const y5_loss_params* p) {
     return static_cast<int64_t>(loss_ws(p).total);
 }
 
-extern "C" Y5_API int y5_loss_fwd_bwd(const y5_loss_params* p, const void* const* pl, const float* targets, const float* anchors,
-                                      float* out_loss, void* const* grad, void* workspace, int64_t workspace_bytes, void* stream) {
-    return y5_loss_fwd_bwd_scaled(p, pl, targets, anchors, out_loss, grad, nullptr, workspace, workspace_bytes, stream);
-}
-
 namespace {
 // the detection launch set; `trow` (segmentation loss only) receives each match's target row
 int loss_launch(const y5_loss_params* p, const void* const* pl, const float* targets, const float* anchors, float* out_loss,

@@ -684,31 +684,32 @@ static int check_operand(const char* what, const char* operand, const void* p, i
     return check_view(p, pitch, channels, name);
 }
 
-// The BatchNorm entry points and their SyncBatchNorm splits share these launches.  `count` (SyncBN) is the fp64 slot after
-// the 2*channels column sums: bn_stats adds this rank's rows to it, and after the caller's SUM all-reduce of the whole
-// workspace it holds N, which the forward and the apply pass divide by instead of the host's `rows`.
-static int bn_stats_launch(const char* what, const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace,
-                           bool sync, void* stream) {
-    if (int e = check_view(y, pitch, channels, what)) return e;
-    if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "%s: dtype must be fp16 or bf16", what);
-    if (!workspace || rows <= 0) return set_error(Y5_E_INVALID, "%s: bad argument", what);
-    double* ws = static_cast<double*>(workspace);
+// `count` (SyncBatchNorm) is one fp64 row count, the slot after the 2*channels column sums: y5_bn_stats adds this rank's
+// rows to it, and after the caller's SUM all-reduce of the whole workspace it holds N, which y5_bn_act_fwd and
+// y5_bn_act_bwd_apply divide by instead of the host's `rows`.  NULL: `rows` is the whole batch.
+extern "C" Y5_API int y5_bn_stats(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace, double* count,
+                                  void* stream) {
+    if (int e = check_view(y, pitch, channels, "bn_stats")) return e;
+    if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "bn_stats: dtype must be fp16 or bf16");
+    if (!workspace || rows <= 0) return set_error(Y5_E_INVALID, "bn_stats: bad argument");
     const RowGeom g = row_geom(channels, rows, true);
     count_launch();
     launch_pdl(col_stats_kernel<0>, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream), 
-        y, pitch, rows, channels, dtype == Y5_BF16, g.cgx, g.rpb, ws, sync ? ws + 2 * static_cast<int64_t>(channels) : static_cast<double*>(nullptr));
-    return launch_status(what);
+        y, pitch, rows, channels, dtype == Y5_BF16, g.cgx, g.rpb, static_cast<double*>(workspace), count);
+    return launch_status("bn_stats");
 }
 
-static int bn_act_fwd_launch(const char* what, const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
-                             float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope, const void* sums,
-                             bool sync, float eps, float momentum, float* running_mean, float* running_var, const void* residual,
-                             int32_t res_pitch, void* stream) {
+extern "C" Y5_API int y5_bn_act_fwd(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
+                                    float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope,
+                                    const void* sums, const void* count, float eps, float momentum, float* running_mean, float* running_var,
+                                    const void* residual, int32_t res_pitch, void* stream) {
+    const char* what = "bn_act_fwd";
     if (int e = check_act(what, act, slope)) return e;
     if (int e = check_operand(what, "y", y, y_pitch, channels)) return e;
     if (int e = check_operand(what, "z", z, z_pitch, channels)) return e;
     if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "%s: dtype must be fp16 or bf16", what);
-    if (!mean || !invstd || !gamma || !beta || rows <= 0 || (sync && !sums)) return set_error(Y5_E_INVALID, "%s: bad argument", what);
+    if (!mean || !invstd || !gamma || !beta || rows <= 0) return set_error(Y5_E_INVALID, "%s: bad argument", what);
+    if (count && !sums) return set_error(Y5_E_INVALID, "%s: count needs the column sums", what);
     if (residual)
         if (int e = check_operand(what, "residual", residual, res_pitch, channels)) return e;
     const RowGeom g = row_geom(channels, rows, false, residual ? 3 : 4);
@@ -721,8 +722,7 @@ static int bn_act_fwd_launch(const char* what, const void* y, int32_t y_pitch, v
                             : (leaky ? bn_act_fwd_kernel<false, true> : bn_act_fwd_kernel<false, false>);
     launch_pdl(kernel, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream),
         y, y_pitch, z, z_pitch, rows, channels, dtype == Y5_BF16, act, g.cgx, g.rpb, mean, invstd, gamma, beta, s,
-        sync ? s + 2 * static_cast<int64_t>(channels) : static_cast<const double*>(nullptr), inv_rows, unbias, eps, momentum,
-        running_mean, running_var, residual, res_pitch, slope);
+        static_cast<const double*>(count), inv_rows, unbias, eps, momentum, running_mean, running_var, residual, res_pitch, slope);
     return launch_status(what);
 }
 
@@ -766,14 +766,6 @@ static void bn_bwd_apply_launch(const void* y, int32_t y_pitch, const void* dz, 
                dbeta);
 }
 
-extern "C" Y5_API int y5_bn_stats(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace, void* stream) {
-    return bn_stats_launch("bn_stats", y, pitch, rows, channels, dtype, workspace, false, stream);
-}
-
-extern "C" Y5_API int y5_bn_stats_sync(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, void* workspace, void* stream) {
-    return bn_stats_launch("bn_stats_sync", y, pitch, rows, channels, dtype, workspace, true, stream);
-}
-
 extern "C" Y5_API int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, float* out, void* workspace,
                                  void* stream) {
     if (int e = check_view(y, pitch, channels, "col_sum")) return e;
@@ -789,9 +781,10 @@ extern "C" Y5_API int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int
     return launch_status("col_sum");
 }
 
-static int bn_act_bwd_impl(const char* what, const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
-                           int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
-                           const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream) {
+extern "C" Y5_API int y5_bn_act_bwd(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
+                                    int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
+                                    const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream) {
+    const char* what = "bn_act_bwd";
     if (int e = check_act(what, act, slope)) return e;
     if (int e = bn_bwd_check(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace)) return e;
     if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "%s: bad argument", what);
@@ -803,9 +796,11 @@ static int bn_act_bwd_impl(const char* what, const void* y, int32_t y_pitch, con
     return launch_status(what);
 }
 
-static int bn_act_bwd_reduce_impl(const char* what, const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
-                                  int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
-                                  const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream) {
+extern "C" Y5_API int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                                           int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
+                                           const float* gamma, const float* beta, int32_t act, float slope, float* dgamma, float* dbeta,
+                                           void* workspace, void* stream) {
+    const char* what = "bn_act_bwd_reduce";
     if (int e = check_act(what, act, slope)) return e;
     if (int e = bn_bwd_check(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace)) return e;
     if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "%s: bad argument", what);
@@ -815,68 +810,6 @@ static int bn_act_bwd_reduce_impl(const char* what, const void* y, int32_t y_pit
     launch_pdl(bn_affine_grad_kernel, dim3((channels + 127) / 128), dim3(128), 0, st, static_cast<const double*>(workspace), static_cast<int>(channels),
                dgamma, dbeta);
     return launch_status(what);
-}
-
-extern "C" Y5_API int y5_bn_act_fwd(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
-                                    float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, const void* sums,
-                                    float eps, float momentum, float* running_mean, float* running_var, const void* residual,
-                                    int32_t res_pitch, void* stream) {
-    return bn_act_fwd_launch("bn_act_fwd", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, 0.0f, sums, false, eps,
-                             momentum, running_mean, running_var, residual, res_pitch, stream);
-}
-
-extern "C" Y5_API int y5_bn_act_fwd_ex(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
-                                       float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope, const void* sums,
-                                       float eps, float momentum, float* running_mean, float* running_var, const void* residual,
-                                       int32_t res_pitch, void* stream) {
-    return bn_act_fwd_launch("bn_act_fwd_ex", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope, sums, false, eps,
-                             momentum, running_mean, running_var, residual, res_pitch, stream);
-}
-
-extern "C" Y5_API int y5_bn_act_fwd_sync(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
-                                         float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, const void* sums,
-                                         float eps, float momentum, float* running_mean, float* running_var, const void* residual,
-                                         int32_t res_pitch, void* stream) {
-    return bn_act_fwd_launch("bn_act_fwd_sync", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, 0.0f, sums, true, eps,
-                             momentum, running_mean, running_var, residual, res_pitch, stream);
-}
-
-extern "C" Y5_API int y5_bn_act_fwd_sync_ex(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels,
-                                            int32_t dtype, float* mean, float* invstd, const float* gamma, const float* beta, int32_t act, float slope,
-                                            const void* sums, float eps, float momentum, float* running_mean, float* running_var,
-                                            const void* residual, int32_t res_pitch, void* stream) {
-    return bn_act_fwd_launch("bn_act_fwd_sync_ex", y, y_pitch, z, z_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope, sums, true,
-                             eps, momentum, running_mean, running_var, residual, res_pitch, stream);
-}
-
-extern "C" Y5_API int y5_bn_act_bwd(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
-                                    int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
-                                    const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace, void* stream) {
-    return bn_act_bwd_impl("bn_act_bwd", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, 0.0f, dgamma,
-                           dbeta, workspace, stream);
-}
-
-extern "C" Y5_API int y5_bn_act_bwd_ex(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
-                                       int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
-                                       const float* beta, int32_t act, float slope, float* dgamma, float* dbeta, void* workspace, void* stream) {
-    return bn_act_bwd_impl("bn_act_bwd_ex", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope,
-                           dgamma, dbeta, workspace, stream);
-}
-
-extern "C" Y5_API int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
-                                           int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
-                                           const float* gamma, const float* beta, int32_t act, float* dgamma, float* dbeta, void* workspace,
-                                           void* stream) {
-    return bn_act_bwd_reduce_impl("bn_act_bwd_reduce", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act,
-                                  0.0f, dgamma, dbeta, workspace, stream);
-}
-
-extern "C" Y5_API int y5_bn_act_bwd_reduce_ex(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
-                                              int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd,
-                                              const float* gamma, const float* beta, int32_t act, float slope, float* dgamma, float* dbeta,
-                                              void* workspace, void* stream) {
-    return bn_act_bwd_reduce_impl("bn_act_bwd_reduce_ex", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta,
-                                  act, slope, dgamma, dbeta, workspace, stream);
 }
 
 extern "C" Y5_API int y5_bn_act_bwd_apply(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,

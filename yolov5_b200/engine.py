@@ -568,9 +568,6 @@ class Program:
             d.inp, d.in_pitch = v.ptr, v.pitch
             d.batch, d.ny, d.nx, d.in_c = self.B, v.h, v.w, v.c
             d.weight, d.bias = wp.data_ptr(), bias.data_ptr()
-            dummy = torch.empty(8, dtype=self.dtype, device=self.device)  # real outputs are bound per call
-            self._keep.append(dummy)
-            d.raw, d.z = dummy.data_ptr(), dummy.data_ptr()
             d.z_rows, d.z_row0 = self.z_rows, row0
             d.na, d.no, d.nc = na, no, nc
             stride = float(m.stride[i])

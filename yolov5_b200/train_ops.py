@@ -429,7 +429,7 @@ def _bn_act_fwd(y, z_ptr: int, z_pitch: int, gamma, beta, running_mean, running_
     b, c, ho, wo = y.shape
     rows = b * ho * wo
     code = _lib.dtype_code(y.dtype)
-    fwd_fn, n_rows = lib.y5_bn_act_fwd_ex, None
+    count = n_rows = None
     if training:
         mean = torch.empty(c, dtype=torch.float32, device=dev)
         invstd = torch.empty(c, dtype=torch.float32, device=dev)
@@ -438,22 +438,22 @@ def _bn_act_fwd(y, z_ptr: int, z_pitch: int, gamma, beta, running_mean, running_
         rv = running_var if running_var is None or running_var.dtype == torch.float32 else running_var.float()
         if pg is None:
             ws = _bn_ws(c, dev)
-            _lib.check(lib.y5_bn_stats(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats")
         else:  # SyncBatchNorm: [column sums | row count] of every rank in one all-reduce, then the statistics of all rows
             ws = _arena.take(2 * c + 1, dev)
-            _lib.check(lib.y5_bn_stats_sync(y.data_ptr(), c, rows, c, code, ws.data_ptr(), _st(dev)), "bn_stats_sync")
+            count = ws[2 * c :].data_ptr()
+        _lib.check(lib.y5_bn_stats(y.data_ptr(), c, rows, c, code, ws.data_ptr(), count, _st(dev)), "bn_stats")
+        if pg is not None:
             _all_reduce(ws[: 2 * c + 1], pg)
             n_rows = ws[2 * c : 2 * c + 1].clone()  # N for the backward: the arena is cleared by the next forward
-            fwd_fn = lib.y5_bn_act_fwd_sync_ex
         sums = ws.data_ptr()
     else:
         mean = running_mean.float().contiguous()
         invstd = torch.rsqrt(running_var.float() + eps)
         rm = rv = sums = None
     g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
-    _lib.check(fwd_fn(y.data_ptr(), c, z_ptr, z_pitch, rows, c, code, mean.data_ptr(), invstd.data_ptr(), g32.data_ptr(),
-                      b32.data_ptr(), *act, sums, eps, momentum, rm.data_ptr() if rm is not None else None,
-                      rv.data_ptr() if rv is not None else None, res[0], res[1], _st(dev)), "bn_act_fwd")
+    _lib.check(lib.y5_bn_act_fwd(y.data_ptr(), c, z_ptr, z_pitch, rows, c, code, mean.data_ptr(), invstd.data_ptr(), g32.data_ptr(),
+                                 b32.data_ptr(), *act, sums, count, eps, momentum, rm.data_ptr() if rm is not None else None,
+                                 rv.data_ptr() if rv is not None else None, res[0], res[1], _st(dev)), "bn_act_fwd")
     if training:
         if rm is not running_mean:
             running_mean.copy_(rm)
@@ -474,13 +474,13 @@ def _bn_act_bwd(y, dz_ptr: int, dz_pitch: int, mean, invstd, g32, b32, act, pg, 
     dbeta = torch.empty(c, dtype=torch.float32, device=dev)
     ws = _bn_ws(c, dev)
     if pg is None:
-        _lib.check(lib.y5_bn_act_bwd_ex(y.data_ptr(), c, dz_ptr, dz_pitch, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
-                                        invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(), dbeta.data_ptr(),
-                                        ws.data_ptr(), _st(dev)), "bn_act_bwd")
+        _lib.check(lib.y5_bn_act_bwd(y.data_ptr(), c, dz_ptr, dz_pitch, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                     invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(), dbeta.data_ptr(),
+                                     ws.data_ptr(), _st(dev)), "bn_act_bwd")
     else:  # SyncBatchNorm: dgamma / dbeta stay this rank's sums (DDP averages them); dy uses the sums of every rank over N
-        _lib.check(lib.y5_bn_act_bwd_reduce_ex(y.data_ptr(), c, dz_ptr, dz_pitch, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
-                                               invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(),
-                                               dbeta.data_ptr(), ws.data_ptr(), _st(dev)), "bn_act_bwd_reduce")
+        _lib.check(lib.y5_bn_act_bwd_reduce(y.data_ptr(), c, dz_ptr, dz_pitch, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
+                                            invstd.data_ptr(), g32.data_ptr(), b32.data_ptr(), *act, dgamma.data_ptr(),
+                                            dbeta.data_ptr(), ws.data_ptr(), _st(dev)), "bn_act_bwd_reduce")
         _all_reduce(ws[: 2 * c], pg)
         _lib.check(lib.y5_bn_act_bwd_apply(y.data_ptr(), c, dz_ptr, dz_pitch, dy.data_ptr(), c, rows, c, code, mean.data_ptr(),
                                            invstd.data_ptr(), g32.data_ptr(), act[0], ws.data_ptr(), n_rows.data_ptr(),

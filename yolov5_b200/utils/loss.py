@@ -1,6 +1,6 @@
 """ComputeLoss with the reference's interface (reference utils/loss.py:101-247): ``ComputeLoss(model)(p, targets) ->
 (loss (1,), items (3,))`` and ``.build_targets(p, targets)``.  build_targets, the gather/CIoU/scatter and both BCE
-terms -- forward and backward -- run in liby5b200 (y5_loss_fwd_bwd); the returned loss carries a custom autograd
+terms -- forward and backward -- run in liby5b200 (y5_loss_fwd_bwd_scaled); the returned loss carries a custom autograd
 node that hands the kernel-computed gradient of every prediction level back to PyTorch.  ``CrossEntropyLoss`` is the
 classification loss (nn.CrossEntropyLoss with label smoothing) on y5_cross_entropy.
 """
