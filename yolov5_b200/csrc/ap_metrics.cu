@@ -524,12 +524,6 @@ static ApWorkspace ap_workspace(char* base, long long n_cap, int n_img, int niou
     return w;
 }
 
-static int last_status(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 static int ap_shape_error(int32_t n_img, int32_t rows_per_image, int32_t niou, int32_t nt, int32_t sets) {
     if (n_img < 0 || rows_per_image < 0 || nt < 0 || niou < 1 || sets < 1 || sets > 2)
         return set_error(Y5_E_INVALID, "ap_per_class: bad shape (images %d, rows %d, niou %d, labels %d, sets %d)", n_img, rows_per_image,
@@ -564,36 +558,40 @@ extern "C" Y5_API int y5_ap_per_class(const uint8_t* tp, const uint8_t* tp2, int
     if (workspace_bytes < w.bytes)
         return set_error(Y5_E_INVALID, "ap_per_class: workspace of %lld bytes, %lld needed", static_cast<long long>(workspace_bytes), w.bytes);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    ap_setup_kernel<<<1, kOneBlock, 0, st>>>(target_cls, nt, count, n_img, rows_per_image, w.img_off, w.label_count, w.pred_count, meta);
-    count_launch();
+    const char* what = "ap_per_class";
+    if (int e = launch(what, ap_setup_kernel, {1, kOneBlock, 0, st}, target_cls, nt, count, n_img, rows_per_image, w.img_off, w.label_count,
+                       w.pred_count, meta))
+        return e;
     if (slots > 0) {
         const long long ntiles = sort_tiles(slots);
         if (256 * ntiles > (1LL << 31) - 1) return set_error(Y5_E_UNSUPPORTED, "ap_per_class: %lld rows", slots);
-        ap_gather_kernel<<<static_cast<unsigned>((slots + kRowThreads - 1) / kRowThreads), kRowThreads, 0, st>>>(
-            tp, tp2, tp_img_stride, tp_row_stride, conf, pred_cls, img_stride, row_stride, count, slots, rows_per_image, niou, w.img_off,
-            w.keys[0], w.vals[0], w.conf, w.tpm[0], tp2 ? w.tpm[1] : nullptr, w.pred_count, meta);
-        count_launch();
+        if (int e = launch(what, ap_gather_kernel, {static_cast<unsigned>((slots + kRowThreads - 1) / kRowThreads), kRowThreads, 0, st}, tp, tp2,
+                           tp_img_stride, tp_row_stride, conf, pred_cls, img_stride, row_stride, count, slots, rows_per_image, niou, w.img_off,
+                           w.keys[0], w.vals[0], w.conf, w.tpm[0], tp2 ? w.tpm[1] : nullptr, w.pred_count, meta))
+            return e;
         for (int pass = 0; pass < kSortPasses; ++pass) {
             const int in = pass & 1, shift = 8 * pass;
-            radix_hist_kernel<<<static_cast<unsigned>(ntiles), kSortThreads, 0, st>>>(w.keys[in], meta, shift, static_cast<int>(ntiles), w.hist);
-            radix_scan_kernel<<<1, kOneBlock, 0, st>>>(w.hist, static_cast<int>(256 * ntiles));
-            radix_scatter_kernel<<<static_cast<unsigned>(ntiles), kSortThreads, 0, st>>>(w.keys[in], w.vals[in], w.keys[in ^ 1], w.vals[in ^ 1],
-                                                                                         meta, shift, static_cast<int>(ntiles), w.hist);
-            count_launch(3);
+            if (int e = launch(what, radix_hist_kernel, {static_cast<unsigned>(ntiles), kSortThreads, 0, st}, w.keys[in], meta, shift,
+                               static_cast<int>(ntiles), w.hist))
+                return e;
+            if (int e = launch(what, radix_scan_kernel, {1, kOneBlock, 0, st}, w.hist, static_cast<int>(256 * ntiles))) return e;
+            if (int e = launch(what, radix_scatter_kernel, {static_cast<unsigned>(ntiles), kSortThreads, 0, st}, w.keys[in], w.vals[in],
+                               w.keys[in ^ 1], w.vals[in ^ 1], meta, shift, static_cast<int>(ntiles), w.hist))
+                return e;
         }
         static_assert(kSortPasses % 2 == 0, "the sorted rows end in buffer 0");
-        ap_permute_kernel<<<static_cast<unsigned>((slots + kRowThreads - 1) / kRowThreads), kRowThreads, 0, st>>>(
-            w.vals[0], meta, w.conf, w.tpm[0], tp2 ? w.tpm[1] : nullptr, w.conf_s, w.tpm_s[0], tp2 ? w.tpm_s[1] : nullptr);
-        count_launch();
+        if (int e = launch(what, ap_permute_kernel, {static_cast<unsigned>((slots + kRowThreads - 1) / kRowThreads), kRowThreads, 0, st}, w.vals[0],
+                           meta, w.conf, w.tpm[0], tp2 ? w.tpm[1] : nullptr, w.conf_s, w.tpm_s[0], tp2 ? w.tpm_s[1] : nullptr))
+            return e;
     }
     if (nc_cap > 0) {
         for (int s = 0; s < sets; ++s) {
             double* o = out + static_cast<long long>(s) * nc_cap * (5 + niou);
-            ap_class_kernel<<<dim3(nc_cap, niou), kClassThreads, 0, st>>>(meta, w.label_count, w.pred_count, w.conf_s, w.tpm_s[s], w.tpc, slots,
-                                                                          grid, eps, niou, w.p_curve, w.r_curve, o + 5LL * nc_cap);
-            ap_tail_kernel<<<1, kOneBlock, 0, st>>>(meta, s, w.label_count, w.p_curve, w.r_curve, eps, nc_cap, o);
-            count_launch(2);
+            if (int e = launch(what, ap_class_kernel, {dim3(nc_cap, niou), kClassThreads, 0, st}, meta, w.label_count, w.pred_count, w.conf_s,
+                               w.tpm_s[s], w.tpc, slots, grid, eps, niou, w.p_curve, w.r_curve, o + 5LL * nc_cap))
+                return e;
+            if (int e = launch(what, ap_tail_kernel, {1, kOneBlock, 0, st}, meta, s, w.label_count, w.p_curve, w.r_curve, eps, nc_cap, o)) return e;
         }
     }
-    return last_status("ap_per_class");
+    return 0;
 }

@@ -445,13 +445,6 @@ constexpr int dq_smem() { return 4 * kTile * Tile<DH>::kStride * 2; }
 template <int DH>
 constexpr int dkv_smem() { return (2 * kTile + 2 * dkv_bq<DH>()) * Tile<DH>::kStride * 2 + 2 * dkv_bq<DH>() * 4; }
 
-int check_launch(const char* what) {
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 template <int DH, bool BF16>
 int launch_fwd(const void* q, const void* k, const void* v, int qkv_pitch, void* o, int o_pitch, float* lse, int B, int L, int heads, float scale,
                cudaStream_t st) {
@@ -460,9 +453,8 @@ int launch_fwd(const void* q, const void* k, const void* v, int qkv_pitch, void*
     cudaError_t e = ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem);
     if (e != cudaSuccess) return set_error(int(e), "attention_fwd: shared memory attribute: %s", cudaGetErrorString(e));
     dim3 grid((L + kTile - 1) / kTile, heads, B);
-    kern<<<grid, kAttnThreads, smem, st>>>(static_cast<const uint16_t*>(q), static_cast<const uint16_t*>(k), static_cast<const uint16_t*>(v),
-                                           qkv_pitch, static_cast<uint16_t*>(o), o_pitch, lse, L, scale * kLog2e);
-    return check_launch("attention_fwd");
+    return launch("attention_fwd", kern, {grid, kAttnThreads, smem, st}, static_cast<const uint16_t*>(q), static_cast<const uint16_t*>(k),
+                  static_cast<const uint16_t*>(v), qkv_pitch, static_cast<uint16_t*>(o), o_pitch, lse, L, scale * kLog2e);
 }
 
 template <int DH, bool BF16>
@@ -477,15 +469,12 @@ int launch_bwd(const void* q, const void* k, const void* v, int qkv_pitch, const
     dim3 grid((L + kTile - 1) / kTile, heads, B);
     const uint16_t *q16 = static_cast<const uint16_t*>(q), *k16 = static_cast<const uint16_t*>(k), *v16 = static_cast<const uint16_t*>(v);
     const uint16_t* d16 = static_cast<const uint16_t*>(dout);
-    kq<<<grid, kAttnThreads, smem_q, st>>>(q16, k16, v16, qkv_pitch, d16, do_pitch, lse, delta, static_cast<uint16_t*>(dq), dqkv_pitch, L, scale);
-    int r = check_launch("attention_bwd dq");
-    if (r) return r;
-    kkv<<<grid, kAttnThreads, smem_kv, st>>>(q16, k16, v16, qkv_pitch, d16, do_pitch, lse, delta, static_cast<uint16_t*>(dk),
-                                             static_cast<uint16_t*>(dv), dqkv_pitch, L, scale);
-    return check_launch("attention_bwd dk dv");
+    if (int r = launch("attention_bwd dq", kq, {grid, kAttnThreads, smem_q, st}, q16, k16, v16, qkv_pitch, d16, do_pitch, lse, delta,
+                       static_cast<uint16_t*>(dq), dqkv_pitch, L, scale))
+        return r;
+    return launch("attention_bwd dk dv", kkv, {grid, kAttnThreads, smem_kv, st}, q16, k16, v16, qkv_pitch, d16, do_pitch, lse, delta,
+                  static_cast<uint16_t*>(dk), static_cast<uint16_t*>(dv), dqkv_pitch, L, scale);
 }
-
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // common argument checks of both passes; returns 0 or the error code (message recorded)
 int check_common(const char* what, const void* q, const void* k, const void* v, int qkv_pitch, int batch, int seq, int heads, int head_dim,
@@ -549,13 +538,9 @@ extern "C" Y5_API int y5_attention_bwd(const void* q, const void* k, const void*
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long warps = static_cast<long long>(batch) * seq * heads;
     const long long blocks = (warps * 32 + 255) / 256;
-    if (dtype == Y5_BF16)
-        attn_delta_kernel<true><<<static_cast<unsigned>(blocks), 256, 0, st>>>(static_cast<const uint16_t*>(o), o_pitch, static_cast<const uint16_t*>(dout),
-                                                                               dout_pitch, delta, batch, seq, heads, head_dim);
-    else
-        attn_delta_kernel<false><<<static_cast<unsigned>(blocks), 256, 0, st>>>(static_cast<const uint16_t*>(o), o_pitch, static_cast<const uint16_t*>(dout),
-                                                                                dout_pitch, delta, batch, seq, heads, head_dim);
-    r = check_launch("attention_bwd delta");
+    r = launch("attention_bwd delta", dtype == Y5_BF16 ? attn_delta_kernel<true> : attn_delta_kernel<false>,
+               {static_cast<unsigned>(blocks), 256, 0, st}, static_cast<const uint16_t*>(o), o_pitch, static_cast<const uint16_t*>(dout), dout_pitch,
+               delta, batch, seq, heads, head_dim);
     if (r) return r;
 #define Y5_BWD(DH, BF) launch_bwd<DH, BF>(q, k, v, qkv_pitch, dout, dout_pitch, lse, delta, dq, dk, dv, dqkv_pitch, batch, seq, heads, scale, st)
     Y5_ATTN_DISPATCH(Y5_BWD)

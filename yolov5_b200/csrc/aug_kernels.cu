@@ -269,12 +269,6 @@ __global__ void __launch_bounds__(kLabelThreads) aug_labels_kernel(const y5_aug_
     if (tid == 0) *count = s_base;
 }
 
-static int aug_status(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 }  // namespace y5
 
 using namespace y5;
@@ -298,23 +292,17 @@ extern "C" Y5_API int y5_aug_gather(const y5_aug_image* table, int32_t n_images,
     const int bf = out_dtype == Y5_BF16;
     if (s2d) {
         const int row_px = out_row_px ? out_row_px : out_w / 2;
-        aug_gather_kernel<3><<<grid, block, 0, st>>>(table, out_h, out_w, hsv_simd_cols, swap_rb, out, bf, row_px, out_x_off);
-    } else if (out_dtype == Y5_U8) {
-        aug_gather_kernel<0><<<grid, block, 0, st>>>(table, out_h, out_w, hsv_simd_cols, swap_rb, out, bf, 0, 0);
-    } else if (out_dtype == Y5_F32) {
-        aug_gather_kernel<2><<<grid, block, 0, st>>>(table, out_h, out_w, hsv_simd_cols, swap_rb, out, bf, 0, 0);
-    } else {
-        aug_gather_kernel<1><<<grid, block, 0, st>>>(table, out_h, out_w, hsv_simd_cols, swap_rb, out, bf, 0, 0);
+        return launch("aug_gather", aug_gather_kernel<3>, {grid, block, 0, st}, table, out_h, out_w, hsv_simd_cols, swap_rb, out, bf, row_px,
+                      out_x_off);
     }
-    count_launch();
-    return aug_status("aug_gather");
+    auto* kernel = out_dtype == Y5_U8 ? aug_gather_kernel<0> : out_dtype == Y5_F32 ? aug_gather_kernel<2> : aug_gather_kernel<1>;
+    return launch("aug_gather", kernel, {grid, block, 0, st}, table, out_h, out_w, hsv_simd_cols, swap_rb, out, bf, 0, 0);
 }
 
 extern "C" Y5_API int y5_aug_labels(const y5_aug_image* table, int32_t n_images, const y5_aug_label* labels, int32_t n_labels, int32_t out_h,
                                     int32_t out_w, float* targets, int32_t* count, void* stream) {
     if (!table || !count || n_images <= 0 || n_labels < 0 || out_h <= 0 || out_w <= 0 || (n_labels > 0 && (!labels || !targets)))
         return set_error(Y5_E_INVALID, "aug_labels: bad argument");
-    aug_labels_kernel<<<1, kLabelThreads, 0, static_cast<cudaStream_t>(stream)>>>(table, labels, n_labels, n_images, out_h, out_w, targets, count);
-    count_launch();
-    return aug_status("aug_labels");
+    return launch("aug_labels", aug_labels_kernel, {1, kLabelThreads, 0, static_cast<cudaStream_t>(stream)}, table, labels, n_labels, n_images,
+                  out_h, out_w, targets, count);
 }

@@ -246,18 +246,6 @@ __global__ void nhwc_to_nchw_kernel(const uint16_t* __restrict__ x, int x_pitch,
 
 using namespace y5;
 
-static int grid_for(long long total, int threads) {
-    long long blocks = (total + threads - 1) / threads;
-    const long long cap = static_cast<long long>(sm_count()) * 16;  // grid-stride beyond 16 CTAs per SM
-    if (blocks > cap) blocks = cap;
-    return static_cast<int>(blocks < 1 ? 1 : blocks);
-}
-static int check_launch(const char* what) {
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
 static bool half_dtype(int d) { return d == Y5_F16 || d == Y5_BF16; }
 // a view the kernels read or write in 16-byte vectors: aligned base, pitch covering its channels
 static bool vec_view(const void* p, int pitch, int c) { return !(reinterpret_cast<uintptr_t>(p) & 15) && pitch >= c; }
@@ -270,18 +258,17 @@ extern "C" Y5_API int y5_stem_s2d(const void* img, int32_t img_dtype, void* out,
     if (!half_dtype(out_dtype)) return set_error(Y5_E_UNSUPPORTED, "stem_s2d: output dtype must be fp16/bf16");
     if (reinterpret_cast<uintptr_t>(out) & 15) return set_error(Y5_E_INVALID, "stem_s2d: output must be 16-byte aligned");
     const long long total = static_cast<long long>(batch) * (h / 2) * (w / 2);
-    const int threads = 256, grid = grid_for(total, threads);
+    const int threads = 256, grid = grid_stride_ctas(total, threads, 16);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int bf = out_dtype == Y5_BF16;
     uint4* o = static_cast<uint4*>(out);
     switch (img_dtype) {
-        case Y5_U8: stem_s2d_kernel<uint8_t><<<grid, threads, 0, st>>>(static_cast<const uint8_t*>(img), o, batch, h, w, bf, row_px, out_x_off); break;
-        case Y5_F16: stem_s2d_kernel<__half><<<grid, threads, 0, st>>>(static_cast<const __half*>(img), o, batch, h, w, bf, row_px, out_x_off); break;
-        case Y5_BF16: stem_s2d_kernel<__nv_bfloat16><<<grid, threads, 0, st>>>(static_cast<const __nv_bfloat16*>(img), o, batch, h, w, bf, row_px, out_x_off); break;
-        case Y5_F32: stem_s2d_kernel<float><<<grid, threads, 0, st>>>(static_cast<const float*>(img), o, batch, h, w, bf, row_px, out_x_off); break;
+        case Y5_U8: return launch("stem_s2d", stem_s2d_kernel<uint8_t>, {grid, threads, 0, st}, static_cast<const uint8_t*>(img), o, batch, h, w, bf, row_px, out_x_off);
+        case Y5_F16: return launch("stem_s2d", stem_s2d_kernel<__half>, {grid, threads, 0, st}, static_cast<const __half*>(img), o, batch, h, w, bf, row_px, out_x_off);
+        case Y5_BF16: return launch("stem_s2d", stem_s2d_kernel<__nv_bfloat16>, {grid, threads, 0, st}, static_cast<const __nv_bfloat16*>(img), o, batch, h, w, bf, row_px, out_x_off);
+        case Y5_F32: return launch("stem_s2d", stem_s2d_kernel<float>, {grid, threads, 0, st}, static_cast<const float*>(img), o, batch, h, w, bf, row_px, out_x_off);
         default: return set_error(Y5_E_UNSUPPORTED, "stem_s2d: image dtype %d", img_dtype);
     }
-    return check_launch("stem_s2d");
 }
 
 extern "C" Y5_API int y5_image_nhwc(const void* img, int32_t img_dtype, void* out, int32_t out_dtype, int32_t batch, int32_t h, int32_t w,
@@ -291,18 +278,17 @@ extern "C" Y5_API int y5_image_nhwc(const void* img, int32_t img_dtype, void* ou
     if (reinterpret_cast<uintptr_t>(out) & 15) return set_error(Y5_E_INVALID, "image_nhwc: output must be 16-byte aligned");
     const int cv = out_c / 8;
     const long long total = static_cast<long long>(batch) * h * w * cv;
-    const int threads = 256, grid = grid_for(total, threads);
+    const int threads = 256, grid = grid_stride_ctas(total, threads, 16);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int bf = out_dtype == Y5_BF16;
     uint4* o = static_cast<uint4*>(out);
     switch (img_dtype) {
-        case Y5_U8: image_nhwc_kernel<uint8_t><<<grid, threads, 0, st>>>(static_cast<const uint8_t*>(img), o, batch, h, w, cv, bf); break;
-        case Y5_F16: image_nhwc_kernel<__half><<<grid, threads, 0, st>>>(static_cast<const __half*>(img), o, batch, h, w, cv, bf); break;
-        case Y5_BF16: image_nhwc_kernel<__nv_bfloat16><<<grid, threads, 0, st>>>(static_cast<const __nv_bfloat16*>(img), o, batch, h, w, cv, bf); break;
-        case Y5_F32: image_nhwc_kernel<float><<<grid, threads, 0, st>>>(static_cast<const float*>(img), o, batch, h, w, cv, bf); break;
+        case Y5_U8: return launch("image_nhwc", image_nhwc_kernel<uint8_t>, {grid, threads, 0, st}, static_cast<const uint8_t*>(img), o, batch, h, w, cv, bf);
+        case Y5_F16: return launch("image_nhwc", image_nhwc_kernel<__half>, {grid, threads, 0, st}, static_cast<const __half*>(img), o, batch, h, w, cv, bf);
+        case Y5_BF16: return launch("image_nhwc", image_nhwc_kernel<__nv_bfloat16>, {grid, threads, 0, st}, static_cast<const __nv_bfloat16*>(img), o, batch, h, w, cv, bf);
+        case Y5_F32: return launch("image_nhwc", image_nhwc_kernel<float>, {grid, threads, 0, st}, static_cast<const float*>(img), o, batch, h, w, cv, bf);
         default: return set_error(Y5_E_UNSUPPORTED, "image_nhwc: image dtype %d", img_dtype);
     }
-    return check_launch("image_nhwc");
 }
 
 extern "C" Y5_API int y5_sppf_pool(const void* x, int32_t x_pitch, void* y1, void* y2, void* y3, int32_t y_pitch, int32_t batch, int32_t h,
@@ -315,17 +301,15 @@ extern "C" Y5_API int y5_sppf_pool(const void* x, int32_t x_pitch, void* y1, voi
     if (smem <= 96 * 1024 && static_cast<long long>(batch) * (c / 8) < 0x7fffffff) {
         if (ensure_dyn_smem(reinterpret_cast<const void*>(sppf_pool_smem_kernel), 96 * 1024) != cudaSuccess)
             return set_error(Y5_E_DRIVER, "sppf_pool: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
-        sppf_pool_smem_kernel<<<batch * (c / 8), 256, smem, static_cast<cudaStream_t>(stream)>>>(
-            static_cast<const uint16_t*>(x), x_pitch, static_cast<uint16_t*>(y1), static_cast<uint16_t*>(y2), static_cast<uint16_t*>(y3),
-            y_pitch, h, w, c, ksize, dtype == Y5_BF16);
-        return check_launch("sppf_pool");
+        return launch("sppf_pool", sppf_pool_smem_kernel, {batch * (c / 8), 256, smem, static_cast<cudaStream_t>(stream)},
+                      static_cast<const uint16_t*>(x), x_pitch, static_cast<uint16_t*>(y1), static_cast<uint16_t*>(y2),
+                      static_cast<uint16_t*>(y3), y_pitch, h, w, c, ksize, dtype == Y5_BF16);
     }
     const long long total = static_cast<long long>(batch) * h * w * (c / 8);
-    const int threads = 128, grid = grid_for(total, threads);
-    sppf_pool_kernel<<<grid, threads, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const uint16_t*>(x), x_pitch, static_cast<uint16_t*>(y1), static_cast<uint16_t*>(y2), static_cast<uint16_t*>(y3),
-        y_pitch, batch, h, w, c, ksize, dtype == Y5_BF16);
-    return check_launch("sppf_pool");
+    const int threads = 128, grid = grid_stride_ctas(total, threads, 16);
+    return launch("sppf_pool", sppf_pool_kernel, {grid, threads, 0, static_cast<cudaStream_t>(stream)}, static_cast<const uint16_t*>(x),
+                  x_pitch, static_cast<uint16_t*>(y1), static_cast<uint16_t*>(y2), static_cast<uint16_t*>(y3), y_pitch, batch, h, w, c,
+                  ksize, dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int y5_upsample2x(const void* x, int32_t x_pitch, void* y, int32_t y_pitch, int32_t batch, int32_t h, int32_t w, int32_t c,
@@ -334,10 +318,9 @@ extern "C" Y5_API int y5_upsample2x(const void* x, int32_t x_pitch, void* y, int
     if (c % 8 || x_pitch % 8 || y_pitch % 8 || !half_dtype(dtype)) return set_error(Y5_E_UNSUPPORTED, "upsample2x: c/pitch %% 8, fp16/bf16 only");
     if (!vec_view(x, x_pitch, c) || !vec_view(y, y_pitch, c)) return set_error(Y5_E_INVALID, "upsample2x: views must be 16-byte aligned with pitch >= c");
     const long long total = static_cast<long long>(batch) * 4 * h * w * (c / 8);
-    const int threads = 256, grid = grid_for(total, threads);
-    launch_pdl(upsample2x_kernel, grid, dim3(threads), 0, static_cast<cudaStream_t>(stream), static_cast<const uint16_t*>(x), x_pitch,
-                                                                                static_cast<uint16_t*>(y), y_pitch, batch, h, w, c);
-    return check_launch("upsample2x");
+    const int threads = 256, grid = grid_stride_ctas(total, threads, 16);
+    return launch("upsample2x", upsample2x_kernel, {grid, threads, 0, static_cast<cudaStream_t>(stream), /*pdl=*/true},
+                  static_cast<const uint16_t*>(x), x_pitch, static_cast<uint16_t*>(y), y_pitch, batch, h, w, c);
 }
 
 extern "C" Y5_API int y5_copy_view(const void* x, int32_t x_pitch, void* y, int32_t y_pitch, int64_t pixels, int32_t c, int32_t dtype,
@@ -346,10 +329,9 @@ extern "C" Y5_API int y5_copy_view(const void* x, int32_t x_pitch, void* y, int3
     if (c % 8 || x_pitch % 8 || y_pitch % 8 || !half_dtype(dtype)) return set_error(Y5_E_UNSUPPORTED, "copy_view: c/pitch %% 8, fp16/bf16 only");
     if (!vec_view(x, x_pitch, c) || !vec_view(y, y_pitch, c)) return set_error(Y5_E_INVALID, "copy_view: views must be 16-byte aligned with pitch >= c");
     const long long total = pixels * (c / 8);
-    const int threads = 256, grid = grid_for(total, threads);
-    launch_pdl(copy_view_kernel, grid, dim3(threads), 0, static_cast<cudaStream_t>(stream), static_cast<const uint16_t*>(x), x_pitch,
-                                                                               static_cast<uint16_t*>(y), y_pitch, pixels, c);
-    return check_launch("copy_view");
+    const int threads = 256, grid = grid_stride_ctas(total, threads, 16);
+    return launch("copy_view", copy_view_kernel, {grid, threads, 0, static_cast<cudaStream_t>(stream), /*pdl=*/true},
+                  static_cast<const uint16_t*>(x), x_pitch, static_cast<uint16_t*>(y), y_pitch, pixels, c);
 }
 
 extern "C" Y5_API int y5_nhwc_to_nchw(const void* x, int32_t x_pitch, void* y, int32_t batch, int32_t h, int32_t w, int32_t c, int32_t dtype,
@@ -358,7 +340,6 @@ extern "C" Y5_API int y5_nhwc_to_nchw(const void* x, int32_t x_pitch, void* y, i
     if (batch > 65535) return set_error(Y5_E_UNSUPPORTED, "nhwc_to_nchw: batch > 65535");
     const int HW = h * w;
     dim3 grid((HW + 31) / 32, (c + 31) / 32, batch), block(32, 8);
-    nhwc_to_nchw_kernel<<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const uint16_t*>(x), x_pitch,
-                                                                               static_cast<uint16_t*>(y), HW, c);
-    return check_launch("nhwc_to_nchw");
+    return launch("nhwc_to_nchw", nhwc_to_nchw_kernel, {grid, block, 0, static_cast<cudaStream_t>(stream)}, static_cast<const uint16_t*>(x),
+                  x_pitch, static_cast<uint16_t*>(y), HW, c);
 }

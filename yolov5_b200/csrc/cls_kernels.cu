@@ -163,29 +163,15 @@ __global__ void __launch_bounds__(kCeThreads) ce_mean_kernel(const float* __rest
 
 using namespace y5;
 
-static int grid_for(long long total, int threads) {
-    long long blocks = (total + threads - 1) / threads;
-    const long long cap = static_cast<long long>(sm_count()) * 16;
-    if (blocks > cap) blocks = cap;
-    return static_cast<int>(blocks < 1 ? 1 : blocks);
-}
-static int check_launch(const char* what) {
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 extern "C" Y5_API int y5_global_avg_pool(const void* x, int32_t x_pitch, void* y, int32_t y_pitch, int32_t batch, int32_t h, int32_t w, int32_t c,
                                          int32_t dtype, void* stream) {
     if (!x || !y || batch <= 0 || h <= 0 || w <= 0 || c <= 0 || x_pitch < c || y_pitch < c) return set_error(Y5_E_INVALID, "global_avg_pool: bad arguments");
     if (c % 8 || x_pitch % 8 || y_pitch % 8 || (dtype != Y5_F16 && dtype != Y5_BF16))
         return set_error(Y5_E_UNSUPPORTED, "global_avg_pool: c/pitch %% 8, fp16/bf16 only");
     const long long total = static_cast<long long>(batch) * (c / 8);
-    const int threads = 128, grid = grid_for(total, threads);
-    gap_fwd_kernel<<<grid, threads, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const uint16_t*>(x), x_pitch, static_cast<uint16_t*>(y),
-                                                                            y_pitch, batch, h * w, c, dtype == Y5_BF16);
-    return check_launch("global_avg_pool");
+    const int threads = 128, grid = grid_stride_ctas(total, threads, 16);
+    return launch("global_avg_pool", gap_fwd_kernel, {grid, threads, 0, static_cast<cudaStream_t>(stream)}, static_cast<const uint16_t*>(x),
+                  x_pitch, static_cast<uint16_t*>(y), y_pitch, batch, h * w, c, dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int y5_global_avg_pool_bwd(const void* dy, int32_t dy_pitch, void* dx, int32_t dx_pitch, int32_t batch, int32_t h, int32_t w,
@@ -195,10 +181,9 @@ extern "C" Y5_API int y5_global_avg_pool_bwd(const void* dy, int32_t dy_pitch, v
     if (c % 8 || dy_pitch % 8 || dx_pitch % 8 || (dtype != Y5_F16 && dtype != Y5_BF16))
         return set_error(Y5_E_UNSUPPORTED, "global_avg_pool_bwd: c/pitch %% 8, fp16/bf16 only");
     const long long total = static_cast<long long>(batch) * h * w * (c / 8);
-    const int threads = 256, grid = grid_for(total, threads);
-    gap_bwd_kernel<<<grid, threads, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const uint16_t*>(dy), dy_pitch, static_cast<uint16_t*>(dx),
-                                                                            dx_pitch, batch, h * w, c, dtype == Y5_BF16);
-    return check_launch("global_avg_pool_bwd");
+    const int threads = 256, grid = grid_stride_ctas(total, threads, 16);
+    return launch("global_avg_pool_bwd", gap_bwd_kernel, {grid, threads, 0, static_cast<cudaStream_t>(stream)},
+                  static_cast<const uint16_t*>(dy), dy_pitch, static_cast<uint16_t*>(dx), dx_pitch, batch, h * w, c, dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int y5_cross_entropy(const void* logits, int32_t dtype, int32_t batch, int32_t nc, int64_t row_stride, const int64_t* labels,
@@ -209,23 +194,22 @@ extern "C" Y5_API int y5_cross_entropy(const void* logits, int32_t dtype, int32_
     if (!(label_smoothing >= 0.0f && label_smoothing <= 1.0f)) return set_error(Y5_E_INVALID, "cross_entropy: label_smoothing outside [0, 1]");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long* lab = reinterpret_cast<const long long*>(labels);
+    int e;
     switch (dtype) {
         case Y5_F16:
-            ce_row_kernel<__half><<<batch, kCeThreads, 0, st>>>(static_cast<const __half*>(logits), row_stride, nc, lab, label_smoothing, grad_scale,
-                                                               static_cast<__half*>(dlogits), dlogits_stride, row_loss, batch);
+            e = launch("cross_entropy", ce_row_kernel<__half>, {batch, kCeThreads, 0, st}, static_cast<const __half*>(logits), row_stride, nc,
+                       lab, label_smoothing, grad_scale, static_cast<__half*>(dlogits), dlogits_stride, row_loss, batch);
             break;
         case Y5_BF16:
-            ce_row_kernel<__nv_bfloat16><<<batch, kCeThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(logits), row_stride, nc, lab, label_smoothing,
-                                                                      grad_scale, static_cast<__nv_bfloat16*>(dlogits), dlogits_stride, row_loss, batch);
+            e = launch("cross_entropy", ce_row_kernel<__nv_bfloat16>, {batch, kCeThreads, 0, st}, static_cast<const __nv_bfloat16*>(logits),
+                       row_stride, nc, lab, label_smoothing, grad_scale, static_cast<__nv_bfloat16*>(dlogits), dlogits_stride, row_loss, batch);
             break;
         case Y5_F32:
-            ce_row_kernel<float><<<batch, kCeThreads, 0, st>>>(static_cast<const float*>(logits), row_stride, nc, lab, label_smoothing, grad_scale,
-                                                              static_cast<float*>(dlogits), dlogits_stride, row_loss, batch);
+            e = launch("cross_entropy", ce_row_kernel<float>, {batch, kCeThreads, 0, st}, static_cast<const float*>(logits), row_stride, nc,
+                       lab, label_smoothing, grad_scale, static_cast<float*>(dlogits), dlogits_stride, row_loss, batch);
             break;
         default: return set_error(Y5_E_UNSUPPORTED, "cross_entropy: logits dtype %d (fp16 / bf16 / fp32)", dtype);
     }
-    int r = check_launch("cross_entropy");
-    if (r) return r;
-    ce_mean_kernel<<<1, kCeThreads, 0, st>>>(row_loss, batch, loss);
-    return check_launch("cross_entropy mean");
+    if (e) return e;
+    return launch("cross_entropy mean", ce_mean_kernel, {1, kCeThreads, 0, st}, row_loss, batch, loss);
 }

@@ -833,29 +833,12 @@ int pick_block_n(int out_c, int64_t m_rows) {
 }
 
 template <int BN, int EPI, int MT, bool OPT>
-cudaError_t launch_conv(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const CUtensorMap& r, const ConvParams& p,
-                        int grid, int cluster, uint32_t smem, cudaStream_t st) {
+int launch_conv(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const CUtensorMap& r, const ConvParams& p, int grid,
+                int cluster, uint32_t smem, cudaStream_t st) {
     auto* kernel = p.is_bf16 ? conv_gemm_kernel<BN, EPI, MT, OPT, true> : conv_gemm_kernel<BN, EPI, MT, OPT, false>;
     const cudaError_t attr_err = ensure_dyn_smem(reinterpret_cast<const void*>(kernel), 227 * 1024);
-    if (attr_err != cudaSuccess) return attr_err;
-    count_launch();
-    if (cluster == 1) return launch_pdl(kernel, dim3(grid), dim3(kThreads), smem, st, a, b, o, r, p);
-    static const bool pdl = [] { const char* e = getenv("Y5_PDL"); return !(e && e[0] == '0'); }();
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl ? 2 : 1;
-    return cudaLaunchKernelEx(&cfg, kernel, a, b, o, r, p);
+    if (attr_err != cudaSuccess) return set_error(int(attr_err), "conv_gemm launch failed: %s", cudaGetErrorString(attr_err));
+    return launch("conv_gemm", kernel, {grid, kThreads, smem, st, /*pdl=*/true, static_cast<unsigned>(cluster)}, a, b, o, r, p);
 }
 
 struct PlanCommon {
@@ -909,38 +892,33 @@ bool plan_staged(const PlanCommon& pc) { return pc.p.stg_bytes > 0 && !pc.p.tma_
 bool plan_opt(const PlanCommon& pc) { return pc.cluster > 1 || pc.p.patch_pw > 0 || plan_staged(pc); }
 
 int run_plan(const PlanCommon& pc, cudaStream_t st) {
-    cudaError_t e = cudaErrorInvalidValue;
     const int key = (plan_opt(pc) ? 100000 : 0) + pc.epi * 10000 + pc.block_n * 10 + pc.mt;
     switch (key) {
-        case 324: e = launch_conv<32, 0, 4, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 642: e = launch_conv<64, 0, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 1281: e = launch_conv<128, 0, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 1282: e = launch_conv<128, 0, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 2561: e = launch_conv<256, 0, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 11281: e = launch_conv<kHeadN, 1, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 100324: e = launch_conv<32, 0, 4, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 100642: e = launch_conv<64, 0, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 101281: e = launch_conv<128, 0, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 101282: e = launch_conv<128, 0, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 102561: e = launch_conv<256, 0, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 324: return launch_conv<32, 0, 4, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 642: return launch_conv<64, 0, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 1281: return launch_conv<128, 0, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 1282: return launch_conv<128, 0, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 2561: return launch_conv<256, 0, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 11281: return launch_conv<kHeadN, 1, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 100324: return launch_conv<32, 0, 4, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 100642: return launch_conv<64, 0, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 101281: return launch_conv<128, 0, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 101282: return launch_conv<128, 0, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 102561: return launch_conv<256, 0, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
         // conv with LeakyReLU (EPI 2)
-        case 20324: e = launch_conv<32, 2, 4, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 20642: e = launch_conv<64, 2, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 21281: e = launch_conv<128, 2, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 21282: e = launch_conv<128, 2, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 22561: e = launch_conv<256, 2, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 120324: e = launch_conv<32, 2, 4, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 120642: e = launch_conv<64, 2, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 121281: e = launch_conv<128, 2, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 121282: e = launch_conv<128, 2, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
-        case 122561: e = launch_conv<256, 2, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st); break;
+        case 20324: return launch_conv<32, 2, 4, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 20642: return launch_conv<64, 2, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 21281: return launch_conv<128, 2, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 21282: return launch_conv<128, 2, 2, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 22561: return launch_conv<256, 2, 1, false>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 120324: return launch_conv<32, 2, 4, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 120642: return launch_conv<64, 2, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 121281: return launch_conv<128, 2, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 121282: return launch_conv<128, 2, 2, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
+        case 122561: return launch_conv<256, 2, 1, true>(pc.tmA, pc.tmB, pc.tmO, pc.tmR, pc.p, pc.grid, pc.cluster, pc.smem_bytes, st);
         default: return set_error(Y5_E_UNSUPPORTED, "conv: no kernel for block_n %d mt %d epi %d", pc.block_n, pc.mt, pc.epi);
     }
-    if (e != cudaSuccess) return set_error(int(e), "conv_gemm launch failed: %s", cudaGetErrorString(e));
-    return 0;
 }
-
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 struct Geo {
     int kh, kw, pad_h, pad_w, Ho, Wo;
@@ -1214,14 +1192,11 @@ extern "C" Y5_API int y5_conv_direct_fwd(const y5_conv_desc* d, void* stream) {
     const long long total = static_cast<long long>(d->batch) * g.Ho * g.Wo * d->out_c;
     const int threads = 256;
     const long long blocks = (total + threads - 1) / threads;
-    conv_direct_kernel<<<static_cast<unsigned>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const uint16_t*>(d->in), g.xs, g.ys, g.ns, d->batch, d->in_h, d->in_w, d->in_c, static_cast<const uint16_t*>(d->weight),
-        cin_pad, d->bias, static_cast<uint16_t*>(d->out), d->out_pitch, d->out_c, static_cast<const uint16_t*>(d->residual), d->res_pitch,
-        g.kh, g.kw, d->stride, g.pad_h, g.pad_w, g.Ho, g.Wo, d->act, d->act_slope, d->dtype == Y5_BF16);
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "conv_direct launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    return launch("conv_direct", conv_direct_kernel, {static_cast<unsigned>(blocks), threads, 0, static_cast<cudaStream_t>(stream)},
+                  static_cast<const uint16_t*>(d->in), g.xs, g.ys, g.ns, d->batch, d->in_h, d->in_w, d->in_c,
+                  static_cast<const uint16_t*>(d->weight), cin_pad, d->bias, static_cast<uint16_t*>(d->out), d->out_pitch, d->out_c,
+                  static_cast<const uint16_t*>(d->residual), d->res_pitch, g.kh, g.kw, d->stride, g.pad_h, g.pad_w, g.Ho, g.Wo, d->act,
+                  d->act_slope, d->dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int y5_detect_plan_create(const y5_detect_desc* d, y5_detect_plan** out) {

@@ -312,9 +312,5 @@ extern "C" Y5_API int y5_conv_wgrad(const y5_wgrad_desc* d, void* stream) {
     const cudaError_t attr_err = ensure_dyn_smem(reinterpret_cast<const void*>(conv_wgrad_kernel), 227 * 1024);
     if (attr_err != cudaSuccess) return set_error(int(attr_err), "wgrad: cudaFuncSetAttribute failed");
     const long long grid = items * p.splits;
-    count_launch();
-    launch_pdl(conv_wgrad_kernel, dim3(static_cast<unsigned>(grid)), dim3(kWgThreads), smem, st, tmDy, tmX, p);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "wgrad launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    return launch("wgrad", conv_wgrad_kernel, {static_cast<unsigned>(grid), kWgThreads, smem, st, /*pdl=*/true}, tmDy, tmX, p);
 }

@@ -206,13 +206,6 @@ namespace {
 
 using namespace y5;
 
-int launched(const char* what) {
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 // a view the kernels read in 32-bit words and that the 16-byte rule of the ABI allows: aligned base, pitch >= c, pitch % 8 == 0
 bool dw_view(const void* p, int pitch, int c) { return p && !(reinterpret_cast<uintptr_t>(p) & 15) && pitch >= c && pitch % 8 == 0; }
 
@@ -251,17 +244,14 @@ extern "C" Y5_API int y5_dwconv_fwd(const void* x, int32_t x_pitch, const void* 
     auto* xrw = static_cast<const uint32_t*>(x_res);
     auto* xow = static_cast<uint32_t*>(x_out);
     // 8 pairs (16 channels) x 32 columns per block where the channels allow, else 4 pairs x 64 columns (c = 8, 24, 40, ...)
-    auto launch = [&](auto kern, int pairs_per_block) {
+    auto fwd = [&](auto kern, int pairs_per_block) {
         const int tw = kFwdThreads / pairs_per_block;
         const dim3 grid(static_cast<unsigned>((cp / pairs_per_block) * ((w + tw - 1) / tw)), static_cast<unsigned>(batch * strips));
-        kern<<<grid, kFwdThreads, 0, st>>>(xw, x_pitch / 2, wp, bias, rw, res_pitch / 2, yw, y_pitch / 2, xrw, x_res_pitch / 2, xow, x_out_pitch / 2,
-                                           h, w, cp, strips, act, act_slope, dtype == Y5_BF16);
+        return launch("dwconv_fwd", kern, {grid, kFwdThreads, 0, st}, xw, x_pitch / 2, wp, bias, rw, res_pitch / 2, yw, y_pitch / 2, xrw,
+                      x_res_pitch / 2, xow, x_out_pitch / 2, h, w, cp, strips, act, act_slope, dtype == Y5_BF16);
     };
-    if (cp % 8 == 0)
-        flip ? launch(dwconv5_fwd_kernel<true, 8>, 8) : launch(dwconv5_fwd_kernel<false, 8>, 8);
-    else
-        flip ? launch(dwconv5_fwd_kernel<true, 4>, 4) : launch(dwconv5_fwd_kernel<false, 4>, 4);
-    return launched("dwconv_fwd");
+    if (cp % 8 == 0) return flip ? fwd(dwconv5_fwd_kernel<true, 8>, 8) : fwd(dwconv5_fwd_kernel<false, 8>, 8);
+    return flip ? fwd(dwconv5_fwd_kernel<true, 4>, 4) : fwd(dwconv5_fwd_kernel<false, 4>, 4);
 }
 
 extern "C" Y5_API int y5_dwconv_wgrad(const void* x, int32_t x_pitch, const void* dy, int32_t dy_pitch, float* dweight, int32_t batch, int32_t h,
@@ -281,9 +271,7 @@ extern "C" Y5_API int y5_dwconv_wgrad(const void* x, int32_t x_pitch, const void
     if (batch * strips > 65535) return set_error(Y5_E_UNSUPPORTED, "dwconv_wgrad: batch %d too large", batch);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     cudaMemsetAsync(dweight, 0, static_cast<size_t>(c) * kTaps * sizeof(float), st);
-    count_launch();
-    dwconv5_wgrad_kernel<<<dim3(static_cast<unsigned>(gx), static_cast<unsigned>(batch * strips)), kWgThreads, 0, st>>>(
-        static_cast<const uint32_t*>(x), x_pitch / 2, static_cast<const uint32_t*>(dy), dy_pitch / 2, dweight, h, w, cp, rows_per,
-        static_cast<int>(strips), dtype == Y5_BF16);
-    return launched("dwconv_wgrad");
+    return launch("dwconv_wgrad", dwconv5_wgrad_kernel, {dim3(static_cast<unsigned>(gx), static_cast<unsigned>(batch * strips)), kWgThreads, 0, st},
+                  static_cast<const uint32_t*>(x), x_pitch / 2, static_cast<const uint32_t*>(dy), dy_pitch / 2, dweight, h, w, cp, rows_per,
+                  static_cast<int>(strips), dtype == Y5_BF16);
 }

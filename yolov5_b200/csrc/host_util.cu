@@ -1,6 +1,7 @@
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
 #include <mutex>
 #include <set>
 #include <utility>
@@ -20,7 +21,38 @@ int set_error(int code, const char* fmt, ...) {
     va_end(ap);
     return code;
 }
-void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+int launch_args(const char* what, const void* kernel, const LaunchDims& d, void** args) {
+    static const bool pdl_on = [] { const char* e = getenv("Y5_PDL"); return !(e && e[0] == '0'); }();
+    cudaLaunchAttribute attr[2];
+    unsigned n = 0;
+    if (d.pdl && pdl_on) {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n++].val.programmaticStreamSerializationAllowed = 1;
+    }
+    if (d.cluster > 1) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n++].val.clusterDim = {d.cluster, 1, 1};
+    }
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = d.grid;
+    cfg.blockDim = d.block;
+    cfg.dynamicSmemBytes = d.smem;
+    cfg.stream = d.stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = n;
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    cudaError_t e = cudaLaunchKernelExC(&cfg, kernel, args);
+    const cudaError_t last = cudaGetLastError();
+    if (e == cudaSuccess) e = last;
+    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
+    return 0;
+}
+
+int grid_stride_ctas(long long total, int threads, int ctas_per_sm) {
+    const long long ctas = (total + threads - 1) / threads, cap = static_cast<long long>(sm_count()) * ctas_per_sm;
+    return static_cast<int>(ctas < cap ? ctas : cap);
+}
 
 int sm_count() {
     static int per_dev[64] = {};

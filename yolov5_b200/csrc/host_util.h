@@ -4,33 +4,40 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <cstdlib>
+#include <utility>
 
 namespace y5 {
 
-// Launch with the programmatic-dependent-launch attribute: the kernel may be scheduled while its predecessor in the
-// stream drains (every such kernel starts with griddepcontrol.wait, which blocks until the predecessor has completed and
-// flushed, then griddepcontrol.launch_dependents).  Y5_PDL=0 turns the attribute off.
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-    static const bool pdl = [] { const char* e = getenv("Y5_PDL"); return !(e && e[0] == '0'); }();
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
 // records a thread-local message retrievable through y5_last_error(); returns `code`
 int set_error(int code, const char* fmt, ...);
-void count_launch(int n = 1);
 int sm_count();
+// CTAs for a grid-stride loop over `total` items: one item per thread, at most `ctas_per_sm` CTAs per SM
+int grid_stride_ctas(long long total, int threads, int ctas_per_sm);
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+struct LaunchDims {
+    dim3 grid, block;
+    size_t smem;
+    cudaStream_t stream;
+    // programmatic dependent launch: the kernel may be scheduled while its predecessor in the stream drains, so it must
+    // begin with griddep_wait().  Y5_PDL=0 turns the attribute off.
+    bool pdl = false;
+    unsigned cluster = 1;  // CTAs per cluster along x
+};
+
+int launch_args(const char* what, const void* kernel, const LaunchDims& d, void** args);
+
+// Every kernel of the library is launched here: counts one launch for y5_launch_count() and returns 0, or records
+// "<what> launch failed: ..." and returns the CUDA error code.  The thread's last runtime error is read and cleared too, so
+// an earlier unchecked runtime call of the entry point surfaces here and no error is left behind for the caller.
+template <typename... KArgs, typename... Args>
+int launch(const char* what, void (*kernel)(KArgs...), const LaunchDims& d, Args&&... args) {
+    return [&](KArgs... coerced) {
+        void* ptrs[] = {&coerced..., nullptr};
+        return launch_args(what, reinterpret_cast<const void*>(kernel), d, ptrs);
+    }(std::forward<Args>(args)...);
+}
+
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device): the attribute is per device, and one process
 // may drive several GPUs (DataParallel, a model on cuda:1 while cuda:0 is current ...)
 cudaError_t ensure_dyn_smem(const void* kernel, int bytes);

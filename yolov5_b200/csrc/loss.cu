@@ -749,19 +749,15 @@ int loss_launch(const y5_loss_params* p, const void* const* pl, const float* tar
     a.trow = trow;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int sms = sm_count();
-    loss_zero_kernel<<<sms * 4, 256, 0, st>>>(a);
-    loss_targets_kernel<<<p->nl, 1024, 0, st>>>(a);
+    if (int e = launch("loss", loss_zero_kernel, {sms * 4, 256, 0, st}, a)) return e;
+    if (int e = launch("loss", loss_targets_kernel, {p->nl, 1024, 0, st}, a)) return e;
     const int match_blocks = min(kPartials, max(1, (a.cap + 127) / 128));
-    loss_match_kernel<<<dim3(match_blocks, p->nl), 128, 0, st>>>(a);
+    if (int e = launch("loss", loss_match_kernel, {dim3(match_blocks, p->nl), 128, 0, st}, a)) return e;
     const int dense_blocks = kPartials;
-    loss_dense_kernel<<<dim3(dense_blocks, p->nl), 512, 0, st>>>(a);
+    if (int e = launch("loss", loss_dense_kernel, {dim3(dense_blocks, p->nl), 512, 0, st}, a)) return e;
     const int cls_blocks = min(kPartials, max(1, (a.cap + 7) / 8));
-    loss_cls_kernel<<<dim3(cls_blocks, p->nl), 256, 0, st>>>(a);
-    loss_finalize_kernel<<<1, 32, 0, st>>>(a, match_blocks, dense_blocks, cls_blocks);
-    count_launch(6);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "loss launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    if (int e = launch("loss", loss_cls_kernel, {dim3(cls_blocks, p->nl), 256, 0, st}, a)) return e;
+    return launch("loss", loss_finalize_kernel, {1, 32, 0, st}, a, match_blocks, dense_blocks, cls_blocks);
 }
 }  // namespace
 
@@ -893,20 +889,14 @@ extern "C" Y5_API int y5_seg_loss_fwd_bwd_scaled(const y5_loss_params* p, const 
     a.det_out = reinterpret_cast<const float*>(ws + S.det_out);
     a.out = out_loss;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    seg_prep_kernel<<<1, 1024, 0, st>>>(a);
-    seg_bucket_kernel<<<p->batch, 256, 0, st>>>(a);
-    seg_match_kernel<<<dim3(min(a.cap, 4 * sm_count()), p->nl), 256, 0, st>>>(a);
-    int n = 4;
+    if (int e = launch("seg_loss", seg_prep_kernel, {1, 1024, 0, st}, a)) return e;
+    if (int e = launch("seg_loss", seg_bucket_kernel, {p->batch, 256, 0, st}, a)) return e;
+    if (int e = launch("seg_loss", seg_match_kernel, {dim3(min(a.cap, 4 * sm_count()), p->nl), 256, 0, st}, a)) return e;
     if (grad_proto) {
         const int tiles = ((mw + kSegTile - 1) / kSegTile) * ((mh + kSegTile - 1) / kSegTile);
-        seg_proto_kernel<<<dim3(tiles, p->batch), kSegTile * kSegTile, 0, st>>>(a);
-        ++n;
+        if (int e = launch("seg_loss", seg_proto_kernel, {dim3(tiles, p->batch), kSegTile * kSegTile, 0, st}, a)) return e;
     }
-    seg_finalize_kernel<<<1, 256, 0, st>>>(a);
-    count_launch(n);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "seg_loss launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    return launch("seg_loss", seg_finalize_kernel, {1, 256, 0, st}, a);
 }
 
 // Copies one level's tidx (int64) and xywhn (fp32 x4) to host memory (synchronises the stream: test / debugging helper).

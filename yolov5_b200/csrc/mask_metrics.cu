@@ -244,12 +244,6 @@ __global__ void match_iou_kernel(const float* __restrict__ det, long long img_st
     match_assign(s_best, s_iou, n, max_det, iouv, niou, correct + static_cast<long long>(b) * max_det * niou);
 }
 
-static int last_status(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 }  // namespace y5
 
 using namespace y5;
@@ -278,23 +272,15 @@ extern "C" Y5_API int y5_mask_pack(const void* src, int32_t src_dtype, int32_t s
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int* li = nullptr;
     if (label_index) {  // also with no targets at all: every image then owns an empty label block
-        mask_labels_kernel<<<1, 1024, 0, st>>>(target_img, target_stride, n_rows, batch, label_index);
-        count_launch();
+        if (int e = launch("mask_pack", mask_labels_kernel, {1, 1024, 0, st}, target_img, target_stride, n_rows, batch, label_index)) return e;
         li = label_index;
-        if (n_rows == 0) return last_status("mask_pack");
+        if (n_rows == 0) return 0;
     }
     const bool resize = src_h != out_h || src_w != out_w;
     const int ov = overlap != 0;
-#define Y5_PACK(O, R)                                                                                                                    \
-    mask_pack_kernel<O, R><<<n_rows, kPackThreads, 0, st>>>(src, src_dtype, src_h, src_w, out_h, out_w, li, batch, n_rows, words, bits, \
-                                                             popcount, nonbinary)
-    if (ov && resize) Y5_PACK(1, 1);
-    else if (ov) Y5_PACK(1, 0);
-    else if (resize) Y5_PACK(0, 1);
-    else Y5_PACK(0, 0);
-#undef Y5_PACK
-    count_launch();
-    return last_status("mask_pack");
+    auto* kernel = ov ? (resize ? mask_pack_kernel<1, 1> : mask_pack_kernel<1, 0>) : (resize ? mask_pack_kernel<0, 1> : mask_pack_kernel<0, 0>);
+    return launch("mask_pack", kernel, {n_rows, kPackThreads, 0, st}, src, src_dtype, src_h, src_w, out_h, out_w, li, batch, n_rows, words, bits,
+                  popcount, nonbinary);
 }
 
 extern "C" Y5_API int y5_mask_iou(const uint32_t* gt_bits, const int32_t* gt_pop, const int32_t* label_index, int32_t n_gt, const uint32_t* pred_bits,
@@ -307,10 +293,8 @@ extern "C" Y5_API int y5_mask_iou(const uint32_t* gt_bits, const int32_t* gt_pop
     if (!label_index && n_gt == 0) return 0;
     if (!gt_bits || !gt_pop || !pred_bits || !pred_pop || !iou) return set_error(Y5_E_INVALID, "mask_iou: null pointer");
     const dim3 grid((rows_per_image + 8 * kIouWarps - 1) / (8 * kIouWarps), n_img);
-    mask_iou_kernel<<<grid, kIouWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(gt_bits, gt_pop, label_index, n_gt, pred_bits, pred_pop, count,
-                                                                                   img0, rows_per_image, words, eps, iou);
-    count_launch();
-    return last_status("mask_iou");
+    return launch("mask_iou", mask_iou_kernel, {grid, kIouWarps * 32, 0, static_cast<cudaStream_t>(stream)}, gt_bits, gt_pop, label_index, n_gt,
+                  pred_bits, pred_pop, count, img0, rows_per_image, words, eps, iou);
 }
 
 extern "C" Y5_API int y5_mask_match_batch(const float* det, int64_t img_stride, int32_t row_stride, const int32_t* count, int32_t batch,
@@ -321,8 +305,6 @@ extern "C" Y5_API int y5_mask_match_batch(const float* det, int64_t img_stride, 
         return set_error(Y5_E_INVALID, "mask_match_batch: bad argument");
     if (!label_index && batch != 1) return set_error(Y5_E_INVALID, "mask_match_batch: more than one image needs label_index");
     if (max_det > kMatchMaxDet) return set_error(Y5_E_UNSUPPORTED, "mask_match_batch: max_det %d > %d", max_det, kMatchMaxDet);
-    match_iou_kernel<<<batch, 256, 0, static_cast<cudaStream_t>(stream)>>>(det, img_stride, row_stride, count, max_det, label_cls, cls_stride,
-                                                                            label_index, batch, nt, iou, iouv, niou, correct);
-    count_launch();
-    return last_status("mask_match_batch");
+    return launch("mask_match_batch", match_iou_kernel, {batch, 256, 0, static_cast<cudaStream_t>(stream)}, det, img_stride, row_stride, count,
+                  max_det, label_cls, cls_stride, label_index, batch, nt, iou, iouv, niou, correct);
 }

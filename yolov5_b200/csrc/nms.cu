@@ -619,27 +619,20 @@ extern "C" Y5_API int y5_nms_batched(const y5_nms_params* p, const void* pred, f
     if (ensure_dyn_smem(reinterpret_cast<const void*>(nms_sort_kernel), kCandCap * 6) != cudaSuccess ||
         ensure_dyn_smem(reinterpret_cast<const void*>(nms_greedy_kernel), kMaxDetCap * 20) != cudaSuccess)
         return set_error(Y5_E_DRIVER, "nms: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
-    nms_pass_kernel<0><<<grid, threads, 0, st>>>(a, 0);
-    nms_scan_kernel<0><<<p->batch, 1024, 0, st>>>(a);
-    int launches = 2;
+    if (int e = launch("nms", nms_pass_kernel<0>, {grid, threads, 0, st}, a, 0)) return e;
+    if (int e = launch("nms", nms_scan_kernel<0>, {p->batch, 1024, 0, st}, a)) return e;
     const long long max_cands = a.multi_label ? static_cast<long long>(p->n_rows) * p->nc : p->n_rows;
     if (max_cands > p->max_nms) {  // the cut can only trigger when more candidates than max_nms are possible at all
-        nms_pass_kernel<1><<<grid, threads, 0, st>>>(a, 0);
-        nms_pick_kernel<<<p->batch, 1024, 0, st>>>(a, 0);
-        nms_pass_kernel<1><<<grid, threads, 0, st>>>(a, 1);
-        nms_pick_kernel<<<p->batch, 1024, 0, st>>>(a, 1);
-        nms_pass_kernel<2><<<grid, threads, 0, st>>>(a, 0);
-        nms_scan_kernel<1><<<p->batch, 1024, 0, st>>>(a);
-        launches += 6;
+        if (int e = launch("nms", nms_pass_kernel<1>, {grid, threads, 0, st}, a, 0)) return e;
+        if (int e = launch("nms", nms_pick_kernel, {p->batch, 1024, 0, st}, a, 0)) return e;
+        if (int e = launch("nms", nms_pass_kernel<1>, {grid, threads, 0, st}, a, 1)) return e;
+        if (int e = launch("nms", nms_pick_kernel, {p->batch, 1024, 0, st}, a, 1)) return e;
+        if (int e = launch("nms", nms_pass_kernel<2>, {grid, threads, 0, st}, a, 0)) return e;
+        if (int e = launch("nms", nms_scan_kernel<1>, {p->batch, 1024, 0, st}, a)) return e;
     }
-    nms_pass_kernel<3><<<grid, threads, 0, st>>>(a, 0);
-    nms_sort_kernel<<<p->batch, 1024, kCandCap * 6, st>>>(a);
-    nms_greedy_kernel<<<p->batch, kGreedyThreads, static_cast<size_t>(p->max_det) * 20, st>>>(a);
-    launches += 3;
-    count_launch(launches);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "nms launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    if (int e = launch("nms", nms_pass_kernel<3>, {grid, threads, 0, st}, a, 0)) return e;
+    if (int e = launch("nms", nms_sort_kernel, {p->batch, 1024, kCandCap * 6, st}, a)) return e;
+    return launch("nms", nms_greedy_kernel, {p->batch, kGreedyThreads, static_cast<size_t>(p->max_det) * 20, st}, a);
 }
 
 extern "C" Y5_API int y5_box_iou(const float* a, int32_t n, const float* b, int32_t m, float eps, float* out, void* stream) {
@@ -648,11 +641,6 @@ extern "C" Y5_API int y5_box_iou(const float* a, int32_t n, const float* b, int3
     if ((reinterpret_cast<uintptr_t>(a) & 15) || (reinterpret_cast<uintptr_t>(b) & 15)) return set_error(Y5_E_INVALID, "box_iou: boxes must be 16-byte aligned");
     const long long total = static_cast<long long>(n) * m;
     const int threads = 256;
-    long long blocks = (total + threads - 1) / threads;
-    if (blocks > sm_count() * 16) blocks = sm_count() * 16;
-    box_iou_kernel<<<static_cast<int>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(a, n, b, m, eps, out);
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "box_iou launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    return launch("box_iou", box_iou_kernel, {grid_stride_ctas(total, threads, 16), threads, 0, static_cast<cudaStream_t>(stream)}, a, n, b, m,
+                  eps, out);
 }

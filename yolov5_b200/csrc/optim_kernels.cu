@@ -254,13 +254,12 @@ extern "C" Y5_API int y5_opt_step(const y5_opt_tensor* table, const int32_t* chu
     if (n_chunks <= 0) return 0;
     if (!table || !chunk_tensor || !chunk_index || !hyper || (do_step && !partial)) return set_error(Y5_E_INVALID, "opt_step: null pointer");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (do_step) opt_grad_norm_kernel<<<n_chunks, kOptThreads, 0, st>>>(table, chunk_tensor, chunk_index, hyper, partial);
-    opt_step_kernel<<<n_chunks, kOptThreads, 0, st>>>(table, chunk_tensor, chunk_index, n_chunks, hyper, partial, do_step, do_ema, zero_grad);
-    opt_tick_kernel<<<1, 1, 0, st>>>(hyper, do_ema);
-    count_launch(do_step ? 3 : 2);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "opt_step launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    if (do_step)
+        if (int e = launch("opt_step", opt_grad_norm_kernel, {n_chunks, kOptThreads, 0, st}, table, chunk_tensor, chunk_index, hyper, partial)) return e;
+    if (int e = launch("opt_step", opt_step_kernel, {n_chunks, kOptThreads, 0, st}, table, chunk_tensor, chunk_index, n_chunks, hyper, partial,
+                       do_step, do_ema, zero_grad))
+        return e;
+    return launch("opt_step", opt_tick_kernel, {1, 1, 0, st}, hyper, do_ema);
 }
 
 extern "C" Y5_API int y5_adam_step(const y5_opt_tensor* table, int32_t n_tensors, const int32_t* chunk_tensor, const int32_t* chunk_index,
@@ -271,14 +270,11 @@ extern "C" Y5_API int y5_adam_step(const y5_opt_tensor* table, int32_t n_tensors
         return set_error(Y5_E_INVALID, "adam_step: null pointer");
     if (n_tensors <= 0 || sq_offset < 0) return set_error(Y5_E_INVALID, "adam_step: n_tensors %d, sq_offset %lld", n_tensors, (long long)sq_offset);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    opt_grad_norm_kernel<<<n_chunks, kOptThreads, 0, st>>>(table, chunk_tensor, chunk_index, hyper, partial);
-    opt_adam_step_kernel<<<n_chunks, kOptThreads, 0, st>>>(table, chunk_tensor, chunk_index, n_chunks, hyper, group_hyper, sq_offset, steps,
-                                                           partial, do_ema, zero_grad);
-    adam_tick_kernel<<<(n_tensors + 255) / 256, 256, 0, st>>>(table, n_tensors, steps, hyper, do_ema);
-    count_launch(3);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "adam_step launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    if (int e = launch("adam_step", opt_grad_norm_kernel, {n_chunks, kOptThreads, 0, st}, table, chunk_tensor, chunk_index, hyper, partial)) return e;
+    if (int e = launch("adam_step", opt_adam_step_kernel, {n_chunks, kOptThreads, 0, st}, table, chunk_tensor, chunk_index, n_chunks, hyper,
+                       group_hyper, sq_offset, steps, partial, do_ema, zero_grad))
+        return e;
+    return launch("adam_step", adam_tick_kernel, {(n_tensors + 255) / 256, 256, 0, st}, table, n_tensors, steps, hyper, do_ema);
 }
 
 extern "C" Y5_API int y5_grad_pack(const y5_opt_tensor* table, const int32_t* chunk_tensor, const int32_t* chunk_index, int32_t n_chunks,
@@ -286,21 +282,14 @@ extern "C" Y5_API int y5_grad_pack(const y5_opt_tensor* table, const int32_t* ch
     if (n_chunks <= 0) return 0;
     if (!table || !chunk_tensor || !chunk_index || !arena_offset || !arena || !present) return set_error(Y5_E_INVALID, "grad_pack: null pointer");
     if (reinterpret_cast<uintptr_t>(arena) & 15) return set_error(Y5_E_INVALID, "grad_pack: the arena must be 16-byte aligned");
-    grad_pack_kernel<<<n_chunks, kOptThreads, 0, static_cast<cudaStream_t>(stream)>>>(table, chunk_tensor, chunk_index, arena_offset, arena,
-                                                                                      present);
-    count_launch(1);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "grad_pack launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    return launch("grad_pack", grad_pack_kernel, {n_chunks, kOptThreads, 0, static_cast<cudaStream_t>(stream)}, table, chunk_tensor, chunk_index,
+                  arena_offset, arena, present);
 }
 
 extern "C" Y5_API int y5_grad_bind(y5_opt_tensor* arena_table, int32_t n_tensors, const int64_t* arena_offset, float* arena, const float* present,
                                    void* stream) {
     if (n_tensors <= 0) return 0;
     if (!arena_table || !arena_offset || !arena || !present) return set_error(Y5_E_INVALID, "grad_bind: null pointer");
-    grad_bind_kernel<<<(n_tensors + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(arena_table, n_tensors, arena_offset, arena, present);
-    count_launch(1);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "grad_bind launch failed: %s", cudaGetErrorString(e));
-    return 0;
+    return launch("grad_bind", grad_bind_kernel, {(n_tensors + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)}, arena_table, n_tensors,
+                  arena_offset, arena, present);
 }

@@ -234,20 +234,6 @@ __global__ void spp_gather_kernel(const T* __restrict__ dcat, int dcat_pitch, co
     }
 }
 
-int grid_for(long long total, int threads) {
-    long long blocks = (total + threads - 1) / threads;
-    const long long cap = static_cast<long long>(sm_count()) * 16;  // grid-stride beyond 16 CTAs per SM
-    if (blocks > cap) blocks = cap;
-    return static_cast<int>(blocks < 1 ? 1 : blocks);
-}
-
-int launched(const char* what) {
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 // a view the kernels move in 16-byte vectors: aligned base, pitch covering its channels and a multiple of 8 elements
 bool vec_view(const void* p, int pitch, int c) { return p && !(reinterpret_cast<uintptr_t>(p) & 15) && pitch >= c && pitch % 8 == 0; }
 
@@ -268,32 +254,28 @@ int pool_out(int mode, int h, int w, int* ho, int* wo) {
 }
 
 template <typename T>
-void fwd_launch(int mode, const void* x, int xp, void* y, int yp, int B, int H, int W, int Ho, int Wo, int C, int bf, cudaStream_t st) {
-    const int threads = 256, grid = grid_for(static_cast<long long>(B) * Ho * Wo * (C / 8), threads);
-    if (mode == Y5_POOL_K2S2)
-        maxpool2_fwd_kernel<T, Y5_POOL_K2S2><<<grid, threads, 0, st>>>(static_cast<const T*>(x), xp, static_cast<T*>(y), yp, B, H, W, Ho, Wo, C, bf);
-    else
-        maxpool2_fwd_kernel<T, Y5_POOL_K2S1_ZPAD><<<grid, threads, 0, st>>>(static_cast<const T*>(x), xp, static_cast<T*>(y), yp, B, H, W, Ho, Wo, C, bf);
+int fwd_launch(int mode, const void* x, int xp, void* y, int yp, int B, int H, int W, int Ho, int Wo, int C, int bf, cudaStream_t st) {
+    const int threads = 256, grid = grid_stride_ctas(static_cast<long long>(B) * Ho * Wo * (C / 8), threads, 16);
+    auto* kernel = mode == Y5_POOL_K2S2 ? maxpool2_fwd_kernel<T, Y5_POOL_K2S2> : maxpool2_fwd_kernel<T, Y5_POOL_K2S1_ZPAD>;
+    return launch("maxpool2d", kernel, {grid, threads, 0, st}, static_cast<const T*>(x), xp, static_cast<T*>(y), yp, B, H, W, Ho, Wo, C, bf);
 }
 
 template <typename T>
-void bwd_launch(int mode, const void* x, int xp, const void* dy, int dyp, void* dx, int dxp, int B, int H, int W, int Ho, int Wo, int C, int bf,
-                cudaStream_t st) {
-    const int threads = 256, grid = grid_for(static_cast<long long>(B) * H * W * (C / 8), threads);
-    if (mode == Y5_POOL_K2S2)
-        maxpool2_bwd_kernel<T, Y5_POOL_K2S2><<<grid, threads, 0, st>>>(static_cast<const T*>(x), xp, static_cast<const T*>(dy), dyp,
-                                                                        static_cast<T*>(dx), dxp, B, H, W, Ho, Wo, C, bf);
-    else
-        maxpool2_bwd_kernel<T, Y5_POOL_K2S1_ZPAD><<<grid, threads, 0, st>>>(static_cast<const T*>(x), xp, static_cast<const T*>(dy), dyp,
-                                                                             static_cast<T*>(dx), dxp, B, H, W, Ho, Wo, C, bf);
+int bwd_launch(int mode, const void* x, int xp, const void* dy, int dyp, void* dx, int dxp, int B, int H, int W, int Ho, int Wo, int C, int bf,
+               cudaStream_t st) {
+    const int threads = 256, grid = grid_stride_ctas(static_cast<long long>(B) * H * W * (C / 8), threads, 16);
+    auto* kernel = mode == Y5_POOL_K2S2 ? maxpool2_bwd_kernel<T, Y5_POOL_K2S2> : maxpool2_bwd_kernel<T, Y5_POOL_K2S1_ZPAD>;
+    return launch("maxpool2d_bwd", kernel, {grid, threads, 0, st}, static_cast<const T*>(x), xp, static_cast<const T*>(dy), dyp,
+                  static_cast<T*>(dx), dxp, B, H, W, Ho, Wo, C, bf);
 }
 
 template <typename T>
-void spp_launch(const void* a, int ap, const void* dcat, int dp, void* da, int dap, int B, int H, int W, int C, int k, int bf, uint16_t* code,
-                cudaStream_t st) {
-    const int threads = 128, grid = grid_for(static_cast<long long>(B) * H * W * (C / 8), threads);
-    spp_argmax_kernel<T><<<grid, threads, 0, st>>>(static_cast<const T*>(a), ap, code, B, H, W, C, k, bf);
-    spp_gather_kernel<T><<<grid, threads, 0, st>>>(static_cast<const T*>(dcat), dp, code, static_cast<T*>(da), dap, B, H, W, C, k, bf);
+int spp_launch(const void* a, int ap, const void* dcat, int dp, void* da, int dap, int B, int H, int W, int C, int k, int bf, uint16_t* code,
+               cudaStream_t st) {
+    const int threads = 128, grid = grid_stride_ctas(static_cast<long long>(B) * H * W * (C / 8), threads, 16);
+    if (int e = launch("spp_pool_bwd", spp_argmax_kernel<T>, {grid, threads, 0, st}, static_cast<const T*>(a), ap, code, B, H, W, C, k, bf)) return e;
+    return launch("spp_pool_bwd", spp_gather_kernel<T>, {grid, threads, 0, st}, static_cast<const T*>(dcat), dp, code, static_cast<T*>(da), dap,
+                  B, H, W, C, k, bf);
 }
 
 }  // namespace
@@ -307,11 +289,8 @@ extern "C" Y5_API int y5_maxpool2d(const void* x, int32_t x_pitch, void* y, int3
     int ho, wo;
     if (int e = pool_out(mode, h, w, &ho, &wo)) return e;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (dtype == Y5_F32)
-        fwd_launch<float>(mode, x, x_pitch, y, y_pitch, batch, h, w, ho, wo, c, 0, st);
-    else
-        fwd_launch<uint16_t>(mode, x, x_pitch, y, y_pitch, batch, h, w, ho, wo, c, dtype == Y5_BF16, st);
-    return launched("maxpool2d");
+    if (dtype == Y5_F32) return fwd_launch<float>(mode, x, x_pitch, y, y_pitch, batch, h, w, ho, wo, c, 0, st);
+    return fwd_launch<uint16_t>(mode, x, x_pitch, y, y_pitch, batch, h, w, ho, wo, c, dtype == Y5_BF16, st);
 }
 
 extern "C" Y5_API int y5_maxpool2d_bwd(const void* x, int32_t x_pitch, const void* dy, int32_t dy_pitch, void* dx, int32_t dx_pitch, int32_t batch,
@@ -323,11 +302,8 @@ extern "C" Y5_API int y5_maxpool2d_bwd(const void* x, int32_t x_pitch, const voi
     int ho, wo;
     if (int e = pool_out(mode, h, w, &ho, &wo)) return e;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (dtype == Y5_F32)
-        bwd_launch<float>(mode, x, x_pitch, dy, dy_pitch, dx, dx_pitch, batch, h, w, ho, wo, c, 0, st);
-    else
-        bwd_launch<uint16_t>(mode, x, x_pitch, dy, dy_pitch, dx, dx_pitch, batch, h, w, ho, wo, c, dtype == Y5_BF16, st);
-    return launched("maxpool2d_bwd");
+    if (dtype == Y5_F32) return bwd_launch<float>(mode, x, x_pitch, dy, dy_pitch, dx, dx_pitch, batch, h, w, ho, wo, c, 0, st);
+    return bwd_launch<uint16_t>(mode, x, x_pitch, dy, dy_pitch, dx, dx_pitch, batch, h, w, ho, wo, c, dtype == Y5_BF16, st);
 }
 
 extern "C" Y5_API int64_t y5_spp_bwd_workspace_bytes(int32_t batch, int32_t h, int32_t w, int32_t c) {
@@ -346,11 +322,6 @@ extern "C" Y5_API int y5_spp_pool_bwd(const void* a, int32_t a_pitch, const void
                                        "and a multiple of 8; workspace 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     uint16_t* code = static_cast<uint16_t*>(workspace);
-    if (dtype == Y5_F32)
-        spp_launch<float>(a, a_pitch, dcat, dcat_pitch, da, da_pitch, batch, h, w, c, ksize, 0, code, st);
-    else
-        spp_launch<uint16_t>(a, a_pitch, dcat, dcat_pitch, da, da_pitch, batch, h, w, c, ksize, dtype == Y5_BF16, code, st);
-    if (int e = launched("spp_pool_bwd")) return e;
-    count_launch();  // two kernels
-    return 0;
+    if (dtype == Y5_F32) return spp_launch<float>(a, a_pitch, dcat, dcat_pitch, da, da_pitch, batch, h, w, c, ksize, 0, code, st);
+    return spp_launch<uint16_t>(a, a_pitch, dcat, dcat_pitch, da, da_pitch, batch, h, w, c, ksize, dtype == Y5_BF16, code, st);
 }

@@ -543,12 +543,6 @@ __global__ void confusion_kernel(const float* __restrict__ det, long long img_st
     }
 }
 
-static int last_status(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 }  // namespace y5
 
 using namespace y5;
@@ -581,29 +575,31 @@ extern "C" Y5_API int y5_letterbox(const y5_letterbox_image* images, int32_t n_i
         for (int i = 0; i < nb; ++i) L.im[i] = images[i0 + i];
         const dim3 grid((out_w / step + block.x - 1) / block.x, (out_h / step + block.y - 1) / block.y, nb);
         const int bf = out_dtype == Y5_BF16;
+        int e;
         if (s2d) {
             const int row_px = out_row_px ? out_row_px : out_w / 2;
             uint8_t* o = static_cast<uint8_t*>(out) + static_cast<size_t>(i0) * (out_h / 2) * row_px * 32;
-            letterbox_kernel<3><<<grid, block, 0, st>>>(L, nb, out_h, out_w, swap_rb, pad_value, o, bf, row_px, out_x_off);
+            e = launch("letterbox", letterbox_kernel<3>, {grid, block, 0, st}, L, nb, out_h, out_w, swap_rb, pad_value, o, bf, row_px, out_x_off);
         } else if (out_dtype == Y5_U8) {
-            letterbox_kernel<0><<<grid, block, 0, st>>>(L, nb, out_h, out_w, swap_rb, pad_value, static_cast<uint8_t*>(out) + i0 * img_elems, bf, 0, 0);
+            e = launch("letterbox", letterbox_kernel<0>, {grid, block, 0, st}, L, nb, out_h, out_w, swap_rb, pad_value,
+                       static_cast<uint8_t*>(out) + i0 * img_elems, bf, 0, 0);
         } else if (out_dtype == Y5_F32) {
-            letterbox_kernel<2><<<grid, block, 0, st>>>(L, nb, out_h, out_w, swap_rb, pad_value, static_cast<float*>(out) + i0 * img_elems, bf, 0, 0);
+            e = launch("letterbox", letterbox_kernel<2>, {grid, block, 0, st}, L, nb, out_h, out_w, swap_rb, pad_value,
+                       static_cast<float*>(out) + i0 * img_elems, bf, 0, 0);
         } else {
-            letterbox_kernel<1><<<grid, block, 0, st>>>(L, nb, out_h, out_w, swap_rb, pad_value, static_cast<uint16_t*>(out) + i0 * img_elems, bf, 0, 0);
+            e = launch("letterbox", letterbox_kernel<1>, {grid, block, 0, st}, L, nb, out_h, out_w, swap_rb, pad_value,
+                       static_cast<uint16_t*>(out) + i0 * img_elems, bf, 0, 0);
         }
-        count_launch();
+        if (e) return e;
     }
-    return last_status("letterbox");
+    return 0;
 }
 
-static void launch_val(const ValBatch& L, int nb, int grid_w, int grid_h, int out_h, int out_w, void* out, int out_dtype, cudaStream_t st) {
+static int launch_val(const ValBatch& L, int nb, int grid_w, int grid_h, int out_h, int out_w, void* out, int out_dtype, cudaStream_t st) {
     const dim3 block(32, 8);
     const dim3 grid((grid_w + block.x - 1) / block.x, (grid_h + block.y - 1) / block.y, nb);
-    if (out_dtype == Y5_U8) val_letterbox_kernel<0><<<grid, block, 0, st>>>(L, out_h, out_w, out, 0);
-    else if (out_dtype == Y5_F32) val_letterbox_kernel<2><<<grid, block, 0, st>>>(L, out_h, out_w, out, 0);
-    else val_letterbox_kernel<1><<<grid, block, 0, st>>>(L, out_h, out_w, out, out_dtype == Y5_BF16);
-    count_launch();
+    auto* kernel = out_dtype == Y5_U8 ? val_letterbox_kernel<0> : out_dtype == Y5_F32 ? val_letterbox_kernel<2> : val_letterbox_kernel<1>;
+    return launch("val_letterbox", kernel, {grid, block, 0, st}, L, out_h, out_w, out, out_dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int y5_val_letterbox(const y5_val_image* images, int32_t n_images, int32_t out_h, int32_t out_w, void* out, int32_t out_dtype,
@@ -653,10 +649,11 @@ extern "C" Y5_API int y5_val_letterbox(const y5_val_image* images, int32_t n_ima
             }
         }
         void* o = static_cast<uint8_t*>(out) + static_cast<size_t>(i0) * img_bytes;
-        launch_val(L, nb, gw, gh, out_h, out_w, o, out_dtype, st);
-        if (again) launch_val(A, nb, out_w, out_h, out_h, out_w, o, out_dtype, st);
+        if (int e = launch_val(L, nb, gw, gh, out_h, out_w, o, out_dtype, st)) return e;
+        if (again)
+            if (int e = launch_val(A, nb, out_w, out_h, out_h, out_w, o, out_dtype, st)) return e;
     }
-    return last_status("val_letterbox");
+    return 0;
 }
 
 extern "C" Y5_API int y5_cls_batch(const y5_cls_image* images, int32_t n_images, int32_t out_h, int32_t out_w, const float* mean, const float* std,
@@ -675,10 +672,8 @@ extern "C" Y5_API int y5_cls_batch(const y5_cls_image* images, int32_t n_images,
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const dim3 block(32, 8);
     const dim3 grid((out_w + block.x - 1) / block.x, (out_h + block.y - 1) / block.y, n_images);
-    if (out_dtype == Y5_F32) cls_batch_kernel<2><<<grid, block, 0, st>>>(images, out_h, out_w, N, out, 0);
-    else cls_batch_kernel<1><<<grid, block, 0, st>>>(images, out_h, out_w, N, out, out_dtype == Y5_BF16);
-    count_launch();
-    return last_status("cls_batch");
+    return launch("cls_batch", out_dtype == Y5_F32 ? cls_batch_kernel<2> : cls_batch_kernel<1>, {grid, block, 0, st}, images, out_h, out_w, N, out,
+                  out_dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int64_t y5_process_mask_workspace_bytes(int32_t n, int32_t mh, int32_t mw, int32_t mode) {
@@ -711,21 +706,16 @@ extern "C" Y5_API int y5_process_mask(const void* protos, int32_t proto_dtype, i
     // python-float ratios rounded once to fp32, as `tensor *= mw / iw` does
     const float sxw = static_cast<float>(static_cast<double>(mw) / static_cast<double>(in_w));
     const float syh = static_cast<float>(static_cast<double>(mh) / static_cast<double>(in_h));
-    if (mode == 0) {
-        mask_lowres_kernel<1><<<grid, 256, smem, st>>>(protos, proto_dtype, c, mh, mw, coef, coef_stride, boxes, box_stride, img_index, n, sxw, syh,
-                                                        1, out, out_dtype == Y5_U8);
-        count_launch();
-    } else {
-        float* low = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~uintptr_t(255));
-        mask_lowres_kernel<0><<<grid, 256, smem, st>>>(protos, proto_dtype, c, mh, mw, coef, coef_stride, boxes, box_stride, img_index, n, sxw, syh,
-                                                        mode == 1, low, 0);
-        const long long total = static_cast<long long>(n) * in_h * in_w;
-        const long long blocks = (total + 255) / 256;
-        mask_upsample_kernel<<<static_cast<unsigned>(blocks < sm_count() * 32LL ? blocks : sm_count() * 32LL), 256, 0, st>>>(
-            low, n, mh, mw, wy, wx, wh, ww, in_h, in_w, mode == 2 ? boxes : nullptr, box_stride, out, out_dtype == Y5_U8);
-        count_launch(2);
-    }
-    return last_status("process_mask");
+    if (mode == 0)
+        return launch("process_mask", mask_lowres_kernel<1>, {grid, 256, smem, st}, protos, proto_dtype, c, mh, mw, coef, coef_stride, boxes,
+                      box_stride, img_index, n, sxw, syh, 1, out, out_dtype == Y5_U8);
+    float* low = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~uintptr_t(255));
+    if (int e = launch("process_mask", mask_lowres_kernel<0>, {grid, 256, smem, st}, protos, proto_dtype, c, mh, mw, coef, coef_stride, boxes,
+                       box_stride, img_index, n, sxw, syh, mode == 1, low, 0))
+        return e;
+    const long long total = static_cast<long long>(n) * in_h * in_w;
+    return launch("process_mask", mask_upsample_kernel, {grid_stride_ctas(total, 256, 32), 256, 0, st}, low, n, mh, mw, wy, wx, wh, ww, in_h, in_w,
+                  mode == 2 ? boxes : nullptr, box_stride, out, out_dtype == Y5_U8);
 }
 
 extern "C" Y5_API int y5_crop_mask(const float* masks, const float* boxes, int32_t box_stride, int32_t n, int32_t h, int32_t w, float* out,
@@ -733,30 +723,22 @@ extern "C" Y5_API int y5_crop_mask(const float* masks, const float* boxes, int32
     if (n == 0) return 0;
     if (!masks || !boxes || !out || n < 0 || h <= 0 || w <= 0 || box_stride < 4) return set_error(Y5_E_INVALID, "crop_mask: bad argument");
     const long long total = static_cast<long long>(n) * h * w;
-    const long long blocks = (total + 255) / 256;
-    crop_mask_kernel<<<static_cast<unsigned>(blocks < sm_count() * 16LL ? blocks : sm_count() * 16LL), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        masks, boxes, box_stride, n, h, w, out);
-    count_launch();
-    return last_status("crop_mask");
+    return launch("crop_mask", crop_mask_kernel, {grid_stride_ctas(total, 256, 16), 256, 0, static_cast<cudaStream_t>(stream)}, masks, boxes,
+                  box_stride, n, h, w, out);
 }
 
 extern "C" Y5_API int y5_scale_boxes(float* boxes, int32_t row_stride, int64_t n_rows, const int32_t* img_index, int32_t rows_per_image,
                                      const int32_t* count, const float* meta, void* stream) {
     if (n_rows == 0) return 0;
     if (!boxes || !meta || n_rows < 0 || row_stride < 4) return set_error(Y5_E_INVALID, "scale_boxes: bad argument");
-    const long long blocks = (n_rows + 255) / 256;
-    scale_boxes_kernel<<<static_cast<unsigned>(blocks < sm_count() * 8 ? blocks : sm_count() * 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        boxes, row_stride, n_rows, img_index, rows_per_image, count, meta);
-    count_launch();
-    return last_status("scale_boxes");
+    return launch("scale_boxes", scale_boxes_kernel, {grid_stride_ctas(n_rows, 256, 8), 256, 0, static_cast<cudaStream_t>(stream)}, boxes,
+                  row_stride, n_rows, img_index, rows_per_image, count, meta);
 }
 
 extern "C" Y5_API int y5_labels_native(const float* targets, int32_t nt, const float* meta, float* out, void* stream) {
     if (nt == 0) return 0;
     if (!targets || !meta || !out || nt < 0) return set_error(Y5_E_INVALID, "labels_native: bad argument");
-    labels_native_kernel<<<(nt + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(targets, nt, meta, out);
-    count_launch();
-    return last_status("labels_native");
+    return launch("labels_native", labels_native_kernel, {(nt + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)}, targets, nt, meta, out);
 }
 
 extern "C" Y5_API int y5_match_batch(const float* det, int64_t img_stride, int32_t row_stride, const int32_t* count, int32_t batch,
@@ -766,10 +748,8 @@ extern "C" Y5_API int y5_match_batch(const float* det, int64_t img_stride, int32
     if (!det || !iouv || !correct || niou <= 0 || row_stride < 6 || nt < 0 || (nt > 0 && !labels))
         return set_error(Y5_E_INVALID, "match_batch: bad argument");
     if (max_det > kMatchMaxDet) return set_error(Y5_E_UNSUPPORTED, "match_batch: max_det %d > %d", max_det, kMatchMaxDet);
-    match_kernel<<<batch, 256, 0, static_cast<cudaStream_t>(stream)>>>(det, img_stride, row_stride, count, max_det, labels, nt, iouv, niou, eps,
-                                                                        correct);
-    count_launch();
-    return last_status("match_batch");
+    return launch("match_batch", match_kernel, {batch, 256, 0, static_cast<cudaStream_t>(stream)}, det, img_stride, row_stride, count, max_det,
+                  labels, nt, iouv, niou, eps, correct);
 }
 
 extern "C" Y5_API int y5_confusion_batch(const float* det, int64_t img_stride, int32_t row_stride, const int32_t* count, int32_t batch,
@@ -780,8 +760,6 @@ extern "C" Y5_API int y5_confusion_batch(const float* det, int64_t img_stride, i
         return set_error(Y5_E_INVALID, "confusion_batch: bad argument");
     if (max_det > kMatchMaxDet) return set_error(Y5_E_UNSUPPORTED, "confusion_batch: max_det %d > %d", max_det, kMatchMaxDet);
     if (nc > (1 << 15)) return set_error(Y5_E_UNSUPPORTED, "confusion_batch: nc %d > %d", nc, 1 << 15);
-    confusion_kernel<<<batch, 256, 0, static_cast<cudaStream_t>(stream)>>>(det, img_stride, row_stride, count, max_det, labels, nt, nc, conf_thres,
-                                                                            iou_thres, eps, reinterpret_cast<unsigned long long*>(matrix), error);
-    count_launch();
-    return last_status("confusion_batch");
+    return launch("confusion_batch", confusion_kernel, {batch, 256, 0, static_cast<cudaStream_t>(stream)}, det, img_stride, row_stride, count,
+                  max_det, labels, nt, nc, conf_thres, iou_thres, eps, reinterpret_cast<unsigned long long*>(matrix), error);
 }

@@ -427,12 +427,6 @@ __global__ void seg_compose_kernel(const y5_aug_image* __restrict__ table, const
     else seg_store<int32_t>(out, o, v);
 }
 
-static int seg_status(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
-
 }  // namespace y5
 
 using namespace y5;
@@ -446,10 +440,8 @@ extern "C" Y5_API int y5_seg_warp(const y5_aug_image* table, int32_t n_images, c
     if (out_h > 16384 || out_w > 16384 || max_points > 8192) return set_error(Y5_E_UNSUPPORTED, "seg_warp: image or polygon too large");
     if (n_labels == 0) return 0;
     const size_t smem = sizeof(float) * 2 * (static_cast<size_t>(max_points) + 1);
-    seg_warp_kernel<<<n_labels, kSegThreads, smem, static_cast<cudaStream_t>(stream)>>>(table, n_images, labels, segments, points, max_points,
-                                                                                          out_h, out_w, verts, rows, keep);
-    count_launch();
-    return seg_status("seg_warp");
+    return launch("seg_warp", seg_warp_kernel, {n_labels, kSegThreads, smem, static_cast<cudaStream_t>(stream)}, table, n_images, labels, segments,
+                  points, max_points, out_h, out_w, verts, rows, keep);
 }
 
 extern "C" Y5_API int y5_seg_raster(const int32_t* verts, int32_t n_verts, const int32_t* keep, int32_t n_labels, int32_t out_h, int32_t out_w,
@@ -465,19 +457,16 @@ extern "C" Y5_API int y5_seg_raster(const int32_t* verts, int32_t n_verts, const
     const int nsrc = ratio == 1 ? 1 : 2;
     const size_t smem = static_cast<size_t>(nsrc) * out_w * (sizeof(int) + 1);
     if (smem > 48 * 1024) cudaFuncSetAttribute(seg_raster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    seg_raster_kernel<<<dim3(out_h / ratio, n_labels), kSegThreads, smem, st>>>(verts, n_verts, keep, out_h, out_w, ratio, masks, areas);
-    count_launch();
-    return seg_status("seg_raster");
+    return launch("seg_raster", seg_raster_kernel, {dim3(out_h / ratio, n_labels), kSegThreads, smem, st}, verts, n_verts, keep, out_h, out_w, ratio,
+                  masks, areas);
 }
 
 extern "C" Y5_API int y5_seg_order(const int32_t* image_rows, int32_t n_images, const int32_t* keep, const int32_t* areas, const float* rows,
                                    int32_t overlap, float* targets, int32_t* plane, int32_t* counts, void* stream) {
     if (!image_rows || !counts || n_images <= 0) return set_error(Y5_E_INVALID, "seg_order: bad argument");
     if (n_images > 65535) return set_error(Y5_E_UNSUPPORTED, "seg_order: batch too large");
-    seg_order_kernel<<<n_images, kSegOrderThreads, 0, static_cast<cudaStream_t>(stream)>>>(image_rows, n_images, keep, areas, rows, overlap,
-                                                                                            targets, plane, counts);
-    count_launch();
-    return seg_status("seg_order");
+    return launch("seg_order", seg_order_kernel, {n_images, kSegOrderThreads, 0, static_cast<cudaStream_t>(stream)}, image_rows, n_images, keep,
+                  areas, rows, overlap, targets, plane, counts);
 }
 
 extern "C" Y5_API int y5_seg_compose(const y5_aug_image* table, const y5_aug_label* labels, const int32_t* counts, const int32_t* plane,
@@ -490,8 +479,6 @@ extern "C" Y5_API int y5_seg_compose(const y5_aug_image* table, const y5_aug_lab
     if (n_out == 0) return 0;
     const long long npx = static_cast<long long>(mask_h) * mask_w;
     const dim3 grid(static_cast<unsigned>((npx + 255) / 256), n_out);
-    seg_compose_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(table, labels, counts, plane, masks, mask_h, mask_w, overlap, out,
-                                                                             out_dtype);
-    count_launch();
-    return seg_status("seg_compose");
+    return launch("seg_compose", seg_compose_kernel, {grid, 256, 0, static_cast<cudaStream_t>(stream)}, table, labels, counts, plane, masks, mask_h,
+                  mask_w, overlap, out, out_dtype);
 }

@@ -658,11 +658,6 @@ static int check_view(const void* p, int pitch, int channels, const char* what) 
 static dim3 row_grid(const RowGeom& g, int channels, long long rows) {
     return dim3((channels / 8 + g.cgx - 1) / g.cgx, static_cast<unsigned>((rows + g.rpb - 1) / g.rpb));
 }
-static int launch_status(const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(int(e), "%s launch failed: %s", what, cudaGetErrorString(e));
-    return 0;
-}
 
 }  // namespace y5
 
@@ -693,10 +688,8 @@ extern "C" Y5_API int y5_bn_stats(const void* y, int32_t pitch, int64_t rows, in
     if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "bn_stats: dtype must be fp16 or bf16");
     if (!workspace || rows <= 0) return set_error(Y5_E_INVALID, "bn_stats: bad argument");
     const RowGeom g = row_geom(channels, rows, true);
-    count_launch();
-    launch_pdl(col_stats_kernel<0>, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream), 
-        y, pitch, rows, channels, dtype == Y5_BF16, g.cgx, g.rpb, static_cast<double*>(workspace), count);
-    return launch_status("bn_stats");
+    return launch("bn_stats", col_stats_kernel<0>, {row_grid(g, channels, rows), kRedThreads, 0, static_cast<cudaStream_t>(stream), /*pdl=*/true},
+                  y, pitch, rows, channels, dtype == Y5_BF16, g.cgx, g.rpb, static_cast<double*>(workspace), count);
 }
 
 extern "C" Y5_API int y5_bn_act_fwd(const void* y, int32_t y_pitch, void* z, int32_t z_pitch, int64_t rows, int32_t channels, int32_t dtype,
@@ -716,14 +709,12 @@ extern "C" Y5_API int y5_bn_act_fwd(const void* y, int32_t y_pitch, void* z, int
     const double inv_rows = 1.0 / static_cast<double>(rows);
     const double unbias = rows > 1 ? static_cast<double>(rows) / static_cast<double>(rows - 1) : 1.0;
     const double* s = static_cast<const double*>(sums);
-    count_launch();
     const bool leaky = act == Y5_ACT_LEAKY;
     auto* kernel = residual ? (leaky ? bn_act_fwd_kernel<true, true> : bn_act_fwd_kernel<true, false>)
                             : (leaky ? bn_act_fwd_kernel<false, true> : bn_act_fwd_kernel<false, false>);
-    launch_pdl(kernel, row_grid(g, channels, rows), dim3(kRedThreads), 0, static_cast<cudaStream_t>(stream),
-        y, y_pitch, z, z_pitch, rows, channels, dtype == Y5_BF16, act, g.cgx, g.rpb, mean, invstd, gamma, beta, s,
-        static_cast<const double*>(count), inv_rows, unbias, eps, momentum, running_mean, running_var, residual, res_pitch, slope);
-    return launch_status(what);
+    return launch(what, kernel, {row_grid(g, channels, rows), kRedThreads, 0, static_cast<cudaStream_t>(stream), /*pdl=*/true}, y, y_pitch, z,
+                  z_pitch, rows, channels, dtype == Y5_BF16, act, g.cgx, g.rpb, mean, invstd, gamma, beta, s, static_cast<const double*>(count),
+                  inv_rows, unbias, eps, momentum, running_mean, running_var, residual, res_pitch, slope);
 }
 
 static int bn_bwd_check(const char* what, const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
@@ -738,9 +729,9 @@ static int bn_bwd_check(const char* what, const void* y, int32_t y_pitch, const 
 
 // reduce pass: du = dz * act'(t) and its two column sums into the workspace.  SiLU and LeakyReLU layers: du is left in the dy
 // buffer and the apply pass finishes it in place; linear layers have du == dz
-static void bn_bwd_reduce_launch(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
-                                 int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, const float* beta,
-                                 int32_t act, float slope, void* workspace, cudaStream_t st) {
+static int bn_bwd_reduce_launch(const char* what, const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                                int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma,
+                                const float* beta, int32_t act, float slope, void* workspace, cudaStream_t st) {
     static const int red_u = env_int("Y5_BN_RED_U", 4);
     const RowGeom g = row_geom(channels, rows, true, red_u == 2 ? 3 : 2);
     using RedFn = void (*)(const void*, int, const void*, int, long long, int, int, int, const float*, const float*, const float*, const float*,
@@ -751,19 +742,19 @@ static void bn_bwd_reduce_launch(const void* y, int32_t y_pitch, const void* dz,
          {bn_act_bwd_reduce_kernel<4, true, N>, bn_act_bwd_reduce_kernel<4, true, S>, bn_act_bwd_reduce_kernel<4, true, L>}},
         {{bn_act_bwd_reduce_kernel<2, false, N>, bn_act_bwd_reduce_kernel<2, false, S>, bn_act_bwd_reduce_kernel<2, false, L>},
          {bn_act_bwd_reduce_kernel<2, true, N>, bn_act_bwd_reduce_kernel<2, true, S>, bn_act_bwd_reduce_kernel<2, true, L>}}};
-    launch_pdl(table[red_u == 2 ? 1 : 0][dtype == Y5_BF16 ? 1 : 0][act], row_grid(g, channels, rows), dim3(kRedThreads), 0, st, y, y_pitch, dz,
-               dz_pitch, rows, channels, g.cgx, g.rpb, mean, invstd, gamma, beta, static_cast<double*>(workspace),
-               act ? dy : static_cast<void*>(nullptr), dy_pitch, slope);
+    return launch(what, table[red_u == 2 ? 1 : 0][dtype == Y5_BF16 ? 1 : 0][act], {row_grid(g, channels, rows), kRedThreads, 0, st, /*pdl=*/true},
+                  y, y_pitch, dz, dz_pitch, rows, channels, g.cgx, g.rpb, mean, invstd, gamma, beta, static_cast<double*>(workspace),
+                  act ? dy : static_cast<void*>(nullptr), dy_pitch, slope);
 }
 
 // apply pass: dy from du and the column sums (count == NULL: divided by this call's rows); dgamma / dbeta written when non-NULL
-static void bn_bwd_apply_launch(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
-                                int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, int32_t act,
-                                const double* sums, const double* count, float* dgamma, float* dbeta, cudaStream_t st) {
+static int bn_bwd_apply_launch(const char* what, const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
+                               int64_t rows, int32_t channels, int32_t dtype, const float* mean, const float* invstd, const float* gamma, int32_t act,
+                               const double* sums, const double* count, float* dgamma, float* dbeta, cudaStream_t st) {
     const RowGeom ga = row_geom(channels, rows, false, 4);
-    launch_pdl(bn_act_bwd_apply_kernel, row_grid(ga, channels, rows), dim3(kRedThreads), 0, st, y, y_pitch, act ? static_cast<const void*>(dy) : dz,
-               act ? dy_pitch : dz_pitch, dy, dy_pitch, rows, channels, dtype == Y5_BF16, ga.cgx, ga.rpb, mean, invstd, gamma, sums, count, dgamma,
-               dbeta);
+    return launch(what, bn_act_bwd_apply_kernel, {row_grid(ga, channels, rows), kRedThreads, 0, st, /*pdl=*/true}, y, y_pitch,
+                  act ? static_cast<const void*>(dy) : dz, act ? dy_pitch : dz_pitch, dy, dy_pitch, rows, channels, dtype == Y5_BF16, ga.cgx,
+                  ga.rpb, mean, invstd, gamma, sums, count, dgamma, dbeta);
 }
 
 extern "C" Y5_API int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int32_t channels, int32_t dtype, float* out, void* workspace,
@@ -774,11 +765,10 @@ extern "C" Y5_API int y5_col_sum(const void* y, int32_t pitch, int64_t rows, int
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     cudaMemsetAsync(workspace, 0, static_cast<size_t>(channels) * sizeof(double), st);
     const RowGeom g = row_geom(channels, rows, true);
-    count_launch(2);
-    launch_pdl(col_stats_kernel<1>, row_grid(g, channels, rows), dim3(kRedThreads), 0, st, y, pitch, rows, channels, dtype == Y5_BF16, g.cgx, g.rpb,
-                                                                              static_cast<double*>(workspace), static_cast<double*>(nullptr));
-    col_sum_finalize_kernel<<<(channels + 127) / 128, 128, 0, st>>>(static_cast<const double*>(workspace), channels, out);
-    return launch_status("col_sum");
+    if (int e = launch("col_sum", col_stats_kernel<1>, {row_grid(g, channels, rows), kRedThreads, 0, st, /*pdl=*/true}, y, pitch, rows, channels,
+                       dtype == Y5_BF16, g.cgx, g.rpb, static_cast<double*>(workspace), static_cast<double*>(nullptr)))
+        return e;
+    return launch("col_sum", col_sum_finalize_kernel, {(channels + 127) / 128, 128, 0, st}, static_cast<const double*>(workspace), channels, out);
 }
 
 extern "C" Y5_API int y5_bn_act_bwd(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch, int64_t rows,
@@ -789,11 +779,11 @@ extern "C" Y5_API int y5_bn_act_bwd(const void* y, int32_t y_pitch, const void* 
     if (int e = bn_bwd_check(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace)) return e;
     if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "%s: bad argument", what);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    count_launch(2);
-    bn_bwd_reduce_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope, workspace, st);
-    bn_bwd_apply_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, act, static_cast<const double*>(workspace),
-                        nullptr, dgamma, dbeta, st);
-    return launch_status(what);
+    if (int e = bn_bwd_reduce_launch(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope,
+                                     workspace, st))
+        return e;
+    return bn_bwd_apply_launch(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, act,
+                               static_cast<const double*>(workspace), nullptr, dgamma, dbeta, st);
 }
 
 extern "C" Y5_API int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
@@ -805,11 +795,11 @@ extern "C" Y5_API int y5_bn_act_bwd_reduce(const void* y, int32_t y_pitch, const
     if (int e = bn_bwd_check(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, workspace)) return e;
     if (!beta || !dgamma || !dbeta) return set_error(Y5_E_INVALID, "%s: bad argument", what);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    count_launch(2);
-    bn_bwd_reduce_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope, workspace, st);
-    launch_pdl(bn_affine_grad_kernel, dim3((channels + 127) / 128), dim3(128), 0, st, static_cast<const double*>(workspace), static_cast<int>(channels),
-               dgamma, dbeta);
-    return launch_status(what);
+    if (int e = bn_bwd_reduce_launch(what, y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, beta, act, slope,
+                                     workspace, st))
+        return e;
+    return launch(what, bn_affine_grad_kernel, {(channels + 127) / 128, 128, 0, st, /*pdl=*/true}, static_cast<const double*>(workspace),
+                  static_cast<int>(channels), dgamma, dbeta);
 }
 
 extern "C" Y5_API int y5_bn_act_bwd_apply(const void* y, int32_t y_pitch, const void* dz, int32_t dz_pitch, void* dy, int32_t dy_pitch,
@@ -818,10 +808,8 @@ extern "C" Y5_API int y5_bn_act_bwd_apply(const void* y, int32_t y_pitch, const 
     if (int e = check_act("bn_act_bwd_apply", act, 0.0f)) return e;
     if (int e = bn_bwd_check("bn_act_bwd_apply", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, sums)) return e;
     if (!count) return set_error(Y5_E_INVALID, "bn_act_bwd_apply: bad argument");
-    count_launch();
-    bn_bwd_apply_launch(y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, act, static_cast<const double*>(sums),
-                        static_cast<const double*>(count), nullptr, nullptr, static_cast<cudaStream_t>(stream));
-    return launch_status("bn_act_bwd_apply");
+    return bn_bwd_apply_launch("bn_act_bwd_apply", y, y_pitch, dz, dz_pitch, dy, dy_pitch, rows, channels, dtype, mean, invstd, gamma, act,
+                               static_cast<const double*>(sums), static_cast<const double*>(count), nullptr, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" Y5_API int y5_zero_stuff2x(const void* x, int32_t x_pitch, void* y, int32_t y_pitch, int32_t batch, int32_t h, int32_t w, int32_t c,
@@ -831,11 +819,8 @@ extern "C" Y5_API int y5_zero_stuff2x(const void* x, int32_t x_pitch, void* y, i
     if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "zero_stuff2x: dtype must be fp16 or bf16");
     if (batch <= 0 || h <= 0 || w <= 0) return set_error(Y5_E_INVALID, "zero_stuff2x: bad shape");
     const long long total = static_cast<long long>(batch) * 4 * h * w * (c / 8);
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 16LL));
-    count_launch();
-    launch_pdl(zero_stuff2x_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), static_cast<const uint4*>(x), x_pitch / 8, static_cast<uint4*>(y),
-                                                                               y_pitch / 8, batch, h, w, c / 8);
-    return launch_status("zero_stuff2x");
+    return launch("zero_stuff2x", zero_stuff2x_kernel, {grid_stride_ctas(total, 256, 16), 256, 0, static_cast<cudaStream_t>(stream), /*pdl=*/true},
+                  static_cast<const uint4*>(x), x_pitch / 8, static_cast<uint4*>(y), y_pitch / 8, batch, h, w, c / 8);
 }
 
 extern "C" Y5_API int y5_weight_pack(const void* w, int32_t w_dtype, int32_t out_c, int32_t in_c, int32_t ksize, void* fwd, int32_t in_c_pad,
@@ -847,11 +832,8 @@ extern "C" Y5_API int y5_weight_pack(const void* w, int32_t w_dtype, int32_t out
         return set_error(Y5_E_INVALID, "weight_pack: bad shape");
     const long long total = (fwd ? static_cast<long long>(out_c) * ksize * ksize * in_c_pad : 0) +
                             (dgrad ? static_cast<long long>(in_c) * ksize * ksize * out_c_pad : 0);
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 8LL));
-    count_launch();
-    launch_pdl(weight_pack_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), w, w_dtype, out_c, in_c, ksize, static_cast<uint16_t*>(fwd), in_c_pad,
-                                                                              static_cast<uint16_t*>(dgrad), out_c_pad, dtype == Y5_BF16);
-    return launch_status("weight_pack");
+    return launch("weight_pack", weight_pack_kernel, {grid_stride_ctas(total, 256, 8), 256, 0, static_cast<cudaStream_t>(stream), /*pdl=*/true}, w,
+                  w_dtype, out_c, in_c, ksize, static_cast<uint16_t*>(fwd), in_c_pad, static_cast<uint16_t*>(dgrad), out_c_pad, dtype == Y5_BF16);
 }
 
 
@@ -862,10 +844,8 @@ extern "C" Y5_API int y5_weight_pack_multi(const y5_pack_item* items, const int3
     if (n_chunks == 0) return 0;
     if (!items || !chunk_item || !chunk_index || n_chunks < 0) return set_error(Y5_E_INVALID, "weight_pack_multi: bad argument");
     if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "weight_pack_multi: packed dtype must be fp16 or bf16");
-    count_launch();
-    launch_pdl(weight_pack_multi_kernel, dim3(static_cast<unsigned>(n_chunks)), dim3(256), 0, static_cast<cudaStream_t>(stream), items, chunk_item,
-               chunk_index, dtype == Y5_BF16);
-    return launch_status("weight_pack_multi");
+    return launch("weight_pack_multi", weight_pack_multi_kernel, {static_cast<unsigned>(n_chunks), 256, 0, static_cast<cudaStream_t>(stream), /*pdl=*/true},
+                  items, chunk_item, chunk_index, dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int y5_fold_pack(const void* w, int32_t w_dtype, int32_t out_c, int32_t in_c, int32_t kh, int32_t kw, const void* conv_bias,
@@ -878,12 +858,9 @@ extern "C" Y5_API int y5_fold_pack(const void* w, int32_t w_dtype, int32_t out_c
     if (out_c <= 0 || in_c <= 0 || kh <= 0 || kw <= 0 || in_c_pad < in_c || out_c_pad < out_c) return set_error(Y5_E_INVALID, "fold_pack: bad shape");
     if (gamma && (!beta || !mean || !var)) return set_error(Y5_E_INVALID, "fold_pack: BatchNorm needs gamma, beta, mean and var");
     const long long total = static_cast<long long>(out_c_pad) * kh * kw * in_c_pad;
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 8LL));
-    count_launch();
-    fold_pack_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(w, w_dtype, out_c, in_c, kh, kw, conv_bias, gamma, beta, mean, var,
-                                                                            bn_dtype, eps, static_cast<uint16_t*>(packed), in_c_pad, out_c_pad,
-                                                                            bias_out, dtype == Y5_BF16);
-    return launch_status("fold_pack");
+    return launch("fold_pack", fold_pack_kernel, {grid_stride_ctas(total, 256, 8), 256, 0, static_cast<cudaStream_t>(stream)}, w, w_dtype, out_c,
+                  in_c, kh, kw, conv_bias, gamma, beta, mean, var, bn_dtype, eps, static_cast<uint16_t*>(packed), in_c_pad, out_c_pad, bias_out,
+                  dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int y5_upsample2x_bwd(const void* dy, int32_t dy_pitch, void* dx, int32_t dx_pitch, int32_t batch, int32_t h, int32_t w, int32_t c,
@@ -893,10 +870,8 @@ extern "C" Y5_API int y5_upsample2x_bwd(const void* dy, int32_t dy_pitch, void* 
     if (dtype != Y5_F16 && dtype != Y5_BF16) return set_error(Y5_E_UNSUPPORTED, "upsample2x_bwd: dtype must be fp16 or bf16");
     if (batch <= 0 || h <= 0 || w <= 0) return set_error(Y5_E_INVALID, "upsample2x_bwd: bad shape");
     const long long total = static_cast<long long>(batch) * h * w * (c / 8);
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 16LL));
-    count_launch();
-    launch_pdl(upsample2x_bwd_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), dy, dy_pitch, dx, dx_pitch, batch, h, w, c, dtype == Y5_BF16);
-    return launch_status("upsample2x_bwd");
+    return launch("upsample2x_bwd", upsample2x_bwd_kernel, {grid_stride_ctas(total, 256, 16), 256, 0, static_cast<cudaStream_t>(stream), /*pdl=*/true},
+                  dy, dy_pitch, dx, dx_pitch, batch, h, w, c, dtype == Y5_BF16);
 }
 
 extern "C" Y5_API int64_t y5_sppf_bwd_workspace_bytes(int32_t batch, int32_t h, int32_t w, int32_t c) {
@@ -915,16 +890,20 @@ extern "C" Y5_API int y5_sppf_pool_bwd(const void* cat, int32_t cat_pitch, const
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long pixels = static_cast<long long>(batch) * h * w, total = pixels * c;
     const int bf = dtype == Y5_BF16;
-    const int blocks = static_cast<int>(std::min<long long>((total + 255) / 256, sm_count() * 16LL));
+    const int blocks = grid_stride_ctas(total, 256, 16);
     float* acc = static_cast<float*>(workspace);
     const uint16_t* cat16 = static_cast<const uint16_t*>(cat);
     const uint16_t* dcat16 = static_cast<const uint16_t*>(dcat);
-    count_launch(5);
-    sppf_bwd_init_kernel<<<blocks, 256, 0, st>>>(dcat, dcat_pitch, acc, pixels, c, bf);
+    const char* what = "sppf_pool_bwd";
+    if (int e = launch(what, sppf_bwd_init_kernel, {blocks, 256, 0, st}, dcat, dcat_pitch, acc, pixels, c, bf)) return e;
     // g3 -> acc2 through the windows of y2 (slice 2);  acc2 -> acc1 through y1 (slice 1);  acc1 -> acc0 through a (slice 0)
-    sppf_bwd_scatter_kernel<true><<<blocks, 256, 0, st>>>(cat16 + 2 * c, cat_pitch, dcat16 + 3 * c, dcat_pitch, acc + 2 * total, batch, h, w, c, ksize, bf);
-    sppf_bwd_scatter_kernel<false><<<blocks, 256, 0, st>>>(cat16 + c, cat_pitch, acc + 2 * total, c, acc + total, batch, h, w, c, ksize, bf);
-    sppf_bwd_scatter_kernel<false><<<blocks, 256, 0, st>>>(cat16, cat_pitch, acc + total, c, acc, batch, h, w, c, ksize, bf);
-    f32_to_lowp_kernel<<<blocks, 256, 0, st>>>(acc, da, da_pitch, pixels, c, bf);
-    return launch_status("sppf_pool_bwd");
+    if (int e = launch(what, sppf_bwd_scatter_kernel<true>, {blocks, 256, 0, st}, cat16 + 2 * c, cat_pitch, dcat16 + 3 * c, dcat_pitch,
+                       acc + 2 * total, batch, h, w, c, ksize, bf))
+        return e;
+    if (int e = launch(what, sppf_bwd_scatter_kernel<false>, {blocks, 256, 0, st}, cat16 + c, cat_pitch, acc + 2 * total, c, acc + total, batch,
+                       h, w, c, ksize, bf))
+        return e;
+    if (int e = launch(what, sppf_bwd_scatter_kernel<false>, {blocks, 256, 0, st}, cat16, cat_pitch, acc + total, c, acc, batch, h, w, c, ksize, bf))
+        return e;
+    return launch(what, f32_to_lowp_kernel, {blocks, 256, 0, st}, acc, da, da_pitch, pixels, c, bf);
 }
