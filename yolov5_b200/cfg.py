@@ -11,6 +11,9 @@ A user-supplied ``*.yaml`` path is still accepted by ``DetectionModel`` (see mod
 C3 (layer 8); it is a built-in name too, pinned by tests/test_transformer_cpu.py against a digest of that YAML.
 ``yolov5s-ghost`` (reference models/hub/yolov5s-ghost.yaml) is yolov5s built from GhostConv and C3Ghost; ``model_cfg`` accepts
 it, pinned by tests/test_ghost_cpu.py, but it is not one of ``model_names()``.
+``yolov5{n,s,m,l,x}6`` (reference models/hub/yolov5*6.yaml) are the P6 models: the same scales with a fifth, stride-64 backbone
+stage and a four-level Detect (P3-P6), trained and validated at 1280.  ``model_cfg`` accepts them, pinned by tests/test_p6_cpu.py;
+they are not among ``model_names()`` either.
 """
 from __future__ import annotations
 
@@ -91,6 +94,29 @@ def _yolov3(name: str) -> dict:
     return {"nc": 80, "depth_multiple": 1.0, "width_multiple": 1.0, "anchors": anchors, "backbone": backbone, "head": head}
 
 
+# reference models/hub/yolov5s6.yaml:12-16 (pixels, P3/P4/P5/P6)
+_ANCHORS_P6 = [[19, 27, 44, 40, 38, 94], [96, 68, 86, 152, 180, 137], [140, 301, 303, 264, 238, 542], [436, 615, 739, 380, 925, 792]]
+
+
+def _p6(scale: str) -> dict:
+    """Reference models/hub/yolov5{n,s,m,l,x}6.yaml as yaml.safe_load returns them: the v6.0 topology with a stride-64 level
+    (backbone Conv(1024, 3, 2) + C3 after a 768-channel P5) and a four-level Detect over P3-P6."""
+    down = lambda c: [-1, 1, "Conv", [c, 3, 2]]  # noqa: E731
+    csp = lambda c, n, *a: [-1, n, "C3", [c, *a]]  # noqa: E731
+    up = [-1, 1, "nn.Upsample", ["None", 2, "nearest"]]
+    backbone = [[-1, 1, "Conv", [64, 6, 2, 2]], down(128), csp(128, 3), down(256), csp(256, 6), down(512), csp(512, 9),
+                down(768), csp(768, 3), down(1024), csp(1024, 3), [-1, 1, "SPPF", [1024, 5]]]  # 11
+    head = []
+    for c, skip in ((768, 8), (512, 6), (256, 4)):  # top-down: layers 12-15, 16-19, 20-23 (P3 out)
+        head += [[-1, 1, "Conv", [c, 1, 1]], copy.deepcopy(up), [[-1, skip], 1, "Concat", [1]], csp(c, 3, False)]
+    for c_down, lat, c in ((256, 20, 512), (512, 16, 768), (768, 12, 1024)):  # bottom-up: P4 26, P5 29, P6 32
+        head += [down(c_down), [[-1, lat], 1, "Concat", [1]], csp(c, 3, False)]
+    head.append([[23, 26, 29, 32], 1, "Detect", ["nc", "anchors"]])
+    gd, gw = _SCALES[scale]
+    return {"nc": 80, "depth_multiple": gd, "width_multiple": gw, "anchors": copy.deepcopy(_ANCHORS_P6), "backbone": backbone,
+            "head": head}
+
+
 def _ghost() -> dict:
     """Reference models/hub/yolov5s-ghost.yaml as yaml.safe_load returns it: yolov5s with every stride-2 Conv and the head's 1x1
     Convs as GhostConv, and every C3 as C3Ghost."""
@@ -109,7 +135,7 @@ def model_names() -> list[str]:
 
 def model_cfg(name: str) -> dict:
     """Return the model dict for ``yolov5s`` / ``yolov5l.yaml`` / ``models/segment/yolov5x-seg.yaml`` /
-    ``models/hub/yolov5s-transformer.yaml`` ..."""
+    ``models/hub/yolov5s-transformer.yaml`` / ``models/hub/yolov5x6.yaml`` ..."""
     stem = Path(str(name)).name
     if stem.endswith(".yaml"):
         stem = stem[: -len(".yaml")]
@@ -121,6 +147,8 @@ def model_cfg(name: str) -> dict:
         return _yolov3(stem)
     if stem == "yolov5s-ghost":
         return _ghost()
+    if len(stem) == 8 and stem.startswith("yolov5") and stem[6] in _SCALES and stem[7] == "6":
+        return _p6(stem[6])
     seg = stem.endswith("-seg")
     key = stem[: -len("-seg")] if seg else stem
     if not (key.startswith("yolov5") and key[6:] in _SCALES):

@@ -77,8 +77,8 @@ def parse_model(d, ch):
     for i, (f, n, m, args) in enumerate(d["backbone"] + d["head"]):
         if isinstance(m, str):
             if m not in _MODULES:
-                raise NotImplementedError(f"y5b200: module '{m}' is outside the engine's hot path (models n/s/m/l/x[-seg], yolov3[-spp|-tiny], "
-                                          "yolov5s-ghost)")
+                raise NotImplementedError(f"y5b200: module '{m}' is outside the engine's hot path (models n/s/m/l/x[-seg], n6-x6, "
+                                          "yolov3[-spp|-tiny], yolov5s-ghost)")
             m = _MODULES[m]
         args = [names.get(a, a) if isinstance(a, str) else a for a in args]
         n = n_ = max(round(n * gd), 1) if n > 1 else n
