@@ -71,7 +71,7 @@ def _mask_term(pmask, proto, masks, b, tidx, xywhn, overlap):
     marea = xywhn[:, 2:].prod(1)
     xy = xywhn * torch.tensor([mw, mh, mw, mh], device=xywhn.device, dtype=xywhn.dtype)
     mxyxy = torch.cat((xy[:, :2] - xy[:, 2:] / 2, xy[:, :2] + xy[:, 2:] / 2), 1)
-    lseg = torch.zeros(1, device=proto.device)
+    lseg = torch.zeros(1, device=proto.device, dtype=proto.dtype)  # float64 inputs accumulate in float64
     for bi in b.unique():
         j = b == bi
         if overlap:
@@ -79,7 +79,7 @@ def _mask_term(pmask, proto, masks, b, tidx, xywhn, overlap):
         else:
             gt = masks[tidx][j]
         pred = (pmask[j] @ proto[bi].reshape(nm, -1)).view(-1, mh, mw)
-        loss = F.binary_cross_entropy_with_logits(pred, gt, reduction="none")
+        loss = F.binary_cross_entropy_with_logits(pred, gt.to(pred.dtype), reduction="none")
         x1, y1, x2, y2 = torch.chunk(mxyxy[j][:, :, None], 4, 1)
         r = torch.arange(mw, device=pred.device, dtype=x1.dtype)[None, None, :]
         c = torch.arange(mh, device=pred.device, dtype=x1.dtype)[None, :, None]
@@ -99,7 +99,7 @@ def compute_seg_loss(p, proto, targets, masks, anchors, hyp, overlap, balance=(4
     lbox, lobj, lcls = items.view(3, 1).unbind(0)
     bt = build_targets_seg(tg, anc, [tuple(pi.shape[2:4]) for pi in p], bs, overlap, hyp["anchor_t"])
     masks = _downsample(torch.as_tensor(masks, dtype=torch.float32), proto)
-    lseg = torch.zeros(1)
+    lseg = torch.zeros(1, dtype=proto.dtype)
     for i, pi in enumerate(p):
         d = bt[i]
         if len(d["b"]):
